@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- routing decisions/s of the EPP scheduling cycle on B200 (BASELINE.json metric).
+"""bench.py -- routing decisions/s of the EPP scheduling cycle on H100 (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload config3] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload config3] [--impl reference] [--dump-outputs DIR]
 
 One "step" = one pass of the whole hot path (prefix-block hashing -> index lookup / global-stop match -> load scoring
 -> weighted sum -> arg-max pick [-> decider -> prefill pick]) over one batch of synthetic requests.
@@ -11,12 +11,15 @@ One "step" = one pass of the whole hot path (prefix-block hashing -> index looku
   roofline  dominant kernel: algorithmic bytes per launch / CUDA-event launch time vs MEASURED_PEAKS.json hbm_gbs
   cpu_baseline  the oracle (C restatement of the reference Go loops, kind "port") on the host cores, bounded sample
 --impl reference: times the reference's CPU algorithm (the oracle port; Go is not installable here) on all host cores.
+--dump-outputs DIR: after the timed steps, the decision records of the last timed step, one float64 array per field, as
+DIR/decision_<field>.npy (inputs are seeded: equal arguments give equal inputs, so two builds can be compared).
 Multi-GPU (--gpus N under torchrun): N independent replicas, each with the full index and its own batch (weak
 scaling, no data-path collective); time = max over ranks.
 """
 from __future__ import annotations
 
 import argparse
+import atexit
 import ctypes as C
 import json
 import os
@@ -44,7 +47,7 @@ def _peaks():
             p = json.load(f)
         return float(p["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "fallback (H100 SXM data sheet HBM3 bandwidth)"
 
 
 class ClockSampler:
@@ -62,6 +65,7 @@ class ClockSampler:
         try:
             self.proc = subprocess.Popen(["nvidia-smi", f"--query-gpu={self.Q}", "--format=csv,noheader,nounits",
                                           "-lms", "100", "-i", str(self.idx)], stdout=subprocess.PIPE, text=True)
+            atexit.register(self.proc.kill)          # never outlive the benchmark, also when it fails before stop()
             self.t = threading.Thread(target=self._read, daemon=True)
             self.t.start()
         except Exception:
@@ -127,6 +131,23 @@ def _pinned(nbytes: int, lib):
     return p, np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_uint8)), shape=(nbytes,))
 
 
+DUMP_MAX_BYTES = 64 << 20
+
+
+def dump_decisions(out_dir: str, dec: np.ndarray):
+    """Decision records as DIR/decision_<field>.npy, float64 (every field is exact in it).  Above 64 MB in all, a fixed
+    seeded sample of rows is written, and its row numbers as DIR/decision_rows.npy."""
+    os.makedirs(out_dir, exist_ok=True)
+    fields = list(dec.dtype.names)
+    max_rows = DUMP_MAX_BYTES // (8 * (len(fields) + 1))
+    if dec.shape[0] > max_rows:
+        rows = np.sort(np.random.default_rng(0).choice(dec.shape[0], max_rows, replace=False))
+        dec = dec[rows]
+        np.save(os.path.join(out_dir, "decision_rows.npy"), rows.astype(np.float64))
+    for f in fields:
+        np.save(os.path.join(out_dir, f"decision_{f}.npy"), dec[f].astype(np.float64))
+
+
 def _workload(name: str, R: int | None):
     from tools import tracegen as tg
     w = tg.baseline_configs()[name]
@@ -143,7 +164,7 @@ def _config_json(w, n_gpus, extra=None):
                         if w.prefill_scorers else ""),
          "endpoints": w.E, "prompt_tokens": w.T, "batch_requests_per_gpu": w.R, "block_size_tokens": w.block_size_tokens,
          "max_prefix_blocks": w.max_prefix_blocks,
-         "l2": f"inputs are {w.R * w.prompt_bytes / 2**20:.0f} MiB per step per GPU, larger than the 126 MB L2 (no flush needed)",
+         "l2": f"inputs are {w.R * w.prompt_bytes / 2**20:.0f} MiB per step per GPU, larger than the 50 MB L2 (no flush needed)",
          "parallelism": f"{n_gpus} independent replicas (index replicated, requests sharded; no data-path collective)",
          "trace_seed": hex(w.seed)}
     if extra:
@@ -397,6 +418,8 @@ def run_gpu(args, rank, world, local_rank):
     torch.cuda.synchronize()
     wall = time.perf_counter() - t0
     timed_ms = eng.event_elapsed_ms()
+    if args.dump_outputs and rank == 0:
+        dump_decisions(args.dump_outputs, epp.decisions_from_torch(dev_dec))     # the last timed step's decisions
     timed_launches = int(eng.stats()["last_kernel_launches"]) * args.steps      # kernels of one async batch x K
     barrier()
     wall = max_over_ranks(wall)
@@ -588,7 +611,7 @@ def run_gpu(args, rank, world, local_rank):
         dist.destroy_process_group()
 
 
-def sharded_leg(args, rank, world, local_rank, steps, warmup):
+def sharded_leg(args, rank, world, local_rank, steps, warmup, dump_dir=None):
     """BASELINE config 5: the endpoint index sharded across the GPUs (4 096 endpoints per GPU, E = 4 096 x N), every
     rank schedules the same batch of R requests; per batch two small exchanges (presence masks, best records) over
     NVLink peer memory (default) or NCCL (--sharded-nccl).  torch.distributed must be initialised when world > 1.
@@ -646,6 +669,8 @@ def sharded_leg(args, rank, world, local_rank, steps, warmup):
     ev1.record()
     torch.cuda.synchronize()
     wall = time.perf_counter() - t0
+    if dump_dir and rank == 0:
+        dump_decisions(dump_dir, epp.decisions_from_torch(dec))                  # the last timed step's decisions
     barrier()
     if world > 1:
         t = torch.tensor([wall], dtype=torch.float64, device="cuda")
@@ -698,7 +723,7 @@ def run_gpu_sharded(args, rank, world, local_rank):
         dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
     epp.build.build()
     tg.build()
-    res = sharded_leg(args, rank, world, local_rank, args.steps, args.warmup)
+    res = sharded_leg(args, rank, world, local_rank, args.steps, args.warmup, dump_dir=args.dump_outputs)
     if rank == 0:
         out = {"metric": METRIC + " (endpoint-sharded index)", "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
                "dtype": "u64 (XXH64) + f64 (scores)", "data": "synthetic"}
@@ -761,6 +786,8 @@ def main():
                          "a table far larger than L2); decisions are unchanged")
     ap.add_argument("--pitch-pad", type=int, default=0,
                     help="experiment: lay the device-resident prompts out with this many pad bytes between requests")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the decisions of the last timed step to DIR/decision_<field>.npy (float64)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
     rank = int(os.environ.get("RANK", "0"))

@@ -1,5 +1,5 @@
 /*
- * epp_engine.h -- C ABI of libepp_engine.so, the B200-native Endpoint-Picker scoring engine.
+ * epp_engine.h -- C ABI of libepp_engine.so, the H100-native Endpoint-Picker scoring engine.
  *
  * The reference (llm-d/llm-d-inference-scheduler @ 520af478, pure Go, CGO_ENABLED=0) has NO FFI; this
  * header is the boundary the build introduces (SURVEY.md 8(b)).  Every entry point names the reference

@@ -1,10 +1,10 @@
-"""llm-d-inference-scheduler_b200 -- B200-native Endpoint-Picker scoring engine (hot path only).
+"""llm-d-inference-scheduler_b200 -- H100-native Endpoint-Picker scoring engine (hot path only).
 
-csrc/        hand-written sm_100a CUDA kernels + the C ABI (include/epp_engine.h) -> libepp_engine.so
+csrc/        hand-written sm_90a CUDA kernels + the C ABI (include/epp_engine.h) -> libepp_engine.so
 _capi.py     ctypes view of the C ABI
 engine.py    Engine: marshals numpy / torch-CUDA buffers into the ABI
 plugins.py   host-side mirror of the reference's Scorer/Filter/Scheduler/DataProducer interface for this path
-build.py     nvcc build (in-tree, sm_100a)
+build.py     nvcc build (in-tree, sm_90a)
 
 The directory name is not a Python identifier; import it with importlib (see epp_b200.py at the repo root).
 """

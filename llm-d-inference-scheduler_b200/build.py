@@ -1,4 +1,4 @@
-"""Builds libepp_engine.so IN-TREE with nvcc for sm_100a (cross-compiles without a GPU).
+"""Builds libepp_engine.so IN-TREE with nvcc for sm_90a (H100; cross-compiles without a GPU).
 
     python llm-d-inference-scheduler_b200/build.py [--force] [--verbose]
 """
@@ -14,7 +14,7 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libepp_engine.so")
 SOURCES = ["engine.cu", "batcher.cu", "hash_kernels.cu", "hash_fused.cu", "hash_staged.cu", "index_kernels.cu", "index_store.cu", "pick_kernels.cu", "match_sparse.cu", "cycle_small.cu", "shard_p2p.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-fmad=false",                      # fp64 scoring must never fuse x*y+z (Go/amd64 semantics)
     "-Xcompiler", "-fPIC,-O2,-Wall,-fvisibility=hidden",

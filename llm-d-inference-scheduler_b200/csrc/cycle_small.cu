@@ -10,8 +10,8 @@
 //              prompt -- into shared memory, from HBM or straight from the caller's pinned host memory over PCIe;
 //   warps 0-7  digest: every thread hashes the 32-byte stripes of "its" blocks out of shared memory and leaves the merged
 //              stripe state of each FULL block there (256 blocks = one per thread);
-//   warp 8     chain: ONE lane walks the blocks in order (the serial part of hashPrompt, hashing.go:80-96; ~84 ns per
-//              block: five dependent 64-bit multiplies), stores every hash to the request's row in HBM (the stash
+//   warp 8     chain: ONE lane walks the blocks in order (the serial part of hashPrompt, hashing.go:80-96; five
+//              dependent 64-bit multiplies per block), stores every hash to the request's row in HBM (the stash
 //              PreRequest needs) and over the block's stripe state in shared memory, and publishes its progress there
 //              every 32 blocks (no global fence on the critical path);
 //   warp 1     match: after its digests, runs sparse::match_request in FOLLOW mode -- it probes the index 32 blocks at
@@ -20,7 +20,7 @@
 //              while the chain is still hashing.  It then copies the decision to host memory and raises the flag.
 // Every prompt byte is consumed before the chain starts (the trailing partial block is parked in shared memory by the idle
 // chain warp): once a request's flag is up, its input may be overwritten.
-// The critical path is the chain (256 blocks x ~84 ns for a 16 KiB prompt) + one PCIe round trip each way.
+// The critical path is the chain (256 dependent blocks for a 16 KiB prompt) + one PCIe round trip each way.
 #include "hash_blocks.cuh"
 #include "match_sparse.cuh"
 
@@ -32,7 +32,7 @@ constexpr int kThreads = kDigestThreads + 32;
 
 // Hand-over of the hashes from the chain lane to the match warp: plain shared-memory stores published by a release
 // store of the progress word, consumed behind an acquire load (CTA scope).  compute-sanitizer's racecheck models
-// barriers only and reports this flag protocol as hazards (profiles/r2_sanitizer_racecheck.log); memcheck is clean.
+// barriers only and reports this flag protocol as hazards.
 __device__ __forceinline__ void st_release_cta(int32_t *p, int32_t v) {
     asm volatile("st.release.cta.shared.s32 [%0], %1;" ::"r"((uint32_t)__cvta_generic_to_shared(p)), "r"(v) : "memory");
 }
@@ -43,7 +43,7 @@ __device__ __forceinline__ int32_t ld_acquire_cta(const int32_t *p) {
 }
 // Poll word written by the copy stream (device memory, so L2 is the point of coherence).  Relaxed on purpose: an acquire at
 // system scope is a MEMBAR.SYS per poll, and a thousand CTAs issuing those while the copy engine streams the prompts in
-// cut its rate by a third to a half (DESIGN.md section 11.2); one GPU-scope fence after the wait orders the reads behind it.
+// slow it down; one GPU-scope fence after the wait orders the reads behind it.
 __device__ __forceinline__ uint32_t ld_relaxed_gpu(const uint32_t *p) {
     uint32_t v;
     asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
@@ -101,7 +101,7 @@ struct ChainFollower {
 
 // kStage: the prompt is staged into shared memory by ONE bulk copy (TMA) per request; else the digest threads load their
 // blocks themselves (prompts too long for the staging buffer).
-template <bool kAlign32, bool kStage>
+template <bool kStage>
 __global__ void __launch_bounds__(kThreads) k_cycle_small(HashParams hp, PickParams pp, SmallOut so, uint32_t stage_off) {
     extern __shared__ __align__(128) uint64_t s_m[];   // [max_blocks] merged stripe state of every full block; then, at byte
                                                        // stage_off, (kStage) the prompt's full blocks and its trailing partial block
@@ -163,7 +163,7 @@ __global__ void __launch_bounds__(kThreads) k_cycle_small(HashParams hp, PickPar
         } else {
             const uint8_t *base = hp.data + s_off;
             for (int32_t b = t; b < nfull; b += kDigestThreads)
-                s_m[b] = block_digest<kAlign32>(base + (uint64_t)b * (uint64_t)bs, n_stripes);
+                s_m[b] = block_digest(base + (uint64_t)b * (uint64_t)bs, n_stripes);
         }
     } else if (warp == kDigestThreads / 32) {
         // The trailing partial block is hashed LAST, long after a cold request may have raised its flag (global stop), and
@@ -236,7 +236,7 @@ bool cycle_small_stages_prompt(int32_t max_blocks, int32_t block_bytes) {
     return m_bytes + (size_t)max_blocks * (size_t)block_bytes <= 160 * 1024;
 }
 
-cudaError_t launch_cycle_small(const HashParams &hp, const PickParams &pp, const SmallOut &so, int align, cudaStream_t s,
+cudaError_t launch_cycle_small(const HashParams &hp, const PickParams &pp, const SmallOut &so, cudaStream_t s,
                                int *launches) {
     if (hp.R <= 0) return cudaSuccess;
     const size_t m_bytes = (sizeof(uint64_t) * (size_t)hp.max_blocks + 127) & ~(size_t)127;
@@ -248,22 +248,15 @@ cudaError_t launch_cycle_small(const HashParams &hp, const PickParams &pp, const
     cudaGetDevice(&dev);
     static bool attr_set[64] = {};                 // function attributes are per device: engines of one process may sit on several GPUs
     if (!attr_set[dev & 63]) {
-        cudaError_t e = cudaFuncSetAttribute(k_cycle_small<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(k_cycle_small<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(k_cycle_small<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(k_cycle_small<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
+        cudaError_t e = cudaFuncSetAttribute(k_cycle_small<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(k_cycle_small<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
         if (e != cudaSuccess) return e;
         attr_set[dev & 63] = true;
     }
     const unsigned grid = (unsigned)hp.R;
     const uint32_t off = (uint32_t)m_bytes;
-    if (stage) {
-        if (align >= 32) k_cycle_small<true, true><<<grid, kThreads, smem, s>>>(hp, pp, so, off);
-        else k_cycle_small<false, true><<<grid, kThreads, smem, s>>>(hp, pp, so, off);
-    } else {
-        if (align >= 32) k_cycle_small<true, false><<<grid, kThreads, smem, s>>>(hp, pp, so, off);
-        else k_cycle_small<false, false><<<grid, kThreads, smem, s>>>(hp, pp, so, off);
-    }
+    if (stage) k_cycle_small<true><<<grid, kThreads, smem, s>>>(hp, pp, so, off);
+    else k_cycle_small<false><<<grid, kThreads, smem, s>>>(hp, pp, so, off);
     if (launches) *launches += 1;
     return cudaGetLastError();
 }

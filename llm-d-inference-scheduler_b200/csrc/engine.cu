@@ -71,7 +71,7 @@ struct epp_engine {
     epp_config cfg;
     int n_profiles = 1;             // profiles of the P/D handler: 1 (single) or 2 (decode + prefill)
     int n_alloc_profiles = 1;       // + the encode profile ([2]) when configured
-    int sm_count = 148;
+    int sm_count = 132;
     int32_t Epad = 0;
     size_t dev_bytes = 0;
     size_t max_smem_optin = 0;
@@ -122,7 +122,8 @@ struct epp_engine {
     DevBuf offsets, lengths, model_ids, multimodal, hashes, nblocks, eff_len, in_len, decisions, details, flag;
     DevBuf dense_match, dense_total, dense_scores;
     int index_load = 0;             // EPP_INDEX_LOAD=n: read-table slots per distinct hash (2 = load factor <= 0.5, 4 = <= 0.25);
-                                    // 0 = automatic: 4 while the table stays L2-sized (<= 48 MiB), else 2
+                                    // 0 = automatic: 4 while the table stays L2-sized (<= l2_table_bytes), else 2
+    uint64_t l2_table_bytes = 24ull << 20;  // half the device's L2: the other half stays for the streamed prompts
     int dev_chunks = 2;             // EPP_DEV_CHUNKS=N: async device batches run as N chunks over both streams (1 = off)
     int staged = 0;                 // EPP_HASH_STAGED: 0 = hash_fused.cu (default), 1 = hash_staged.cu default shape, else a shape
     int pick_grid = 0;
@@ -280,6 +281,7 @@ extern "C" int32_t epp_engine_create(const epp_config *cfg, epp_engine **out) {
     CUDA_TRY(cudaGetDeviceProperties(&prop, cfg->device));
     e->sm_count = prop.multiProcessorCount;
     e->max_smem_optin = prop.sharedMemPerBlockOptin;
+    if (prop.l2CacheSize > 0) e->l2_table_bytes = (uint64_t)prop.l2CacheSize / 2;
     int32_t Ep = 1;
     while (Ep < cfg->max_endpoints) Ep <<= 1;
     e->Epad = Ep;
@@ -315,7 +317,7 @@ extern "C" int32_t epp_engine_create(const epp_config *cfg, epp_engine **out) {
         const epp_profile_cfg &pc = pi == 0 ? cfg->primary : (pi == 1 ? cfg->prefill : cfg->encode);
         if (pc.affinity_threshold > 0.0) e->general = true;
     }
-    e->store.reset(new IndexStore((uint32_t)cfg->max_endpoints, cfg->lru_capacity_per_server));
+    e->store.reset(new IndexStore((uint32_t)cfg->max_endpoints, cfg->lru_capacity_per_server, e->sm_count));
     { const char *v1 = getenv("EPP_INDEX_PATCH"); e->patch_enabled = v1 ? atoi(v1) : 1; }
     { const char *v1 = getenv("EPP_INDEX_LOAD"); e->index_load = v1 ? std::max(2, atoi(v1)) : 0; }
     { const char *v1 = getenv("EPP_DEV_CHUNKS"); e->dev_chunks = v1 ? std::max(1, atoi(v1)) : 2; }
@@ -594,9 +596,9 @@ static int32_t build_index_from_device_pairs(epp_engine *h, uint64_t n, uint64_t
     uint32_t cursor[4] = {0, 0, 0, 0};
     uint64_t cap = 16;
     for (int pass = 0; pass < 2; pass++) {
-        // load factor <= 0.5 over the distinct hashes (<= 0.25 while the table stays L2-sized: shorter probe chains, measured
-        // 10 % faster match kernel); the first pass only knows an upper bound (the pair count)
-        const uint64_t load = h->index_load ? (uint64_t)h->index_load : (4 * distinct * sizeof(IndexSlot) <= (48ull << 20) ? 4 : 2);
+        // load factor <= 0.5 over the distinct hashes (<= 0.25 while the table stays L2-sized: shorter probe chains, a faster
+        // step on H100, profiles/h100_index_load_ab.jsonl); the first pass only knows an upper bound (the pair count)
+        const uint64_t load = h->index_load ? (uint64_t)h->index_load : (4 * distinct * sizeof(IndexSlot) <= h->l2_table_bytes ? 4 : 2);
         uint64_t want = std::max<uint64_t>(16, load * distinct);
         cap = 16;
         while (cap < want) cap <<= 1;
@@ -612,7 +614,7 @@ static int32_t build_index_from_device_pairs(epp_engine *h, uint64_t n, uint64_t
         CUDA_TRY(cudaMemcpyAsync(cursor, h->idx_cursor.p, sizeof cursor, cudaMemcpyDeviceToHost, s));
         CUDA_TRY(cudaStreamSynchronize(s));
         uint64_t true_distinct = std::max<uint64_t>(1, cursor[2]);
-        const uint64_t load2 = h->index_load ? (uint64_t)h->index_load : (4 * true_distinct * sizeof(IndexSlot) <= (48ull << 20) ? 4 : 2);
+        const uint64_t load2 = h->index_load ? (uint64_t)h->index_load : (4 * true_distinct * sizeof(IndexSlot) <= h->l2_table_bytes ? 4 : 2);
         uint64_t tight = 16;
         while (tight < load2 * true_distinct) tight <<= 1;
         if (tight >= cap) break;            // already as small as the load factor allows
@@ -1036,7 +1038,7 @@ static int32_t launch_match(epp_engine *h, Slot &sl, PickParams pp, int *launche
 }
 
 // The whole cycle for one Work item: hash kernel, then the standalone match / score / pick kernel (every fused or
-// concurrently scheduled arrangement of the two was measured slower, DESIGN.md section 11).
+// concurrently scheduled arrangement of the two was measured slower).
 static int32_t launch_cycle(epp_engine *h, Slot &sl, const HashParams &hp, PickParams pp, int *launches, cudaEvent_t *ev) {
     CUDA_TRY(launch_hash_prompts(hp, sl.stream, launches, ev));
     return launch_match(h, sl, pp, launches);
@@ -1096,8 +1098,8 @@ static const uint8_t *device_view_of_pinned(const void *p) {
 
 // Is this host batch one for the single-launch path?  Returns 0 = no; 1 = the kernel reads the prompts from the
 // caller's pinned memory over PCIe (*data_dev = their device view); 2 = one DMA copy into HBM first (SM-issued PCIe
-// reads top out near 20 GB/s, the copy engine reaches 55: beyond a handful of prompts the copy wins).
-static int small_batch_mode(epp_engine *h, const BatchView &v, const uint8_t **data_dev, int *align) {
+// reads are slower than the copy engine: beyond a handful of prompts the copy wins).
+static int small_batch_mode(epp_engine *h, const BatchView &v, const uint8_t **data_dev) {
     if (v.device || h->small_max <= 0 || v.R > h->small_max || h->general) return 0;
     if (h->shard_begin != 0 || h->shard_end != 0xFFFFFFFFu) return 0;
     const int64_t bs = (int64_t)h->cfg.block_size_tokens * 4;
@@ -1107,13 +1109,11 @@ static int small_batch_mode(epp_engine *h, const BatchView &v, const uint8_t **d
         *data_dev = v.total_bytes ? device_view_of_pinned(v.data) : nullptr;
         if (*data_dev || !v.total_bytes) {
             const uint64_t bits = reinterpret_cast<uintptr_t>(*data_dev) | layout_bits;
-            *align = (bits & 31) == 0 ? 32 : ((bits & 15) == 0 ? 16 : 0);
-            if (*align >= 16) return 1;
+            if ((bits & 15) == 0) return 1;
         }
     }
     // the staged copy keeps the caller's layout modulo 32 (see run_batch), so only the layout decides the alignment
-    *align = (layout_bits & 31) == 0 ? 32 : ((layout_bits & 15) == 0 ? 16 : 0);
-    return *align >= 16 ? 2 : 0;
+    return (layout_bits & 15) == 0 ? 2 : 0;
 }
 
 // cuStreamWriteValue32 through the runtime's driver-entry-point lookup (no link against libcuda); nullptr when absent.
@@ -1131,8 +1131,8 @@ static StreamWriteValue32 stream_write_value32() {
     return fn;
 }
 
-static int32_t run_small(epp_engine *h, const BatchView &v, int mode, const uint8_t *data_dev, int align,
-                         epp_decision *out_dec, epp_decision_detail *out_detail) {
+static int32_t run_small(epp_engine *h, const BatchView &v, int mode, const uint8_t *data_dev, epp_decision *out_dec,
+                         epp_decision_detail *out_detail) {
     const int64_t R = v.R;
     cudaStream_t s0 = h->slot[0].stream;
     EPP_TRY(reserve_batch(h, R));
@@ -1195,7 +1195,7 @@ static int32_t run_small(epp_engine *h, const BatchView &v, int mode, const uint
     SmallOut so{h->small_dec, h->small_det, h->small_flags, epoch, arrive};
     int launches = 0;
     CUDA_TRY(cudaEventRecord(h->ev[0], s0));
-    CUDA_TRY(launch_cycle_small(hash_params(h, w), pp, so, align, s0, &launches));
+    CUDA_TRY(launch_cycle_small(hash_params(h, w), pp, so, s0, &launches));
     CUDA_TRY(cudaEventRecord(h->ev[1], s0));
 
     // wait for the flag word of every request (written after a system-scope fence behind its decision)
@@ -1350,9 +1350,8 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
     // ---- small host batch in pinned memory: one zero-copy launch, no copy engine, no stream synchronisation
     if (mode == Mode::Schedule && !tk && out_dec) {
         const uint8_t *data_dev = nullptr;
-        int align = 0;
-        const int sm = small_batch_mode(h, v, &data_dev, &align);
-        if (sm) return run_small(h, v, sm, data_dev, align, out_dec, out_detail);
+        const int sm = small_batch_mode(h, v, &data_dev);
+        if (sm) return run_small(h, v, sm, data_dev, out_dec, out_detail);
     }
 
     // ---- host batch: upload the small per-request arrays once, then pipeline the prompt bytes

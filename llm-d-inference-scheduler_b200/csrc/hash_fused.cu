@@ -1,7 +1,7 @@
 // hash_fused.cu -- a1 (hashPrompt, approximateprefix/hashing.go:35-99) as one CTA-cooperative kernel with register-fed
-// 128/256-bit global loads: the DEFAULT hash kernel of the throughput path (block sizes that are a multiple of 32
+// 128-bit global loads: the DEFAULT hash kernel of the throughput path (block sizes that are a multiple of 32
 // bytes, 16-byte aligned prompts; everything else takes the generic kernels of hash_kernels.cu).  hash_staged.cu is the
-// cp.async-staged alternative behind EPP_HASH_STAGED=1 (measured slower, DESIGN.md section 4.1).
+// cp.async-staged alternative behind EPP_HASH_STAGED=1 (DESIGN.md section 4.1).
 //
 // HBM traffic per request: every prompt byte is read exactly once, the 8-byte pre-chain digests never leave the SM
 // (shared-memory ring), the block hashes are written once (the PluginState stash PreRequest needs, plugin.go:150-157).
@@ -93,7 +93,6 @@ __device__ __forceinline__ uint64_t chain_window(uint64_t (*sm)[W + 1], const in
 }
 }  // namespace
 
-template <bool kAlign32>
 __global__ void __launch_bounds__(32 * kWin + 32, kHashMinCtas) k_hash_fused(HashParams p, int n_tiles) {
     constexpr int TR = 32, W = kWin;
     constexpr int kDigestWarps = TR * W / 32;
@@ -129,7 +128,7 @@ __global__ void __launch_bounds__(32 * kWin + 32, kHashMinCtas) k_hash_fused(Has
                 if (k >= kStages) bar_sync(kBarEmpty + s, kProducers);
 #pragma unroll
                 for (int u = 0; u < kSub; u++, src += win_bytes, left -= W)
-                    if (left > 0) s_m[s][u][r][j] = block_digest<kAlign32>(src, n_stripes);
+                    if (left > 0) s_m[s][u][r][j] = block_digest(src, n_stripes);
                 bar_arrive(kBarFull + s, kProducers);     // bar.arrive orders the stores above for the threads of the barrier
             }
             const int first = n_st > kStages ? n_st - kStages : 0;
@@ -158,23 +157,20 @@ __global__ void __launch_bounds__(32 * kWin + 32, kHashMinCtas) k_hash_fused(Has
     }
 }
 
-cudaError_t launch_hash_fused(const HashParams &p, int align, int sm_count, cudaStream_t s, int *launches) {
+cudaError_t launch_hash_fused(const HashParams &p, int sm_count, cudaStream_t s, int *launches) {
     if (p.R <= 0) return cudaSuccess;
-    const bool a32 = align >= 32;
     int dev = 0;
     cudaGetDevice(&dev);
-    static int occ_dev[2][64] = {};                  // resident CTAs per SM, per variant and device
-    int &occ = occ_dev[a32 ? 1 : 0][dev & 63];
+    static int occ_dev[64] = {};                     // resident CTAs per SM, per device
+    int &occ = occ_dev[dev & 63];
     if (!occ) {
-        if (a32) cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_hash_fused<true>, 32 * kWin + 32, 0);
-        else cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_hash_fused<false>, 32 * kWin + 32, 0);
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_hash_fused, 32 * kWin + 32, 0);
         if (occ < 1) occ = 1;
     }
-    if (sm_count <= 0) sm_count = 148;
+    if (sm_count <= 0) sm_count = 132;
     const int n_tiles = (int)((p.R + 31) / 32);
     const int grid = n_tiles < sm_count * occ ? n_tiles : sm_count * occ;
-    if (a32) k_hash_fused<true><<<grid, 32 * kWin + 32, 0, s>>>(p, n_tiles);
-    else k_hash_fused<false><<<grid, 32 * kWin + 32, 0, s>>>(p, n_tiles);
+    k_hash_fused<<<grid, 32 * kWin + 32, 0, s>>>(p, n_tiles);
     if (launches) *launches += 1;
     return cudaGetLastError();
 }

@@ -88,7 +88,7 @@ __global__ void __launch_bounds__(128) k_hash_generic(HashParams p) {
 }
 
 // Common alignment (0, 16 or 32 bytes) of every block start of the batch; the vectorised paths need
-// block_bytes % 32 == 0 and alignment >= 16 (128-bit loads) or 32 (256-bit loads, one per XXH64 stripe).
+// block_bytes % 32 == 0 and alignment >= 16 (128-bit loads).
 int hash_batch_alignment(const HashParams &p) {
     if (p.block_bytes <= 0 || (p.block_bytes % 32) != 0) return 0;
     uint64_t bits = reinterpret_cast<uintptr_t>(p.data);
@@ -107,7 +107,7 @@ cudaError_t launch_check_offsets_aligned(const uint64_t *offsets, int64_t n, int
     return cudaGetLastError();
 }
 
-cudaError_t launch_hash_fused(const HashParams &p, int align, int sm_count, cudaStream_t s, int *launches);
+cudaError_t launch_hash_fused(const HashParams &p, int sm_count, cudaStream_t s, int *launches);
 
 // ev (optional, 4 events): recorded around the hash kernel(s): [1]..[2] brackets the kernel that reads the prompt bytes.
 cudaError_t launch_hash_prompts(const HashParams &p, cudaStream_t s, int *launches, cudaEvent_t *ev) {
@@ -117,7 +117,7 @@ cudaError_t launch_hash_prompts(const HashParams &p, cudaStream_t s, int *launch
         if (ev) { cudaEventRecord(ev[0], s); cudaEventRecord(ev[1], s); }
         cudaError_t e;
         if (p.staged > 0 && hash_staged_supported(p)) e = launch_hash_staged(p, p.staged, s, launches);
-        else e = launch_hash_fused(p, align, p.sm_count, s, launches);
+        else e = launch_hash_fused(p, p.sm_count, s, launches);
         if (ev) { cudaEventRecord(ev[2], s); cudaEventRecord(ev[3], s); }
         return e;
     }

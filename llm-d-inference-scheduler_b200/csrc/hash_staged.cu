@@ -13,7 +13,7 @@
 //       TR requests per instruction, 8 steps per window; hashes written as 64-byte segments (the PluginState stash
 //       PreRequest needs, plugin.go:150-157).
 //
-// Why this shape (round-2 measurements, profiles/r2_hash_variants.txt): in the CTA-cooperative kernels (hash_fused.cu
+// Why this shape: in the CTA-cooperative kernels (hash_fused.cu
 // and three staged variants of it) ONE chain warp per CTA carries the serial ~25-instruction dependency chain per
 // block for 32 requests, and at 3-4 CTAs per SM those 3-4 latency-bound streams plus the named-barrier hand-over bound
 // the kernel.  Here every warp chains its own requests and the chain phase of one warp overlaps the digest phases of
@@ -224,7 +224,7 @@ cudaError_t launch_hash_staged(const HashParams &p, int shape, cudaStream_t s, i
     switch (shape) {
         case 3244: e = launch_shape<32, 4, 4>(p, s); break;
         case 1634: e = launch_shape<16, 3, 4>(p, s); break;
-        default: e = launch_shape<16, 4, 4>(p, s); break;      // 1644: measured best (profiles/r2_hash_variants.txt)
+        default: e = launch_shape<16, 4, 4>(p, s); break;      // 1644
     }
     if (launches) *launches += 1;
     return e;

@@ -11,8 +11,9 @@ struct Hit {
 };
 
 __device__ __forceinline__ void load_slot(const IndexSlot *p, uint64_t &key, Hit &h) {
-    uint64_t a, b, c, d;   // one 256-bit load = the whole slot
-    asm volatile("ld.global.nc.v4.u64 {%0,%1,%2,%3}, [%4];" : "=l"(a), "=l"(b), "=l"(c), "=l"(d) : "l"(p));
+    uint64_t a, b, c, d;   // the whole slot: two 128-bit loads (sm_90's widest) of the same 32-byte sector
+    asm volatile("ld.global.nc.v2.u64 {%0,%1}, [%2];" : "=l"(a), "=l"(b) : "l"(p));
+    asm volatile("ld.global.nc.v2.u64 {%0,%1}, [%2];" : "=l"(c), "=l"(d) : "l"(reinterpret_cast<const uint8_t *>(p) + 16));
     key = a;
     h.cnt = (uint32_t)b;
     h.w[0] = (uint32_t)(b >> 32);

@@ -707,7 +707,7 @@ __global__ void k_store_rehash(const StoreEntry *old_pt, uint64_t old_capacity, 
 }
 
 // Scan of the pair table: kExportPer slots per thread, all loads issued before any is used (the scan is pure
-// streaming; with one 32-byte load per thread it ran at 1.1 TB/s).
+// streaming: loads in flight set its rate).
 constexpr int kExportPer = 4;
 __global__ void k_store_export(View v, uint64_t capacity, unsigned long long *out_hash, uint32_t *out_ep) {
     const uint32_t lane = threadIdx.x & 31;
@@ -1156,7 +1156,7 @@ cudaError_t IndexStore::apply(const StoreCalls &calls, cudaStream_t s) {
         ST_TRY(blockmask_.reserve(sizeof(uint32_t) * (log_cap_ / kEvictBlock + 1) * (kEvictBlock / 32), &bytes_));
         ST_TRY(log_hash_spare_.reserve(sizeof(unsigned long long) * std::max<uint64_t>(log_cap_, 64), &bytes_));
         ST_TRY(log_seq_spare_.reserve(sizeof(unsigned long long) * std::max<uint64_t>(log_cap_, 64), &bytes_));
-        const unsigned cg = 148 * 8;
+        const unsigned cg = (unsigned)sm_count_ * 8;                // persistent: CTAs stride over the flat block space
         unsigned long long *nh = new_off_.as<unsigned long long>();          // scratch until repack_logs rewrites it
         k_compact_count<<<cg, kEvictBlock, 0, s>>>(v, list_e_.as<uint32_t>(), list_start_.as<unsigned long long>(),
                                                    blockcnt_.as<uint32_t>(), blockmask_.as<uint32_t>());
@@ -1194,7 +1194,7 @@ cudaError_t IndexStore::apply(const StoreCalls &calls, cudaStream_t s) {
         ST_TRY(list_start_.reserve(sizeof(unsigned long long) * E_, &bytes_));
         ST_TRY(cudaMemsetAsync(&v.ctr[kCtrEvict], 0, sizeof(unsigned long long), s));
         k_store_advance<<<blocks_for(E_, 256), 256, 0, s>>>(v, list_e_.as<uint32_t>(), list_start_.as<unsigned long long>());
-        const unsigned eg = 148 * 8;                     // persistent: CTAs stride over the flat block space
+        const unsigned eg = (unsigned)sm_count_ * 8;     // persistent: CTAs stride over the flat block space
         k_evict_count<<<eg, kEvictBlock, 0, s>>>(v, list_e_.as<uint32_t>(), list_start_.as<unsigned long long>(), blockcnt_.as<uint32_t>());
         tm.mark("ev_count");
         k_evict_cut<<<blocks_for((uint64_t)E_ * 32, 256), 256, 0, s>>>(v, blockcnt_.as<uint32_t>());

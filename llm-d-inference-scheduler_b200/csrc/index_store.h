@@ -58,7 +58,9 @@ struct ReadTableRef {
 
 class IndexStore {
   public:
-    IndexStore(uint32_t max_endpoints, int32_t default_lru_size) : E_(max_endpoints), default_cap_(default_lru_size) {}
+    // sm_count: SMs of the engine's device; sizes the persistent grids of the compaction and eviction kernels.
+    IndexStore(uint32_t max_endpoints, int32_t default_lru_size, int sm_count)
+        : E_(max_endpoints), default_cap_(default_lru_size), sm_count_(sm_count > 0 ? sm_count : 1) {}
 
     // Applies the calls (Add + eviction).  Synchronises `s` (two small read-backs size the tables).
     cudaError_t apply(const StoreCalls &calls, cudaStream_t s);
@@ -97,6 +99,7 @@ class IndexStore {
 
     uint32_t E_;
     int32_t default_cap_;
+    int sm_count_;
     bool init_ = false, dirty_ = false, used_ = false;
     size_t bytes_ = 0;
     uint64_t pt_cap_ = 0, log_cap_ = 0, in_map_ = 0, pt_used_ = 0;

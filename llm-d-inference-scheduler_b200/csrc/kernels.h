@@ -1,4 +1,4 @@
-// kernels.h -- host-callable launchers of the sm_100a kernels (internal to libepp_engine.so).
+// kernels.h -- host-callable launchers of the sm_90a kernels (internal to libepp_engine.so).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -46,7 +46,7 @@ cudaError_t launch_hash_staged(const HashParams &p, int shape, cudaStream_t s, i
 // prefix index (a2): open-addressed table  hash -> (posting offset, count)
 // ------------------------------------------------------------------------------------------------
 constexpr int kInlineIds = 5;
-// One 32-byte slot = one DRAM/L2 sector, fetched by a single 256-bit load.  Posting lists of up to kInlineIds
+// One 32-byte slot = one DRAM/L2 sector, fetched by two 128-bit loads.  Posting lists of up to kInlineIds
 // endpoints live IN the slot (no dependent load); longer lists live in `postings` at offset ids[0].  Lists are
 // sorted by endpoint id and duplicate-free.
 struct __align__(32) IndexSlot {
@@ -198,8 +198,7 @@ size_t cycle_small_max_blocks();
 // Does the kernel bring a whole prompt into shared memory (one bulk copy) before it hashes?  Then a request's flag is
 // raised only after its last read of the prompt bytes, and the staging buffer may be refilled as soon as all flags are up.
 bool cycle_small_stages_prompt(int32_t max_blocks, int32_t block_bytes);
-cudaError_t launch_cycle_small(const HashParams &hp, const PickParams &pp, const SmallOut &so, int align, cudaStream_t s,
-                               int *launches);
+cudaError_t launch_cycle_small(const HashParams &hp, const PickParams &pp, const SmallOut &so, cudaStream_t s, int *launches);
 // Decision logic on injected dense match info (plugin parity / KAT mode).
 struct DensePickParams {
     int64_t R;

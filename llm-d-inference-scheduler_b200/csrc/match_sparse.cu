@@ -41,7 +41,7 @@ cudaError_t launch_one(const PickParams &p, int sm_count, cudaStream_t s) {
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_match_pick_sparse<MINCTA, kSharded, kTie, kStages>, kWarps * 32, 0);
         if (occ < 1) occ = 1;
     }
-    if (sm_count <= 0) sm_count = 148;
+    if (sm_count <= 0) sm_count = 132;
     const int64_t need = (p.R + kWarps - 1) / kWarps;
     const int grid = (int)(need < (int64_t)sm_count * occ ? need : (int64_t)sm_count * occ);
     k_match_pick_sparse<MINCTA, kSharded, kTie, kStages><<<grid, kWarps * 32, 0, s>>>(p);
@@ -51,7 +51,7 @@ cudaError_t launch_one(const PickParams &p, int sm_count, cudaStream_t s) {
 
 cudaError_t launch_match_pick_sparse(const PickParams &p, int sm_count, cudaStream_t s, int *launches) {
     if (p.R <= 0) return cudaSuccess;
-    static int ctas = 0;                               // EPP_MATCH_CTAS=6: the 40-register variant (A/B; 8 measured faster)
+    static int ctas = 0;                               // EPP_MATCH_CTAS=6: the 40-register variant (A/B switch)
     if (!ctas) { const char *v = getenv("EPP_MATCH_CTAS"); ctas = (v && atoi(v) == 6) ? 6 : 8; }
     const bool tie = p.tie_seed != 0;
     const int stages = p.encode_on ? 3 : (p.n_profiles >= 2 ? 2 : 1);

@@ -1,4 +1,4 @@
-"""CPU-side checks of the drop-in boundary: libepp_engine.so builds for sm_100a, loads, exports every symbol
+"""CPU-side checks of the drop-in boundary: libepp_engine.so builds for sm_90a, loads, exports every symbol
 include/epp_engine.h declares, matches the ctypes struct layouts, and FAILS LOUDLY without a GPU (no CPU fallback).
 No compute calls here."""
 import ctypes as C
@@ -38,9 +38,9 @@ def test_every_declared_symbol_is_exported(epp):
     assert lib.epp_abi_version() == 5
 
 
-def test_library_contains_sm100a_code(epp):
+def test_library_contains_sm90a_code(epp):
     out = subprocess.run(["cuobjdump", "-lelf", epp.capi.LIB_PATH], capture_output=True, text=True).stdout
-    assert "sm_100a" in out, out[:400]
+    assert "sm_90a" in out, out[:400]
 
 
 def test_struct_layouts_match_header(epp, tmp_path):

@@ -1,6 +1,6 @@
 """GPU parity tests: the CUDA engine (through the C ABI) vs the CPU oracle on the same seeded inputs, vs the
 committed golden vectors, and through the reference-interface mirror (KATs of the reference's own tests).
-Bar: bit-exact for hashes / counts / picks, bit-exact fp64 score bits.  Run on the B200 box: pytest -m gpu."""
+Bar: bit-exact for hashes / counts / picks, bit-exact fp64 score bits.  Run on an H100: pytest -m gpu."""
 import dataclasses
 import json
 import os
@@ -113,7 +113,7 @@ def test_hash_ragged_vs_oracle(epp, orc, bst):
 
 
 def test_hash_ragged_aligned_starts_with_lengths(epp, orc):
-    """Ragged prompts whose STARTS sit on 32-byte boundaries (epp_batch.lengths): the fused 256-bit-load kernel with
+    """Ragged prompts whose STARTS sit on 32-byte boundaries (epp_batch.lengths): the fused kernel with
     per-request block counts, partial tail blocks, prompts shorter than a block and truncation, hashes AND decisions."""
     rng = random.Random(77)
     maxb = 20

@@ -1,6 +1,6 @@
 """GPU parity of the general profile evaluation (csrc/pick_general.cuh) vs the CPU oracle and the reference's own KATs:
 the k best endpoints of the max-score picker (picker/maxscore/picker.go:87-115) and the prefix-cache-affinity-filter
-(filter/prefixcacheaffinity/plugin.go:105-151).  Run on the B200 box: pytest -m gpu."""
+(filter/prefixcacheaffinity/plugin.go:105-151).  Run on an H100: pytest -m gpu."""
 import numpy as np
 import pytest
 

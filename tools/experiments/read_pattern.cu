@@ -1,12 +1,14 @@
 // read_pattern.cu -- microbenchmark: HBM read bandwidth of the hash kernels' access pattern (R requests of 16 KiB, each
 // CTA walks 32 requests 512 bytes at a time) against a linear sweep of the same 1 GiB, with no hashing at all.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/_build/read_pattern tools/experiments/read_pattern.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/_build/read_pattern tools/experiments/read_pattern.cu
 #include <cuda_runtime.h>
 #include <cstdint>
 #include <cstdio>
 
+// 32 bytes as two 128-bit loads (the widest global load of sm_90)
 __device__ __forceinline__ void ld256(const uint8_t *p, uint64_t x[4]) {
-    asm volatile("ld.global.nc.v4.u64 {%0,%1,%2,%3}, [%4];" : "=l"(x[0]), "=l"(x[1]), "=l"(x[2]), "=l"(x[3]) : "l"(p));
+    asm volatile("ld.global.nc.v2.u64 {%0,%1}, [%2];" : "=l"(x[0]), "=l"(x[1]) : "l"(p));
+    asm volatile("ld.global.nc.v2.u64 {%0,%1}, [%2];" : "=l"(x[2]), "=l"(x[3]) : "l"(p + 16));
 }
 
 // linear sweep: thread reads 64 B at consecutive positions, grid-stride
@@ -77,8 +79,8 @@ int main() {
     uint8_t *d; uint64_t *out;
     cudaMalloc(&d, bytes); cudaMalloc(&out, 64);
     cudaMemset(d, 1, bytes);
-    const int sm = 148;
-    timeit("linear sweep, 148x8 CTAs x 256", bytes, [&] { k_linear<<<sm * 8, 256>>>(d, bytes / 64, out); });
+    const int sm = 132;
+    timeit("linear sweep, 132x8 CTAs x 256", bytes, [&] { k_linear<<<sm * 8, 256>>>(d, bytes / 64, out); });
     timeit("request-major (v1 digest pattern)", bytes, [&] { k_request<<<sm * 8, 256>>>(d, R, row, out); });
     timeit("tiled 32 req x 512 B, depth 1, 4 CTA/SM", bytes, [&] { k_tiled<1><<<sm * 4, 256>>>(d, R, row, R / 32, out); });
     timeit("tiled 32 req x 512 B, depth 1, 8 CTA/SM", bytes, [&] { k_tiled<1><<<sm * 8, 256>>>(d, R, row, R / 32, out); });

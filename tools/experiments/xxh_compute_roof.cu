@@ -1,6 +1,6 @@
 // xxh_compute_roof.cu -- how many prompt bytes per second can the SMs DIGEST (XXH64 stripe rounds + merge per 64-byte
 // block, xxh64.cuh) with the data already in registers?  The compute roof of a1, measured: no loads, no stores.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -I llm-d-inference-scheduler_b200/csrc -o tools/_build/xxh_compute_roof tools/experiments/xxh_compute_roof.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -I llm-d-inference-scheduler_b200/csrc -o tools/_build/xxh_compute_roof tools/experiments/xxh_compute_roof.cu
 #include <cuda_runtime.h>
 #include <cstdint>
 #include <cstdio>
@@ -55,7 +55,7 @@ static float timeit(F launch) {
 
 int main() {
     uint64_t *out; cudaMalloc(&out, 64);
-    const int sm = 148, iters = 4096;
+    const int sm = 132, iters = 4096;
     printf("digest of 64-byte blocks from registers (rounds + merge), bytes/s the SMs can hash:\n");
     for (int wps : {4, 8, 16, 32, 48, 64}) {           // warps per SM
         const int threads = 128, ctas = sm * wps / 4;
