@@ -126,6 +126,7 @@ struct epp_engine {
     uint64_t l2_table_bytes = 24ull << 20;  // half the device's L2: the other half stays for the streamed prompts
     int dev_chunks = 2;             // EPP_DEV_CHUNKS=N: async device batches run as N chunks over both streams (1 = off)
     int staged = 0;                 // EPP_HASH_STAGED: 0 = hash_fused.cu (default), 1 = hash_staged.cu default shape, else a shape
+    int match_ctas = 8;             // EPP_MATCH_CTAS=6: k_match_pick_sparse's one-profile build bounded to 40 registers, not 32
     int pick_grid = 0;
     bool pick_global = false;
     size_t pick_smem = 0;
@@ -322,6 +323,7 @@ extern "C" int32_t epp_engine_create(const epp_config *cfg, epp_engine **out) {
     { const char *v1 = getenv("EPP_INDEX_LOAD"); e->index_load = v1 ? std::max(2, atoi(v1)) : 0; }
     { const char *v1 = getenv("EPP_DEV_CHUNKS"); e->dev_chunks = v1 ? std::max(1, atoi(v1)) : 2; }
     { const char *v1 = getenv("EPP_HASH_STAGED"); e->staged = v1 ? atoi(v1) : 0; }
+    { const char *v1 = getenv("EPP_MATCH_CTAS"); e->match_ctas = (v1 && atoi(v1) == 6) ? 6 : 8; }
     { const char *v1 = getenv("EPP_SMALL_BATCH"); e->small_max = v1 ? std::max(0, atoi(v1)) : 1024; }
     { const char *v1 = getenv("EPP_SMALL_ZEROCOPY"); e->small_zc_max = v1 ? std::max(0, atoi(v1)) : 8; }
     { const char *v1 = getenv("EPP_SMALL_PIPELINE"); e->small_pipe_min = v1 ? std::max(0, atoi(v1)) : 1; }
@@ -1033,7 +1035,7 @@ static int32_t launch_match(epp_engine *h, Slot &sl, PickParams pp, int *launche
     CUDA_TRY(cudaMemsetAsync(sl.overflow_n.p, 0, sizeof(int32_t), s));
     pp.overflow_list = sl.overflow_list.as<int32_t>();
     pp.overflow_n = sl.overflow_n.as<int32_t>();
-    CUDA_TRY(launch_match_pick_sparse(pp, h->sm_count, s, launches));
+    CUDA_TRY(launch_match_pick_sparse(pp, h->sm_count, h->match_ctas, s, launches));
     return launch_overflow_pass(h, sl, pp, launches);
 }
 

@@ -2,7 +2,7 @@
 // the device counterpart of indexer.hashToPods (approximateprefix/indexer.go:32-37).
 //
 // Layout in HBM: one open-addressed table of 32-byte slots {key u64, count u32, 5 x endpoint u32} -- one sector,
-// one 256-bit load per probe -- linear probing from key & mask (XXH64 output is already uniformly mixed), load
+// two 128-bit loads per probe -- linear probing from key & mask (XXH64 output is already uniformly mixed), load
 // factor <= 0.5.  Lists longer than five endpoints spill to a contiguous u32 postings array.  Every list is
 // sorted by endpoint id and duplicate-free (podSet is a set, indexer.go:78-82).
 //

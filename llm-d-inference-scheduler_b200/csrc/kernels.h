@@ -180,8 +180,9 @@ int match_pick_warps_per_cta();
 cudaError_t launch_match_pick(const PickParams &p, uint32_t *gscratch, int grid, size_t smem, cudaStream_t s,
                               int *launches);
 // The same decision per request with a lane-distributed register map of the matched endpoints (requests whose set
-// overflows it are appended to p.overflow_list for the dense-counter kernel).  8 warps per CTA, 6-8 CTAs per SM.
-cudaError_t launch_match_pick_sparse(const PickParams &p, int sm_count, cudaStream_t s, int *launches);
+// overflows it are appended to p.overflow_list for the dense-counter kernel).  8 warps per CTA, 6-8 CTAs per SM;
+// ctas = 6 bounds the one-profile lowest-slot build to 40 registers instead of 32 (the engine's EPP_MATCH_CTAS).
+cudaError_t launch_match_pick_sparse(const PickParams &p, int sm_count, int ctas, cudaStream_t s, int *launches);
 // cycle_small.cu: a1-a14 of a small host batch in ONE launch, one CTA per request, prompts read from and decisions
 // written to PINNED HOST memory (zero-copy); flags[r] = epoch (| 0x80000000 when the request overflowed the sparse map and
 // was appended to pp.overflow_list instead of being decided) is written last, after a system-scope fence.

@@ -1,7 +1,5 @@
 // match_sparse.cu -- a2-a14 over the hash rows of a batch: the match / score / pick kernel of the throughput path (and of
 // the endpoint-sharded mode): one warp per request, the per-request work is match_sparse.cuh.
-#include <cstdlib>
-
 #include "match_sparse.cuh"
 
 namespace epp {
@@ -49,17 +47,15 @@ cudaError_t launch_one(const PickParams &p, int sm_count, cudaStream_t s) {
 }
 }  // namespace
 
-cudaError_t launch_match_pick_sparse(const PickParams &p, int sm_count, cudaStream_t s, int *launches) {
+cudaError_t launch_match_pick_sparse(const PickParams &p, int sm_count, int ctas, cudaStream_t s, int *launches) {
     if (p.R <= 0) return cudaSuccess;
-    static int ctas = 0;                               // EPP_MATCH_CTAS=6: the 40-register variant (A/B switch)
-    if (!ctas) { const char *v = getenv("EPP_MATCH_CTAS"); ctas = (v && atoi(v) == 6) ? 6 : 8; }
     const bool tie = p.tie_seed != 0;
     const int stages = p.encode_on ? 3 : (p.n_profiles >= 2 ? 2 : 1);
     cudaError_t e;
     // the hot configuration (one profile, lowest-slot ties) gets the 32-register build; the variants that carry more
     // code (stages, tie rule, sharding) keep 40 registers
     if (p.global_masks) e = launch_one<6, true, false, 1>(p, sm_count, s);
-    else if (stages == 1 && !tie) e = ctas == 8 ? launch_one<8, false, false, 1>(p, sm_count, s) : launch_one<6, false, false, 1>(p, sm_count, s);
+    else if (stages == 1 && !tie) e = ctas == 6 ? launch_one<6, false, false, 1>(p, sm_count, s) : launch_one<8, false, false, 1>(p, sm_count, s);
     else if (stages == 1) e = launch_one<6, false, true, 1>(p, sm_count, s);
     else if (stages == 2) e = tie ? launch_one<6, false, true, 2>(p, sm_count, s) : launch_one<6, false, false, 2>(p, sm_count, s);
     else e = tie ? launch_one<6, false, true, 3>(p, sm_count, s) : launch_one<6, false, false, 3>(p, sm_count, s);

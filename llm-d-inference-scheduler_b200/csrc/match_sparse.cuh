@@ -7,7 +7,7 @@
 // endpoint-sharded variant) and by the latency kernel (cycle_small.cu: one warp of the request's CTA follows the hash
 // chain as it is produced).
 //
-//   * 32 blocks are probed per step, one 256-bit load per 32-byte slot.  Probe chains are followed only as far as the
+//   * 32 blocks are probed per step, two 128-bit loads per 32-byte slot.  Probe chains are followed only as far as the
 //     stop rule needs them: once a lane has proven its block absent, the lanes behind it (which cannot change the walk)
 //     stop probing -- a cold prompt costs the probe chain of block 0, not the longest chain of 32 unrelated blocks;
 //   * matched endpoints live in a LANE-DISTRIBUTED register map: lane j holds (endpoint E_j, count C_j), j <

@@ -40,20 +40,6 @@ def _pack(prompts):
     return data, offs
 
 
-def _pack_aligned(prompts, align=16):
-    offs = np.zeros(len(prompts) + 1, dtype=np.uint64)
-    chunks, pos = [], 0
-    starts = []
-    for p in prompts:
-        pad = (-pos) % align
-        chunks.append(b"\0" * pad)
-        pos += pad
-        starts.append(pos)
-        chunks.append(p)
-        pos += len(p)
-    return np.frombuffer(b"".join(chunks) + b"\0" * 16, dtype=np.uint8).copy(), starts
-
-
 # ------------------------------------------------------------------------------------------------
 # a1 hashing
 # ------------------------------------------------------------------------------------------------
@@ -100,10 +86,8 @@ def test_hash_ragged_vs_oracle(epp, orc, bst):
             want = orc.hash_prompt(p, b"mdl", bst, maxb)
             assert nb[i] == len(want), (i, len(p))
             assert [int(x) for x in hs[i, : nb[i]]] == want, (i, len(p))
-        # (b) 16-byte aligned prompt starts with explicit offsets (vector path when bs % 32 == 0)
-        d2, starts = _pack_aligned(prompts)
-        offs2 = np.array(starts + [starts[-1] + len(prompts[-1])], dtype=np.uint64)
-        # offsets[r+1]-offsets[r] must equal the prompt length: use per-request spans via a gather copy
+        # (b) single requests at offset 0 (vector path when bs % 32 == 0); multi-request aligned layouts are covered by
+        # test_kernel_paths_gpu.py
         for i in (0, 1, 2, 3, 10, 33):
             di = np.zeros(((len(prompts[i]) + 31) // 16) * 16 + 16, np.uint8)
             di[: len(prompts[i])] = np.frombuffer(prompts[i], np.uint8)
@@ -812,13 +796,15 @@ def test_small_batch_prompt_buffer_may_be_rewritten_when_the_call_returns(epp, o
     and epp_schedule returns as soon as every request is decided.  From then on the caller may rewrite its prompt
     buffer, and the next batch's copy may refill the engine's staging buffer -- the hashes PreRequest indexes afterwards
     (incl. the one of the trailing PARTIAL block, hashing.go:90-96, which the chain reaches last) must still be those
-    of the prompts that were scheduled.  1 request = the kernel reads the caller's pinned buffer; 24 = DMA-copied."""
-    E, bst, B = 8, 8, 2048                         # 64 KiB prompts: the chain runs for > 100 us
-    bb = 4 * bst
+    of the prompts that were scheduled.  1 request = the kernel reads the caller's pinned buffer; 24 = DMA-copied.
+    64 KiB prompts of 32-byte blocks are staged into shared memory by one bulk copy (the chain runs for > 100 us);
+    200 KiB prompts of 1 KiB blocks do not fit there, and the digest threads read them from the row themselves."""
+    E = 8
     rng = np.random.default_rng(99)
     role = np.full(E, 3, dtype=np.uint8)
     spec = epp.ProfileSpec(1, [epp.ScorerSpec(2, 1.0, 0)])
-    for n in (1, 24):
+    for bst, B, n in ((8, 2048, 1), (8, 2048, 24), (256, 200, 1), (256, 200, 24)):
+        bb = 4 * bst
         with epp.Engine(E, spec, None, block_size_tokens=bst, max_prefix_blocks=B, lru_capacity_per_server=100000) as eng:
             eng.register_model(b"m")
             eng.pool_set(np.arange(E), role, np.zeros(E), np.zeros(E, dtype=np.int32))
