@@ -112,7 +112,7 @@ struct epp_engine {
     uint64_t idx_capacity = 0, idx_pairs = 0;
     // incremental maintenance of the read table (IndexStore::patch_read_table)
     bool rt_from_store = false;     // the table mirrors the store's inverted map (bulk-built from its export)
-    uint64_t post_cap = 0, post_used = 0, rt_slots_used = 0;
+    uint64_t post_cap = 0, post_used = 0, rt_slots_used = 0, rt_intern_used = 0;
     int patches_since_build = 0;
     int patch_enabled = 1;          // EPP_INDEX_PATCH=0: always rebuild
     IndexSlot idx_special_host{};
@@ -632,6 +632,7 @@ static int32_t build_index_from_device_pairs(epp_engine *h, uint64_t n, uint64_t
     h->post_cap = h->postings.cap / sizeof(uint32_t);
     h->post_used = cursor[0];
     h->rt_slots_used = cursor[2];
+    h->rt_intern_used = cursor[3];
     h->rt_from_store = from_store;
     h->patches_since_build = 0;
     return EPP_OK;
@@ -707,11 +708,13 @@ static int32_t commit_locked(epp_engine *h) {
         rt.head = h->idx_scratch.as<uint32_t>();
         rt.intern_keys = h->intern_keys.as<uint64_t>();
         rt.intern_vals = h->intern_vals.as<uint32_t>();
-        uint64_t np = 0, nu = 0, npost = 0;
-        CUDA_TRY(h->store->patch_read_table(rt, h->idx_pairs, s, &patched, &np, &nu, &npost));
+        rt.intern_used = h->rt_intern_used;
+        uint64_t np = 0, nu = 0, npost = 0, ni = 0;
+        CUDA_TRY(h->store->patch_read_table(rt, h->idx_pairs, s, &patched, &np, &nu, &npost, &ni));
         if (patched) {
             h->idx_pairs = np;
             h->rt_slots_used = nu;
+            h->rt_intern_used = ni;
             h->post_used = npost;
             h->stats.index_pairs = np;
             h->stats.index_hashes = nu;

@@ -33,6 +33,7 @@ __global__ void k_index_clear(IndexSlot *slots, uint32_t *fill, uint64_t capacit
         cursor[0] = 0;   // posting cursor
         cursor[1] = 0;   // special fill
         cursor[2] = 0;   // distinct hashes
+        cursor[3] = 0;   // claimed keys of the interning table
         special->key = kEmptyKey;
         special->cnt = 0;
         for (int q = 0; q < kInlineIds; q++) special->ids[q] = 0;
@@ -155,7 +156,9 @@ __global__ void k_intern_clear(uint64_t *ikeys, uint32_t *ivals, uint64_t capaci
     if (i < capacity) { ikeys[i] = kEmptyKey; ivals[i] = 0xFFFFFFFFu; }
 }
 
-__device__ __forceinline__ uint64_t intern_find_or_claim(uint64_t *ikeys, uint64_t mask, uint64_t key, bool claim) {
+// keys_used (claim only): counts the keys this call claims, so that patches can bound the table's fill (index_store.cu)
+__device__ __forceinline__ uint64_t intern_find_or_claim(uint64_t *ikeys, uint64_t mask, uint64_t key, bool claim,
+                                                         uint32_t *keys_used = nullptr) {
     uint64_t i = key & mask;
     for (;;) {
         unsigned long long *kp = reinterpret_cast<unsigned long long *>(&ikeys[i]);
@@ -164,6 +167,7 @@ __device__ __forceinline__ uint64_t intern_find_or_claim(uint64_t *ikeys, uint64
         if (cur == kEmptyKey) {
             if (!claim) return i;
             unsigned long long old = atomicCAS(kp, (unsigned long long)kEmptyKey, (unsigned long long)key);
+            if (old == kEmptyKey) atomicAdd(keys_used, 1u);
             if (old == kEmptyKey || old == key) return i;
         }
         i = (i + 1) & mask;
@@ -171,11 +175,11 @@ __device__ __forceinline__ uint64_t intern_find_or_claim(uint64_t *ikeys, uint64
 }
 
 __global__ void k_intern_claim(const IndexSlot *slots, uint64_t capacity, const uint32_t *postings, uint64_t *ikeys,
-                               uint32_t *ivals) {
+                               uint32_t *ivals, uint32_t *cursor) {
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= capacity || slots[i].cnt <= (uint32_t)kInlineIds) return;
     uint32_t off = slots[i].ids[0];
-    uint64_t j = intern_find_or_claim(ikeys, capacity - 1, list_hash(postings + off, slots[i].cnt), true);
+    uint64_t j = intern_find_or_claim(ikeys, capacity - 1, list_hash(postings + off, slots[i].cnt), true, &cursor[3]);
     atomicMin(&ivals[j], (uint32_t)i);  // canonical copy = the list of the lowest slot among equal-hash lists
 }
 
@@ -211,7 +215,7 @@ cudaError_t launch_index_build(const uint64_t *pair_hash, const uint32_t *pair_e
         k_index_fill<<<gn, 256, 0, s>>>(pair_hash, pair_ep, n, slots, mask, scratch, postings, cursor, special_dev);
         k_index_finalize<<<gc, 256, 0, s>>>(slots, capacity, postings, special_dev);
         k_intern_clear<<<gc, 256, 0, s>>>(intern_keys, intern_vals, capacity);
-        k_intern_claim<<<gc, 256, 0, s>>>(slots, capacity, postings, intern_keys, intern_vals);
+        k_intern_claim<<<gc, 256, 0, s>>>(slots, capacity, postings, intern_keys, intern_vals, cursor);
         k_intern_apply<<<gc, 256, 0, s>>>(slots, capacity, postings, intern_keys, intern_vals);
         nl += 7;
     }

@@ -15,7 +15,8 @@ constexpr unsigned long long kTmpBit = 1ull << 62;    // scratch of k_store_leak
 constexpr unsigned long long kSeqMask = ~(kLeakBit | kTmpBit);
 constexpr int kCallChunk = 1024;                      // calls per ordering chunk (= threads of k_store_offsets)
 enum { kCtrPtUsed = 0, kCtrTotalItems, kCtrNeedRepack, kCtrInMap, kCtrCursor, kCtrAlive, kCtrEvict, kCtrTouch,
-       kCtrTouchLost, kCtrPatchFlag, kCtrPatchDirty, kCtrPatchClaims, kCtrPatchAdd, kCtrPatchDel, kCtrPatchPost, kCtrN = 16 };
+       kCtrTouchLost, kCtrPatchFlag, kCtrPatchDirty, kCtrPatchClaims, kCtrPatchAdd, kCtrPatchDel, kCtrPatchIntern,
+       kCtrPatchPost, kCtrN = 16 };
 
 // One (hash, endpoint) pair of the write side: 32 bytes = one sector.
 struct __align__(32) StoreEntry {
@@ -772,6 +773,7 @@ struct PatchView {
     uint32_t *dirty;             // [n_touch] slots with pending entries
     uint64_t *intern_keys;       // interning table of the last bulk build (capacity entries)
     uint32_t *intern_vals;
+    unsigned long long *intern_claims;   // keys this patch claimed in it
 };
 
 __device__ __forceinline__ uint64_t rt_find_or_claim(const PatchView &pv, uint64_t key, uint32_t &claimed) {
@@ -922,6 +924,7 @@ __device__ __forceinline__ uint64_t patch_intern_slot(const PatchView &pv, uint6
         if (cur == kEmptyKey) {
             if (!claim) return i;
             unsigned long long old = atomicCAS(kp, (unsigned long long)kEmptyKey, (unsigned long long)key);
+            if (old == kEmptyKey) atomicAdd(pv.intern_claims, 1ull);
             if (old == kEmptyKey || old == key) return i;
         }
         i = (i + 1) & pv.mask;
@@ -1253,9 +1256,11 @@ cudaError_t IndexStore::touch_reset(cudaStream_t s) {
 }
 
 // Brings a bulk-built read table up to date from the touch log.  *patched = false: nothing was done (log unusable, the
-// table lacks room, the sentinel hash is involved, or the change set is too large to be worth it) -> bulk build.
+// table or its interning table lacks room, the sentinel hash is involved, or the change set is too large to be worth
+// it) -> bulk build.
 cudaError_t IndexStore::patch_read_table(const ReadTableRef &rt, uint64_t table_pairs, cudaStream_t s, bool *patched,
-                                         uint64_t *new_pairs, uint64_t *new_slots_used, uint64_t *new_post_used) {
+                                         uint64_t *new_pairs, uint64_t *new_slots_used, uint64_t *new_post_used,
+                                         uint64_t *new_intern_used) {
     *patched = false;
     if (!init_ || touch_disabled_) return cudaSuccess;
     View v;
@@ -1264,10 +1269,21 @@ cudaError_t IndexStore::patch_read_table(const ReadTableRef &rt, uint64_t table_
     ST_TRY(cudaStreamSynchronize(s));
     const uint64_t n_touch = ctr_host_[kCtrTouch];
     if (ctr_host_[kCtrTouchLost] || n_touch > touch_cap_) return cudaSuccess;
-    if (n_touch == 0) { *patched = true; *new_pairs = table_pairs; *new_slots_used = rt.slots_used; *new_post_used = rt.post_used; return cudaSuccess; }
+    if (n_touch == 0) {
+        *patched = true;
+        *new_pairs = table_pairs;
+        *new_slots_used = rt.slots_used;
+        *new_post_used = rt.post_used;
+        *new_intern_used = rt.intern_used;
+        return cudaSuccess;
+    }
     // worth it only when the change set is small next to the table; and the table must keep its load factor
     if (n_touch > std::max<uint64_t>(1 << 16, table_pairs / 2)) return cudaSuccess;
     if ((rt.slots_used + n_touch) * 10 > rt.capacity * 6) return cudaSuccess;
+    // so must the interning table, which only the bulk build empties: every spilled list a patch writes claims a key
+    // (at most one per dirty slot, n_dirty <= n_touch) and the key of the list it replaces stays; its probes end only
+    // at a free key
+    if ((rt.intern_used + n_touch) * 10 > rt.capacity * 6) return cudaSuccess;
     if (n_touch >= 0xFFFFFFF0ull) return cudaSuccess;
     ST_TRY(patch_next_.reserve(sizeof(uint32_t) * n_touch, &bytes_));
     ST_TRY(patch_dirty_.reserve(sizeof(uint32_t) * n_touch, &bytes_));
@@ -1282,7 +1298,8 @@ cudaError_t IndexStore::patch_read_table(const ReadTableRef &rt, uint64_t table_
     pv.dirty = patch_dirty_.as<uint32_t>();
     pv.intern_keys = rt.intern_keys;
     pv.intern_vals = rt.intern_vals;
-    ST_TRY(cudaMemsetAsync(&v.ctr[kCtrPatchFlag], 0, sizeof(unsigned long long) * 5, s));     // flag, dirty, claims, add, del
+    pv.intern_claims = &v.ctr[kCtrPatchIntern];
+    ST_TRY(cudaMemsetAsync(&v.ctr[kCtrPatchFlag], 0, sizeof(unsigned long long) * 6, s));     // flag .. intern
     ctr_host_[kCtrPatchPost] = rt.post_used;
     ST_TRY(cudaMemcpyAsync(&v.ctr[kCtrPatchPost], &ctr_host_[kCtrPatchPost], sizeof(unsigned long long), cudaMemcpyHostToDevice, s));
     ST_TRY(cudaStreamSynchronize(s));
@@ -1298,10 +1315,13 @@ cudaError_t IndexStore::patch_read_table(const ReadTableRef &rt, uint64_t table_
     if (ctr_host_[kCtrPatchFlag]) return cudaSuccess;                    // out of posting space mid-way: bulk build
     k_patch_intern_claim<<<blocks_for(n_dirty, 128), 128, 0, s>>>(pv, n_dirty);
     k_patch_intern_apply<<<blocks_for(n_dirty, 128), 128, 0, s>>>(pv, n_dirty);
+    ST_TRY(cudaMemcpyAsync(&ctr_host_[kCtrPatchIntern], &v.ctr[kCtrPatchIntern], sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
+    ST_TRY(cudaStreamSynchronize(s));
     ST_TRY(cudaGetLastError());
     *new_pairs = table_pairs + ctr_host_[kCtrPatchAdd] - ctr_host_[kCtrPatchDel];
     *new_slots_used = rt.slots_used + ctr_host_[kCtrPatchClaims];
     *new_post_used = ctr_host_[kCtrPatchPost];
+    *new_intern_used = rt.intern_used + ctr_host_[kCtrPatchIntern];
     last_patch_touches = n_touch;
     last_patch_dirty = n_dirty;
     *patched = true;

@@ -54,6 +54,7 @@ struct ReadTableRef {
     uint32_t *head = nullptr;     // device: [capacity], all 0xFFFFFFFF between patches
     uint64_t *intern_keys = nullptr;
     uint32_t *intern_vals = nullptr;
+    uint64_t intern_used = 0;     // claimed keys of the interning table, retired ones included (`capacity` entries)
 };
 
 class IndexStore {
@@ -74,7 +75,8 @@ class IndexStore {
     // Every (hash, endpoint) pair of the inverted map, for the bulk build of the read table.
     // Incremental read-table maintenance from the log of changed (hash, endpoint) pairs (see index_store.cu).
     cudaError_t patch_read_table(const ReadTableRef &rt, uint64_t table_pairs, cudaStream_t s, bool *patched,
-                                 uint64_t *new_pairs, uint64_t *new_slots_used, uint64_t *new_post_used);
+                                 uint64_t *new_pairs, uint64_t *new_slots_used, uint64_t *new_post_used,
+                                 uint64_t *new_intern_used);
     cudaError_t touch_reset(cudaStream_t s);
     uint64_t last_patch_touches = 0, last_patch_dirty = 0;
     cudaError_t export_pairs(DevBuf &pair_hash, DevBuf &pair_ep, uint64_t *n_pairs, size_t *accounted, cudaStream_t s);

@@ -65,7 +65,8 @@ struct IndexView {
     uint32_t ep_begin, ep_end;  // shard range (postings outside are ignored for counting but keep the walk alive)
 };
 // Builds table + postings from n pairs (device arrays).  slots must hold `capacity` entries, postings n,
-// scratch `capacity` uint32, cursor 4 uint32 (cursor[2] returns the number of distinct hashes).  *special_dev
+// scratch `capacity` uint32, cursor 4 uint32 (cursor[2] returns the number of distinct hashes, cursor[3] the keys
+// claimed in the interning table).  *special_dev
 // receives the record of key == kEmptyKey.  Deduplicates pairs, sorts every posting list and interns equal spilled
 // lists (intern_keys / intern_vals: `capacity` entries each).
 cudaError_t launch_index_build(const uint64_t *pair_hash, const uint32_t *pair_ep, uint64_t n, IndexSlot *slots,

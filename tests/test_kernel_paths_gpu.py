@@ -10,6 +10,8 @@ from collections import defaultdict
 import numpy as np
 import pytest
 
+from helpers import assert_ran, kernels_launched, ran
+
 pytestmark = pytest.mark.gpu
 
 GOLD = os.path.join(os.path.dirname(__file__), "golden", "xxh64_vectors.json")
@@ -26,41 +28,6 @@ def epp():
     import epp_b200
     epp_b200.build.build()
     return epp_b200
-
-
-def kernels_launched(fn):
-    """Runs fn() under torch.profiler with CUDA activities -> (fn's result, names of the CUDA kernels it launched).
-    Two torch kernels before and two behind fn's launches show that the trace kept its device records; a trace that
-    lost them is taken again with one more call of fn (every caller passes a call whose repetition changes nothing
-    the test checks later), and the first call's result is returned."""
-    import torch
-    from torch.profiler import ProfilerActivity, profile
-    out, names = None, set()
-    for attempt in range(3):
-        torch.cuda.synchronize()
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            torch.ones(1, device="cuda").add_(1)
-            r = fn()
-            torch.cuda.synchronize()
-            torch.ones(1, device="cuda").add_(1)
-            torch.cuda.synchronize()
-        if attempt == 0:
-            out = r
-        events = prof.events()
-        names = {e.name for e in events}
-        if sum("at::native::" in e.name for e in events) >= 4:
-            break
-    return out, names
-
-
-def ran(names, kernel):
-    return any(kernel in n for n in names)
-
-
-def assert_ran(names, kernel, absent=(), where=""):
-    assert ran(names, kernel), f"{where}: {kernel} did not run; kernels: {sorted(names)}"
-    for k in absent:
-        assert not ran(names, k), f"{where}: {k} ran; kernels: {sorted(names)}"
 
 
 def _pack(prompts, first=0):
