@@ -215,9 +215,9 @@ __global__ void __launch_bounds__(kThreads) k_cycle_small(HashParams hp, PickPar
     }
     if (warp != 1) return;                         // not warp 0: that one shares its scheduler with the chain warp (8 % 4)
 
-    sparse::Work wk;
+    int32_t unused = 0;
     const ChainFollower fw{&s_progress, s_m};
-    const bool decided = sparse::match_request<true, false, true, 3, ChainFollower>(pp, r, lane, false, wk, fw);
+    const bool decided = sparse::match_request<true, false, true, 3, ChainFollower>(pp, r, lane, false, nullptr, nullptr, unused, fw);
     if (lane == 0) {
         if (decided) {
             so.dec[r] = pp.out[r];

@@ -60,7 +60,8 @@ struct ProfileState {
 struct Slot {                       // per-stream staging for host-pointer batches
     cudaStream_t stream = nullptr;
     DevBuf data;
-    DevBuf overflow_list, overflow_n;   // requests handed from a sparse pass to the dense-counter pass (per stream)
+    DevBuf overflow_list, overflow_n;   // requests handed from a sparse pass to the dense-counter pass (per stream);
+                                        // overflow_n[1] is the sparse pass's request counter
     DevBuf pick_scratch;                // zeroed global match counters of the dense-counter kernel when max_endpoints is too
                                         // large for shared memory: per stream, two streams may run that kernel at once
     cudaEvent_t done = nullptr;
@@ -996,6 +997,7 @@ static PickParams pick_params(epp_engine *h, const Work &w, epp_decision *out, e
     p.req_list_n = nullptr;
     p.overflow_list = nullptr;
     p.overflow_n = nullptr;
+    p.req_next = nullptr;
     p.gen = gen_view(h);
     return p;
 }
@@ -1035,9 +1037,11 @@ static int32_t launch_match(epp_engine *h, Slot &sl, PickParams pp, int *launche
         CUDA_TRY(launch_match_pick(pp, gs, h->pick_grid, h->pick_smem, s, launches));
         return EPP_OK;
     }
-    CUDA_TRY(cudaMemsetAsync(sl.overflow_n.p, 0, sizeof(int32_t), s));
+    // overflow_n[0]: the overflow count, [1]: the sparse kernel's request counter; one memset clears both
+    CUDA_TRY(cudaMemsetAsync(sl.overflow_n.p, 0, sizeof(int32_t) * 2, s));
     pp.overflow_list = sl.overflow_list.as<int32_t>();
     pp.overflow_n = sl.overflow_n.as<int32_t>();
+    pp.req_next = sl.overflow_n.as<int32_t>() + 1;
     CUDA_TRY(launch_match_pick_sparse(pp, h->sm_count, h->match_ctas, s, launches));
     return launch_overflow_pass(h, sl, pp, launches);
 }

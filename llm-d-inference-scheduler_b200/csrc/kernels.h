@@ -168,6 +168,8 @@ struct PickParams {
     // sparse kernels only: requests whose matched-endpoint set overflowed the per-warp map are appended here
     int32_t *overflow_list;
     int32_t *overflow_n;
+    // k_match_pick_sparse only: requests taken beyond each warp's first one (zero at launch; R < 2^31)
+    int32_t *req_next;
     // tie rule: 0 = lowest slot of the arg-max set; else the member of rank tie_rank(seed, 4 * (tie_base + r) + profile)
     uint64_t tie_seed;
     uint64_t tie_base;         // ordinal of request 0 of this launch

@@ -10,20 +10,35 @@ constexpr int kWarps = 8;
 
 // MINCTA: resident CTAs per SM the register allocation is bounded for (8 -> 32 registers: 64 resident warps hide the
 // probe latency; 6 -> 40 registers).  kTie / kStages: see match_sparse.cuh.
+// Requests are taken dynamically: a warp's first request is its index in the grid, every further one comes off the
+// launch's counter (p.req_next), so the warps that draw cheap (cold) prompts take more of them while the warps on long
+// cached prefixes are busy, instead of the launch ending on the warps whose fixed share happened to be costliest.  The
+// ticket is taken once the current request's probes are done, so the atomic's latency hides behind its scoring.
 template <int MINCTA, bool kSharded, bool kTie, int kStages>
 __global__ void __launch_bounds__(kWarps * 32, MINCTA) k_match_pick_sparse(PickParams p) {
+    __shared__ sparse::Work s_work[kWarps];           // when counting
     const int lane = threadIdx.x & 31;
     const int warp = threadIdx.x >> 5;
-    const int64_t gwarp = (int64_t)blockIdx.x * kWarps + warp;
-    const int64_t nwarps = (int64_t)gridDim.x * kWarps;
+    const uint32_t nwarps = gridDim.x * kWarps;
+    const uint32_t R = (uint32_t)p.R;                  // < 2^31 (launch_match_pick_sparse)
     const bool counting = p.work_counters != nullptr;
-    sparse::Work wk;
-    for (int64_t r = gwarp; r < p.R; r += nwarps) sparse::match_request<false, kSharded, kTie, kStages>(p, r, lane, counting, wk);
+    sparse::Work *wk = &s_work[warp];
     if (counting) {
-        for (int o = 16; o; o >>= 1) wk.postings += __shfl_xor_sync(0xffffffffu, wk.postings, o);
+        wk->postings[lane] = 0;
+        if (lane == 0) wk->probes = 0;
+    }
+    uint32_t r = blockIdx.x * kWarps + warp;
+    while (r < R) {
+        int32_t ticket = 0;
+        sparse::match_request<false, kSharded, kTie, kStages>(p, r, lane, counting, wk, p.req_next, ticket);
+        r = nwarps + (uint32_t)__shfl_sync(0xffffffffu, ticket, 0);
+    }
+    if (counting) {
+        unsigned long long postings = wk->postings[lane];
+        for (int o = 16; o; o >>= 1) postings += __shfl_xor_sync(0xffffffffu, postings, o);
         if (lane == 0) {
-            atomicAdd(&p.work_counters[0], wk.probes);
-            atomicAdd(&p.work_counters[1], wk.postings);
+            atomicAdd(&p.work_counters[0], wk->probes);
+            atomicAdd(&p.work_counters[1], postings);
         }
     }
 }
@@ -49,6 +64,7 @@ cudaError_t launch_one(const PickParams &p, int sm_count, cudaStream_t s) {
 
 cudaError_t launch_match_pick_sparse(const PickParams &p, int sm_count, int ctas, cudaStream_t s, int *launches) {
     if (p.R <= 0) return cudaSuccess;
+    if (!p.req_next || p.R > INT32_MAX) return cudaErrorInvalidValue;
     const bool tie = p.tie_seed != 0;
     const int stages = p.encode_on ? 3 : (p.n_profiles >= 2 ? 2 : 1);
     cudaError_t e;

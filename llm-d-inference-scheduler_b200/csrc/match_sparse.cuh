@@ -1,7 +1,8 @@
 // match_sparse.cuh -- a2-a14 for ONE request by ONE warp over hashes resident in HBM / L2: index lookup with the
 // global-stop rule (approximateprefix/plugin.go:214-230), per-endpoint match counts, ordered weighted sum
 // (scheduler_profile.go:151-174), arg-max pick (maxscore/picker.go:87-115) and the decode -> decider -> prefill second
-// stage (disagg_profile_handler.go:264-308).  No shared memory, no atomics on the common path.
+// stage (disagg_profile_handler.go:264-308).  No shared memory (except the optional work tally), one atomic per request
+// (the throughput kernel's request counter).
 //
 // Shared by the throughput kernel (match_sparse.cu: one warp per request over the hash rows of a whole batch, incl. the
 // endpoint-sharded variant) and by the latency kernel (cycle_small.cu: one warp of the request's CTA follows the hash
@@ -32,8 +33,8 @@ constexpr uint32_t kFull = 0xffffffffu;
 struct LaneMap {                   // one entry per lane
     uint32_t e;                    // endpoint held by this lane (kNoKey = none)
     uint32_t c;                    // its match count
-    uint32_t n;                    // distinct endpoints so far (warp-uniform)
-    bool overflow;                 // warp-uniform
+    uint32_t n;                    // distinct endpoints so far (warp-uniform); 33 = overflowed (one register, no flag)
+    __device__ __forceinline__ bool overflow() const { return n > 32; }
 };
 
 // count[e] += c for a warp-uniform (e, c).
@@ -45,7 +46,7 @@ __device__ __forceinline__ void map_add(LaneMap &m, uint32_t e, uint32_t c, int 
         if (lane == (int)m.n) { m.e = e; m.c = c; }
         m.n++;
     } else {
-        m.overflow = true;
+        m.n = 33;
     }
 }
 
@@ -188,10 +189,10 @@ __device__ __forceinline__ void count_chunk(LaneMap &m, const IndexView &ix, uin
             if (rc > 4) { const uint32_t e = __shfl_sync(kFull, w4, s); if (e >= shard_lo && e < shard_hi) map_add(m, e, len, lane); }
         } else {
             // spilled (interned) list: r0 is the offset into the postings array
-            for (uint32_t k0 = 0; k0 < rc && !m.overflow; k0 += 32) {
+            for (uint32_t k0 = 0; k0 < rc && !m.overflow(); k0 += 32) {
                 const uint32_t mine = (k0 + lane < rc) ? ix.postings[r0 + k0 + lane] : kNoKey;
                 const uint32_t nk = min(32u, rc - k0);
-                for (uint32_t k = 0; k < nk && !m.overflow; k++) {
+                for (uint32_t k = 0; k < nk && !m.overflow(); k++) {
                     const uint32_t e = __shfl_sync(kFull, mine, (int)k);
                     if (e >= shard_lo && e < shard_hi) map_add(m, e, len, lane);
                 }
@@ -206,9 +207,11 @@ __device__ __forceinline__ T ld_row(const T *p) {
     return *p;
 }
 
-// Work a warp did for its requests (SURVEY 8(d) P and M); flushed by the caller.
+// Work a warp did for its requests (SURVEY 8(d) P and M), tallied in the calling kernel's shared memory so that the
+// probe loop carries no totals in registers: blocks probed (added by lane 0) and postings counted (one total per lane).
 struct Work {
-    unsigned long long probes = 0, postings = 0;
+    unsigned long long probes;
+    unsigned long long postings[32];
 };
 
 // The whole decision for request r (all 32 lanes of one warp call it together).  kCg: the per-request inputs
@@ -225,20 +228,22 @@ struct NoFollow {
     __device__ __forceinline__ uint64_t hash(int32_t) const { return 0; }
 };
 // Returns false when the request was handed to the dense-counter kernel (p.overflow_list) instead of being decided.
+// req_next != nullptr: once the probes are done, lane 0 takes a ticket off *req_next into `ticket` (k_match_pick_sparse:
+// the warp's next request, fetched while this one is scored).
 template <bool kCg, bool kSharded, bool kTie, int kStages, typename Follow = NoFollow>
-__device__ __forceinline__ bool match_request(const PickParams &p, const int64_t r, const int lane, const bool counting,
-                                              Work &wk, const Follow fw = Follow()) {
+__device__ __forceinline__ bool match_request(const PickParams &p, const uint32_t r, const int lane, const bool counting,
+                                              Work *wk, int32_t *req_next, int32_t &ticket, const Follow fw = Follow()) {
     const uint32_t shard_lo = p.index.ep_begin, shard_hi = min(p.index.ep_end, (uint32_t)p.E);
     const IndexSlot *slots = p.index.slots;
     const uint32_t mask32 = (uint32_t)p.index.mask;
     const int32_t total = ld_row<kCg>(p.nblocks + r);
     const uint64_t *row = p.hashes + r * (int64_t)p.max_blocks;
     LaneMap m;
-    m.e = kNoKey; m.c = 0; m.n = 0; m.overflow = false;
+    m.e = kNoKey; m.c = 0; m.n = 0;
     // ---- a2/a3: probe in block order, 32 blocks per step; global stop at the first block nobody holds
-    bool stopped = false;
+    int32_t limit = total;                                        // < total once the walk has stopped at block `limit`
     uint64_t hnext = (!Follow::kOn && lane < total) ? ld_row<kCg>(row + lane) : 0;
-    for (int32_t cq = 0; cq < total && !stopped; cq += 32) {
+    for (int32_t cq = 0; cq < total && limit == total; cq += 32) {
         const int32_t i = cq + lane;
         uint64_t hcur;
         if (Follow::kOn) {
@@ -276,41 +281,40 @@ __device__ __forceinline__ bool match_request(const PickParams &p, const int64_t
                 if (!((below0 >> lane) & 1u)) pending = false;
             }
             if (pending) {
+                // straight into (cnt, w0..w4), which a pending lane holds as zeros: no second set of slot registers
                 uint64_t key;
                 Hit hs;
                 load_slot(slots + idx, key, hs);
+                cnt = hs.cnt; w0 = hs.w[0]; w1 = hs.w[1]; w2 = hs.w[2]; w3 = hs.w[3]; w4 = hs.w[4];
                 if (key == hcur) {                                // cnt == 0: every holder was evicted (tombstone)
-                    cnt = hs.cnt; w0 = hs.w[0]; w1 = hs.w[1]; w2 = hs.w[2]; w3 = hs.w[3]; w4 = hs.w[4];
-                    pending = false;
-                } else if (key == kEmptyKey) {                    // a never-used slot ends the probe chain: absent
                     pending = false;
                 } else {
-                    idx = (idx + 1) & mask32;
+                    cnt = 0; w0 = 0; w1 = 0; w2 = 0; w3 = 0; w4 = 0;
+                    if (key == kEmptyKey) pending = false;        // a never-used slot ends the probe chain: absent
+                    else idx = (idx + 1) & mask32;
                 }
             }
         }
         // lanes that stopped early (pending) hold cnt == 0 and sit behind the stop
         const uint32_t miss = kSharded ? gmiss : __ballot_sync(kFull, valid && cnt == 0);
-        const int32_t limit = miss ? cq + (__ffs(miss) - 1) : total;
+        limit = miss ? cq + (__ffs(miss) - 1) : total;
         if (i >= limit) { cnt = 0; w0 = 0; w1 = 0; w2 = 0; w3 = 0; w4 = 0; }
-        if (counting) {
-            if (lane == 0) wk.probes += (unsigned long long)((miss ? limit + 1 : min(total, cq + 32)) - cq);
-            wk.postings += cnt;
-        }
+        if (counting) wk->postings[lane] += cnt;
         if (limit > cq) count_chunk(m, p.index, cnt, w0, w1, w2, w3, w4, shard_lo, shard_hi, lane);
-        if (miss) stopped = true;
     }
+    if (counting && lane == 0) wk->probes += (unsigned long long)min(limit + 1, total);   // up to and including the stop
+    if (req_next && lane == 0) ticket = atomicAdd(req_next, 1);
     // ---- lora-affinity: the endpoints where the request's adapter is active or waiting get a request-dependent
     //      score, so they join the map (count 0) and are evaluated one by one like the prefix holders
     int lora_st = 0;
-    if (p.lora.enabled && p.lora.ptr && !m.overflow) {
+    if (p.lora.enabled && p.lora.ptr && !m.overflow()) {
         const uint32_t a = p.model_ids ? p.model_ids[r] : 0u;
         if (a < (uint32_t)p.lora.n_models) {
             const uint32_t lo = p.lora.ptr[a], hi = p.lora.ptr[a + 1];
-            for (uint32_t k0 = lo; k0 < hi && !m.overflow; k0 += 32) {
+            for (uint32_t k0 = lo; k0 < hi && !m.overflow(); k0 += 32) {
                 const uint32_t mine_e = (k0 + lane < hi) ? p.lora.ep[k0 + lane] : kNoKey;
                 const uint32_t nk = min(32u, hi - k0);
-                for (uint32_t k = 0; k < nk && !m.overflow; k++) {
+                for (uint32_t k = 0; k < nk && !m.overflow(); k++) {
                     const uint32_t e = __shfl_sync(kFull, mine_e, (int)k);
                     if (e >= shard_lo && e < shard_hi) map_add(m, e, 0, lane);
                 }
@@ -318,7 +322,7 @@ __device__ __forceinline__ bool match_request(const PickParams &p, const int64_t
             if ((uint32_t)lane < m.n) lora_st = lora_lookup(p.lora, a, m.e);
         }
     }
-    if (m.overflow) {
+    if (m.overflow()) {
         // hand the request to the dense-counter kernel
         if (lane == 0 && p.overflow_list) p.overflow_list[atomicAdd(p.overflow_n, 1)] = (int32_t)r;
         return false;

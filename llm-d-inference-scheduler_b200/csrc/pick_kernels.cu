@@ -276,6 +276,10 @@ __global__ void __launch_bounds__(kPickWarps * 32) k_match_pick(PickParams p, in
     const int warp = threadIdx.x >> 5;
     const int64_t gwarp = (int64_t)blockIdx.x * kPickWarps + warp;
     const int64_t nwarps = (int64_t)gridDim.x * kPickWarps;
+    // the overflow pass runs over a full grid and its list is almost always empty: a warp without a request leaves
+    // before it clears its counters (no block-wide barrier below)
+    const int64_t n_work = p.req_list ? (int64_t)*p.req_list_n : p.R;
+    if (gwarp >= n_work) return;
     uint32_t *cnt32;
     uint32_t *list;
     if (gscratch) {
@@ -291,7 +295,6 @@ __global__ void __launch_bounds__(kPickWarps * 32) k_match_pick(PickParams p, in
     unsigned long long w_probes = 0, w_postings = 0;    // algorithmic work of this warp's requests
     __syncwarp();
 
-    const int64_t n_work = p.req_list ? (int64_t)*p.req_list_n : p.R;
     for (int64_t wi = gwarp; wi < n_work; wi += nwarps) {
         const int64_t r = p.req_list ? (int64_t)p.req_list[wi] : wi;
         const int32_t total = p.nblocks[r];
