@@ -257,6 +257,10 @@ typedef struct {
     uint64_t last_index_items;         /* hashes added by the last applied batch                               */
     uint64_t last_index_launches;      /* kernels launched by it                                               */
     uint64_t last_index_patched;       /* 1: the last commit patched the read table from the change log; 0: bulk build */
+    /* bytes of hash rows k_hash_fused stored for the last synchronous device batch (8 per hash; a Schedule batch without
+     * keep_hashes stores each row only up to the first block the index cannot hold, EPP_HASH_TRIM; 0 when another hash
+     * kernel ran) */
+    uint64_t last_hash_bytes_stored;
 } epp_stats;
 
 /* ---- lifecycle --------------------------------------------------------------------------------- */
@@ -328,7 +332,8 @@ EPP_API int32_t epp_score(epp_engine *h, int64_t n_requests, const int32_t *matc
 
 /* ---- a1-a14 fused: Scheduler.Schedule for a batch (scheduling/scheduler.go:54-102) ---------------
  * out: [R]; detail: [R] or NULL; keep_hashes != 0 keeps the batch's prefix hashes resident on the device
- * for epp_index_add_picked (the PluginState stash of plugin.go:150-157). */
+ * for epp_index_add_picked (the PluginState stash of plugin.go:150-157).  Without it the engine may store each row
+ * only up to the first block the index cannot hold (EPP_HASH_TRIM). */
 EPP_API int32_t epp_schedule(epp_engine *h, const epp_batch *batch, epp_decision *out, epp_decision_detail *detail,
                      int32_t keep_hashes);
 

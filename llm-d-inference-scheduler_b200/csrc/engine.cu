@@ -85,7 +85,7 @@ struct epp_engine {
     bool s1_unjoined = false;       // chunk-pipelined async batches left work on stream 1 that stream 0 has not waited for
     int64_t pipe_R = 0, pipe_per = 0;   // chunk layout of the pipelined batches in flight (row ranges are per stream)
     int async_launches = 0;
-    DevBuf work_counters;           // u64[2] probes, postings
+    DevBuf work_counters;           // u64[3] probes, postings, hash bytes stored
 
     // models
     DevBuf seeds;                   // u64[kMaxModels]
@@ -117,10 +117,15 @@ struct epp_engine {
     int patches_since_build = 0;
     int patch_enabled = 1;          // EPP_INDEX_PATCH=0: always rebuild
     IndexSlot idx_special_host{};
+    // presence bitmap of the read table (index.cuh presence_maybe): rebuilt by every bulk build, bits added by patches
+    DevBuf presence;
+    int presence_log2 = 0;          // log2 of its bits
+    int presence_log2_env = 0;      // EPP_PRESENCE_LOG2BITS=n (6..26): fixed size instead of 16 bits per table slot
+    int hash_trim = 1;              // EPP_HASH_TRIM=0: Schedule batches store whole hash rows
     uint32_t shard_begin = 0, shard_end = 0xFFFFFFFFu;
 
     // batch buffers (sized for the largest batch seen)
-    DevBuf offsets, lengths, model_ids, multimodal, hashes, nblocks, eff_len, in_len, decisions, details, flag;
+    DevBuf offsets, lengths, model_ids, multimodal, hashes, nblocks, bound, eff_len, in_len, decisions, details, flag;
     DevBuf dense_match, dense_total, dense_scores;
     int index_load = 0;             // EPP_INDEX_LOAD=n: read-table slots per distinct hash (2 = load factor <= 0.5, 4 = <= 0.25);
                                     // 0 = automatic: 4 while the table stays L2-sized (<= l2_table_bytes), else 2
@@ -248,6 +253,8 @@ static int32_t alloc_profile(epp_engine *e, ProfileState &ps) {
     return EPP_OK;
 }
 
+static int32_t rebuild_presence(epp_engine *h);
+
 extern "C" int32_t epp_engine_create(const epp_config *cfg, epp_engine **out) {
     if (!cfg || !out) return fail(EPP_ERR_INVALID, "cfg/out is NULL");
     *out = nullptr;
@@ -293,7 +300,7 @@ extern "C" int32_t epp_engine_create(const epp_config *cfg, epp_engine **out) {
     }
     for (auto &ev : e->ev) CUDA_TRY(cudaEventCreate(&ev));
     for (auto &ev : e->user_ev) CUDA_TRY(cudaEventCreate(&ev));
-    CUDA_TRY(cudaHostAlloc(reinterpret_cast<void **>(&e->wc_host), sizeof(unsigned long long) * 2, cudaHostAllocDefault));
+    CUDA_TRY(cudaHostAlloc(reinterpret_cast<void **>(&e->wc_host), sizeof(unsigned long long) * 3, cudaHostAllocDefault));
     size_t E = (size_t)cfg->max_endpoints;
     CUDA_TRY(e->seeds.reserve(sizeof(uint64_t) * kMaxModels, &e->dev_bytes));
     CUDA_TRY(e->seed_msg.reserve(4096, &e->dev_bytes));
@@ -307,7 +314,7 @@ extern "C" int32_t epp_engine_create(const epp_config *cfg, epp_engine **out) {
     CUDA_TRY(e->idx_special.reserve(sizeof(IndexSlot), &e->dev_bytes));
     CUDA_TRY(e->get_out.reserve(sizeof(uint32_t) * 4096 + 16, &e->dev_bytes));
     CUDA_TRY(e->flag.reserve(sizeof(int) * 4, &e->dev_bytes));
-    CUDA_TRY(e->work_counters.reserve(sizeof(unsigned long long) * 2, &e->dev_bytes));
+    CUDA_TRY(e->work_counters.reserve(sizeof(unsigned long long) * 3, &e->dev_bytes));
     memset(&e->idx_special_host, 0, sizeof(IndexSlot));
     e->idx_special_host.key = kEmptyKey;
     for (int pi = 0; pi < e->n_alloc_profiles; pi++) {
@@ -324,6 +331,8 @@ extern "C" int32_t epp_engine_create(const epp_config *cfg, epp_engine **out) {
     { const char *v1 = getenv("EPP_INDEX_LOAD"); e->index_load = v1 ? std::max(2, atoi(v1)) : 0; }
     { const char *v1 = getenv("EPP_DEV_CHUNKS"); e->dev_chunks = v1 ? std::max(1, atoi(v1)) : 2; }
     { const char *v1 = getenv("EPP_HASH_STAGED"); e->staged = v1 ? atoi(v1) : 0; }
+    { const char *v1 = getenv("EPP_HASH_TRIM"); e->hash_trim = v1 ? atoi(v1) : 1; }
+    { const char *v1 = getenv("EPP_PRESENCE_LOG2BITS"); e->presence_log2_env = v1 ? std::min(26, std::max(6, atoi(v1))) : 0; }
     { const char *v1 = getenv("EPP_MATCH_CTAS"); e->match_ctas = (v1 && atoi(v1) == 6) ? 6 : 8; }
     { const char *v1 = getenv("EPP_SMALL_BATCH"); e->small_max = v1 ? std::max(0, atoi(v1)) : 1024; }
     { const char *v1 = getenv("EPP_SMALL_ZEROCOPY"); e->small_zc_max = v1 ? std::max(0, atoi(v1)) : 8; }
@@ -334,6 +343,7 @@ extern "C" int32_t epp_engine_create(const epp_config *cfg, epp_engine **out) {
     CUDA_TRY(e->small_overflow_n.reserve(sizeof(int32_t) * 4, &e->dev_bytes));
     CUDA_TRY(cudaMemset(e->small_overflow_n.p, 0, sizeof(int32_t) * 4));
     for (int i = 0; i < 2; i++) CUDA_TRY(e->slot[i].overflow_n.reserve(sizeof(int32_t) * 4, &e->dev_bytes));
+    EPP_TRY(rebuild_presence(e.get()));              // the empty index: every bit clear
 
     // match/pick launch geometry: counters in shared memory when they fit, else zeroed global scratch
     size_t smem_local = match_pick_smem_bytes(cfg->max_endpoints, false);
@@ -587,6 +597,20 @@ extern "C" int32_t epp_pool_set_lora(epp_engine *h, int32_t n, const uint32_t *i
 // ------------------------------------------------------------------------------------------------
 // prefix index
 // ------------------------------------------------------------------------------------------------
+// Clears the presence bitmap and sets the bits of every key the read table holds.  16 bits per table slot, which is
+// >= 26 per distinct key at the load factors the build and the patches allow, up to 2^26 bits (8 MiB, L2-resident).
+static int32_t rebuild_presence(epp_engine *h) {
+    int l = 6;
+    while (l < 26 && (1ull << l) < 16 * h->idx_capacity) l++;
+    if (h->presence_log2_env) l = h->presence_log2_env;
+    h->presence_log2 = l;
+    CUDA_TRY(h->presence.reserve(((size_t)1 << l) / 8, &h->dev_bytes));
+    int launches = 0;
+    CUDA_TRY(launch_presence_build(h->idx_capacity ? h->slots.as<IndexSlot>() : nullptr, h->idx_capacity,
+                                   h->presence.as<uint32_t>(), l, h->slot[0].stream, &launches));
+    return EPP_OK;
+}
+
 // Bulk build of the read table from n (hash, endpoint) pairs already in h->pair_hash / h->pair_ep.
 static int32_t build_index_from_device_pairs(epp_engine *h, uint64_t n, uint64_t n_distinct_hint, bool from_store = false) {
     cudaStream_t s = h->slot[0].stream;
@@ -636,7 +660,7 @@ static int32_t build_index_from_device_pairs(epp_engine *h, uint64_t n, uint64_t
     h->rt_intern_used = cursor[3];
     h->rt_from_store = from_store;
     h->patches_since_build = 0;
-    return EPP_OK;
+    return rebuild_presence(h);
 }
 
 static int32_t build_device_index(epp_engine *h, const uint64_t *hashes, const uint32_t *eps, uint64_t n,
@@ -710,6 +734,8 @@ static int32_t commit_locked(epp_engine *h) {
         rt.intern_keys = h->intern_keys.as<uint64_t>();
         rt.intern_vals = h->intern_vals.as<uint32_t>();
         rt.intern_used = h->rt_intern_used;
+        rt.presence = h->presence.as<uint32_t>();
+        rt.presence_shift = 64 - h->presence_log2;
         uint64_t np = 0, nu = 0, npost = 0, ni = 0;
         CUDA_TRY(h->store->patch_read_table(rt, h->idx_pairs, s, &patched, &np, &nu, &npost, &ni));
         if (patched) {
@@ -902,6 +928,7 @@ static int32_t reserve_batch(epp_engine *h, int64_t R) {
     size_t n = (size_t)std::max<int64_t>(R, 1);
     CUDA_TRY(h->hashes.reserve(sizeof(uint64_t) * n * B, &h->dev_bytes));
     CUDA_TRY(h->nblocks.reserve(sizeof(int32_t) * n, &h->dev_bytes));
+    CUDA_TRY(h->bound.reserve(sizeof(int32_t) * n, &h->dev_bytes));
     CUDA_TRY(h->eff_len.reserve(sizeof(int64_t) * n, &h->dev_bytes));
     CUDA_TRY(h->in_len.reserve(sizeof(int64_t) * n, &h->dev_bytes));
     CUDA_TRY(h->decisions.reserve(sizeof(epp_decision) * n, &h->dev_bytes));
@@ -946,6 +973,10 @@ static HashParams hash_params(epp_engine *h, const Work &w) {
     p.offsets_or_bits = w.offsets_or_bits;
     p.sm_count = h->sm_count;
     p.staged = h->staged;
+    p.presence = nullptr;
+    p.presence_shift = 0;
+    p.bound = nullptr;
+    p.stored = nullptr;
     return p;
 }
 
@@ -982,6 +1013,7 @@ static PickParams pick_params(epp_engine *h, const Work &w, epp_decision *out, e
     p.tie_base = h->stats.n_decisions + (uint64_t)w.r0;
     p.hashes = w.hashes_out;
     p.nblocks = w.nblocks_out;
+    p.bound = nullptr;
     p.in_len = h->in_len.as<int64_t>() + w.r0;
     p.model_ids = w.model_ids_dev ? w.model_ids_dev + w.r0 : nullptr;
     p.lora = lora_dev(h);
@@ -1046,6 +1078,17 @@ static int32_t launch_match(epp_engine *h, Slot &sl, PickParams pp, int *launche
     return launch_overflow_pass(h, sl, pp, launches);
 }
 
+// A Schedule batch's hash rows are read by nothing but its match kernel, whose global stop never lies beyond the first
+// block the presence bitmap proves absent: k_hash_fused stores each row only up to there and both match kernels honour
+// the bound.  Only on the k_hash_fused + k_match_pick_sparse path (not the dense-counter or general evaluation).
+static void trim_rows(epp_engine *h, const Work &w, HashParams &hp, PickParams &pp) {
+    if (!hash_fused_selected(hp) || pp.out_match || pp.gen.on) return;
+    hp.presence = h->presence.as<uint32_t>();
+    hp.presence_shift = 64 - h->presence_log2;
+    hp.bound = h->bound.as<int32_t>() + w.r0;
+    pp.bound = hp.bound;
+}
+
 // The whole cycle for one Work item: hash kernel, then the standalone match / score / pick kernel (every fused or
 // concurrently scheduled arrangement of the two was measured slower).
 static int32_t launch_cycle(epp_engine *h, Slot &sl, const HashParams &hp, PickParams pp, int *launches, cudaEvent_t *ev) {
@@ -1068,6 +1111,7 @@ static int32_t finish_async(epp_engine *h) {
     h->stats.last_h2d_ms = h->stats.last_d2h_ms = 0;
     h->stats.last_probes = h->wc_host[0];
     h->stats.last_postings = h->wc_host[1];
+    h->stats.last_hash_bytes_stored = h->wc_host[2];
     h->stats.last_kernel_launches = (uint64_t)h->async_launches;
     return EPP_OK;
 }
@@ -1252,9 +1296,10 @@ static int32_t run_small(epp_engine *h, const BatchView &v, int mode, const uint
 
 // Runs hashing (+ match/pick) for a batch.  Host batches are split into chunks whose H2D copy overlaps the
 // kernels of the previous chunk (two streams, two staging buffers); device batches run in one pass.
+// keep_hashes: the hash rows of a Schedule batch stay for epp_index_add_picked (whole rows, no trimming).
 static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t *out_hashes, int32_t *out_nblocks,
                          epp_decision *out_dec, epp_decision_detail *out_detail, int32_t *out_match,
-                         int32_t *out_total) {
+                         int32_t *out_total, bool keep_hashes = false) {
     const int64_t R = v.R;
     const size_t B = (size_t)h->cfg.max_prefix_blocks;
     if (R == 0) return EPP_OK;
@@ -1296,6 +1341,8 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
         }
     }
     const bool pipelined = v.device && v.async && mode == Mode::Schedule && h->dev_chunks > 1 && R >= 2 * 4096 && !h->pick_global;
+    // the endpoint-sharded mode's local table is not the global one: its rows stay whole
+    const bool trim = mode == Mode::Schedule && !keep_hashes && h->hash_trim && h->shard_begin == 0 && h->shard_end == 0xFFFFFFFFu;
     if (!pipelined) EPP_TRY(join_streams(h));
     EPP_TRY(reserve_batch(h, R));
     int launches = 0;
@@ -1308,7 +1355,7 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
                (mode == Mode::HashOnly && out_hashes) ? out_hashes : h->hashes.as<uint64_t>(),
                (mode == Mode::HashOnly && out_nblocks) ? out_nblocks : (mode == Mode::Match && out_total ? out_total : h->nblocks.as<int32_t>()),
                v.multimodal};
-        CUDA_TRY(cudaMemsetAsync(h->work_counters.p, 0, sizeof(unsigned long long) * 2, s0));
+        CUDA_TRY(cudaMemsetAsync(h->work_counters.p, 0, sizeof(unsigned long long) * 3, s0));
         const int64_t min_chunk = 4096;
         if (pipelined) {
             // Throughput mode: the batch runs as C chunks alternating between the engine's two streams, so the hash
@@ -1333,7 +1380,9 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
                 PickParams pp = pick_params(h, w, dec_base + r0, out_detail ? out_detail + r0 : nullptr, nullptr);
                 if (tk) attach_topk(h, pp.gen, tk_picks, tk_scores, r0);
                 Slot &sl = h->slot[k & 1];
-                EPP_TRY(launch_cycle(h, sl, hash_params(h, w), pp, &launches, nullptr));
+                HashParams hp = hash_params(h, w);
+                if (trim) trim_rows(h, w, hp, pp);
+                EPP_TRY(launch_cycle(h, sl, hp, pp, &launches, nullptr));
             }
             h->s1_unjoined = true;
             h->pipe_R = R;
@@ -1345,10 +1394,13 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
             PickParams pp = pick_params(h, w, dec, mode == Mode::Schedule ? out_detail : nullptr, mode == Mode::Match ? out_match : nullptr);
             pp.work_counters = h->work_counters.as<unsigned long long>();
             if (tk) attach_topk(h, pp.gen, tk_picks, tk_scores, 0);
-            EPP_TRY(launch_cycle(h, h->slot[0], hash_params(h, w), pp, &launches, h->ev));
+            HashParams hp = hash_params(h, w);
+            hp.stored = h->work_counters.as<unsigned long long>() + 2;
+            if (trim) trim_rows(h, w, hp, pp);
+            EPP_TRY(launch_cycle(h, h->slot[0], hp, pp, &launches, h->ev));
         }
         CUDA_TRY(cudaEventRecord(h->ev[4], s0));
-        CUDA_TRY(cudaMemcpyAsync(h->wc_host, h->work_counters.p, sizeof(unsigned long long) * 2, cudaMemcpyDeviceToHost, s0));
+        CUDA_TRY(cudaMemcpyAsync(h->wc_host, h->work_counters.p, sizeof(unsigned long long) * 3, cudaMemcpyDeviceToHost, s0));
         h->async_pending = true;
         h->async_launches = launches;
         if (v.async && mode != Mode::Match) return EPP_OK;         // epp_synchronize() (or the next call that needs the
@@ -1439,7 +1491,9 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
             epp_decision_detail *det = h->details.as<epp_decision_detail>() + c.r0;
             PickParams pp = pick_params(h, w, dec, det, dm);
             if (tk) attach_topk(h, pp.gen, tk_picks, tk_scores, c.r0);
-            EPP_TRY(launch_cycle(h, sl, hash_params(h, w), pp, &launches, nullptr));
+            HashParams hp = hash_params(h, w);
+            if (trim) trim_rows(h, w, hp, pp);
+            EPP_TRY(launch_cycle(h, sl, hp, pp, &launches, nullptr));
             if (mode == Mode::Schedule) {
                 if (out_dec) CUDA_TRY(cudaMemcpyAsync(out_dec + c.r0, dec, sizeof(epp_decision) * nreq, cudaMemcpyDeviceToHost, s));
                 if (out_detail) CUDA_TRY(cudaMemcpyAsync(out_detail + c.r0, det, sizeof(epp_decision_detail) * nreq, cudaMemcpyDeviceToHost, s));
@@ -1508,7 +1562,7 @@ static int32_t schedule_impl(epp_engine *h, const epp_batch *batch, epp_decision
     if (h->cfg.encode_enabled && v.multimodal && !detail) return fail(EPP_ERR_INVALID, "an encode profile is configured and the batch flags multimodal requests: `detail` (which carries the encode pick) must not be NULL");
     h->kept_R = 0;
     h->cur_topk = topk;
-    const int32_t rc = run_batch(h, v, Mode::Schedule, nullptr, nullptr, out, detail, nullptr, nullptr);
+    const int32_t rc = run_batch(h, v, Mode::Schedule, nullptr, nullptr, out, detail, nullptr, nullptr, keep_hashes != 0);
     h->cur_topk = nullptr;
     EPP_TRY(rc);
     h->stats.n_batches++;

@@ -4,7 +4,9 @@
 // cp.async-staged alternative behind EPP_HASH_STAGED=1 (DESIGN.md section 4.1).
 //
 // HBM traffic per request: every prompt byte is read exactly once, the 8-byte pre-chain digests never leave the SM
-// (shared-memory ring), the block hashes are written once (the PluginState stash PreRequest needs, plugin.go:150-157).
+// (shared-memory ring), the block hashes are written once (the PluginState stash PreRequest needs, plugin.go:150-157)
+// -- or, with a presence bitmap (HashParams::presence), only up to the first block no endpoint can hold: the match
+// kernel's global stop never lies beyond it.
 //
 // CTA = 9 warps, tile = 32 requests:
 //   warps 0-7 (digest): thread (r = t/8, j = t%8) owns block k*8+j of request r in window k: 4 independent XXH64
@@ -14,7 +16,7 @@
 //   Stages are handed over with named barriers (bar.arrive / bar.sync), 4-deep ring of stages of TWO windows each: full
 //   (digest -> chain), empty (chain -> digest).
 #include "hash_blocks.cuh"
-#include "kernels.h"
+#include "index.cuh"
 
 namespace epp {
 
@@ -63,14 +65,35 @@ __device__ __forceinline__ void tile_lengths(const HashParams &p, int64_t r0, in
     if (t == 0) *s_maxfull = mx;
 }
 
+// Per-lane stop bound of the chain warp: the first window whose leading block reads as absent in the presence bitmap
+// (one lookup per window of W blocks).  The word is loaded right after the window is chained and examined only once the
+// NEXT window has been chained, so the L2 latency hides behind that work instead of stalling the ring; a window is
+// stored while no earlier one has been proven absent, so a row may run up to W - 1 hashes past its bound (never read).
+struct StopBound {
+    int32_t bnd = INT32_MAX;        // a block proven absent (bound >= the global stop); INT32_MAX while none is
+    int32_t pending = -1;           // block whose presence word is in flight, or -1
+    uint32_t word = 0, bit = 0;
+
+    __device__ __forceinline__ void issue(const HashParams &p, int32_t block, uint64_t h) {
+        const uint32_t b = (uint32_t)(h >> p.presence_shift);
+        word = __ldg(p.presence + (b >> 5));
+        bit = h == kEmptyKey ? 32u : (b & 31);   // the all-ones hash lives in the side record: always present
+        pending = block;
+    }
+    __device__ __forceinline__ void resolve() {
+        if (bit < 32 && !((word >> bit) & 1u)) bnd = pending;
+        pending = -1;
+    }
+};
+
 // Chain warp, one window: the serial part of the digest for 32 requests at once (lane = request); every lane then
 // writes its request's 8 hashes straight from registers (64 bytes = two full sectors per lane, 128-bit stores when the
-// row pitch allows) -- no transpose through shared memory.
+// row pitch allows) -- no transpose through shared memory.  With p.presence, hashes at or past a proven-absent block
+// are not stored (the match kernel never reads past it); every hash is still computed.
 template <int TR, int W = kWin>
-__device__ __forceinline__ uint64_t chain_window(uint64_t (*sm)[W + 1], const int32_t *s_nfull, const HashParams &p,
-                                                 int64_t r0, int k, int lane, int32_t nfull, uint64_t lenp8,
-                                                 uint64_t prev) {
-    (void)s_nfull;
+__device__ __forceinline__ uint64_t chain_window(uint64_t (*sm)[W + 1], const HashParams &p, int64_t r0, int k,
+                                                 int lane, int32_t nfull, uint64_t lenp8, uint64_t prev,
+                                                 StopBound &sb, uint32_t &n_stored) {
     const int32_t n_here = min(W, nfull - k * W);              // hashes of this window for my request (<= 0: none)
     if (lane >= TR || n_here <= 0) return prev;
     uint64_t hv[W];
@@ -79,16 +102,21 @@ __device__ __forceinline__ uint64_t chain_window(uint64_t (*sm)[W + 1], const in
         if (j < n_here) prev = xxh_chain_step32(sm[lane][j], lenp8, prev);
         hv[j] = prev;
     }
+    if (sb.pending >= 0) sb.resolve();                         // the previous window's word has had this window's time
+    const int32_t n_store = min(n_here, sb.bnd - k * W);
+    if (n_store <= 0) return prev;
+    n_stored += (uint32_t)n_store;
     uint64_t *dst = p.hashes + (r0 + lane) * (int64_t)p.max_blocks + (int64_t)k * W;
-    if (n_here == W && !(p.max_blocks & 1) && !(reinterpret_cast<uintptr_t>(p.hashes) & 15)) {   // the window starts 16-byte aligned
+    if (n_store == W && !(p.max_blocks & 1) && !(reinterpret_cast<uintptr_t>(p.hashes) & 15)) {   // the window starts 16-byte aligned
 #pragma unroll
         for (int j = 0; j < W; j += 2)
             asm volatile("st.global.v2.u64 [%0], {%1, %2};" ::"l"(dst + j), "l"(hv[j]), "l"(hv[j + 1]) : "memory");
     } else {
 #pragma unroll
         for (int j = 0; j < W; j++)
-            if (j < n_here) dst[j] = hv[j];
+            if (j < n_store) dst[j] = hv[j];
     }
+    if (p.presence && sb.bnd == INT32_MAX) sb.issue(p, k * W, hv[0]);        // closed requests issue no loads
     return prev;
 }
 }  // namespace
@@ -137,20 +165,37 @@ __global__ void __launch_bounds__(32 * kWin + 32, kHashMinCtas) k_hash_fused(Has
             const int64_t r = r0 + lane;
             const int32_t nfull = s_nfull[lane];
             uint64_t prev = 0;
+            StopBound sb;
+            uint32_t n_stored = 0;
             if (r < p.R) prev = p.seeds[p.model_ids ? p.model_ids[r] : 0];
             for (int k = 0; k < n_st; k++) {
                 const int s = k % kStages;
                 bar_sync(kBarFull + s, kProducers);
 #pragma unroll
                 for (int u = 0; u < kSub; u++)
-                    prev = chain_window<TR, W>(s_m[s][u], s_nfull, p, r0, k * kSub + u, lane, nfull, lenp8, prev);
+                    prev = chain_window<TR, W>(s_m[s][u], p, r0, k * kSub + u, lane, nfull, lenp8, prev, sb, n_stored);
                 bar_arrive(kBarEmpty + s, kProducers);
             }
+            if (sb.pending >= 0) sb.resolve();
+            int32_t &bnd = sb.bnd;
             if (r < p.R) {                           // trailing partial block (hashing.go:90-96): generic tail, rare
                 const int64_t eff = s_eff[lane];
-                if ((int64_t)nfull * bs < eff)
-                    p.hashes[r * (int64_t)p.max_blocks + nfull] = hash_block_generic(
-                        p.data + s_off[lane] + (uint64_t)nfull * (uint64_t)bs, eff - (int64_t)nfull * bs, prev);
+                int32_t nb = nfull;
+                if ((int64_t)nfull * bs < eff) {
+                    nb++;
+                    const uint64_t h = hash_block_generic(p.data + s_off[lane] + (uint64_t)nfull * (uint64_t)bs,
+                                                          eff - (int64_t)nfull * bs, prev);
+                    if (bnd == INT32_MAX && p.presence && !presence_maybe(p.presence, p.presence_shift, h)) bnd = nfull;
+                    if (nfull < bnd) {
+                        p.hashes[r * (int64_t)p.max_blocks + nfull] = h;
+                        n_stored++;
+                    }
+                }
+                if (p.presence) p.bound[r] = min(bnd, nb);
+            }
+            if (p.stored) {
+                for (int o = 16; o; o >>= 1) n_stored += __shfl_xor_sync(0xffffffffu, n_stored, o);
+                if (lane == 0) atomicAdd(p.stored, 8ull * n_stored);
             }
         }
         __syncthreads();

@@ -109,6 +109,10 @@ cudaError_t launch_check_offsets_aligned(const uint64_t *offsets, int64_t n, int
 
 cudaError_t launch_hash_fused(const HashParams &p, int sm_count, cudaStream_t s, int *launches);
 
+bool hash_fused_selected(const HashParams &p) {
+    return hash_batch_alignment(p) >= 16 && !(p.staged > 0 && hash_staged_supported(p));
+}
+
 // ev (optional, 4 events): recorded around the hash kernel(s): [1]..[2] brackets the kernel that reads the prompt bytes.
 cudaError_t launch_hash_prompts(const HashParams &p, cudaStream_t s, int *launches, cudaEvent_t *ev) {
     if (p.R <= 0) return cudaSuccess;
@@ -116,7 +120,7 @@ cudaError_t launch_hash_prompts(const HashParams &p, cudaStream_t s, int *launch
     if (align >= 16) {                          // one kernel: lengths + digests + chain
         if (ev) { cudaEventRecord(ev[0], s); cudaEventRecord(ev[1], s); }
         cudaError_t e;
-        if (p.staged > 0 && hash_staged_supported(p)) e = launch_hash_staged(p, p.staged, s, launches);
+        if (!hash_fused_selected(p)) e = launch_hash_staged(p, p.staged, s, launches);
         else e = launch_hash_fused(p, p.sm_count, s, launches);
         if (ev) { cudaEventRecord(ev[2], s); cudaEventRecord(ev[3], s); }
         return e;

@@ -46,6 +46,18 @@ __device__ __forceinline__ bool probe(const IndexView &ix, uint64_t hash, Hit &h
     }
 }
 
+// Presence bitmap of the read table: one bit per bucket of the key's top log2(bits) bits (shift = 64 - log2(bits);
+// the table's `key & mask` uses the low bits).  A clear bit proves that no endpoint holds the key, a set bit means
+// "maybe".  The all-ones key lives in the side record and always reads as present.
+__device__ __forceinline__ bool presence_maybe(const uint32_t *bits, int shift, uint64_t h) {
+    const uint32_t b = (uint32_t)(h >> shift);
+    return h == kEmptyKey || ((__ldg(bits + (b >> 5)) >> (b & 31)) & 1u);
+}
+__device__ __forceinline__ void presence_set(uint32_t *bits, int shift, uint64_t h) {
+    const uint32_t b = (uint32_t)(h >> shift);
+    atomicOr(bits + (b >> 5), 1u << (b & 31));
+}
+
 // k-th endpoint of a hit (k < h.cnt).
 __device__ __forceinline__ uint32_t posting(const IndexView &ix, const Hit &h, uint32_t k) {
     if (h.cnt > (uint32_t)kInlineIds) return ix.postings[h.w[0] + k];

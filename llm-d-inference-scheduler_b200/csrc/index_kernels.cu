@@ -223,6 +223,23 @@ cudaError_t launch_index_build(const uint64_t *pair_hash, const uint32_t *pair_e
     return cudaGetLastError();
 }
 
+// Presence bitmap of the table (index.cuh): cleared, then one bit per key that some endpoint holds.
+__global__ void k_presence_build(const IndexSlot *slots, uint64_t capacity, uint32_t *bits, int shift) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= capacity) return;
+    const uint64_t key = slots[i].key;
+    if (key != kEmptyKey && slots[i].cnt) presence_set(bits, shift, key);
+}
+
+cudaError_t launch_presence_build(const IndexSlot *slots, uint64_t capacity, uint32_t *bits, int log2bits, cudaStream_t s,
+                                  int *launches) {
+    cudaError_t e = cudaMemsetAsync(bits, 0, ((size_t)1 << log2bits) / 8, s);
+    if (e != cudaSuccess || !slots || !capacity) return e;
+    k_presence_build<<<(unsigned)((capacity + 255) / 256), 256, 0, s>>>(slots, capacity, bits, 64 - log2bits);
+    if (launches) *launches += 1;
+    return cudaGetLastError();
+}
+
 __global__ void k_index_get(IndexView ix, uint64_t hash, uint32_t *out_eps, int32_t cap, int32_t *out_n) {
     if (threadIdx.x || blockIdx.x) return;
     Hit h;

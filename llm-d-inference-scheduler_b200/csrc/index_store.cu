@@ -1,4 +1,5 @@
 // index_store.cu -- kernels and host logic of the HBM-resident write side of the prefix index (see index_store.h).
+#include "index.cuh"
 #include "index_store.h"
 
 #include <algorithm>
@@ -774,6 +775,8 @@ struct PatchView {
     uint64_t *intern_keys;       // interning table of the last bulk build (capacity entries)
     uint32_t *intern_vals;
     unsigned long long *intern_claims;   // keys this patch claimed in it
+    uint32_t *presence;          // presence bitmap of the read table; a key that loses its last endpoint keeps its bit
+    int32_t presence_shift;
 };
 
 __device__ __forceinline__ uint64_t rt_find_or_claim(const PatchView &pv, uint64_t key, uint32_t &claimed) {
@@ -909,6 +912,7 @@ __global__ void k_patch_apply(View v, PatchView pv, unsigned long long n_dirty) 
     }
     sl->cnt = n_new;
     pv.head[si] = kNil;
+    if (n_new) presence_set(pv.presence, pv.presence_shift, hsh);
     if (n_new > cnt) atomicAdd(&v.ctr[kCtrPatchAdd], (unsigned long long)(n_new - cnt));
     if (n_new < cnt) atomicAdd(&v.ctr[kCtrPatchDel], (unsigned long long)(cnt - n_new));
 }
@@ -1299,6 +1303,8 @@ cudaError_t IndexStore::patch_read_table(const ReadTableRef &rt, uint64_t table_
     pv.intern_keys = rt.intern_keys;
     pv.intern_vals = rt.intern_vals;
     pv.intern_claims = &v.ctr[kCtrPatchIntern];
+    pv.presence = rt.presence;
+    pv.presence_shift = rt.presence_shift;
     ST_TRY(cudaMemsetAsync(&v.ctr[kCtrPatchFlag], 0, sizeof(unsigned long long) * 6, s));     // flag .. intern
     ctr_host_[kCtrPatchPost] = rt.post_used;
     ST_TRY(cudaMemcpyAsync(&v.ctr[kCtrPatchPost], &ctr_host_[kCtrPatchPost], sizeof(unsigned long long), cudaMemcpyHostToDevice, s));

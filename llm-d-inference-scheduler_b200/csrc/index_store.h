@@ -55,6 +55,8 @@ struct ReadTableRef {
     uint64_t *intern_keys = nullptr;
     uint32_t *intern_vals = nullptr;
     uint64_t intern_used = 0;     // claimed keys of the interning table, retired ones included (`capacity` entries)
+    uint32_t *presence = nullptr; // presence bitmap (index.cuh): the patch sets the bits of keys whose list is not empty
+    int32_t presence_shift = 0;
 };
 
 class IndexStore {

@@ -27,9 +27,18 @@ struct HashParams {
     uint64_t offsets_or_bits;   // OR of every offsets[r] (low bits decide the common alignment)
     int32_t sm_count;
     int32_t staged;             // hash_staged.cu (cp.async-staged, warp-per-task) kernel: 0 off, 1 default shape, else a launch shape (A/B)
+    // k_hash_fused only: presence != nullptr trims the rows to the read table's reach.  bound[r] = the first block at a
+    // window start (every 8th block is looked up) whose presence bit is clear (index.cuh), else nblocks[r]: the global
+    // stop is <= bound[r].  Hashes [0, bound[r]) are stored, plus at most the rest of bound's window.
+    const uint32_t *presence;
+    int32_t presence_shift;
+    int32_t *bound;             // [R]
+    unsigned long long *stored; // += bytes of hash rows stored by k_hash_fused, or nullptr
 };
 // Common alignment (0, 16, 32) of every block start; >= 16 (and block_bytes % 32 == 0) enables the fused kernel.
 int hash_batch_alignment(const HashParams &p);
+// Does launch_hash_prompts run k_hash_fused for this batch (the only kernel that trims rows and counts stored bytes)?
+bool hash_fused_selected(const HashParams &p);
 // Generic single-message XXH64 (model || salt seeds).  msg on device.
 cudaError_t launch_hash_bytes(const uint8_t *msg, size_t len, uint64_t *out, cudaStream_t s);
 cudaError_t launch_check_offsets_aligned(const uint64_t *offsets, int64_t n, int *flag_dev, cudaStream_t s);
@@ -75,6 +84,9 @@ cudaError_t launch_index_build(const uint64_t *pair_hash, const uint32_t *pair_e
                                cudaStream_t s, int *launches);
 cudaError_t launch_index_get(const IndexView &ix, uint64_t hash, uint32_t *out_eps, int32_t cap, int32_t *out_n,
                              cudaStream_t s);
+// Presence bitmap of 2^log2bits bits (6..26) over the table's keys (index.cuh presence_maybe); slots == nullptr: clear.
+cudaError_t launch_presence_build(const IndexSlot *slots, uint64_t capacity, uint32_t *bits, int log2bits, cudaStream_t s,
+                                  int *launches);
 
 // ------------------------------------------------------------------------------------------------
 // pool state -> request-independent scorer terms (a5-a9 precompute)
@@ -150,6 +162,9 @@ struct PickParams {
     ProfileDev prof[kMaxProfiles];
     const uint64_t *hashes;    // [R][max_blocks]
     const int32_t *nblocks;    // [R]
+    // [R] rows trimmed by k_hash_fused (HashParams::bound): hashes [bound, nblocks) were not stored and block `bound`
+    // (< nblocks) is a proven miss.  nullptr: every row is whole.
+    const int32_t *bound;
     const int64_t *in_len;     // [R] prompt bytes (decider)
     const uint32_t *model_ids; // [R] registered model (= LoRA adapter) of each request, or nullptr => model 0
     LoraDev lora;

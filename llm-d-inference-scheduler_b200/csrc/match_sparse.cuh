@@ -237,12 +237,14 @@ __device__ __forceinline__ bool match_request(const PickParams &p, const uint32_
     const IndexSlot *slots = p.index.slots;
     const uint32_t mask32 = (uint32_t)p.index.mask;
     const int32_t total = ld_row<kCg>(p.nblocks + r);
+    // hashes [0, stored) are in the row; block `stored` < total is a proven miss (PickParams::bound)
+    const int32_t stored = (!Follow::kOn && p.bound) ? ld_row<kCg>(p.bound + r) : total;
     const uint64_t *row = p.hashes + r * (int64_t)p.max_blocks;
     LaneMap m;
     m.e = kNoKey; m.c = 0; m.n = 0;
     // ---- a2/a3: probe in block order, 32 blocks per step; global stop at the first block nobody holds
     int32_t limit = total;                                        // < total once the walk has stopped at block `limit`
-    uint64_t hnext = (!Follow::kOn && lane < total) ? ld_row<kCg>(row + lane) : 0;
+    uint64_t hnext = (!Follow::kOn && lane < stored) ? ld_row<kCg>(row + lane) : 0;
     for (int32_t cq = 0; cq < total && limit == total; cq += 32) {
         const int32_t i = cq + lane;
         uint64_t hcur;
@@ -251,7 +253,7 @@ __device__ __forceinline__ bool match_request(const PickParams &p, const uint32_
             hcur = i < total ? fw.hash(i) : 0;
         } else {
             hcur = hnext;
-            if (i + 32 < total) hnext = ld_row<kCg>(row + i + 32);    // next chunk's hashes in flight during this one
+            if (i + 32 < stored) hnext = ld_row<kCg>(row + i + 32);   // next chunk's hashes in flight during this one
         }
         const bool valid = i < total;
         // endpoint-sharded mode: a block is missing only if NO rank holds it, and that is known up front
@@ -263,7 +265,7 @@ __device__ __forceinline__ bool match_request(const PickParams &p, const uint32_
         }
         const uint32_t relevant = (kSharded && gmiss) ? ((1u << (__ffs(gmiss) - 1)) - 1u) : kFull;
         uint32_t cnt = 0, w0 = 0, w1 = 0, w2 = 0, w3 = 0, w4 = 0;
-        bool pending = valid && ((relevant >> lane) & 1u);
+        bool pending = i < stored && ((relevant >> lane) & 1u);     // lanes in [stored, total): absent, never probed
         if (pending && (hcur == kEmptyKey || !slots)) {           // the sentinel hash lives in a side record
             Hit hs;
             if (probe(p.index, hcur, hs)) { cnt = hs.cnt; w0 = hs.w[0]; w1 = hs.w[1]; w2 = hs.w[2]; w3 = hs.w[3]; w4 = hs.w[4]; }

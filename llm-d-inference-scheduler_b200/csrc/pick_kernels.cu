@@ -298,6 +298,7 @@ __global__ void __launch_bounds__(kPickWarps * 32) k_match_pick(PickParams p, in
     for (int64_t wi = gwarp; wi < n_work; wi += nwarps) {
         const int64_t r = p.req_list ? (int64_t)p.req_list[wi] : wi;
         const int32_t total = p.nblocks[r];
+        const int32_t stored = p.bound ? p.bound[r] : total;      // block `stored` < total: a proven miss
         if (lane == 0) *list_n = 0;
         __syncwarp();
         // ---- a2/a3: probe in block order, global stop at the first block nobody holds (plugin.go:214-230)
@@ -308,7 +309,7 @@ __global__ void __launch_bounds__(kPickWarps * 32) k_match_pick(PickParams p, in
             Hit hit;
             hit.cnt = 0;
             bool found = false;
-            if (active) found = probe(p.index, row[i], hit);
+            if (i < stored) found = probe(p.index, row[i], hit);
             if (!found) hit.cnt = 0;
             const uint32_t cnt = hit.cnt;
             uint32_t miss;

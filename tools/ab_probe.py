@@ -100,6 +100,7 @@ def main():
                 out["sync_kernel_ms"] = [round(x, 4) for x in st["last_kernel_ms"][:4]]
                 out["launches"] = int(st["last_kernel_launches"])
                 out["probes"], out["postings"] = int(st["last_probes"]), int(st["last_postings"])
+                out["hash_bytes_stored"] = int(st["last_hash_bytes_stored"])
                 dec = epp.decisions_from_torch(dev_dec)
                 if ref_dec is None:
                     ref_dec = dec.copy()
