@@ -52,6 +52,40 @@ func Register(e *Engine) {
 	})
 }
 
+// NoHitLRUType is the reference's plugin type of the no-hit-lru scorer (scorer/nohitlru/no_hit_lru.go).
+const NoHitLRUType = "no-hit-lru-scorer"
+
+// NoHitLRUScorer turns the parameters of a "no-hit-lru-scorer" entry (nohitlru.Parameters: lruSize, prefixPluginType,
+// prefixPluginName) into the engine's scorer of the profile.  The prefix plugin names are accepted and ignored: the
+// engine's own prefix match decides whether a request is cold.  lruSize <= 0 means 1024 (no_hit_lru.go:93-95); every
+// profile that lists the scorer must use the same lruSize, because they share one LRU (epp_engine_create rejects others).
+func NoHitLRUScorer(weight float64, params json.RawMessage) (ScorerSpec, error) {
+	var p struct {
+		LRUSize          int    `json:"lruSize"`
+		PrefixPluginType string `json:"prefixPluginType"`
+		PrefixPluginName string `json:"prefixPluginName"`
+	}
+	if len(params) > 0 {
+		if err := json.Unmarshal(params, &p); err != nil {
+			return ScorerSpec{}, err
+		}
+	}
+	return ScorerSpec{Kind: int(C.EPP_SCORER_NO_HIT_LRU), Weight: weight, Param: float64(p.LRUSize)}, nil
+}
+
+// NoHitLRUKeys returns the slots of the scorer's LRU, oldest first (golang-lru Cache.Keys, epp_nohit_lru_get).
+func (e *Engine) NoHitLRUKeys() ([]uint32, error) {
+	out := make([]uint32, e.cfg.MaxEndpoints)
+	var n C.int32_t
+	if rc := C.epp_nohit_lru_get(e.h, (*C.uint32_t)(unsafe.Pointer(&out[0])), C.int32_t(len(out)), &n); rc != C.EPP_OK {
+		return nil, lastError()
+	}
+	if int(n) < len(out) {
+		out = out[:n]
+	}
+	return out, nil
+}
+
 // matchRow runs epp_prefix_match for one request: dense matchBlocks per slot + totalBlocks.
 func (e *Engine) matchRow(model uint32, prompt []byte) ([]int32, int32, error) {
 	match := make([]int32, e.cfg.MaxEndpoints)

@@ -26,7 +26,10 @@
  *
  * Batch semantics (SURVEY.md App. A.8): the reference schedules one request at a time; a batch evaluates
  * all R requests against ONE frozen snapshot (pool state + prefix index).  Index updates (PreRequest)
- * are applied between batches.
+ * are applied between batches.  The same holds for the no-hit-lru scorer's LRU: every scheduling call (epp_schedule[_topk],
+ * epp_schedule_with_match[_topk], the micro-batcher's flushes) scores against the LRU as it stood when the call started
+ * and then applies its cold requests' Adds in request order (on the device, in enqueue order for async batches), so cold
+ * requests inside one batch do not rotate; epp_score, epp_prefix_match and epp_hash_prompts never update it.
  *
  * Tie rule: the reference's max-score picker shuffles with math/rand before its stable sort, i.e. it returns a
  * uniformly random member of the arg-max set (picker/maxscore/picker.go:91-102).  The engine always returns the bit
@@ -97,8 +100,15 @@ typedef enum {
     EPP_SCORER_ACTIVE_REQUEST = 7, /* "active-request-scorer"    scorer/activerequest/active_request.go:140-173; column = ext
                                   column holding InFlightLoad.Requests, param = maxBusyScore (outside [0,1]: 1.0),
                                   param2 = idleThreshold (< 0: 0)                                                 */
-    EPP_SCORER_LORA_AFFINITY = 8  /* "lora-affinity-scorer"      scorer/loraaffinity/lora_affinity.go:76-100; the adapter is the
+    EPP_SCORER_LORA_AFFINITY = 8, /* "lora-affinity-scorer"      scorer/loraaffinity/lora_affinity.go:76-100; the adapter is the
                                   request's model id; residency comes from epp_pool_set_lora                     */
+    EPP_SCORER_NO_HIT_LRU = 9  /* "no-hit-lru-scorer"            scorer/nohitlru/no_hit_lru.go:259-321; param = lruSize (<= 0:
+                                  1024), the same in every profile that lists it (they share ONE LRU).  A request is cold
+                                  for a profile when no candidate holds a block of its prompt (the engine's own match is
+                                  the producer).  Every scheduling call scores against the LRU as it stood when the call
+                                  started and then Adds, for each cold request in request order, its pick and its
+                                  prefill pick (PreRequest, :279-321): inside one batch cold requests do not rotate.
+                                  Not available in the endpoint-sharded and peer-memory modes.                    */
 } epp_scorer_kind;
 
 /* Value of the llm-d.ai/role label (filter/bylabel/roles.go:25-44). */
@@ -246,7 +256,8 @@ typedef struct {
     uint64_t last_kernel_launches;
     uint64_t device_bytes;
     /* device-pointer batches only: CUDA-event time of each kernel of the last batch on the launch stream.
-     * [0] prompt lengths  [1] block digests (dominant: reads every token once)  [2] chain  [3] match+score+pick */
+     * [0] prompt lengths  [1] block digests (dominant: reads every token once)  [2] chain  [3] match+score+pick
+     * [4] the no-hit-lru update after the picks (engines with that scorer; 0 otherwise) */
     double last_kernel_ms[8];
     /* algorithmic work of the last batch (SURVEY.md 8(d)): table probes P = sum_r min(stop_r+1, B_r) and
      * postings consumed M = sum_r sum_{i<stop_r} |servers(h_i)| */
@@ -368,6 +379,10 @@ EPP_API int32_t epp_schedule_with_match_topk(epp_engine *h, int64_t n_requests, 
 /* PreRequest (approximateprefix/plugin.go:164-200): index the hashes of the LAST epp_schedule batch
  * (keep_hashes=1) for each request's primary pick and prefill pick. */
 EPP_API int32_t epp_index_add_picked(epp_engine *h);
+
+/* The no-hit-lru scorer's LRU, oldest first (golang-lru Cache.Keys): *out_n = its length, the first min(cap, *out_n)
+ * slot ids go to out_eps.  Waits for the batches in flight.  EPP_ERR_STATE when no profile has the scorer. */
+EPP_API int32_t epp_nohit_lru_get(epp_engine *h, uint32_t *out_eps, int32_t cap, int32_t *out_n);
 
 EPP_API int32_t epp_get_stats(epp_engine *h, epp_stats *out);
 

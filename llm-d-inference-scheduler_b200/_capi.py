@@ -18,7 +18,7 @@ EPP_BATCH_LENGTHS_EXCEED_ROWS = 4
 EPP_OK, EPP_ERR_INVALID, EPP_ERR_CUDA, EPP_ERR_NO_DEVICE, EPP_ERR_CAPACITY, EPP_ERR_STATE, EPP_ERR_NCCL = \
     0, -1, -2, -3, -4, -5, -6
 (SCORER_PREFIX, SCORER_KV_UTIL, SCORER_QUEUE, SCORER_LOAD_AWARE, SCORER_EXTERNAL, SCORER_RUNNING, SCORER_TOKEN_LOAD,
- SCORER_ACTIVE_REQUEST, SCORER_LORA_AFFINITY) = range(9)
+ SCORER_ACTIVE_REQUEST, SCORER_LORA_AFFINITY, SCORER_NO_HIT_LRU) = range(10)
 (ROLE_NONE, ROLE_DECODE, ROLE_PREFILL, ROLE_PREFILL_DECODE, ROLE_BOTH, ROLE_ENCODE, ROLE_ENCODE_PREFILL,
  ROLE_ENCODE_PREFILL_DECODE, ROLE_OTHER) = range(9)
 FILTER_NONE, FILTER_DECODE, FILTER_PREFILL, FILTER_ENCODE = range(4)
@@ -128,6 +128,7 @@ SIGNATURES = {
     "epp_schedule_with_match_topk": (C.c_int32, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                                  C.c_int32, C.c_void_p, C.c_void_p, C.c_uint32, C.POINTER(TopkOut)]),
     "epp_index_add_picked": (C.c_int32, [C.c_void_p]),
+    "epp_nohit_lru_get": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(C.c_int32)]),
     "epp_get_stats": (C.c_int32, [C.c_void_p, C.POINTER(Stats)]),
     "epp_synchronize": (C.c_int32, [C.c_void_p]),
     "epp_event_record": (C.c_int32, [C.c_void_p, C.c_int32]),

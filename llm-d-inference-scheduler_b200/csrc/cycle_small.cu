@@ -101,8 +101,9 @@ struct ChainFollower {
 
 // kStage: the prompt is staged into shared memory by ONE bulk copy (TMA) per request; else the digest threads load their
 // blocks themselves (prompts too long for the staging buffer).
-template <bool kStage>
-__global__ void __launch_bounds__(kThreads) k_cycle_small(HashParams hp, PickParams pp, SmallOut so, uint32_t stage_off) {
+// kNoHit: a profile has the no-hit-lru scorer (match_sparse.cuh match_request); those engines launch k_cycle_small_nohit.
+template <bool kStage, bool kNoHit>
+__device__ __forceinline__ void cycle_small(const HashParams &hp, const PickParams &pp, const SmallOut &so, uint32_t stage_off) {
     extern __shared__ __align__(128) uint64_t s_m[];   // [max_blocks] merged stripe state of every full block; then, at byte
                                                        // stage_off, (kStage) the prompt's full blocks and its trailing partial block
     __shared__ __align__(8) uint64_t s_bar;
@@ -217,7 +218,7 @@ __global__ void __launch_bounds__(kThreads) k_cycle_small(HashParams hp, PickPar
 
     int32_t unused = 0;
     const ChainFollower fw{&s_progress, s_m};
-    const bool decided = sparse::match_request<true, false, true, 3, ChainFollower>(pp, r, lane, false, nullptr, nullptr, unused, fw);
+    const bool decided = sparse::match_request<true, false, true, 3, ChainFollower, kNoHit>(pp, r, lane, false, nullptr, nullptr, unused, fw);
     if (lane == 0) {
         if (decided) {
             so.dec[r] = pp.out[r];
@@ -226,6 +227,15 @@ __global__ void __launch_bounds__(kThreads) k_cycle_small(HashParams hp, PickPar
         __threadfence_system();
         *reinterpret_cast<volatile uint32_t *>(so.flags + r) = decided ? so.epoch : (so.epoch | 0x80000000u);
     }
+}
+
+template <bool kStage>
+__global__ void __launch_bounds__(kThreads) k_cycle_small(HashParams hp, PickParams pp, SmallOut so, uint32_t stage_off) {
+    cycle_small<kStage, false>(hp, pp, so, stage_off);
+}
+template <bool kStage>
+__global__ void __launch_bounds__(kThreads) k_cycle_small_nohit(HashParams hp, PickParams pp, SmallOut so, uint32_t stage_off) {
+    cycle_small<kStage, true>(hp, pp, so, stage_off);
 }
 }  // namespace
 
@@ -250,13 +260,21 @@ cudaError_t launch_cycle_small(const HashParams &hp, const PickParams &pp, const
     if (!attr_set[dev & 63]) {
         cudaError_t e = cudaFuncSetAttribute(k_cycle_small<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
         if (e == cudaSuccess) e = cudaFuncSetAttribute(k_cycle_small<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(k_cycle_small_nohit<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(k_cycle_small_nohit<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
         if (e != cudaSuccess) return e;
         attr_set[dev & 63] = true;
     }
     const unsigned grid = (unsigned)hp.R;
     const uint32_t off = (uint32_t)m_bytes;
-    if (stage) k_cycle_small<true><<<grid, kThreads, smem, s>>>(hp, pp, so, off);
-    else k_cycle_small<false><<<grid, kThreads, smem, s>>>(hp, pp, so, off);
+    if (pp.nohit.mask) {                           // no-hit-lru builds (match_sparse.cuh match_request)
+        if (stage) k_cycle_small_nohit<true><<<grid, kThreads, smem, s>>>(hp, pp, so, off);
+        else k_cycle_small_nohit<false><<<grid, kThreads, smem, s>>>(hp, pp, so, off);
+    } else if (stage) {
+        k_cycle_small<true><<<grid, kThreads, smem, s>>>(hp, pp, so, off);
+    } else {
+        k_cycle_small<false><<<grid, kThreads, smem, s>>>(hp, pp, so, off);
+    }
     if (launches) *launches += 1;
     return cudaGetLastError();
 }

@@ -100,6 +100,14 @@ struct epp_engine {
     bool lora_set = false, lora_enabled = false;
     int32_t lora_models = 0;
     ProfileState prof[kMaxProfiles];
+    // no-hit-lru scorer (nohit_lru.cu), allocated only when a profile lists it
+    int nohit_mask = 0;             // bit pi: profile pi has the scorer
+    int32_t nohit_lru = 0;          // lruSize
+    uint64_t nohit_seq = 1;         // sequence number of the next call's first Add (0 = not in the LRU)
+    bool nohit_timed = false;       // ev[5] / ev[6] bracket the update of the device batch in flight
+    ProfileState prof_cold[kMaxProfiles];   // cold sets: base / order / groups with the LRU column
+    DevBuf nh_last_seq, nh_pos, nh_misc, nh_sort_key, nh_order, nh_cold, nh_col[kMaxProfiles];
+    DevBuf nh_prof;                 // ProfileDev[kMaxProfiles] of the cold sets (NoHitView::cold)
 
     // index
     std::unique_ptr<IndexStore> store;          // write side: LRU bookkeeping in HBM (index_store.cu)
@@ -226,7 +234,7 @@ static int32_t validate_profile(const epp_profile_cfg &p, int n_ext, const char 
     if (p.n_scorers < 0 || p.n_scorers > EPP_MAX_SCORERS) return fail(EPP_ERR_INVALID, "%s: n_scorers %d out of range", name, p.n_scorers);
     for (int s = 0; s < p.n_scorers; s++) {
         const epp_scorer_cfg &sc = p.scorers[s];
-        if (sc.kind < EPP_SCORER_PREFIX || sc.kind > EPP_SCORER_LORA_AFFINITY) return fail(EPP_ERR_INVALID, "%s: scorer %d has unknown kind %d", name, s, sc.kind);
+        if (sc.kind < EPP_SCORER_PREFIX || sc.kind > EPP_SCORER_NO_HIT_LRU) return fail(EPP_ERR_INVALID, "%s: scorer %d has unknown kind %d", name, s, sc.kind);
         if (!std::isfinite(sc.weight)) return fail(EPP_ERR_INVALID, "%s: scorer %d weight is not finite", name, s);
         if ((sc.kind == EPP_SCORER_TOKEN_LOAD || sc.kind == EPP_SCORER_ACTIVE_REQUEST) && (sc.column < 0 || sc.column >= n_ext))
             return fail(EPP_ERR_INVALID, "%s: scorer %d reads ext column %d, out of range [0,%d)", name, s, sc.column, n_ext);
@@ -254,6 +262,7 @@ static int32_t alloc_profile(epp_engine *e, ProfileState &ps) {
 }
 
 static int32_t rebuild_presence(epp_engine *h);
+static ProfileDev cold_profile_dev(epp_engine *h, int p);
 
 extern "C" int32_t epp_engine_create(const epp_config *cfg, epp_engine **out) {
     if (!cfg || !out) return fail(EPP_ERR_INVALID, "cfg/out is NULL");
@@ -321,6 +330,36 @@ extern "C" int32_t epp_engine_create(const epp_config *cfg, epp_engine **out) {
         const epp_profile_cfg &pc = pi == 0 ? cfg->primary : (pi == 1 ? cfg->prefill : cfg->encode);
         for (int si = 0; si < pc.n_scorers; si++) if (pc.scorers[si].kind == EPP_SCORER_LORA_AFFINITY) e->lora_enabled = true;
     }
+    for (int pi = 0; pi < e->n_alloc_profiles; pi++) {
+        const epp_profile_cfg &pc = pi == 0 ? cfg->primary : (pi == 1 ? cfg->prefill : cfg->encode);
+        for (int si = 0; si < pc.n_scorers; si++) {
+            if (pc.scorers[si].kind != EPP_SCORER_NO_HIT_LRU) continue;
+            if (e->nohit_mask & (1 << pi)) return fail(EPP_ERR_INVALID, "profile %d lists the no-hit-lru scorer twice", pi);
+            const double p = pc.scorers[si].param;
+            if (std::isnan(p) || p > (double)(1 << 30) || (p > 0.0 && p != std::floor(p)))
+                return fail(EPP_ERR_INVALID, "no-hit-lru lruSize %g must be an integer <= 2^30 (<= 0: 1024)", p);
+            const int32_t lru = p <= 0.0 ? 1024 : (int32_t)p;             // no_hit_lru.go:93-95
+            if (e->nohit_mask && lru != e->nohit_lru)
+                return fail(EPP_ERR_INVALID, "the no-hit-lru scorer has lruSize %d in one profile and %d in another: the profiles share one LRU", e->nohit_lru, lru);
+            e->nohit_mask |= 1 << pi;
+            e->nohit_lru = lru;
+        }
+    }
+    if (e->nohit_mask) {
+        CUDA_TRY(e->nh_last_seq.reserve(sizeof(uint64_t) * E, &e->dev_bytes));
+        CUDA_TRY(e->nh_pos.reserve(sizeof(int32_t) * E, &e->dev_bytes));
+        CUDA_TRY(e->nh_misc.reserve(sizeof(int32_t) * 4, &e->dev_bytes));
+        CUDA_TRY(e->nh_sort_key.reserve(sizeof(uint64_t) * (size_t)e->Epad, &e->dev_bytes));
+        CUDA_TRY(e->nh_order.reserve(sizeof(uint32_t) * (size_t)e->Epad, &e->dev_bytes));
+        CUDA_TRY(cudaMemset(e->nh_last_seq.p, 0, sizeof(uint64_t) * E));
+        CUDA_TRY(cudaMemset(e->nh_pos.p, 0xFF, sizeof(int32_t) * E));
+        CUDA_TRY(cudaMemset(e->nh_misc.p, 0, sizeof(int32_t) * 4));
+        for (int pi = 0; pi < e->n_alloc_profiles; pi++)
+            if (e->nohit_mask & (1 << pi)) {
+                EPP_TRY(alloc_profile(e.get(), e->prof_cold[pi]));
+                CUDA_TRY(e->nh_col[pi].reserve(sizeof(double) * E, &e->dev_bytes));
+            }
+    }
     e->general = cfg->pick_k > 1;
     for (int pi = 0; pi < e->n_alloc_profiles; pi++) {
         const epp_profile_cfg &pc = pi == 0 ? cfg->primary : (pi == 1 ? cfg->prefill : cfg->encode);
@@ -344,6 +383,14 @@ extern "C" int32_t epp_engine_create(const epp_config *cfg, epp_engine **out) {
     CUDA_TRY(cudaMemset(e->small_overflow_n.p, 0, sizeof(int32_t) * 4));
     for (int i = 0; i < 2; i++) CUDA_TRY(e->slot[i].overflow_n.reserve(sizeof(int32_t) * 4, &e->dev_bytes));
     EPP_TRY(rebuild_presence(e.get()));              // the empty index: every bit clear
+    if (e->nohit_mask) {
+        ProfileDev cold[kMaxProfiles];
+        memset(cold, 0, sizeof cold);
+        for (int pi = 0; pi < e->n_alloc_profiles; pi++)
+            if (e->nohit_mask & (1 << pi)) cold[pi] = cold_profile_dev(e.get(), pi);
+        CUDA_TRY(e->nh_prof.reserve(sizeof cold, &e->dev_bytes));
+        CUDA_TRY(cudaMemcpy(e->nh_prof.p, cold, sizeof cold, cudaMemcpyHostToDevice));
+    }
 
     // match/pick launch geometry: counters in shared memory when they fit, else zeroed global scratch
     size_t smem_local = match_pick_smem_bytes(cfg->max_endpoints, false);
@@ -471,6 +518,90 @@ static ProfileDev profile_dev(epp_engine *h, int p) {
     return pd;
 }
 
+static NoHitState nohit_state(epp_engine *h) {
+    NoHitState st;
+    st.last_seq = h->nh_last_seq.as<uint64_t>();
+    st.pos = h->nh_pos.as<int32_t>();
+    st.n_members = h->nh_misc.as<int32_t>();
+    st.dirty = h->nh_misc.as<int32_t>() + 1;
+    st.sort_key = h->nh_sort_key.as<uint64_t>();
+    st.order = h->nh_order.as<uint32_t>();
+    st.lru_size = h->nohit_lru;
+    return st;
+}
+
+// The cold set of every profile with the no-hit-lru scorer: its LRU column over the profile's candidates, and the base
+// sums / order / groups with that column (the warm set holds 0.5).  gated: only if an Add happened since the last time.
+static int32_t nohit_derive(epp_engine *h, cudaStream_t s, bool gated, int *launches) {
+    if (!h->nohit_mask) return EPP_OK;
+    const NoHitState st = nohit_state(h);
+    PoolArrays pa = pool_arrays(h);
+    for (int p = 0; p < h->n_alloc_profiles; p++) {
+        if (!(h->nohit_mask & (1 << p))) continue;
+        ProfileDerived d;
+        d.cand = h->prof[p].cand.as<uint8_t>();
+        d.n_cand = h->prof[p].n_cand.as<int32_t>();
+        d.qminmax = h->prof[p].qminmax.as<int64_t>();
+        d.contrib = h->prof_cold[p].contrib.as<double>();
+        d.base = h->prof_cold[p].base.as<double>();
+        d.order = h->prof_cold[p].order.as<uint32_t>();
+        d.grp_size = h->prof_cold[p].grp_size.as<uint32_t>();
+        d.sort_key = h->prof_cold[p].sort_key.as<uint64_t>();
+        double *col = h->nh_col[p].as<double>();
+        CUDA_TRY(launch_nohit_column(st, h->cfg.max_endpoints, d.cand, d.n_cand, col, gated, s, launches));
+        CUDA_TRY(launch_pool_order(pa, p == 0 ? h->cfg.primary : (p == 1 ? h->cfg.prefill : h->cfg.encode), d, h->Epad, col,
+                                   gated ? st.dirty : nullptr, s, launches));
+    }
+    return EPP_OK;
+}
+
+// PreRequest of the no-hit-lru scorer for one scheduling call (no_hit_lru.go:279-321), enqueued on s behind the call's
+// last pick kernel: the cold requests' picks are Added in request order, then the LRU is trimmed and re-ranked and the
+// cold sets re-derived -- all on the device, and all but the first kernel return at once when no request was cold.
+// dec / the cold scratch hold the call's R requests.
+static int32_t nohit_update(epp_engine *h, const epp_decision *dec, int64_t R, cudaStream_t s, int *launches) {
+    if (!h->nohit_mask || R <= 0) return EPP_OK;
+    const NoHitState st = nohit_state(h);
+    CUDA_TRY(launch_nohit_touch(st, dec, h->nh_cold.as<uint8_t>(), R, h->nohit_seq, s, launches));
+    h->nohit_seq += 2 * (uint64_t)R;
+    CUDA_TRY(launch_nohit_rank(st, h->cfg.max_endpoints, h->Epad, true, s, launches));
+    EPP_TRY(nohit_derive(h, s, true, launches));
+    CUDA_TRY(launch_nohit_clear(st, s, launches));
+    return EPP_OK;
+}
+
+// The same on stream 0 of a device batch, bracketed by ev[5] / ev[6] (epp_stats.last_kernel_ms[4]).
+static int32_t nohit_update_timed(epp_engine *h, const epp_decision *dec, int64_t R, int *launches) {
+    if (!h->nohit_mask) return EPP_OK;
+    cudaStream_t s0 = h->slot[0].stream;
+    CUDA_TRY(cudaEventRecord(h->ev[5], s0));
+    EPP_TRY(nohit_update(h, dec, R, s0, launches));
+    CUDA_TRY(cudaEventRecord(h->ev[6], s0));
+    h->nohit_timed = true;
+    return EPP_OK;
+}
+
+// Profile p's cold set: its candidates, with the cold base / order / groups / contributions.
+static ProfileDev cold_profile_dev(epp_engine *h, int p) {
+    ProfileDev c = profile_dev(h, p);
+    c.contrib = h->prof_cold[p].contrib.as<double>();
+    c.base = h->prof_cold[p].base.as<double>();
+    c.order = h->prof_cold[p].order.as<uint32_t>();
+    c.grp_size = h->prof_cold[p].grp_size.as<uint32_t>();
+    return c;
+}
+
+// The no-hit-lru view of a pick launch whose first request is r0.
+static NoHitView nohit_view(epp_engine *h, int64_t r0) {
+    NoHitView v;
+    memset(&v, 0, sizeof v);
+    v.mask = h->nohit_mask;
+    if (!v.mask) return v;
+    v.cold = h->nh_prof.as<ProfileDev>();
+    v.cold_out = h->nh_cold.as<uint8_t>() + r0;
+    return v;
+}
+
 // Request-independent scorer terms of every profile from the current pool (+ LoRA) snapshot, on the device.
 static int32_t derive_pool(epp_engine *h) {
     cudaStream_t s = h->slot[0].stream;
@@ -488,7 +619,7 @@ static int32_t derive_pool(epp_engine *h) {
         d.qminmax = h->prof[p].qminmax.as<int64_t>();
         CUDA_TRY(launch_pool_prepare(pa, p == 0 ? h->cfg.primary : (p == 1 ? h->cfg.prefill : h->cfg.encode), d, h->Epad, h->shard_begin, h->shard_end, s, &launches));
     }
-    return EPP_OK;
+    return nohit_derive(h, s, false, &launches);
 }
 
 extern "C" int32_t epp_pool_set(epp_engine *h, int32_t n, const uint32_t *ids, const uint8_t *role,
@@ -937,6 +1068,7 @@ static int32_t reserve_batch(epp_engine *h, int64_t R) {
     CUDA_TRY(h->lengths.reserve(sizeof(uint64_t) * n, &h->dev_bytes));
     CUDA_TRY(h->model_ids.reserve(sizeof(uint32_t) * n, &h->dev_bytes));
     for (int i = 0; i < 2; i++) CUDA_TRY(h->slot[i].overflow_list.reserve(sizeof(int32_t) * n, &h->dev_bytes));
+    if (h->nohit_mask) CUDA_TRY(h->nh_cold.reserve(n, &h->dev_bytes));
     return EPP_OK;
 }
 
@@ -1031,6 +1163,7 @@ static PickParams pick_params(epp_engine *h, const Work &w, epp_decision *out, e
     p.overflow_n = nullptr;
     p.req_next = nullptr;
     p.gen = gen_view(h);
+    p.nohit = nohit_view(h, w.r0);
     return p;
 }
 
@@ -1113,6 +1246,12 @@ static int32_t finish_async(epp_engine *h) {
     h->stats.last_postings = h->wc_host[1];
     h->stats.last_hash_bytes_stored = h->wc_host[2];
     h->stats.last_kernel_launches = (uint64_t)h->async_launches;
+    if (h->nohit_timed) {
+        float tn = 0;
+        cudaEventElapsedTime(&tn, h->ev[5], h->ev[6]);
+        h->stats.last_kernel_ms[4] = tn;
+        h->nohit_timed = false;
+    }
     return EPP_OK;
 }
 
@@ -1286,6 +1425,7 @@ static int32_t run_small(epp_engine *h, const BatchView &v, int mode, const uint
         CUDA_TRY(cudaMemcpyAsync(h->small_det, h->details.p, sizeof(epp_decision_detail) * (size_t)R, cudaMemcpyDeviceToHost, s0));
         CUDA_TRY(cudaStreamSynchronize(s0));
     }
+    EPP_TRY(nohit_update(h, h->small_dec, R, s0, &launches));   // reads the decisions from the pinned copy (UVA)
     memcpy(out_dec, h->small_dec, sizeof(epp_decision) * (size_t)R);
     if (out_detail) memcpy(out_detail, h->small_det, sizeof(epp_decision_detail) * (size_t)R);
     h->small_stats_pending = true;
@@ -1385,6 +1525,9 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
                 EPP_TRY(launch_cycle(h, sl, hp, pp, &launches, nullptr));
             }
             h->s1_unjoined = true;
+            // the next call's picks must see both chunks' Adds: join the chunks on stream 0 for the update (below), and the
+            // next call's stream-1 chunk waits for stream 0 again (engines without the scorer stay unjoined)
+            if (h->nohit_mask) EPP_TRY(join_streams(h));
             h->pipe_R = R;
             h->pipe_per = per;
         } else if (mode == Mode::HashOnly) {
@@ -1400,6 +1543,8 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
             EPP_TRY(launch_cycle(h, h->slot[0], hp, pp, &launches, h->ev));
         }
         CUDA_TRY(cudaEventRecord(h->ev[4], s0));
+        if (mode == Mode::Schedule)                // after ev[4]: last_kernel_ms[3] stays the match + pick time
+            EPP_TRY(nohit_update_timed(h, out_dec ? out_dec : h->decisions.as<epp_decision>(), R, &launches));
         CUDA_TRY(cudaMemcpyAsync(h->wc_host, h->work_counters.p, sizeof(unsigned long long) * 3, cudaMemcpyDeviceToHost, s0));
         h->async_pending = true;
         h->async_launches = launches;
@@ -1510,6 +1655,7 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
         }
     }
     CUDA_TRY(cudaStreamSynchronize(h->slot[1].stream));
+    if (mode == Mode::Schedule) EPP_TRY(nohit_update(h, h->decisions.as<epp_decision>(), R, s0, &launches));
     CUDA_TRY(cudaEventRecord(h->ev[1], s0));
     CUDA_TRY(cudaStreamSynchronize(s0));
     float t_all = 0;
@@ -1647,7 +1793,17 @@ extern "C" int32_t epp_score(epp_engine *h, int64_t n_requests, const int32_t *m
         d_models = h->score_models.as<uint32_t>();
     }
     int launches = 0;
-    CUDA_TRY(launch_score_dense(n_requests, h->cfg.max_endpoints, profile_dev(h, profile), pool_arrays(h),
+    // no-hit-lru: each request's cold bit for this profile selects its cold set (no_hit_lru.go:259-275)
+    const bool nh = (h->nohit_mask >> profile) & 1;
+    const ProfileDev pw = profile_dev(h, profile);
+    uint8_t *cold = nullptr;
+    if (nh) {
+        CUDA_TRY(h->nh_cold.reserve((size_t)n_requests, &h->dev_bytes));
+        cold = h->nh_cold.as<uint8_t>();
+        CUDA_TRY(launch_nohit_cold_rows(n_requests, h->cfg.max_endpoints, pw.cand, d_match, cold, s, &launches));
+    }
+    CUDA_TRY(launch_score_dense(n_requests, h->cfg.max_endpoints, pw, nh ? cold_profile_dev(h, profile) : pw, cold,
+                                nh ? h->nh_col[profile].as<double>() : nullptr, pool_arrays(h),
                                 h->prof[profile].qminmax.as<int64_t>(), d_match, d_total, d_models, scorer_index, d_out, s, &launches));
     if (!dev) CUDA_TRY(cudaMemcpyAsync(out_scores, d_out, sizeof(double) * n, cudaMemcpyDeviceToHost, s));
     CUDA_TRY(cudaStreamSynchronize(s));
@@ -1682,6 +1838,9 @@ static int32_t with_match_impl(epp_engine *h, int64_t n_requests, const int32_t 
     p.tie_seed = h->cfg.tie_seed;
     p.tie_base = h->stats.n_decisions;
     p.gen = gen_view(h);
+    p.nohit = nohit_view(h, 0);
+    if (h->nohit_mask) CUDA_TRY(h->nh_cold.reserve(R, &h->dev_bytes));
+    p.nohit.cold_out = h->nohit_mask ? h->nh_cold.as<uint8_t>() : nullptr;
     const size_t K = (size_t)h->cfg.pick_k;
     uint32_t *tk_host[kMaxProfiles] = {nullptr, nullptr, nullptr};
     uint32_t *tk_picks[kMaxProfiles] = {nullptr, nullptr, nullptr};
@@ -1725,6 +1884,7 @@ static int32_t with_match_impl(epp_engine *h, int64_t n_requests, const int32_t 
     }
     int launches = 0;
     CUDA_TRY(launch_dense_pick(p, s, &launches));
+    EPP_TRY(nohit_update(h, p.out, n_requests, s, &launches));
     if (!dev) {
         CUDA_TRY(cudaMemcpyAsync(out, p.out, sizeof(epp_decision) * R, cudaMemcpyDeviceToHost, s));
         if (detail) CUDA_TRY(cudaMemcpyAsync(detail, p.detail, sizeof(epp_decision_detail) * R, cudaMemcpyDeviceToHost, s));
@@ -1750,6 +1910,23 @@ extern "C" int32_t epp_schedule_with_match_topk(epp_engine *h, int64_t n_request
                                                 const epp_topk_out *topk) {
     if (!topk) return fail(EPP_ERR_INVALID, "topk is NULL");
     return with_match_impl(h, n_requests, match, total, model_ids, input_len_bytes, block_size_tokens, out, detail, flags, topk);
+}
+
+extern "C" int32_t epp_nohit_lru_get(epp_engine *h, uint32_t *out_eps, int32_t cap, int32_t *out_n) {
+    if (!h || !out_n || cap < 0 || (cap > 0 && !out_eps)) return fail(EPP_ERR_INVALID, "bad arguments");
+    std::lock_guard<std::mutex> lk(h->mu);
+    EPP_TRY(set_device(h));
+    if (!h->nohit_mask) return fail(EPP_ERR_STATE, "no profile has the no-hit-lru scorer");
+    EPP_TRY(finish_async(h));
+    const size_t E = (size_t)h->cfg.max_endpoints;
+    std::vector<uint64_t> seq(E);
+    CUDA_TRY(cudaMemcpy(seq.data(), h->nh_last_seq.p, sizeof(uint64_t) * E, cudaMemcpyDeviceToHost));
+    std::vector<std::pair<uint64_t, uint32_t>> m;
+    for (size_t e = 0; e < E; e++) if (seq[e]) m.push_back({seq[e], (uint32_t)e});
+    std::sort(m.begin(), m.end());
+    *out_n = (int32_t)m.size();
+    for (int32_t i = 0; i < std::min<int32_t>(cap, (int32_t)m.size()); i++) out_eps[i] = m[(size_t)i].second;
+    return EPP_OK;
 }
 
 extern "C" int32_t epp_get_config(epp_engine *h, epp_config *out) {
@@ -1816,6 +1993,7 @@ extern "C" int32_t epp_shard_set(epp_engine *h, uint32_t ep_begin, uint32_t ep_e
     std::lock_guard<std::mutex> lk(h->mu);
     if (h->cfg.handler != EPP_HANDLER_SINGLE) return fail(EPP_ERR_INVALID, "endpoint-sharded mode supports the single-profile handler only");
     if (h->general) return fail(EPP_ERR_INVALID, "endpoint-sharded mode supports neither pick_k > 1 nor the prefix-cache-affinity-filter (both need every candidate's score on one rank)");
+    if (h->nohit_mask) return fail(EPP_ERR_INVALID, "endpoint-sharded mode does not support the no-hit-lru scorer (coldness needs every rank's match)");
     h->shard_begin = ep_begin;
     h->shard_end = ep_end;
     h->pool_ready = false;          // candidates are derived per shard: epp_pool_set must follow
@@ -1919,6 +2097,7 @@ extern "C" int32_t epp_shard_p2p_export(epp_engine *h, int64_t max_requests, uin
 extern "C" int32_t epp_shard_p2p_connect(epp_engine *h, int32_t n_ranks, int32_t rank, const void *peers, int32_t ipc_handles) {
     if (!h || n_ranks <= 0 || n_ranks > 64 || rank < 0 || rank >= n_ranks || !peers) return fail(EPP_ERR_INVALID, "bad arguments");
     std::lock_guard<std::mutex> lk(h->mu);
+    if (h->nohit_mask) return fail(EPP_ERR_INVALID, "endpoint-sharded mode does not support the no-hit-lru scorer (coldness needs every rank's match)");
     EPP_TRY(set_device(h));
     EPP_TRY(join_streams(h));
     if (!h->p2p_buf) return fail(EPP_ERR_STATE, "epp_shard_p2p_export has not been called");

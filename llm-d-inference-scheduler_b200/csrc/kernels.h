@@ -126,8 +126,42 @@ struct ProfileDerived {
     int64_t *qminmax;          // [4] waiting min,max, running min,max over candidates
 };
 // [shard_begin, shard_end): only these slots become candidates (queue min/max still span the whole pool).
+// A no-hit-lru scorer gets its warm score 0.5 here (the cold set comes from launch_pool_order).
 cudaError_t launch_pool_prepare(const PoolArrays &pool, const epp_profile_cfg &prof, const ProfileDerived &d,
                                 int32_t Epad, uint32_t shard_begin, uint32_t shard_end, cudaStream_t s, int *launches);
+// The contribution rows, base sums, (base desc, slot asc) order and groups of d over d.cand / d.n_cand / d.qminmax (already
+// derived), with the raw no-hit-lru score of slot e = nohit_col[e] (nullptr: the warm 0.5).  gate != nullptr: every kernel
+// returns at once unless *gate != 0.
+// (key asc, order asc) sort of Epad (a power of two) entries by one CTA; gate as below.
+cudaError_t launch_pool_sort(uint64_t *key, uint32_t *order, int32_t Epad, const int32_t *gate, cudaStream_t s);
+cudaError_t launch_pool_order(const PoolArrays &pool, const epp_profile_cfg &prof, const ProfileDerived &d, int32_t Epad,
+                              const double *nohit_col, const int32_t *gate, cudaStream_t s, int *launches);
+
+// ------------------------------------------------------------------------------------------------
+// no-hit-lru scorer state (nohit_lru.cu): the LRU of endpoints that received a cold request
+// ------------------------------------------------------------------------------------------------
+struct NoHitState {
+    uint64_t *last_seq;        // [E] sequence number of the endpoint's last Add, 0 = not in the LRU
+    int32_t *pos;              // [E] position in the LRU (oldest = 0), -1 = not in it
+    int32_t *n_members;        // [1] LRU length
+    int32_t *dirty;            // [1] some Add happened since the cold sets were derived
+    uint64_t *sort_key;        // [Epad] scratch
+    uint32_t *order;           // [Epad] scratch
+    int32_t lru_size;
+};
+// Applies the Adds of one scheduling call's decisions (request r: its pick, then its prefill pick, when cold[r] != 0) as
+// last_seq[e] = max(last_seq[e], seq0 + 2r (+1)), then trims the LRU to lru_size members and re-ranks it.
+// dec / cold are indexed by r in [0, R).
+cudaError_t launch_nohit_touch(const NoHitState &st, const epp_decision *dec, const uint8_t *cold, int64_t R, uint64_t seq0,
+                               cudaStream_t s, int *launches);
+cudaError_t launch_nohit_rank(const NoHitState &st, int32_t E, int32_t Epad, bool gated, cudaStream_t s, int *launches);
+// The raw cold no-hit-lru column of one profile (no_hit_lru.go:198-242) over its candidates -> col[E].
+cudaError_t launch_nohit_column(const NoHitState &st, int32_t E, const uint8_t *cand, const int32_t *n_cand, double *col,
+                                bool gated, cudaStream_t s, int *launches);
+cudaError_t launch_nohit_clear(const NoHitState &st, cudaStream_t s, int *launches);
+// Cold bit of each request of a dense match matrix for one profile (epp_score): no candidate has match > 0.
+cudaError_t launch_nohit_cold_rows(int64_t R, int32_t E, const uint8_t *cand, const int32_t *match, uint8_t *cold,
+                                   cudaStream_t s, int *launches);
 
 // ------------------------------------------------------------------------------------------------
 // match + score + pick (a3-a14)
@@ -140,6 +174,14 @@ struct ProfileDev {            // what the pick kernels read (device pointers + 
     const uint32_t *order;
     const uint32_t *grp_size;
     const int32_t *n_cand;
+};
+// no-hit-lru scorer (nohitlru/no_hit_lru.go): a profile whose bit is set in `mask` evaluates a cold request (no candidate
+// holds a block of its prompt) with cold[pi] -- the same candidates, with the LRU column in place of the warm 0.5 -- and
+// every decision writes the cold bit of the last such profile that ran (decode -> encode -> prefill) to cold_out[r].
+struct NoHitView {
+    int32_t mask;              // 0: no profile has the scorer
+    const ProfileDev *cold;    // [kMaxProfiles] in device memory (keeps the launch parameters of the default builds small)
+    uint8_t *cold_out;         // [R] (this launch's rows), or nullptr
 };
 // General evaluation (pick_general.cuh): set when a profile configures the prefix-cache-affinity-filter or pick_k > 1.
 struct GenView {
@@ -189,6 +231,7 @@ struct PickParams {
     uint64_t tie_seed;
     uint64_t tie_base;         // ordinal of request 0 of this launch
     GenView gen;
+    NoHitView nohit;
 };
 // Fused lookup + match + score + pick, one warp per request.  Per-warp match counters live in shared memory
 // (smem = match_pick_smem_bytes(E, false)) or, when E is too large for that, in a zero-initialised global
@@ -239,10 +282,14 @@ struct DensePickParams {
     uint64_t tie_seed;
     uint64_t tie_base;
     GenView gen;
+    NoHitView nohit;
 };
 cudaError_t launch_dense_pick(const DensePickParams &p, cudaStream_t s, int *launches);
 // Scorer.Score parity: out[R][E].  scorer_index -1 => weighted ordered sum (-1.0 for non-candidates).
-cudaError_t launch_score_dense(int64_t R, int32_t E, const ProfileDev &prof, const PoolArrays &pool,
+// cold != nullptr (the profile has a no-hit-lru scorer): cold[r] selects prof_cold and the raw cold column nohit_col
+// for request r.
+cudaError_t launch_score_dense(int64_t R, int32_t E, const ProfileDev &prof, const ProfileDev &prof_cold,
+                               const uint8_t *cold, const double *nohit_col, const PoolArrays &pool,
                                const int64_t *qminmax, const int32_t *match, const int32_t *total,
                                const uint32_t *model_ids, int32_t scorer_index, double *out, cudaStream_t s,
                                int *launches);

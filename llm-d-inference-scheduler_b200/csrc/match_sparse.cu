@@ -14,8 +14,9 @@ constexpr int kWarps = 8;
 // launch's counter (p.req_next), so the warps that draw cheap (cold) prompts take more of them while the warps on long
 // cached prefixes are busy, instead of the launch ending on the warps whose fixed share happened to be costliest.  The
 // ticket is taken once the current request's probes are done, so the atomic's latency hides behind its scoring.
-template <int MINCTA, bool kSharded, bool kTie, int kStages>
-__global__ void __launch_bounds__(kWarps * 32, MINCTA) k_match_pick_sparse(PickParams p) {
+// kNoHit: the no-hit-lru builds (match_sparse.cuh match_request), launched as k_match_pick_sparse_nohit.
+template <bool kSharded, bool kTie, int kStages, bool kNoHit>
+__device__ __forceinline__ void match_pick_sparse(const PickParams &p) {
     __shared__ sparse::Work s_work[kWarps];           // when counting
     const int lane = threadIdx.x & 31;
     const int warp = threadIdx.x >> 5;
@@ -30,7 +31,7 @@ __global__ void __launch_bounds__(kWarps * 32, MINCTA) k_match_pick_sparse(PickP
     uint32_t r = blockIdx.x * kWarps + warp;
     while (r < R) {
         int32_t ticket = 0;
-        sparse::match_request<false, kSharded, kTie, kStages>(p, r, lane, counting, wk, p.req_next, ticket);
+        sparse::match_request<false, kSharded, kTie, kStages, sparse::NoFollow, kNoHit>(p, r, lane, counting, wk, p.req_next, ticket);
         r = nwarps + (uint32_t)__shfl_sync(0xffffffffu, ticket, 0);
     }
     if (counting) {
@@ -43,22 +44,39 @@ __global__ void __launch_bounds__(kWarps * 32, MINCTA) k_match_pick_sparse(PickP
     }
 }
 
-namespace {
 template <int MINCTA, bool kSharded, bool kTie, int kStages>
-cudaError_t launch_one(const PickParams &p, int sm_count, cudaStream_t s) {
+__global__ void __launch_bounds__(kWarps * 32, MINCTA) k_match_pick_sparse(PickParams p) {
+    match_pick_sparse<kSharded, kTie, kStages, false>(p);
+}
+template <int MINCTA, bool kTie, int kStages>
+__global__ void __launch_bounds__(kWarps * 32, MINCTA) k_match_pick_sparse_nohit(PickParams p) {
+    match_pick_sparse<false, kTie, kStages, true>(p);
+}
+
+namespace {
+template <void (*kernel)(PickParams)>
+cudaError_t launch_kernel(const PickParams &p, int sm_count, cudaStream_t s) {
     int dev = 0;
     cudaGetDevice(&dev);
-    static int occ_dev[64] = {};                       // per device: engines of one process may sit on different GPUs
+    static int occ_dev[64] = {};                       // per kernel and device: engines of one process may sit on different GPUs
     int &occ = occ_dev[dev & 63];
     if (!occ) {
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_match_pick_sparse<MINCTA, kSharded, kTie, kStages>, kWarps * 32, 0);
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, kWarps * 32, 0);
         if (occ < 1) occ = 1;
     }
     if (sm_count <= 0) sm_count = 132;
     const int64_t need = (p.R + kWarps - 1) / kWarps;
     const int grid = (int)(need < (int64_t)sm_count * occ ? need : (int64_t)sm_count * occ);
-    k_match_pick_sparse<MINCTA, kSharded, kTie, kStages><<<grid, kWarps * 32, 0, s>>>(p);
+    kernel<<<grid, kWarps * 32, 0, s>>>(p);
     return cudaGetLastError();
+}
+template <int MINCTA, bool kSharded, bool kTie, int kStages>
+cudaError_t launch_one(const PickParams &p, int sm_count, cudaStream_t s) {
+    return launch_kernel<k_match_pick_sparse<MINCTA, kSharded, kTie, kStages>>(p, sm_count, s);
+}
+template <bool kTie, int kStages>
+cudaError_t launch_nohit(const PickParams &p, int sm_count, cudaStream_t s) {
+    return launch_kernel<k_match_pick_sparse_nohit<6, kTie, kStages>>(p, sm_count, s);
 }
 }  // namespace
 
@@ -71,6 +89,11 @@ cudaError_t launch_match_pick_sparse(const PickParams &p, int sm_count, int ctas
     // the hot configuration (one profile, lowest-slot ties) gets the 32-register build; the variants that carry more
     // code (stages, tie rule, sharding) keep 40 registers
     if (p.global_masks) e = launch_one<6, true, false, 1>(p, sm_count, s);
+    else if (p.nohit.mask) {
+        if (stages == 1) e = tie ? launch_nohit<true, 1>(p, sm_count, s) : launch_nohit<false, 1>(p, sm_count, s);
+        else if (stages == 2) e = tie ? launch_nohit<true, 2>(p, sm_count, s) : launch_nohit<false, 2>(p, sm_count, s);
+        else e = tie ? launch_nohit<true, 3>(p, sm_count, s) : launch_nohit<false, 3>(p, sm_count, s);
+    }
     else if (stages == 1 && !tie) e = ctas == 6 ? launch_one<6, false, false, 1>(p, sm_count, s) : launch_one<8, false, false, 1>(p, sm_count, s);
     else if (stages == 1) e = launch_one<6, false, true, 1>(p, sm_count, s);
     else if (stages == 2) e = tie ? launch_one<6, false, true, 2>(p, sm_count, s) : launch_one<6, false, false, 2>(p, sm_count, s);

@@ -230,7 +230,9 @@ struct NoFollow {
 // Returns false when the request was handed to the dense-counter kernel (p.overflow_list) instead of being decided.
 // req_next != nullptr: once the probes are done, lane 0 takes a ticket off *req_next into `ticket` (k_match_pick_sparse:
 // the warp's next request, fetched while this one is scored).
-template <bool kCg, bool kSharded, bool kTie, int kStages, typename Follow = NoFollow>
+// kNoHit: a profile has a no-hit-lru scorer (PickParams::nohit): the lane map decides, with one ballot, whether the request
+// is cold for the profile, which selects the profile's warm or cold set (same candidates, different base / order / groups).
+template <bool kCg, bool kSharded, bool kTie, int kStages, typename Follow = NoFollow, bool kNoHit = false>
 __device__ __forceinline__ bool match_request(const PickParams &p, const uint32_t r, const int lane, const bool counting,
                                               Work *wk, int32_t *req_next, int32_t &ticket, const Follow fw = Follow()) {
     const uint32_t shard_lo = p.index.ep_begin, shard_hi = min(p.index.ep_end, (uint32_t)p.E);
@@ -332,9 +334,18 @@ __device__ __forceinline__ bool match_request(const PickParams &p, const uint32_
     // ---- a5-a14: the profiles of the handler
     epp_decision d;
     epp_decision_detail dd;
+    bool cold = false;
     decide_stages<kStages>(p, r, total, (kStages >= 2 && p.n_profiles >= 2) ? ld_row<kCg>(p.in_len + r) : 0,
-                  [&](int pi, uint64_t key) { return eval_profile_lanes<kTie>(p.prof[pi], p.E, m, total, lane, p.lora, lora_st, p.tie_seed, key); },
+                  [&](int pi, uint64_t key) {
+                      if (!kNoHit) return eval_profile_lanes<kTie>(p.prof[pi], p.E, m, total, lane, p.lora, lora_st, p.tie_seed, key);
+                      // a hit = a matched candidate with count > 0 (lora-affinity entries join the map with count 0)
+                      const ProfileDev &pf = nohit_select(p, pi, cold, [&](const ProfileDev &w) {
+                          return !__ballot_sync(kFull, (uint32_t)lane < m.n && m.c > 0 && w.cand[m.e]);
+                      });
+                      return eval_profile_lanes<kTie>(pf, p.E, m, total, lane, p.lora, lora_st, p.tie_seed, key);
+                  },
                   [&](uint32_t e) { return m.n ? (int32_t)map_get(m, e) : 0; }, d, dd);
+    if (kNoHit && lane == 0 && p.nohit.cold_out) p.nohit.cold_out[r] = cold ? 1 : 0;
     if (lane == 0) {
         if (p.shard_out) {
             epp_shard_best sb;

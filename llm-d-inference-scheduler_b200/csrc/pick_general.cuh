@@ -92,7 +92,8 @@ __device__ inline void affinity_filter(const ProfileDev &pf, const GenView &g, i
 }
 
 // runScorerPlugins over the narrowed set: the same ordered, clamped, unfused sum as weighted_sum(), with every scorer
-// evaluated from the pool arrays and the set's own normalisation constants.
+// evaluated from the pool arrays and the set's own normalisation constants.  A narrowed set holds sticky endpoints only
+// (matchBlocks > 0), so the request is warm for it and a no-hit-lru scorer adds its 0.5 (pool_score).
 __device__ inline double weighted_sum_over(const ProfileDev &pf, const GenView &g, const Norm &nm, uint32_t e,
                                            int32_t match, int32_t total, const LoraDev &L, int lora_st) {
     double acc = 0.0;

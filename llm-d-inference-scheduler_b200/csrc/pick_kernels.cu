@@ -95,8 +95,11 @@ __device__ __forceinline__ uint64_t desc_key(double x) {
     return ~asc;
 }
 
+// nohit_col: raw cold no-hit-lru score per slot, nullptr = the warm 0.5 (no_hit_lru.go:159-165).
 __global__ void k_pool_terms(PoolArrays pool, epp_profile_cfg cfg, const uint8_t *cand, const int64_t *qminmax,
-                             double *contrib, double *base, uint64_t *sort_key, uint32_t *order, int32_t Epad) {
+                             double *contrib, double *base, uint64_t *sort_key, uint32_t *order, int32_t Epad,
+                             const double *nohit_col, const int32_t *gate) {
+    if (gate && !*gate) return;
     int32_t e = blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= Epad) return;
     if (e >= pool.E || !cand[e]) {
@@ -110,7 +113,10 @@ __global__ void k_pool_terms(PoolArrays pool, epp_profile_cfg cfg, const uint8_t
     }
     double acc = 0.0;
     for (int s = 0; s < cfg.n_scorers; s++) {
-        double raw = cfg.scorers[s].kind == EPP_SCORER_PREFIX ? 0.0 : pool_score(cfg.scorers[s], s, pool, qminmax, e);
+        double raw;
+        if (cfg.scorers[s].kind == EPP_SCORER_PREFIX) raw = 0.0;
+        else if (cfg.scorers[s].kind == EPP_SCORER_NO_HIT_LRU) raw = nohit_col ? nohit_col[e] : 0.5;
+        else raw = pool_score(cfg.scorers[s], s, pool, qminmax, e);
         double term = __dmul_rn(clamp01(raw), cfg.scorers[s].weight);
         contrib[(size_t)s * (size_t)pool.E + e] = term;
         acc = __dadd_rn(acc, term);
@@ -121,7 +127,8 @@ __global__ void k_pool_terms(PoolArrays pool, epp_profile_cfg cfg, const uint8_t
 }
 
 // Single-CTA bitonic sort of (sort_key asc, slot asc) over Epad (power of two) entries in global memory.
-__global__ void __launch_bounds__(1024) k_pool_sort(uint64_t *key, uint32_t *order, int32_t Epad) {
+__global__ void __launch_bounds__(1024) k_pool_sort(uint64_t *key, uint32_t *order, int32_t Epad, const int32_t *gate) {
+    if (gate && !*gate) return;
     for (int32_t k = 2; k <= Epad; k <<= 1) {
         for (int32_t j = k >> 1; j > 0; j >>= 1) {
             for (int32_t i = threadIdx.x; i < Epad; i += blockDim.x) {
@@ -142,7 +149,9 @@ __global__ void __launch_bounds__(1024) k_pool_sort(uint64_t *key, uint32_t *ord
     }
 }
 
-__global__ void k_pool_groups(const double *base, const uint32_t *order, const int32_t *n_cand, uint32_t *grp_size) {
+__global__ void k_pool_groups(const double *base, const uint32_t *order, const int32_t *n_cand, uint32_t *grp_size,
+                              const int32_t *gate) {
+    if (gate && !*gate) return;
     int32_t k = blockIdx.x * blockDim.x + threadIdx.x;
     int32_t n = *n_cand;
     if (k >= n) return;
@@ -151,6 +160,21 @@ __global__ void k_pool_groups(const double *base, const uint32_t *order, const i
     int32_t end = k + 1;
     while (end < n && base[order[end]] == b) end++;
     for (int32_t i = k; i < end; i++) grp_size[i] = (uint32_t)(end - k);
+}
+
+cudaError_t launch_pool_sort(uint64_t *key, uint32_t *order, int32_t Epad, const int32_t *gate, cudaStream_t s) {
+    k_pool_sort<<<1, 1024, 0, s>>>(key, order, Epad, gate);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_pool_order(const PoolArrays &pool, const epp_profile_cfg &prof, const ProfileDerived &d, int32_t Epad,
+                              const double *nohit_col, const int32_t *gate, cudaStream_t s, int *launches) {
+    k_pool_terms<<<(Epad + 255) / 256, 256, 0, s>>>(pool, prof, d.cand, d.qminmax, d.contrib, d.base, d.sort_key,
+                                                    d.order, Epad, nohit_col, gate);
+    k_pool_sort<<<1, 1024, 0, s>>>(d.sort_key, d.order, Epad, gate);
+    k_pool_groups<<<(pool.E + 255) / 256, 256, 0, s>>>(d.base, d.order, d.n_cand, d.grp_size, gate);
+    if (launches) *launches += 3;
+    return cudaGetLastError();
 }
 
 cudaError_t launch_pool_prepare(const PoolArrays &pool, const epp_profile_cfg &prof, const ProfileDerived &d,
@@ -162,12 +186,8 @@ cudaError_t launch_pool_prepare(const PoolArrays &pool, const epp_profile_cfg &p
             if (launches) *launches += 1;
             break;
         }
-    k_pool_terms<<<(Epad + 255) / 256, 256, 0, s>>>(pool, prof, d.cand, d.qminmax, d.contrib, d.base, d.sort_key,
-                                                    d.order, Epad);
-    k_pool_sort<<<1, 1024, 0, s>>>(d.sort_key, d.order, Epad);
-    k_pool_groups<<<(pool.E + 255) / 256, 256, 0, s>>>(d.base, d.order, d.n_cand, d.grp_size);
-    if (launches) *launches += 4;
-    return cudaGetLastError();
+    if (launches) *launches += 1;
+    return launch_pool_order(pool, prof, d, Epad, nullptr, nullptr, s, launches);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -256,15 +276,15 @@ __device__ inline Best eval_profile_inner(const ProfileDev &pf, int32_t E, const
 // gen::eval for profile pi of request r, with the request's top-k rows (all rows are reset first: a stage that does
 // not run leaves EPP_NO_ENDPOINT).
 template <typename P, typename CntOf>
-__device__ inline Best gen_eval_profile(const P &p, int pi, int64_t r, int32_t total, int lane, uint32_t adapter,
-                                        uint64_t key, CntOf cnt_of) {
+__device__ inline Best gen_eval_profile(const P &p, const ProfileDev &pf, int pi, int64_t r, int32_t total, int lane,
+                                        uint32_t adapter, uint64_t key, CntOf cnt_of) {
     const int32_t k = p.gen.topk > 1 ? p.gen.topk : 1;
     if (pi == 0 && k > 1) {
         for (int q = 0; q < kMaxProfiles; q++)
             if (p.gen.topk_picks[q]) for (int j = lane; j < k; j += 32) p.gen.topk_picks[q][r * k + j] = EPP_NO_ENDPOINT;
         __syncwarp();
     }
-    return gen::eval(p.prof[pi], p.gen, p.E, total, lane, p.lora, adapter, p.tie_seed, key, cnt_of, k,
+    return gen::eval(pf, p.gen, p.E, total, lane, p.lora, adapter, p.tie_seed, key, cnt_of, k,
                      (k > 1 && p.gen.topk_picks[pi]) ? p.gen.topk_picks[pi] + r * k : nullptr,
                      (k > 1 && pi == 0 && p.gen.topk_scores) ? p.gen.topk_scores + r * k : nullptr);
 }
@@ -346,15 +366,18 @@ __global__ void __launch_bounds__(kPickWarps * 32) k_match_pick(PickParams p, in
         epp_decision d;
         epp_decision_detail dd;
         auto cnt_of = [&](uint32_t e) { return (int32_t)cnt_get(cnt32, e); };
+        bool cold = false;
+        auto is_cold = [&](const ProfileDev &pf) { return cold_scan(pf, p.E, lane, cnt_of); };
         if (p.gen.on) {       // affinity filter / top-k: full-scan evaluation (pick_general.cuh)
             decide_stages<3>(p, r, total, p.n_profiles >= 2 ? p.in_len[r] : 0,
-                          [&](int pi, uint64_t key) { return gen_eval_profile(p, pi, r, total, lane, adapter, key, cnt_of); },
+                          [&](int pi, uint64_t key) { return gen_eval_profile(p, nohit_select(p, pi, cold, is_cold), pi, r, total, lane, adapter, key, cnt_of); },
                           cnt_of, d, dd);
         } else {
             decide_stages<3>(p, r, total, p.n_profiles >= 2 ? p.in_len[r] : 0,
-                          [&](int pi, uint64_t key) { return eval_profile(p.prof[pi], p.E, cnt32, list, nl, total, lane, p.lora, adapter, p.tie_seed, key); },
+                          [&](int pi, uint64_t key) { return eval_profile(nohit_select(p, pi, cold, is_cold), p.E, cnt32, list, nl, total, lane, p.lora, adapter, p.tie_seed, key); },
                           cnt_of, d, dd);
         }
+        if (lane == 0 && p.nohit.cold_out) p.nohit.cold_out[r] = cold ? 1 : 0;
         if (lane == 0) {
             if (p.shard_out) {
                 epp_shard_best sb;
@@ -450,15 +473,18 @@ __global__ void __launch_bounds__(256) k_dense_pick(DensePickParams p) {
     epp_decision d;
     epp_decision_detail dd;
     auto cnt_of = [&](uint32_t e) { return mrow[e]; };
+    bool cold = false;
+    auto is_cold = [&](const ProfileDev &pf) { return cold_scan(pf, p.E, lane, cnt_of); };
     if (p.gen.on) {
         decide_stages<3>(p, r, total, p.in_len ? p.in_len[r] : 0,
-                      [&](int pi, uint64_t key) { return gen_eval_profile(p, pi, r, total, lane, adapter, key, cnt_of); },
+                      [&](int pi, uint64_t key) { return gen_eval_profile(p, nohit_select(p, pi, cold, is_cold), pi, r, total, lane, adapter, key, cnt_of); },
                       cnt_of, d, dd);
     } else {
         decide_stages<3>(p, r, total, p.in_len ? p.in_len[r] : 0,
-                      [&](int pi, uint64_t key) { return eval_profile_dense(p.prof[pi], p.E, mrow, total, lane, p.lora, adapter, p.tie_seed, key); },
+                      [&](int pi, uint64_t key) { return eval_profile_dense(nohit_select(p, pi, cold, is_cold), p.E, mrow, total, lane, p.lora, adapter, p.tie_seed, key); },
                       cnt_of, d, dd);
     }
+    if (lane == 0 && p.nohit.cold_out) p.nohit.cold_out[r] = cold ? 1 : 0;
     if (lane == 0) {
         p.out[r] = d;
         if (p.detail) p.detail[r] = dd;
@@ -474,13 +500,15 @@ cudaError_t launch_dense_pick(const DensePickParams &p, cudaStream_t s, int *lau
 }
 
 // Scorer.Score parity (dense [R][E] output).
-__global__ void k_score_dense(int64_t R, int32_t E, ProfileDev pf, PoolArrays pool, const int64_t *qminmax,
-                              const int32_t *match, const int32_t *total, const uint32_t *model_ids,
+__global__ void k_score_dense(int64_t R, int32_t E, ProfileDev pw, ProfileDev pcold, const uint8_t *cold,
+                              const double *nohit_col, PoolArrays pool,
+                              const int64_t *qminmax, const int32_t *match, const int32_t *total, const uint32_t *model_ids,
                               int32_t scorer_index, double *out) {
     int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= R * (int64_t)E) return;
     int64_t r = idx / E;
     int32_t e = (int32_t)(idx % E);
+    const ProfileDev &pf = (cold && cold[r]) ? pcold : pw;
     bool c = pf.cand[e] != 0;
     const int lora_st = (pool.lora.enabled && pool.lora.ptr) ? lora_lookup(pool.lora, model_ids ? model_ids[r] : 0u, (uint32_t)e) : 0;
     double v;
@@ -490,21 +518,25 @@ __global__ void k_score_dense(int64_t R, int32_t E, ProfileDev pf, PoolArrays po
         v = 0.0;
     } else {
         const epp_scorer_cfg &sc = pf.cfg.scorers[scorer_index];
-        v = sc.kind == EPP_SCORER_PREFIX ? prefix_score(match[idx], total[r])
-            : (sc.kind == EPP_SCORER_LORA_AFFINITY ? lora_score(pool.lora, (uint32_t)e, lora_st)
-                                                   : pool_score(sc, scorer_index, pool, qminmax, e));
+        if (sc.kind == EPP_SCORER_NO_HIT_LRU)        // no_hit_lru.go:259-275
+            v = (cold && cold[r]) ? nohit_col[e] : 0.5;
+        else
+            v = sc.kind == EPP_SCORER_PREFIX ? prefix_score(match[idx], total[r])
+                : (sc.kind == EPP_SCORER_LORA_AFFINITY ? lora_score(pool.lora, (uint32_t)e, lora_st)
+                                                       : pool_score(sc, scorer_index, pool, qminmax, e));
     }
     out[idx] = v;
 }
 
-cudaError_t launch_score_dense(int64_t R, int32_t E, const ProfileDev &prof, const PoolArrays &pool,
+cudaError_t launch_score_dense(int64_t R, int32_t E, const ProfileDev &prof, const ProfileDev &prof_cold,
+                               const uint8_t *cold, const double *nohit_col, const PoolArrays &pool,
                                const int64_t *qminmax, const int32_t *match, const int32_t *total,
                                const uint32_t *model_ids, int32_t scorer_index, double *out, cudaStream_t s,
                                int *launches) {
     int64_t n = R * (int64_t)E;
     if (n <= 0) return cudaSuccess;
-    k_score_dense<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(R, E, prof, pool, qminmax, match, total, model_ids,
-                                                             scorer_index, out);
+    k_score_dense<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(R, E, prof, prof_cold, cold, nohit_col, pool, qminmax, match, total,
+                                                             model_ids, scorer_index, out);
     if (launches) *launches += 1;
     return cudaGetLastError();
 }

@@ -114,6 +114,8 @@ __device__ __forceinline__ double pool_score(const epp_scorer_cfg &sc, int s_ind
         }
         case EPP_SCORER_LORA_AFFINITY:      // request-independent part: the adapter is not resident on the endpoint
             return lora_score(pool.lora, (uint32_t)e, 0);
+        case EPP_SCORER_NO_HIT_LRU:         // the warm score (no_hit_lru.go:159-165); the cold column is never read here
+            return 0.5;
         default: return 0.0;
     }
 }
@@ -195,6 +197,27 @@ __device__ inline uint32_t select_kth_scan(const ProfileDev &pf, int32_t E, doub
         k -= c;
     }
     return EPP_NO_ENDPOINT;
+}
+
+// no-hit-lru isColdRequest (nohitlru/no_hit_lru.go:140-155) by a full scan: does no candidate of pf hold a block?
+// cnt_of(slot) = the request's matchBlocks on the slot.  All lanes call it.
+template <typename CntOf>
+__device__ inline bool cold_scan(const ProfileDev &pf, int32_t E, int lane, CntOf cnt_of) {
+    bool hit = false;
+    for (uint32_t e = lane; e < (uint32_t)E && !hit; e += 32) hit = pf.cand[e] && cnt_of(e) > 0;
+    return !__any_sync(0xffffffffu, hit);
+}
+
+// The profile set request-evaluation uses for profile pi: the cold set when the profile has a no-hit-lru scorer, has
+// candidates and the request is cold for it (is_cold() is called only then, by all lanes); `cold` records the decision
+// of the last such profile (no_hit_lru.go:264-266: every Score call overwrites the request's flag).
+template <typename P, typename IsCold>
+__device__ __forceinline__ const ProfileDev &nohit_select(const P &p, int pi, bool &cold, IsCold is_cold) {
+    if (((p.nohit.mask >> pi) & 1) && *p.prof[pi].n_cand > 0) {
+        cold = is_cold(p.prof[pi]);
+        if (cold) return p.nohit.cold[pi];
+    }
+    return p.prof[pi];
 }
 
 // PrefixBasedPDDecider.disaggregate, prefix_based_pd_decider.go:99-149

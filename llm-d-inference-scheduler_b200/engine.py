@@ -193,6 +193,13 @@ class Engine:
     def index_add_picked(self):
         self._check(self._lib.epp_index_add_picked(self._h))
 
+    def nohit_lru_get(self) -> list:
+        """The no-hit-lru scorer's LRU, oldest first (golang-lru Cache.Keys): slot ids."""
+        out = np.zeros(self.E, dtype=np.uint32)
+        n = C.c_int32()
+        self._check(self._lib.epp_nohit_lru_get(self._h, _ptr(out), out.shape[0], C.byref(n)))
+        return [int(x) for x in out[:min(n.value, out.shape[0])]]
+
     # ---- batches ----
     def _batch(self, data, offsets=None, uniform_len=None, model_ids=None, n_requests=None, lengths=None, multimodal=None):
         """data: bytes-like numpy array / torch CUDA tensor (any dtype, viewed as bytes)."""

@@ -150,6 +150,13 @@ def LoraAffinityScorer():
     return _Scorer(capi.SCORER_LORA_AFFINITY, 0.0, "lora-affinity-scorer")
 
 
+def NoHitLRU(lruSize: int = 1024):
+    """ "no-hit-lru-scorer" (scorer/nohitlru/no_hit_lru.go:80-110, 259-321): cold requests (no candidate holds a block of
+    the prompt) prefer the endpoints that least recently received a cold request; lruSize <= 0 means 1024.  The engine's
+    own prefix match decides coldness, and every Schedule call updates the LRU with its cold requests' picks."""
+    return _Scorer(capi.SCORER_NO_HIT_LRU, float(lruSize), "no-hit-lru-scorer")
+
+
 def ExternalScorer(column: int):                 # host-computed column (e.g. lora-affinity)
     return _Scorer(capi.SCORER_EXTERNAL, float(column), "external")
 
