@@ -130,7 +130,8 @@ __device__ inline Best eval(const ProfileDev &pf, const GenView &g, int32_t E, i
         const int st = use_lora ? lora_lookup(lora, adapter, e) : 0;
         return nm.sticky ? weighted_sum_over(pf, g, nm, e, c, total, lora, st) : weighted_sum(pf, E, e, c, total, lora, st);
     };
-    double v = CUDART_INF;            // score of the current group
+    double v = 0.0;                   // score of the current group
+    bool have_v = false;              // a group is open: the next one lies strictly below v (the first may be +inf)
     uint32_t n_rem = 0;               // its members not emitted yet
     uint32_t g0 = EPP_NO_ENDPOINT, g1 = EPP_NO_ENDPOINT;   // emitted members of the current group: lane l holds #l and #l+32
     uint32_t n_taken = 0;
@@ -142,11 +143,12 @@ __device__ inline Best eval(const ProfileDev &pf, const GenView &g, int32_t E, i
                 const int32_t c = cnt_of(e);
                 if (!cand(e, c)) continue;
                 const double sc = score(e, c);
-                if (sc < v) best_add(b, sc, e);
+                if (!have_v || sc < v) best_add(b, sc, e);
             }
             b = best_warp_reduce(b);
             if (!b.ties) break;       // fewer candidates than k
             v = b.val;
+            have_v = true;
             n_rem = b.ties;
             n_taken = 0;
             g0 = g1 = EPP_NO_ENDPOINT;
