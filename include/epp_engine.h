@@ -272,6 +272,10 @@ typedef struct {
      * keep_hashes stores each row only up to the first block the index cannot hold, EPP_HASH_TRIM; 0 when another hash
      * kernel ran) */
     uint64_t last_hash_bytes_stored;
+    /* prompt bytes k_hash_fused read for the last synchronous device batch or epp_hash_prompts call: every byte the
+     * hashes need, or, for a trimmed Schedule batch, each prompt only up to shortly past its first absent block
+     * (EPP_HASH_SKIP); 0 when another hash kernel ran */
+    uint64_t last_prompt_bytes_read;
 } epp_stats;
 
 /* ---- lifecycle --------------------------------------------------------------------------------- */

@@ -70,7 +70,7 @@ class Stats(C.Structure):
                 ("device_bytes", C.c_uint64), ("last_kernel_ms", C.c_double * 8), ("last_probes", C.c_uint64),
                 ("last_postings", C.c_uint64), ("last_index_apply_ms", C.c_double), ("last_index_build_ms", C.c_double),
                 ("last_index_items", C.c_uint64), ("last_index_launches", C.c_uint64), ("last_index_patched", C.c_uint64),
-                ("last_hash_bytes_stored", C.c_uint64)]
+                ("last_hash_bytes_stored", C.c_uint64), ("last_prompt_bytes_read", C.c_uint64)]
 
 
 class TopkOut(C.Structure):

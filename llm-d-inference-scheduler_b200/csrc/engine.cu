@@ -62,6 +62,7 @@ struct Slot {                       // per-stream staging for host-pointer batch
     DevBuf data;
     DevBuf overflow_list, overflow_n;   // requests handed from a sparse pass to the dense-counter pass (per stream);
                                         // overflow_n[1] is the sparse pass's request counter
+    DevBuf hash_next;                   // k_hash_fused's request counter
     DevBuf pick_scratch;                // zeroed global match counters of the dense-counter kernel when max_endpoints is too
                                         // large for shared memory: per stream, two streams may run that kernel at once
     cudaEvent_t done = nullptr;
@@ -85,7 +86,7 @@ struct epp_engine {
     bool s1_unjoined = false;       // chunk-pipelined async batches left work on stream 1 that stream 0 has not waited for
     int64_t pipe_R = 0, pipe_per = 0;   // chunk layout of the pipelined batches in flight (row ranges are per stream)
     int async_launches = 0;
-    DevBuf work_counters;           // u64[3] probes, postings, hash bytes stored
+    DevBuf work_counters;           // u64[4] probes, postings, hash bytes stored, prompt bytes read
 
     // models
     DevBuf seeds;                   // u64[kMaxModels]
@@ -128,8 +129,9 @@ struct epp_engine {
     // presence bitmap of the read table (index.cuh presence_maybe): rebuilt by every bulk build, bits added by patches
     DevBuf presence;
     int presence_log2 = 0;          // log2 of its bits
-    int presence_log2_env = 0;      // EPP_PRESENCE_LOG2BITS=n (6..26): fixed size instead of 16 bits per table slot
+    int presence_log2_env = 0;      // EPP_PRESENCE_LOG2BITS=n (6..30): fixed size instead of 16 bits per table slot
     int hash_trim = 1;              // EPP_HASH_TRIM=0: Schedule batches store whole hash rows
+    int hash_skip = 1;              // EPP_HASH_SKIP=0: trimmed batches still read and hash every prompt byte
     uint32_t shard_begin = 0, shard_end = 0xFFFFFFFFu;
 
     // batch buffers (sized for the largest batch seen)
@@ -309,7 +311,7 @@ extern "C" int32_t epp_engine_create(const epp_config *cfg, epp_engine **out) {
     }
     for (auto &ev : e->ev) CUDA_TRY(cudaEventCreate(&ev));
     for (auto &ev : e->user_ev) CUDA_TRY(cudaEventCreate(&ev));
-    CUDA_TRY(cudaHostAlloc(reinterpret_cast<void **>(&e->wc_host), sizeof(unsigned long long) * 3, cudaHostAllocDefault));
+    CUDA_TRY(cudaHostAlloc(reinterpret_cast<void **>(&e->wc_host), sizeof(unsigned long long) * 4, cudaHostAllocDefault));
     size_t E = (size_t)cfg->max_endpoints;
     CUDA_TRY(e->seeds.reserve(sizeof(uint64_t) * kMaxModels, &e->dev_bytes));
     CUDA_TRY(e->seed_msg.reserve(4096, &e->dev_bytes));
@@ -323,7 +325,7 @@ extern "C" int32_t epp_engine_create(const epp_config *cfg, epp_engine **out) {
     CUDA_TRY(e->idx_special.reserve(sizeof(IndexSlot), &e->dev_bytes));
     CUDA_TRY(e->get_out.reserve(sizeof(uint32_t) * 4096 + 16, &e->dev_bytes));
     CUDA_TRY(e->flag.reserve(sizeof(int) * 4, &e->dev_bytes));
-    CUDA_TRY(e->work_counters.reserve(sizeof(unsigned long long) * 3, &e->dev_bytes));
+    CUDA_TRY(e->work_counters.reserve(sizeof(unsigned long long) * 4, &e->dev_bytes));
     memset(&e->idx_special_host, 0, sizeof(IndexSlot));
     e->idx_special_host.key = kEmptyKey;
     for (int pi = 0; pi < e->n_alloc_profiles; pi++) {
@@ -371,7 +373,8 @@ extern "C" int32_t epp_engine_create(const epp_config *cfg, epp_engine **out) {
     { const char *v1 = getenv("EPP_DEV_CHUNKS"); e->dev_chunks = v1 ? std::max(1, atoi(v1)) : 2; }
     { const char *v1 = getenv("EPP_HASH_STAGED"); e->staged = v1 ? atoi(v1) : 0; }
     { const char *v1 = getenv("EPP_HASH_TRIM"); e->hash_trim = v1 ? atoi(v1) : 1; }
-    { const char *v1 = getenv("EPP_PRESENCE_LOG2BITS"); e->presence_log2_env = v1 ? std::min(26, std::max(6, atoi(v1))) : 0; }
+    { const char *v1 = getenv("EPP_HASH_SKIP"); e->hash_skip = v1 ? atoi(v1) : 1; }
+    { const char *v1 = getenv("EPP_PRESENCE_LOG2BITS"); e->presence_log2_env = v1 ? std::min(30, std::max(6, atoi(v1))) : 0; }
     { const char *v1 = getenv("EPP_MATCH_CTAS"); e->match_ctas = (v1 && atoi(v1) == 6) ? 6 : 8; }
     { const char *v1 = getenv("EPP_SMALL_BATCH"); e->small_max = v1 ? std::max(0, atoi(v1)) : 1024; }
     { const char *v1 = getenv("EPP_SMALL_ZEROCOPY"); e->small_zc_max = v1 ? std::max(0, atoi(v1)) : 8; }
@@ -382,6 +385,7 @@ extern "C" int32_t epp_engine_create(const epp_config *cfg, epp_engine **out) {
     CUDA_TRY(e->small_overflow_n.reserve(sizeof(int32_t) * 4, &e->dev_bytes));
     CUDA_TRY(cudaMemset(e->small_overflow_n.p, 0, sizeof(int32_t) * 4));
     for (int i = 0; i < 2; i++) CUDA_TRY(e->slot[i].overflow_n.reserve(sizeof(int32_t) * 4, &e->dev_bytes));
+    for (int i = 0; i < 2; i++) CUDA_TRY(e->slot[i].hash_next.reserve(sizeof(uint32_t), &e->dev_bytes));
     EPP_TRY(rebuild_presence(e.get()));              // the empty index: every bit clear
     if (e->nohit_mask) {
         ProfileDev cold[kMaxProfiles];
@@ -729,10 +733,13 @@ extern "C" int32_t epp_pool_set_lora(epp_engine *h, int32_t n, const uint32_t *i
 // prefix index
 // ------------------------------------------------------------------------------------------------
 // Clears the presence bitmap and sets the bits of every key the read table holds.  16 bits per table slot, which is
-// >= 26 per distinct key at the load factors the build and the patches allow, up to 2^26 bits (8 MiB, L2-resident).
+// >= 26 per distinct key at the load factors the build and the patches allow, up to 2^26 bits (8 MiB, L2-resident) while
+// the table fits its L2 budget.  A larger table is read from DRAM anyway: its bitmap may grow to 2^30 bits (128 MiB), as
+// 2^26 bits over 1.3e8 keys would be mostly set and prove few misses (the lookup's latency hides behind a window).
 static int32_t rebuild_presence(epp_engine *h) {
+    const int cap = h->idx_capacity * sizeof(IndexSlot) > h->l2_table_bytes ? 30 : 26;
     int l = 6;
-    while (l < 26 && (1ull << l) < 16 * h->idx_capacity) l++;
+    while (l < cap && (1ull << l) < 16 * h->idx_capacity) l++;
     if (h->presence_log2_env) l = h->presence_log2_env;
     h->presence_log2 = l;
     CUDA_TRY(h->presence.reserve(((size_t)1 << l) / 8, &h->dev_bytes));
@@ -1086,7 +1093,7 @@ struct Work {
     const uint8_t *multimodal_dev = nullptr;   // absolute, or nullptr
 };
 
-static HashParams hash_params(epp_engine *h, const Work &w) {
+static HashParams hash_params(epp_engine *h, const Work &w, Slot &sl) {
     HashParams p;
     int64_t n = w.r1 - w.r0;
     p.data = w.data_base;
@@ -1109,6 +1116,9 @@ static HashParams hash_params(epp_engine *h, const Work &w) {
     p.presence_shift = 0;
     p.bound = nullptr;
     p.stored = nullptr;
+    p.skip = 0;
+    p.read = nullptr;
+    p.req_next = sl.hash_next.as<uint32_t>();
     return p;
 }
 
@@ -1213,9 +1223,11 @@ static int32_t launch_match(epp_engine *h, Slot &sl, PickParams pp, int *launche
 
 // A Schedule batch's hash rows are read by nothing but its match kernel, whose global stop never lies beyond the first
 // block the presence bitmap proves absent: k_hash_fused stores each row only up to there and both match kernels honour
-// the bound.  Only on the k_hash_fused + k_match_pick_sparse path (not the dense-counter or general evaluation).
+// the bound.  Only on the k_hash_fused + k_match_pick_sparse path (not the dense-counter or general evaluation).  Since
+// a block hash depends on the blocks before it alone, the kernel also stops reading each prompt there (EPP_HASH_SKIP).
 static void trim_rows(epp_engine *h, const Work &w, HashParams &hp, PickParams &pp) {
     if (!hash_fused_selected(hp) || pp.out_match || pp.gen.on) return;
+    hp.skip = h->hash_skip;
     hp.presence = h->presence.as<uint32_t>();
     hp.presence_shift = 64 - h->presence_log2;
     hp.bound = h->bound.as<int32_t>() + w.r0;
@@ -1245,6 +1257,7 @@ static int32_t finish_async(epp_engine *h) {
     h->stats.last_probes = h->wc_host[0];
     h->stats.last_postings = h->wc_host[1];
     h->stats.last_hash_bytes_stored = h->wc_host[2];
+    h->stats.last_prompt_bytes_read = h->wc_host[3];
     h->stats.last_kernel_launches = (uint64_t)h->async_launches;
     if (h->nohit_timed) {
         float tn = 0;
@@ -1387,7 +1400,7 @@ static int32_t run_small(epp_engine *h, const BatchView &v, int mode, const uint
     SmallOut so{h->small_dec, h->small_det, h->small_flags, epoch, arrive};
     int launches = 0;
     CUDA_TRY(cudaEventRecord(h->ev[0], s0));
-    CUDA_TRY(launch_cycle_small(hash_params(h, w), pp, so, s0, &launches));
+    CUDA_TRY(launch_cycle_small(hash_params(h, w, h->slot[0]), pp, so, s0, &launches));
     CUDA_TRY(cudaEventRecord(h->ev[1], s0));
 
     // wait for the flag word of every request (written after a system-scope fence behind its decision)
@@ -1495,7 +1508,7 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
                (mode == Mode::HashOnly && out_hashes) ? out_hashes : h->hashes.as<uint64_t>(),
                (mode == Mode::HashOnly && out_nblocks) ? out_nblocks : (mode == Mode::Match && out_total ? out_total : h->nblocks.as<int32_t>()),
                v.multimodal};
-        CUDA_TRY(cudaMemsetAsync(h->work_counters.p, 0, sizeof(unsigned long long) * 3, s0));
+        CUDA_TRY(cudaMemsetAsync(h->work_counters.p, 0, sizeof(unsigned long long) * 4, s0));
         const int64_t min_chunk = 4096;
         if (pipelined) {
             // Throughput mode: the batch runs as C chunks alternating between the engine's two streams, so the hash
@@ -1520,7 +1533,7 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
                 PickParams pp = pick_params(h, w, dec_base + r0, out_detail ? out_detail + r0 : nullptr, nullptr);
                 if (tk) attach_topk(h, pp.gen, tk_picks, tk_scores, r0);
                 Slot &sl = h->slot[k & 1];
-                HashParams hp = hash_params(h, w);
+                HashParams hp = hash_params(h, w, sl);
                 if (trim) trim_rows(h, w, hp, pp);
                 EPP_TRY(launch_cycle(h, sl, hp, pp, &launches, nullptr));
             }
@@ -1531,21 +1544,24 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
             h->pipe_R = R;
             h->pipe_per = per;
         } else if (mode == Mode::HashOnly) {
-            CUDA_TRY(launch_hash_prompts(hash_params(h, w), s0, &launches, h->ev));
+            HashParams hp = hash_params(h, w, h->slot[0]);
+            hp.read = h->work_counters.as<unsigned long long>() + 3;
+            CUDA_TRY(launch_hash_prompts(hp, s0, &launches, h->ev));
         } else {
             epp_decision *dec = (mode == Mode::Schedule && out_dec) ? out_dec : h->decisions.as<epp_decision>();
             PickParams pp = pick_params(h, w, dec, mode == Mode::Schedule ? out_detail : nullptr, mode == Mode::Match ? out_match : nullptr);
             pp.work_counters = h->work_counters.as<unsigned long long>();
             if (tk) attach_topk(h, pp.gen, tk_picks, tk_scores, 0);
-            HashParams hp = hash_params(h, w);
+            HashParams hp = hash_params(h, w, h->slot[0]);
             hp.stored = h->work_counters.as<unsigned long long>() + 2;
+            hp.read = h->work_counters.as<unsigned long long>() + 3;
             if (trim) trim_rows(h, w, hp, pp);
             EPP_TRY(launch_cycle(h, h->slot[0], hp, pp, &launches, h->ev));
         }
         CUDA_TRY(cudaEventRecord(h->ev[4], s0));
         if (mode == Mode::Schedule)                // after ev[4]: last_kernel_ms[3] stays the match + pick time
             EPP_TRY(nohit_update_timed(h, out_dec ? out_dec : h->decisions.as<epp_decision>(), R, &launches));
-        CUDA_TRY(cudaMemcpyAsync(h->wc_host, h->work_counters.p, sizeof(unsigned long long) * 3, cudaMemcpyDeviceToHost, s0));
+        CUDA_TRY(cudaMemcpyAsync(h->wc_host, h->work_counters.p, sizeof(unsigned long long) * 4, cudaMemcpyDeviceToHost, s0));
         h->async_pending = true;
         h->async_launches = launches;
         if (v.async && mode != Mode::Match) return EPP_OK;         // epp_synchronize() (or the next call that needs the
@@ -1627,7 +1643,7 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
         w.hashes_out = h->hashes.as<uint64_t>() + (size_t)c.r0 * B;
         w.nblocks_out = h->nblocks.as<int32_t>() + c.r0;
         if (mode == Mode::HashOnly) {
-            CUDA_TRY(launch_hash_prompts(hash_params(h, w), s, &launches));
+            CUDA_TRY(launch_hash_prompts(hash_params(h, w, sl), s, &launches));
             if (out_hashes) CUDA_TRY(cudaMemcpyAsync(out_hashes + (size_t)c.r0 * B, w.hashes_out, sizeof(uint64_t) * nreq * B, cudaMemcpyDeviceToHost, s));
             if (out_nblocks) CUDA_TRY(cudaMemcpyAsync(out_nblocks + c.r0, w.nblocks_out, sizeof(int32_t) * nreq, cudaMemcpyDeviceToHost, s));
         } else {
@@ -1636,7 +1652,7 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
             epp_decision_detail *det = h->details.as<epp_decision_detail>() + c.r0;
             PickParams pp = pick_params(h, w, dec, det, dm);
             if (tk) attach_topk(h, pp.gen, tk_picks, tk_scores, c.r0);
-            HashParams hp = hash_params(h, w);
+            HashParams hp = hash_params(h, w, sl);
             if (trim) trim_rows(h, w, hp, pp);
             EPP_TRY(launch_cycle(h, sl, hp, pp, &launches, nullptr));
             if (mode == Mode::Schedule) {
@@ -2190,7 +2206,7 @@ static int32_t p2p_phase_rows(epp_engine *h, const BatchView &v, epp_decision *o
         // hashes + local presence masks -> own exchange buffer, raise flag 1
         Work w{r0, r1, v.offsets ? v.data : v.data + (uint64_t)r0 * v.uniform_len, v.offsets, v.lengths, v.uniform_len, v.model_ids,
                or_bits, hashes, nbs, nullptr};
-        CUDA_TRY(launch_hash_prompts(hash_params(h, w), s, &launches));
+        CUDA_TRY(launch_hash_prompts(hash_params(h, w, sl), s, &launches));
         CUDA_TRY(launch_shard_probe(R, h->cfg.max_prefix_blocks, hashes, nbs, index_view(h),
                                     reinterpret_cast<uint32_t *>(own + mask_off), (int32_t)W, s, &launches));
         CUDA_TRY(launch_p2p_signal(reinterpret_cast<unsigned long long *>(own + flag1), epoch, s));

@@ -34,6 +34,11 @@ struct HashParams {
     int32_t presence_shift;
     int32_t *bound;             // [R]
     unsigned long long *stored; // += bytes of hash rows stored by k_hash_fused, or nullptr
+    // with presence: stop loading each prompt at its closing window (bound's window; the trailing partial block only
+    // while no block is proven absent).  0: every prompt byte is read and hashed.
+    int32_t skip;
+    unsigned long long *read;   // += prompt bytes loaded by k_hash_fused, or nullptr
+    uint32_t *req_next;         // k_hash_fused's request counter (device; zeroed by its launcher): one per stream
 };
 // Common alignment (0, 16, 32) of every block start; >= 16 (and block_bytes % 32 == 0) enables the fused kernel.
 int hash_batch_alignment(const HashParams &p);
@@ -84,7 +89,7 @@ cudaError_t launch_index_build(const uint64_t *pair_hash, const uint32_t *pair_e
                                cudaStream_t s, int *launches);
 cudaError_t launch_index_get(const IndexView &ix, uint64_t hash, uint32_t *out_eps, int32_t cap, int32_t *out_n,
                              cudaStream_t s);
-// Presence bitmap of 2^log2bits bits (6..26) over the table's keys (index.cuh presence_maybe); slots == nullptr: clear.
+// Presence bitmap of 2^log2bits bits (6..30) over the table's keys (index.cuh presence_maybe); slots == nullptr: clear.
 cudaError_t launch_presence_build(const IndexSlot *slots, uint64_t capacity, uint32_t *bits, int log2bits, cudaStream_t s,
                                   int *launches);
 

@@ -101,6 +101,7 @@ def main():
                 out["launches"] = int(st["last_kernel_launches"])
                 out["probes"], out["postings"] = int(st["last_probes"]), int(st["last_postings"])
                 out["hash_bytes_stored"] = int(st["last_hash_bytes_stored"])
+                out["prompt_bytes_read"] = int(st["last_prompt_bytes_read"])
                 dec = epp.decisions_from_torch(dev_dec)
                 if ref_dec is None:
                     ref_dec = dec.copy()
