@@ -53,11 +53,12 @@ type AffinitySpec struct {
 	TTFTColumn             int // ext column carrying LatencyPredictionInfo.TTFT; -1 = attribute absent
 }
 
-// ProfileSpec mirrors epp_profile_cfg: role filter -> [prefix-cache-affinity-filter] -> scorers in order -> max-score picker.
+// ProfileSpec mirrors epp_profile_cfg: role filter -> [prefix-cache-affinity-filter] -> scorers in order -> picker.
 type ProfileSpec struct {
 	Filter   int // C.EPP_FILTER_*
 	Scorers  []ScorerSpec
 	Affinity *AffinitySpec
+	Picker   int // C.EPP_PICKER_* (0 = max-score-picker); see RandomPicker / WeightedRandomPicker
 }
 
 // Config mirrors epp_config (EndpointPickerConfig fields that define this path).
@@ -110,6 +111,7 @@ func fillProfile(dst *C.epp_profile_cfg, p ProfileSpec) error {
 		dst.scorers[i].param2 = C.double(s.Param2)
 	}
 	dst.ttft_column = -1
+	dst.picker = C.int32_t(p.Picker)
 	if a := p.Affinity; a != nil {
 		dst.affinity_threshold = C.double(a.AffinityThreshold)
 		dst.exploration_probability = C.double(a.ExplorationProbability)

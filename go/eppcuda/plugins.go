@@ -73,6 +73,42 @@ func NoHitLRUScorer(weight float64, params json.RawMessage) (ScorerSpec, error) 
 	return ScorerSpec{Kind: int(C.EPP_SCORER_NO_HIT_LRU), Weight: weight, Param: float64(p.LRUSize)}, nil
 }
 
+// RandomPickerType and WeightedRandomPickerType are the reference's plugin types of the two random pickers
+// (picker/random/picker.go, picker/weightedrandom/picker.go).
+const (
+	RandomPickerType         = "random-picker"
+	WeightedRandomPickerType = "weighted-random-picker"
+)
+
+// pickerMaxEndpoints parses picker.PickerParameters (maxNumOfEndpoints); <= 0 means 1, as in the reference factories.
+func pickerMaxEndpoints(params json.RawMessage) (int, error) {
+	p := struct {
+		MaxNumOfEndpoints int `json:"maxNumOfEndpoints"`
+	}{MaxNumOfEndpoints: 1}
+	if len(params) > 0 {
+		if err := json.Unmarshal(params, &p); err != nil {
+			return 0, err
+		}
+	}
+	if p.MaxNumOfEndpoints <= 0 {
+		p.MaxNumOfEndpoints = 1
+	}
+	return p.MaxNumOfEndpoints, nil
+}
+
+// RandomPicker turns a "random-picker" entry into the profile's picker kind and maxNumOfEndpoints (Config.PickK; the
+// engine has one maxNumOfEndpoints for all profiles).
+func RandomPicker(params json.RawMessage) (kind int, maxNumOfEndpoints int, err error) {
+	k, err := pickerMaxEndpoints(params)
+	return int(C.EPP_PICKER_RANDOM), k, err
+}
+
+// WeightedRandomPicker turns a "weighted-random-picker" entry into the profile's picker kind and maxNumOfEndpoints.
+func WeightedRandomPicker(params json.RawMessage) (kind int, maxNumOfEndpoints int, err error) {
+	k, err := pickerMaxEndpoints(params)
+	return int(C.EPP_PICKER_WEIGHTED_RANDOM), k, err
+}
+
 // NoHitLRUKeys returns the slots of the scorer's LRU, oldest first (golang-lru Cache.Keys, epp_nohit_lru_get).
 func (e *Engine) NoHitLRUKeys() ([]uint32, error) {
 	out := make([]uint32, e.cfg.MaxEndpoints)

@@ -53,6 +53,28 @@
  * Exploration draw of the prefix-cache-affinity-filter (rand.Float64() < explorationProbability,
  * filter/prefixcacheaffinity/plugin.go:113): u = (mix64((tie_seed ^ 0xA0761D6478BD642F) ^ mix64(key)) >> 11) * 2^-53 when
  * tie_seed != 0; with tie_seed == 0 (the deterministic mode) the filter never explores.
+ *
+ * Random pickers (epp_profile_cfg.picker): the draw u = (mix64((tie_seed ^ 0xE7037ED1A0B428DB) ^
+ * mix64(key)) >> 11) * 2^-53 (same key as the tie rule) is made for every tie_seed, 0 included.  The population is the
+ * profile's candidates c_0 < c_1 < ... < c_{n-1} (ascending slot order, after the affinity filter); s(c) is c's weighted score.
+ *   random-picker: c_min(floor(u * n), n - 1)  (u * n rounded to nearest).
+ *   weighted-random-picker: P(c_i) = s_i+ / W.  s+ = s when 0 < s < +inf (times sigma = 2^-128 when the profile's
+ *       sum of |weight| exceeds 2^960, which keeps every sum finite; exact, a power of two), 0 when s <= 0 or NaN.
+ *       The sequence folded is: the request's EXPLICIT candidates (matchBlocks > 0, or the request's LoRA adapter is
+ *       active / waiting on them; under a narrowing affinity filter every candidate) with their own s+, and between
+ *       them the GAPS, runs [a, b) of the other candidates, whose mass is wcum[b] - wcum[a], wcum[i] = the left fold
+ *       (+0.0 first, round-to-nearest) of s+(base) over c_0 .. c_{i-1}, base = the score with no match (computed once
+ *       per pool snapshot / no-hit-lru update).  W = the left fold of that sequence.
+ *       - some candidate scores +inf: the pick is the one of rank min(floor(u * N), N - 1) among the N +inf candidates;
+ *       - else W == 0 (every score <= 0): the random-picker's pick (weightedrandom/picker.go:113-116);
+ *       - else t = u * W (rounded; t >= W becomes the largest double below W); the pick is the first item whose
+ *         running sum exceeds t -- inside a gap [a, b) that followed the running sum S, the first c_i (a <= i < b) with
+ *         S + (wcum[i+1] - wcum[a]) > t (the last one reproduces the gap's own sum, so the search stays inside it).
+ *       The draw has the distribution of A-Res's largest key (picker.go:121-154) and costs O(explicit + log n).
+ *   First k (pick_k > 1): draw j = 0 .. min(k, n) - 1 is the draw above with the seed tie_seed + j * 0x9E3779B97F4A7C15 over
+ *       the candidates not emitted yet (the random rank counts only those); the emitted ones stay in the weighted sequence
+ *       as explicit items of mass 0, so once the positive scores are used up W == 0 and the rest follow in uniform random
+ *       order.  Pick 0 is the one-endpoint pick.
  */
 #ifndef EPP_ENGINE_H
 #define EPP_ENGINE_H
@@ -146,8 +168,17 @@ typedef struct {
     double param2;
 } epp_scorer_cfg;
 
+/* Pickers (the last plugin of a profile).  Under the random pickers an epp_decision's score is the pick's own weighted
+ * score (bit-exact), tie_count the size of the population the draw was made from (the profile's candidates), and
+ * match_blocks / the P/D decider read the pick's match count, as under max-score.  See "Random pickers" above. */
+typedef enum {
+    EPP_PICKER_MAX_SCORE = 0,        /* "max-score-picker"       picker/maxscore/picker.go:87-115                    */
+    EPP_PICKER_RANDOM = 1,           /* "random-picker"          picker/random/picker.go:86-104                      */
+    EPP_PICKER_WEIGHTED_RANDOM = 2   /* "weighted-random-picker" picker/weightedrandom/picker.go:111-155             */
+} epp_picker_kind;
+
 /* One SchedulerProfile (scheduling/scheduler_profile.go:117-128): role filter -> [prefix-cache-affinity-filter] ->
- * scorers IN ORDER -> max-score picker. */
+ * scorers IN ORDER -> picker. */
 typedef struct {
     int32_t filter;            /* epp_filter_kind */
     int32_t n_scorers;
@@ -163,7 +194,7 @@ typedef struct {
     double max_ttft_penalty_ms;        /* >= 0; 0 = always stick                                              */
     int32_t ttft_column;               /* ext column holding LatencyPredictionInfo.TTFT per endpoint; < 0 = no
                                           prediction attached (the gate then never breaks stickiness, :169-180) */
-    int32_t reserved;
+    int32_t picker;                    /* epp_picker_kind of the profile (0 = max-score)                      */
 } epp_profile_cfg;
 
 /* Mirrors the EndpointPickerConfig fields that define this path (apix/config/v1alpha1, and

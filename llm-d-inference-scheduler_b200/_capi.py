@@ -22,6 +22,7 @@ EPP_OK, EPP_ERR_INVALID, EPP_ERR_CUDA, EPP_ERR_NO_DEVICE, EPP_ERR_CAPACITY, EPP_
 (ROLE_NONE, ROLE_DECODE, ROLE_PREFILL, ROLE_PREFILL_DECODE, ROLE_BOTH, ROLE_ENCODE, ROLE_ENCODE_PREFILL,
  ROLE_ENCODE_PREFILL_DECODE, ROLE_OTHER) = range(9)
 FILTER_NONE, FILTER_DECODE, FILTER_PREFILL, FILTER_ENCODE = range(4)
+PICKER_MAX_SCORE, PICKER_RANDOM, PICKER_WEIGHTED_RANDOM = range(3)
 HANDLER_SINGLE, HANDLER_DISAGG = 0, 1
 
 
@@ -33,7 +34,7 @@ class ScorerCfg(C.Structure):
 class ProfileCfg(C.Structure):
     _fields_ = [("filter", C.c_int32), ("n_scorers", C.c_int32), ("scorers", ScorerCfg * EPP_MAX_SCORERS),
                 ("affinity_threshold", C.c_double), ("exploration_probability", C.c_double),
-                ("max_ttft_penalty_ms", C.c_double), ("ttft_column", C.c_int32), ("reserved", C.c_int32)]
+                ("max_ttft_penalty_ms", C.c_double), ("ttft_column", C.c_int32), ("picker", C.c_int32)]
 
 
 class Config(C.Structure):

@@ -102,7 +102,8 @@ struct ChainFollower {
 // kStage: the prompt is staged into shared memory by ONE bulk copy (TMA) per request; else the digest threads load their
 // blocks themselves (prompts too long for the staging buffer).
 // kNoHit: a profile has the no-hit-lru scorer (match_sparse.cuh match_request); those engines launch k_cycle_small_nohit.
-template <bool kStage, bool kNoHit>
+// kRand: some profile has a random picker (k_cycle_small_rand, which also carries the no-hit-lru logic).
+template <bool kStage, bool kNoHit, bool kRand = false>
 __device__ __forceinline__ void cycle_small(const HashParams &hp, const PickParams &pp, const SmallOut &so, uint32_t stage_off) {
     extern __shared__ __align__(128) uint64_t s_m[];   // [max_blocks] merged stripe state of every full block; then, at byte
                                                        // stage_off, (kStage) the prompt's full blocks and its trailing partial block
@@ -218,7 +219,7 @@ __device__ __forceinline__ void cycle_small(const HashParams &hp, const PickPara
 
     int32_t unused = 0;
     const ChainFollower fw{&s_progress, s_m};
-    const bool decided = sparse::match_request<true, false, true, 3, ChainFollower, kNoHit>(pp, r, lane, false, nullptr, nullptr, unused, fw);
+    const bool decided = sparse::match_request<true, false, true, 3, ChainFollower, kNoHit, kRand>(pp, r, lane, false, nullptr, nullptr, unused, fw);
     if (lane == 0) {
         if (decided) {
             so.dec[r] = pp.out[r];
@@ -236,6 +237,10 @@ __global__ void __launch_bounds__(kThreads) k_cycle_small(HashParams hp, PickPar
 template <bool kStage>
 __global__ void __launch_bounds__(kThreads) k_cycle_small_nohit(HashParams hp, PickParams pp, SmallOut so, uint32_t stage_off) {
     cycle_small<kStage, true>(hp, pp, so, stage_off);
+}
+template <bool kStage>
+__global__ void __launch_bounds__(kThreads) k_cycle_small_rand(HashParams hp, PickParams pp, SmallOut so, uint32_t stage_off) {
+    cycle_small<kStage, true, true>(hp, pp, so, stage_off);
 }
 }  // namespace
 
@@ -262,12 +267,17 @@ cudaError_t launch_cycle_small(const HashParams &hp, const PickParams &pp, const
         if (e == cudaSuccess) e = cudaFuncSetAttribute(k_cycle_small<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
         if (e == cudaSuccess) e = cudaFuncSetAttribute(k_cycle_small_nohit<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
         if (e == cudaSuccess) e = cudaFuncSetAttribute(k_cycle_small_nohit<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(k_cycle_small_rand<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(k_cycle_small_rand<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
         if (e != cudaSuccess) return e;
         attr_set[dev & 63] = true;
     }
     const unsigned grid = (unsigned)hp.R;
     const uint32_t off = (uint32_t)m_bytes;
-    if (pp.nohit.mask) {                           // no-hit-lru builds (match_sparse.cuh match_request)
+    if (any_random_picker(pp)) {                   // random-picker builds (match_sparse.cuh eval_random_lanes)
+        if (stage) k_cycle_small_rand<true><<<grid, kThreads, smem, s>>>(hp, pp, so, off);
+        else k_cycle_small_rand<false><<<grid, kThreads, smem, s>>>(hp, pp, so, off);
+    } else if (pp.nohit.mask) {                    // no-hit-lru builds (match_sparse.cuh match_request)
         if (stage) k_cycle_small_nohit<true><<<grid, kThreads, smem, s>>>(hp, pp, so, off);
         else k_cycle_small_nohit<false><<<grid, kThreads, smem, s>>>(hp, pp, so, off);
     } else if (stage) {

@@ -55,6 +55,7 @@ static int32_t fail(int32_t code, const char *fmt, ...) {
 
 struct ProfileState {
     DevBuf cand, contrib, base, order, grp_size, sort_key, n_cand, qminmax;
+    DevBuf cands, wcum, icum;       // random pickers only (ProfileDerived)
 };
 
 struct Slot {                       // per-stream staging for host-pointer batches
@@ -247,11 +248,17 @@ static int32_t validate_profile(const epp_profile_cfg &p, int n_ext, const char 
     if (!(p.exploration_probability >= 0.0 && p.exploration_probability <= 1.0)) return fail(EPP_ERR_INVALID, "%s: explorationProbability must be in [0, 1], got %f", name, p.exploration_probability);
     if (!(p.max_ttft_penalty_ms >= 0.0)) return fail(EPP_ERR_INVALID, "%s: maxTTFTPenaltyMs must be >= 0, got %f", name, p.max_ttft_penalty_ms);
     if (p.affinity_threshold > 0.0 && p.ttft_column >= n_ext) return fail(EPP_ERR_INVALID, "%s: ttft_column %d out of range [0,%d)", name, p.ttft_column, n_ext);
+    if (p.picker < EPP_PICKER_MAX_SCORE || p.picker > EPP_PICKER_WEIGHTED_RANDOM) return fail(EPP_ERR_INVALID, "%s: unknown picker %d", name, p.picker);
     return EPP_OK;
 }
 
-static int32_t alloc_profile(epp_engine *e, ProfileState &ps) {
+static int32_t alloc_profile(epp_engine *e, ProfileState &ps, bool random_picker) {
     size_t E = (size_t)e->cfg.max_endpoints, Ep = (size_t)e->Epad;
+    if (random_picker) {
+        CUDA_TRY(ps.cands.reserve(sizeof(uint32_t) * E, &e->dev_bytes));
+        CUDA_TRY(ps.wcum.reserve(sizeof(double) * (E + 1), &e->dev_bytes));
+        CUDA_TRY(ps.icum.reserve(sizeof(uint32_t) * (E + 1), &e->dev_bytes));
+    }
     CUDA_TRY(ps.cand.reserve(E, &e->dev_bytes));
     CUDA_TRY(ps.contrib.reserve(sizeof(double) * EPP_MAX_SCORERS * E, &e->dev_bytes));
     CUDA_TRY(ps.base.reserve(sizeof(double) * E, &e->dev_bytes));
@@ -265,6 +272,15 @@ static int32_t alloc_profile(epp_engine *e, ProfileState &ps) {
 
 static int32_t rebuild_presence(epp_engine *h);
 static ProfileDev cold_profile_dev(epp_engine *h, int p);
+static const epp_profile_cfg &profile_cfg(const epp_engine *h, int p) {
+    return p == 0 ? h->cfg.primary : (p == 1 ? h->cfg.prefill : h->cfg.encode);
+}
+// Does any profile of the handler use a random picker?
+static bool any_random_picker(const epp_engine *h) {
+    for (int p = 0; p < h->n_alloc_profiles; p++)
+        if (profile_cfg(h, p).picker != EPP_PICKER_MAX_SCORE) return true;
+    return false;
+}
 
 extern "C" int32_t epp_engine_create(const epp_config *cfg, epp_engine **out) {
     if (!cfg || !out) return fail(EPP_ERR_INVALID, "cfg/out is NULL");
@@ -320,7 +336,7 @@ extern "C" int32_t epp_engine_create(const epp_config *cfg, epp_engine **out) {
     CUDA_TRY(e->waiting.reserve(sizeof(int32_t) * E, &e->dev_bytes));
     CUDA_TRY(e->running.reserve(sizeof(int32_t) * E, &e->dev_bytes));
     if (cfg->n_ext_cols) CUDA_TRY(e->ext.reserve(sizeof(double) * E * (size_t)cfg->n_ext_cols, &e->dev_bytes));
-    for (int p = 0; p < e->n_alloc_profiles; p++) EPP_TRY(alloc_profile(e.get(), e->prof[p]));
+    for (int p = 0; p < e->n_alloc_profiles; p++) EPP_TRY(alloc_profile(e.get(), e->prof[p], profile_cfg(e.get(), p).picker != 0));
     CUDA_TRY(e->idx_cursor.reserve(sizeof(uint32_t) * 4, &e->dev_bytes));
     CUDA_TRY(e->idx_special.reserve(sizeof(IndexSlot), &e->dev_bytes));
     CUDA_TRY(e->get_out.reserve(sizeof(uint32_t) * 4096 + 16, &e->dev_bytes));
@@ -358,7 +374,7 @@ extern "C" int32_t epp_engine_create(const epp_config *cfg, epp_engine **out) {
         CUDA_TRY(cudaMemset(e->nh_misc.p, 0, sizeof(int32_t) * 4));
         for (int pi = 0; pi < e->n_alloc_profiles; pi++)
             if (e->nohit_mask & (1 << pi)) {
-                EPP_TRY(alloc_profile(e.get(), e->prof_cold[pi]));
+                EPP_TRY(alloc_profile(e.get(), e->prof_cold[pi], profile_cfg(e.get(), pi).picker != 0));
                 CUDA_TRY(e->nh_col[pi].reserve(sizeof(double) * E, &e->dev_bytes));
             }
     }
@@ -519,6 +535,9 @@ static ProfileDev profile_dev(epp_engine *h, int p) {
     pd.order = h->prof[p].order.as<uint32_t>();
     pd.grp_size = h->prof[p].grp_size.as<uint32_t>();
     pd.n_cand = h->prof[p].n_cand.as<int32_t>();
+    pd.cands = h->prof[p].cands.as<uint32_t>();
+    pd.wcum = h->prof[p].wcum.as<double>();
+    pd.icum = h->prof[p].icum.as<uint32_t>();
     return pd;
 }
 
@@ -542,9 +561,12 @@ static int32_t nohit_derive(epp_engine *h, cudaStream_t s, bool gated, int *laun
     PoolArrays pa = pool_arrays(h);
     for (int p = 0; p < h->n_alloc_profiles; p++) {
         if (!(h->nohit_mask & (1 << p))) continue;
-        ProfileDerived d;
+        ProfileDerived d{};
         d.cand = h->prof[p].cand.as<uint8_t>();
         d.n_cand = h->prof[p].n_cand.as<int32_t>();
+        d.cands = h->prof_cold[p].cands.as<uint32_t>();
+        d.wcum = h->prof_cold[p].wcum.as<double>();
+        d.icum = h->prof_cold[p].icum.as<uint32_t>();
         d.qminmax = h->prof[p].qminmax.as<int64_t>();
         d.contrib = h->prof_cold[p].contrib.as<double>();
         d.base = h->prof_cold[p].base.as<double>();
@@ -592,6 +614,9 @@ static ProfileDev cold_profile_dev(epp_engine *h, int p) {
     c.base = h->prof_cold[p].base.as<double>();
     c.order = h->prof_cold[p].order.as<uint32_t>();
     c.grp_size = h->prof_cold[p].grp_size.as<uint32_t>();
+    c.cands = h->prof_cold[p].cands.as<uint32_t>();
+    c.wcum = h->prof_cold[p].wcum.as<double>();
+    c.icum = h->prof_cold[p].icum.as<uint32_t>();
     return c;
 }
 
@@ -612,9 +637,12 @@ static int32_t derive_pool(epp_engine *h) {
     PoolArrays pa = pool_arrays(h);
     int launches = 0;
     for (int p = 0; p < h->n_alloc_profiles; p++) {
-        ProfileDerived d;
+        ProfileDerived d{};
         d.cand = h->prof[p].cand.as<uint8_t>();
         d.contrib = h->prof[p].contrib.as<double>();
+        d.cands = h->prof[p].cands.as<uint32_t>();
+        d.wcum = h->prof[p].wcum.as<double>();
+        d.icum = h->prof[p].icum.as<uint32_t>();
         d.base = h->prof[p].base.as<double>();
         d.order = h->prof[p].order.as<uint32_t>();
         d.grp_size = h->prof[p].grp_size.as<uint32_t>();
@@ -2010,6 +2038,7 @@ extern "C" int32_t epp_shard_set(epp_engine *h, uint32_t ep_begin, uint32_t ep_e
     if (h->cfg.handler != EPP_HANDLER_SINGLE) return fail(EPP_ERR_INVALID, "endpoint-sharded mode supports the single-profile handler only");
     if (h->general) return fail(EPP_ERR_INVALID, "endpoint-sharded mode supports neither pick_k > 1 nor the prefix-cache-affinity-filter (both need every candidate's score on one rank)");
     if (h->nohit_mask) return fail(EPP_ERR_INVALID, "endpoint-sharded mode does not support the no-hit-lru scorer (coldness needs every rank's match)");
+    if (any_random_picker(h)) return fail(EPP_ERR_INVALID, "endpoint-sharded mode does not support the random pickers (a weighted draw needs every rank's scores)");
     h->shard_begin = ep_begin;
     h->shard_end = ep_end;
     h->pool_ready = false;          // candidates are derived per shard: epp_pool_set must follow
@@ -2114,6 +2143,7 @@ extern "C" int32_t epp_shard_p2p_connect(epp_engine *h, int32_t n_ranks, int32_t
     if (!h || n_ranks <= 0 || n_ranks > 64 || rank < 0 || rank >= n_ranks || !peers) return fail(EPP_ERR_INVALID, "bad arguments");
     std::lock_guard<std::mutex> lk(h->mu);
     if (h->nohit_mask) return fail(EPP_ERR_INVALID, "endpoint-sharded mode does not support the no-hit-lru scorer (coldness needs every rank's match)");
+    if (any_random_picker(h)) return fail(EPP_ERR_INVALID, "endpoint-sharded mode does not support the random pickers (a weighted draw needs every rank's scores)");
     EPP_TRY(set_device(h));
     EPP_TRY(join_streams(h));
     if (!h->p2p_buf) return fail(EPP_ERR_STATE, "epp_shard_p2p_export has not been called");

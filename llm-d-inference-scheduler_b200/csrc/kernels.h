@@ -129,6 +129,11 @@ struct ProfileDerived {
     uint64_t *sort_key;        // [Epad] scratch
     int32_t *n_cand;           // [1]
     int64_t *qminmax;          // [4] waiting min,max, running min,max over candidates
+    // random pickers only (nullptr otherwise): the candidates in ascending slot order, and over them the prefix sums of
+    // the weighted-random masses of their bases (pick_random.cuh) and the prefix counts of +inf bases
+    uint32_t *cands;           // [E]
+    double *wcum;              // [E + 1]
+    uint32_t *icum;            // [E + 1]
 };
 // [shard_begin, shard_end): only these slots become candidates (queue min/max still span the whole pool).
 // A no-hit-lru scorer gets its warm score 0.5 here (the cold set comes from launch_pool_order).
@@ -137,6 +142,7 @@ cudaError_t launch_pool_prepare(const PoolArrays &pool, const epp_profile_cfg &p
 // The contribution rows, base sums, (base desc, slot asc) order and groups of d over d.cand / d.n_cand / d.qminmax (already
 // derived), with the raw no-hit-lru score of slot e = nohit_col[e] (nullptr: the warm 0.5).  gate != nullptr: every kernel
 // returns at once unless *gate != 0.
+// With d.wcum != nullptr (a random picker) also d.cands / d.wcum / d.icum.
 // (key asc, order asc) sort of Epad (a power of two) entries by one CTA; gate as below.
 cudaError_t launch_pool_sort(uint64_t *key, uint32_t *order, int32_t Epad, const int32_t *gate, cudaStream_t s);
 cudaError_t launch_pool_order(const PoolArrays &pool, const epp_profile_cfg &prof, const ProfileDerived &d, int32_t Epad,
@@ -179,6 +185,9 @@ struct ProfileDev {            // what the pick kernels read (device pointers + 
     const uint32_t *order;
     const uint32_t *grp_size;
     const int32_t *n_cand;
+    const uint32_t *cands;     // random pickers (cfg.picker != 0): ProfileDerived::cands / wcum / icum
+    const double *wcum;
+    const uint32_t *icum;
 };
 // no-hit-lru scorer (nohitlru/no_hit_lru.go): a profile whose bit is set in `mask` evaluates a cold request (no candidate
 // holds a block of its prompt) with cold[pi] -- the same candidates, with the LRU column in place of the warm 0.5 -- and
@@ -249,6 +258,8 @@ cudaError_t launch_match_pick(const PickParams &p, uint32_t *gscratch, int grid,
 // overflows it are appended to p.overflow_list for the dense-counter kernel).  8 warps per CTA, 6-8 CTAs per SM;
 // ctas = 6 bounds the one-profile lowest-slot build to 40 registers instead of 32 (the engine's EPP_MATCH_CTAS).
 cudaError_t launch_match_pick_sparse(const PickParams &p, int sm_count, int ctas, cudaStream_t s, int *launches);
+// Does some profile of the launch have a random picker?  Then the sparse and small-batch paths launch their _rand builds.
+bool any_random_picker(const PickParams &p);
 // cycle_small.cu: a1-a14 of a small host batch in ONE launch, one CTA per request, prompts read from and decisions
 // written to PINNED HOST memory (zero-copy); flags[r] = epoch (| 0x80000000 when the request overflowed the sparse map and
 // was appended to pp.overflow_list instead of being decided) is written last, after a system-scope fence.

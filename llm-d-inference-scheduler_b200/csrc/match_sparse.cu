@@ -15,7 +15,8 @@ constexpr int kWarps = 8;
 // cached prefixes are busy, instead of the launch ending on the warps whose fixed share happened to be costliest.  The
 // ticket is taken once the current request's probes are done, so the atomic's latency hides behind its scoring.
 // kNoHit: the no-hit-lru builds (match_sparse.cuh match_request), launched as k_match_pick_sparse_nohit.
-template <bool kSharded, bool kTie, int kStages, bool kNoHit>
+// kRand: the random-picker build (k_match_pick_sparse_rand).
+template <bool kSharded, bool kTie, int kStages, bool kNoHit, bool kRand = false>
 __device__ __forceinline__ void match_pick_sparse(const PickParams &p) {
     __shared__ sparse::Work s_work[kWarps];           // when counting
     const int lane = threadIdx.x & 31;
@@ -31,7 +32,7 @@ __device__ __forceinline__ void match_pick_sparse(const PickParams &p) {
     uint32_t r = blockIdx.x * kWarps + warp;
     while (r < R) {
         int32_t ticket = 0;
-        sparse::match_request<false, kSharded, kTie, kStages, sparse::NoFollow, kNoHit>(p, r, lane, counting, wk, p.req_next, ticket);
+        sparse::match_request<false, kSharded, kTie, kStages, sparse::NoFollow, kNoHit, kRand>(p, r, lane, counting, wk, p.req_next, ticket);
         r = nwarps + (uint32_t)__shfl_sync(0xffffffffu, ticket, 0);
     }
     if (counting) {
@@ -51,6 +52,11 @@ __global__ void __launch_bounds__(kWarps * 32, MINCTA) k_match_pick_sparse(PickP
 template <int MINCTA, bool kTie, int kStages>
 __global__ void __launch_bounds__(kWarps * 32, MINCTA) k_match_pick_sparse_nohit(PickParams p) {
     match_pick_sparse<false, kTie, kStages, true>(p);
+}
+// Engines where some profile has a random picker: one build for every handler shape, tie rule and no-hit-lru setting
+// (each is a run-time branch here: nohit_select reads a zero mask as "no scorer").
+__global__ void __launch_bounds__(kWarps * 32, 6) k_match_pick_sparse_rand(PickParams p) {
+    match_pick_sparse<false, true, 3, true, true>(p);
 }
 
 namespace {
@@ -80,6 +86,13 @@ cudaError_t launch_nohit(const PickParams &p, int sm_count, cudaStream_t s) {
 }
 }  // namespace
 
+bool any_random_picker(const PickParams &p) {
+    const int np = p.encode_on ? 3 : (p.n_profiles >= 2 ? 2 : 1);
+    for (int i = 0; i < np; i++)
+        if (p.prof[i].cfg.picker) return true;
+    return false;
+}
+
 cudaError_t launch_match_pick_sparse(const PickParams &p, int sm_count, int ctas, cudaStream_t s, int *launches) {
     if (p.R <= 0) return cudaSuccess;
     if (!p.req_next || p.R > INT32_MAX) return cudaErrorInvalidValue;
@@ -89,6 +102,7 @@ cudaError_t launch_match_pick_sparse(const PickParams &p, int sm_count, int ctas
     // the hot configuration (one profile, lowest-slot ties) gets the 32-register build; the variants that carry more
     // code (stages, tie rule, sharding) keep 40 registers
     if (p.global_masks) e = launch_one<6, true, false, 1>(p, sm_count, s);
+    else if (any_random_picker(p)) e = launch_kernel<k_match_pick_sparse_rand>(p, sm_count, s);
     else if (p.nohit.mask) {
         if (stages == 1) e = tie ? launch_nohit<true, 1>(p, sm_count, s) : launch_nohit<false, 1>(p, sm_count, s);
         else if (stages == 2) e = tie ? launch_nohit<true, 2>(p, sm_count, s) : launch_nohit<false, 2>(p, sm_count, s);

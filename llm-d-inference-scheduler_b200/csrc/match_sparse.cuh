@@ -22,6 +22,7 @@
 // PickParams::overflow_list and handled by the dense-counter kernel (pick_kernels.cu), never approximated.
 #pragma once
 #include "index.cuh"
+#include "pick_random.cuh"
 #include "score.cuh"
 
 namespace epp {
@@ -159,6 +160,64 @@ __device__ __forceinline__ Best eval_profile_lanes(const ProfileDev &pf, int32_t
     return b;
 }
 
+// One profile with a random picker (include/epp_engine.h "Random pickers"): the explicit candidates are the map's (matched
+// endpoints and lora-affinity entries), at most 32.  Each lane finds its entry's rank in slot order and its position among
+// the candidates (one binary search per lane, in parallel); the fold then walks the items and the gaps between them in
+// warp-uniform steps, and a pick inside a gap costs one binary search over wcum.  Kept out of line: the builds that carry
+// it are launched only for engines with a random picker.
+static __device__ __noinline__ Best eval_random_lanes(const ProfileDev &pf, int32_t E, const LaneMap &m, int32_t total,
+                                                      int lane, const LoraDev &lora, int lora_st, uint64_t seed,
+                                                      uint64_t key) {
+    Best b;
+    best_init(b);
+    const uint32_t n = (uint32_t)*pf.n_cand;
+    if (n == 0) return b;
+    const double u = rnd::pick_u(seed, key);
+    const bool x = (uint32_t)lane < m.n && pf.cand[m.e];
+    const double s = x ? weighted_sum(pf, E, m.e, (int32_t)m.c, total, lora, lora_st) : 0.0;
+    uint32_t pick;
+    if (pf.cfg.picker == EPP_PICKER_RANDOM) {
+        pick = pf.cands[rnd::pick_rank(u, n)];
+    } else {
+        const double mass = x ? rnd::mass_of(s, rnd::mass_scale(pf.cfg)) : 0.0;
+        const bool inf = x && rnd::is_pinf(s);
+        const uint32_t xmask = __ballot_sync(kFull, x);
+        uint32_t rk = 0;                               // rank of my entry among the explicit ones, ascending slot
+        for (uint32_t j = 0; j < m.n; j++) {
+            const uint32_t ej = __shfl_sync(kFull, m.e, (int)j);
+            rk += ((xmask >> j) & 1u) && ej < m.e;
+        }
+        uint32_t pos = 0;                              // its position among the candidates
+        if (x) {
+            uint32_t lo = 0, hi = n;
+            while (lo < hi) {
+                const uint32_t mid = (lo + hi) >> 1;
+                if (pf.cands[mid] < m.e) lo = mid + 1; else hi = mid;
+            }
+            pos = lo;
+        }
+        const uint32_t nx = __popc(xmask);
+        auto feed = [&](rnd::Walker &w) {
+            for (uint32_t q = 0; q < nx && w.pick == rnd::kNone; q++) {
+                const int l = __ffs(__ballot_sync(kFull, x && rk == q)) - 1;
+                const uint32_t pl = __shfl_sync(kFull, pos, l);
+                const double ml = __shfl_sync(kFull, mass, l);
+                const bool il = __shfl_sync(kFull, (int)inf, l) != 0;
+                w.item(pl, ml, il, __shfl_sync(kFull, m.e, l));
+            }
+            w.finish(n);
+        };
+        pick = rnd::weighted_pick(pf, true, u, n, feed, [&](uint32_t r) { return pf.cands[r]; });
+    }
+    // the pick's score: its own weighted sum when it is an explicit entry, else its base
+    const uint32_t holder = __ballot_sync(kFull, x && m.e == pick);
+    const double hs = __shfl_sync(kFull, s, holder ? __ffs(holder) - 1 : 0);
+    b.val = holder ? hs : pf.base[pick];
+    b.pick = pick;
+    b.ties = n;
+    return b;
+}
+
 // Adds one chunk's postings to the lane map.  (cnt, w0..w4) = this lane's slot words, all zero when the block is
 // beyond the stop or absent.  Runs of lanes with identical words are added at once.
 __device__ __forceinline__ void count_chunk(LaneMap &m, const IndexView &ix, uint32_t cnt, uint32_t w0, uint32_t w1,
@@ -232,7 +291,8 @@ struct NoFollow {
 // the warp's next request, fetched while this one is scored).
 // kNoHit: a profile has a no-hit-lru scorer (PickParams::nohit): the lane map decides, with one ballot, whether the request
 // is cold for the profile, which selects the profile's warm or cold set (same candidates, different base / order / groups).
-template <bool kCg, bool kSharded, bool kTie, int kStages, typename Follow = NoFollow, bool kNoHit = false>
+// kRand: some profile has a random picker (epp_profile_cfg.picker): those profiles are decided by eval_random_lanes.
+template <bool kCg, bool kSharded, bool kTie, int kStages, typename Follow = NoFollow, bool kNoHit = false, bool kRand = false>
 __device__ __forceinline__ bool match_request(const PickParams &p, const uint32_t r, const int lane, const bool counting,
                                               Work *wk, int32_t *req_next, int32_t &ticket, const Follow fw = Follow()) {
     const uint32_t shard_lo = p.index.ep_begin, shard_hi = min(p.index.ep_end, (uint32_t)p.E);
@@ -337,11 +397,16 @@ __device__ __forceinline__ bool match_request(const PickParams &p, const uint32_
     bool cold = false;
     decide_stages<kStages>(p, r, total, (kStages >= 2 && p.n_profiles >= 2) ? ld_row<kCg>(p.in_len + r) : 0,
                   [&](int pi, uint64_t key) {
-                      if (!kNoHit) return eval_profile_lanes<kTie>(p.prof[pi], p.E, m, total, lane, p.lora, lora_st, p.tie_seed, key);
+                      if (!kNoHit) {
+                          if (kRand && p.prof[pi].cfg.picker)
+                              return eval_random_lanes(p.prof[pi], p.E, m, total, lane, p.lora, lora_st, p.tie_seed, key);
+                          return eval_profile_lanes<kTie>(p.prof[pi], p.E, m, total, lane, p.lora, lora_st, p.tie_seed, key);
+                      }
                       // a hit = a matched candidate with count > 0 (lora-affinity entries join the map with count 0)
                       const ProfileDev &pf = nohit_select(p, pi, cold, [&](const ProfileDev &w) {
                           return !__ballot_sync(kFull, (uint32_t)lane < m.n && m.c > 0 && w.cand[m.e]);
                       });
+                      if (kRand && pf.cfg.picker) return eval_random_lanes(pf, p.E, m, total, lane, p.lora, lora_st, p.tie_seed, key);
                       return eval_profile_lanes<kTie>(pf, p.E, m, total, lane, p.lora, lora_st, p.tie_seed, key);
                   },
                   [&](uint32_t e) { return m.n ? (int32_t)map_get(m, e) : 0; }, d, dd);

@@ -12,6 +12,7 @@
 #include <cfloat>
 #include <climits>
 
+#include "pick_random.cuh"
 #include "score.cuh"
 
 namespace epp {
@@ -111,7 +112,8 @@ __device__ inline double weighted_sum_over(const ProfileDev &pf, const GenView &
 
 // One profile for one request: filter chain, scores, and the first max(1, k) endpoints in picker order.  Returns the
 // record of the arg-max set (value, pick 0, set size); picks_row / scores_row (k entries, or nullptr) receive the list.
-template <typename CntOf>
+// kRand: some profile of the engine has a random picker (the max-score builds carry none of that code).
+template <bool kRand, typename CntOf>
 __device__ inline Best eval(const ProfileDev &pf, const GenView &g, int32_t E, int32_t total, int lane,
                             const LoraDev &lora, uint32_t adapter, uint64_t seed, uint64_t key, CntOf cnt_of,
                             int32_t k, uint32_t *picks_row, double *scores_row) {
@@ -130,6 +132,36 @@ __device__ inline Best eval(const ProfileDev &pf, const GenView &g, int32_t E, i
         const int st = use_lora ? lora_lookup(lora, adapter, e) : 0;
         return nm.sticky ? weighted_sum_over(pf, g, nm, e, c, total, lora, st) : weighted_sum(pf, E, e, c, total, lora, st);
     };
+    if (kRand && pf.cfg.picker) {     // random pickers: a narrowed set is all explicit, else the gaps of wcum
+        uint32_t n = 0;
+        for (uint32_t e0 = 0; e0 < (uint32_t)E; e0 += 32) {
+            const uint32_t e = e0 + lane;
+            n += __popc(__ballot_sync(kFull, e < (uint32_t)E && cand(e, cnt_of(e))));
+        }
+        // first k: successive draws without replacement, draw j with the seed tie_seed + j * kGolden; the endpoints
+        // already emitted stay in the sequence with mass 0 (lane l holds emitted #l and #l + 32)
+        uint32_t g0 = EPP_NO_ENDPOINT, g1 = EPP_NO_ENDPOINT;
+        for (int32_t j = 0; j < k && (uint32_t)j < n; j++) {
+            auto out_of = [&](uint32_t e) {
+                bool o = false;
+                for (int32_t t = 0; t < j; t++)
+                    o |= e == __shfl_sync(kFull, t < 32 ? g0 : g1, t & 31);
+                return o;
+            };
+            const Best b = rnd::draw_scan(pf, E, lane, !nm.sticky, n - (uint32_t)j, (uint32_t)j,
+                                          seed + (uint64_t)j * kGolden, key,
+                                          [&](uint32_t e) { return cand(e, cnt_of(e)); },
+                                          [&](uint32_t e) { return cnt_of(e) > 0 || (use_lora && lora_lookup(lora, adapter, e) != 0); },
+                                          [&](uint32_t e) { return score(e, cnt_of(e)); }, out_of);
+            if (j == 0) first = b;
+            if (lane == (j & 31)) { if (j < 32) g0 = b.pick; else g1 = b.pick; }
+            if (lane == 0) {
+                if (picks_row) picks_row[j] = b.pick;
+                if (scores_row) scores_row[j] = b.val;
+            }
+        }
+        return first;
+    }
     double v = 0.0;                   // score of the current group
     bool have_v = false;              // a group is open: the next one lies strictly below v (the first may be +inf)
     uint32_t n_rem = 0;               // its members not emitted yet

@@ -17,6 +17,7 @@
 
 #include "index.cuh"
 #include "pick_general.cuh"
+#include "pick_random.cuh"
 #include "score.cuh"
 
 namespace epp {
@@ -162,6 +163,50 @@ __global__ void k_pool_groups(const double *base, const uint32_t *order, const i
     for (int32_t i = k; i < end; i++) grp_size[i] = (uint32_t)(end - k);
 }
 
+// Random pickers (pick_random.cuh): the candidates in ascending slot order, and over them wcum[i] = the left fold (+0.0
+// first) of the weighted-random masses of the bases of cands[0 .. i), icum[i] = how many of those bases are +inf.  One
+// CTA: each chunk of 1024 slots is compacted by the block, then one thread folds it in order (the fold is sequential by
+// definition: round-to-nearest addition is not associative).
+__global__ void __launch_bounds__(1024) k_pool_cum(const uint8_t *cand, const double *base, int32_t E, epp_profile_cfg cfg,
+                                                   uint32_t *cands, double *wcum, uint32_t *icum, const int32_t *gate) {
+    if (gate && !*gate) return;
+    __shared__ double s_m[1024];
+    __shared__ uint8_t s_inf[1024];
+    __shared__ uint32_t s_wc[32];
+    const double sigma = rnd::mass_scale(cfg);
+    const int t = threadIdx.x, lane = t & 31, w = t >> 5;
+    uint32_t q = 0;                                   // candidates before the chunk (every thread keeps the same count)
+    double acc = 0.0;                                 // thread 0: wcum[q]
+    uint32_t ic = 0;                                  // thread 0: icum[q]
+    if (t == 0) { wcum[0] = 0.0; icum[0] = 0; }
+    for (int32_t e0 = 0; e0 < E; e0 += 1024) {
+        const int32_t e = e0 + t;
+        const bool c = e < E && cand[e];
+        const uint32_t bal = __ballot_sync(0xffffffffu, c);
+        if (lane == 0) s_wc[w] = __popc(bal);
+        __syncthreads();
+        uint32_t before = 0, nc = 0;
+        for (int i = 0; i < 32; i++) { if (i < w) before += s_wc[i]; nc += s_wc[i]; }
+        if (c) {
+            const uint32_t pos = before + __popc(bal & ((1u << lane) - 1u));
+            const double b = base[e];
+            s_m[pos] = rnd::mass_of(b, sigma);
+            s_inf[pos] = rnd::is_pinf(b) ? 1 : 0;
+            cands[q + pos] = (uint32_t)e;
+        }
+        __syncthreads();
+        if (t == 0)
+            for (uint32_t i = 0; i < nc; i++) {
+                acc = __dadd_rn(acc, s_m[i]);
+                ic += s_inf[i];
+                wcum[q + i + 1] = acc;
+                icum[q + i + 1] = ic;
+            }
+        q += nc;
+        __syncthreads();
+    }
+}
+
 cudaError_t launch_pool_sort(uint64_t *key, uint32_t *order, int32_t Epad, const int32_t *gate, cudaStream_t s) {
     k_pool_sort<<<1, 1024, 0, s>>>(key, order, Epad, gate);
     return cudaGetLastError();
@@ -174,6 +219,10 @@ cudaError_t launch_pool_order(const PoolArrays &pool, const epp_profile_cfg &pro
     k_pool_sort<<<1, 1024, 0, s>>>(d.sort_key, d.order, Epad, gate);
     k_pool_groups<<<(pool.E + 255) / 256, 256, 0, s>>>(d.base, d.order, d.n_cand, d.grp_size, gate);
     if (launches) *launches += 3;
+    if (d.wcum) {
+        k_pool_cum<<<1, 1024, 0, s>>>(d.cand, d.base, pool.E, prof, d.cands, d.wcum, d.icum, gate);
+        if (launches) *launches += 1;
+    }
     return cudaGetLastError();
 }
 
@@ -206,9 +255,22 @@ __device__ inline Best eval_profile_inner(const ProfileDev &pf, int32_t E, const
                                           uint32_t nl, int32_t total, int lane, const LoraDev &lora, uint32_t adapter);
 
 // + the tie rule (score.cuh): the member of rank k of the arg-max set, found by one more scan over the slots
+template <bool kRand>
 __device__ inline Best eval_profile(const ProfileDev &pf, int32_t E, const uint32_t *cnt32, const uint32_t *list,
                                     uint32_t nl, int32_t total, int lane, const LoraDev &lora, uint32_t adapter,
                                     uint64_t tie_seed, uint64_t tie_key) {
+    if (kRand && pf.cfg.picker) {                     // random pickers: explicit = matched or lora-resident candidates
+        const bool use_lora = lora.enabled && lora.ptr;
+        return rnd::draw_scan(pf, E, lane, true, (uint32_t)*pf.n_cand, 0u, tie_seed, tie_key,
+                              [&](uint32_t e) { return pf.cand[e] != 0; },
+                              [&](uint32_t e) { return cnt_get(cnt32, e) > 0 || (use_lora && lora_lookup(lora, adapter, e) != 0); },
+                              [&](uint32_t e) {
+                                  const uint32_t c = cnt_get(cnt32, e);
+                                  if (use_lora) return weighted_sum(pf, E, e, (int32_t)c, total, lora, lora_lookup(lora, adapter, e));
+                                  return c ? weighted_sum(pf, E, e, (int32_t)c, total) : pf.base[e];
+                              },
+                              [](uint32_t) { return false; });
+    }
     Best b = eval_profile_inner(pf, E, cnt32, list, nl, total, lane, lora, adapter);
     if (tie_seed && b.ties > 1) {
         const bool use_lora = lora.enabled && lora.ptr;
@@ -275,7 +337,7 @@ __device__ inline Best eval_profile_inner(const ProfileDev &pf, int32_t E, const
 
 // gen::eval for profile pi of request r, with the request's top-k rows (all rows are reset first: a stage that does
 // not run leaves EPP_NO_ENDPOINT).
-template <typename P, typename CntOf>
+template <bool kRand, typename P, typename CntOf>
 __device__ inline Best gen_eval_profile(const P &p, const ProfileDev &pf, int pi, int64_t r, int32_t total, int lane,
                                         uint32_t adapter, uint64_t key, CntOf cnt_of) {
     const int32_t k = p.gen.topk > 1 ? p.gen.topk : 1;
@@ -284,13 +346,14 @@ __device__ inline Best gen_eval_profile(const P &p, const ProfileDev &pf, int pi
             if (p.gen.topk_picks[q]) for (int j = lane; j < k; j += 32) p.gen.topk_picks[q][r * k + j] = EPP_NO_ENDPOINT;
         __syncwarp();
     }
-    return gen::eval(pf, p.gen, p.E, total, lane, p.lora, adapter, p.tie_seed, key, cnt_of, k,
+    return gen::eval<kRand>(pf, p.gen, p.E, total, lane, p.lora, adapter, p.tie_seed, key, cnt_of, k,
                      (k > 1 && p.gen.topk_picks[pi]) ? p.gen.topk_picks[pi] + r * k : nullptr,
                      (k > 1 && pi == 0 && p.gen.topk_scores) ? p.gen.topk_scores + r * k : nullptr);
 }
 
-__global__ void __launch_bounds__(kPickWarps * 32) k_match_pick(PickParams p, int32_t cnt_words,
-                                                                uint32_t *gscratch) {
+// kRand: the engine has a random picker (k_match_pick_rand); the max-score build carries none of its code.
+template <bool kRand>
+__device__ __forceinline__ void match_pick_dense(const PickParams &p, int32_t cnt_words, uint32_t *gscratch) {
     extern __shared__ uint32_t smem[];
     const int lane = threadIdx.x & 31;
     const int warp = threadIdx.x >> 5;
@@ -370,11 +433,11 @@ __global__ void __launch_bounds__(kPickWarps * 32) k_match_pick(PickParams p, in
         auto is_cold = [&](const ProfileDev &pf) { return cold_scan(pf, p.E, lane, cnt_of); };
         if (p.gen.on) {       // affinity filter / top-k: full-scan evaluation (pick_general.cuh)
             decide_stages<3>(p, r, total, p.n_profiles >= 2 ? p.in_len[r] : 0,
-                          [&](int pi, uint64_t key) { return gen_eval_profile(p, nohit_select(p, pi, cold, is_cold), pi, r, total, lane, adapter, key, cnt_of); },
+                          [&](int pi, uint64_t key) { return gen_eval_profile<kRand>(p, nohit_select(p, pi, cold, is_cold), pi, r, total, lane, adapter, key, cnt_of); },
                           cnt_of, d, dd);
         } else {
             decide_stages<3>(p, r, total, p.n_profiles >= 2 ? p.in_len[r] : 0,
-                          [&](int pi, uint64_t key) { return eval_profile(nohit_select(p, pi, cold, is_cold), p.E, cnt32, list, nl, total, lane, p.lora, adapter, p.tie_seed, key); },
+                          [&](int pi, uint64_t key) { return eval_profile<kRand>(nohit_select(p, pi, cold, is_cold), p.E, cnt32, list, nl, total, lane, p.lora, adapter, p.tie_seed, key); },
                           cnt_of, d, dd);
         }
         if (lane == 0 && p.nohit.cold_out) p.nohit.cold_out[r] = cold ? 1 : 0;
@@ -418,6 +481,13 @@ __global__ void __launch_bounds__(kPickWarps * 32) k_match_pick(PickParams p, in
     }
 }
 
+__global__ void __launch_bounds__(kPickWarps * 32) k_match_pick(PickParams p, int32_t cnt_words, uint32_t *gscratch) {
+    match_pick_dense<false>(p, cnt_words, gscratch);
+}
+__global__ void __launch_bounds__(kPickWarps * 32) k_match_pick_rand(PickParams p, int32_t cnt_words, uint32_t *gscratch) {
+    match_pick_dense<true>(p, cnt_words, gscratch);
+}
+
 // The engine allocates gscratch when E does not fit in shared memory; see engine.cu.
 size_t match_pick_smem_bytes(int32_t E, bool global_counts) {
     int32_t cnt_words = (E + 1) / 2;
@@ -433,11 +503,13 @@ cudaError_t launch_match_pick(const PickParams &p, uint32_t *gscratch, int grid,
     static bool attr_set[64] = {};                 // function attributes are per device: engines of one process may sit on several GPUs
     if (!attr_set[dev & 63]) {
         cudaError_t e = cudaFuncSetAttribute(k_match_pick, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(k_match_pick_rand, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
         if (e != cudaSuccess) return e;
         attr_set[dev & 63] = true;
     }
     int32_t cnt_words = (p.E + 1) / 2;
-    k_match_pick<<<grid, kPickWarps * 32, smem, s>>>(p, cnt_words, gscratch);
+    if (any_random_picker(p)) k_match_pick_rand<<<grid, kPickWarps * 32, smem, s>>>(p, cnt_words, gscratch);
+    else k_match_pick<<<grid, kPickWarps * 32, smem, s>>>(p, cnt_words, gscratch);
     if (launches) *launches += 1;
     return cudaGetLastError();
 }
@@ -445,6 +517,7 @@ cudaError_t launch_match_pick(const PickParams &p, uint32_t *gscratch, int grid,
 // ------------------------------------------------------------------------------------------------
 // decision logic on injected dense match info (KAT / plugin-parity mode)
 // ------------------------------------------------------------------------------------------------
+template <bool kRand>
 __device__ inline Best eval_profile_dense(const ProfileDev &pf, int32_t E, const int32_t *mrow, int32_t total,
                                           int lane, const LoraDev &lora, uint32_t adapter, uint64_t tie_seed,
                                           uint64_t tie_key) {
@@ -454,6 +527,11 @@ __device__ inline Best eval_profile_dense(const ProfileDev &pf, int32_t E, const
     auto score_of = [&](uint32_t e) {
         return weighted_sum(pf, E, e, mrow[e], total, lora, use_lora ? lora_lookup(lora, adapter, e) : 0);
     };
+    if (kRand && pf.cfg.picker)
+        return rnd::draw_scan(pf, E, lane, true, (uint32_t)*pf.n_cand, 0u, tie_seed, tie_key,
+                              [&](uint32_t e) { return pf.cand[e] != 0; },
+                              [&](uint32_t e) { return mrow[e] > 0 || (use_lora && lora_lookup(lora, adapter, e) != 0); }, score_of,
+                              [](uint32_t) { return false; });
     for (uint32_t e = lane; e < (uint32_t)E; e += 32) {
         if (!pf.cand[e]) continue;
         best_add(b, score_of(e), e);
@@ -463,7 +541,8 @@ __device__ inline Best eval_profile_dense(const ProfileDev &pf, int32_t E, const
     return b;
 }
 
-__global__ void __launch_bounds__(256) k_dense_pick(DensePickParams p) {
+template <bool kRand>
+__device__ __forceinline__ void dense_pick(const DensePickParams &p) {
     const int lane = threadIdx.x & 31;
     const int64_t r = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (r >= p.R) return;
@@ -477,11 +556,11 @@ __global__ void __launch_bounds__(256) k_dense_pick(DensePickParams p) {
     auto is_cold = [&](const ProfileDev &pf) { return cold_scan(pf, p.E, lane, cnt_of); };
     if (p.gen.on) {
         decide_stages<3>(p, r, total, p.in_len ? p.in_len[r] : 0,
-                      [&](int pi, uint64_t key) { return gen_eval_profile(p, nohit_select(p, pi, cold, is_cold), pi, r, total, lane, adapter, key, cnt_of); },
+                      [&](int pi, uint64_t key) { return gen_eval_profile<kRand>(p, nohit_select(p, pi, cold, is_cold), pi, r, total, lane, adapter, key, cnt_of); },
                       cnt_of, d, dd);
     } else {
         decide_stages<3>(p, r, total, p.in_len ? p.in_len[r] : 0,
-                      [&](int pi, uint64_t key) { return eval_profile_dense(nohit_select(p, pi, cold, is_cold), p.E, mrow, total, lane, p.lora, adapter, p.tie_seed, key); },
+                      [&](int pi, uint64_t key) { return eval_profile_dense<kRand>(nohit_select(p, pi, cold, is_cold), p.E, mrow, total, lane, p.lora, adapter, p.tie_seed, key); },
                       cnt_of, d, dd);
     }
     if (lane == 0 && p.nohit.cold_out) p.nohit.cold_out[r] = cold ? 1 : 0;
@@ -491,10 +570,17 @@ __global__ void __launch_bounds__(256) k_dense_pick(DensePickParams p) {
     }
 }
 
+__global__ void __launch_bounds__(256) k_dense_pick(DensePickParams p) { dense_pick<false>(p); }
+__global__ void __launch_bounds__(256) k_dense_pick_rand(DensePickParams p) { dense_pick<true>(p); }
+
 cudaError_t launch_dense_pick(const DensePickParams &p, cudaStream_t s, int *launches) {
     if (p.R <= 0) return cudaSuccess;
     int64_t threads = p.R * 32;
-    k_dense_pick<<<(unsigned)((threads + 255) / 256), 256, 0, s>>>(p);
+    const int np = p.encode_on ? 3 : (p.n_profiles >= 2 ? 2 : 1);
+    bool rand = false;
+    for (int i = 0; i < np; i++) rand |= p.prof[i].cfg.picker != EPP_PICKER_MAX_SCORE;
+    if (rand) k_dense_pick_rand<<<(unsigned)((threads + 255) / 256), 256, 0, s>>>(p);
+    else k_dense_pick<<<(unsigned)((threads + 255) / 256), 256, 0, s>>>(p);
     if (launches) *launches += 1;
     return cudaGetLastError();
 }

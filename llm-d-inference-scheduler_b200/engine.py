@@ -47,10 +47,12 @@ class AffinityFilterSpec:
 
 @dataclass
 class ProfileSpec:
-    """One SchedulerProfile: role filter -> [prefix-cache-affinity-filter] -> scorers in order -> max-score picker."""
+    """One SchedulerProfile: role filter -> [prefix-cache-affinity-filter] -> scorers in order -> picker
+    (capi.PICKER_MAX_SCORE / PICKER_RANDOM / PICKER_WEIGHTED_RANDOM)."""
     filter: int = capi.FILTER_NONE
     scorers: list = field(default_factory=list)
     affinity: AffinityFilterSpec | None = None
+    picker: int = capi.PICKER_MAX_SCORE
 
 
 def _fill_profile(dst: capi.ProfileCfg, spec: ProfileSpec):
@@ -67,6 +69,7 @@ def _fill_profile(dst: capi.ProfileCfg, spec: ProfileSpec):
         dst.scorers[i].column = s.column
         dst.scorers[i].param2 = s.param2
     dst.ttft_column = -1
+    dst.picker = spec.picker
     if spec.affinity is not None:
         a = spec.affinity
         dst.affinity_threshold, dst.exploration_probability = a.affinity_threshold, a.exploration_probability

@@ -207,6 +207,32 @@ def NewMaxScorePicker(maxNumOfEndpoints: int = 1):
     return MaxScorePicker(maxNumOfEndpoints)
 
 
+@dataclass
+class RandomPicker:                              # picker/random; draw: include/epp_engine.h "Random pickers"
+    maxNumOfEndpoints: int = 1
+
+
+def NewRandomPicker(maxNumOfEndpoints: int = 1):
+    if maxNumOfEndpoints <= 0:                   # random/picker.go:65-67
+        maxNumOfEndpoints = 1
+    return RandomPicker(maxNumOfEndpoints)
+
+
+@dataclass
+class WeightedRandomPicker:                      # picker/weightedrandom; P(endpoint) = score+ / sum of scores+
+    maxNumOfEndpoints: int = 1
+
+
+def NewWeightedRandomPicker(maxNumOfEndpoints: int = 1):
+    if maxNumOfEndpoints <= 0:                   # weightedrandom/picker.go:67-69
+        maxNumOfEndpoints = 1
+    return WeightedRandomPicker(maxNumOfEndpoints)
+
+
+_PICKER_KIND = {MaxScorePicker: capi.PICKER_MAX_SCORE, RandomPicker: capi.PICKER_RANDOM,
+                WeightedRandomPicker: capi.PICKER_WEIGHTED_RANDOM}
+
+
 class SchedulerProfile:
     def __init__(self):
         self.filters: list = []
@@ -232,11 +258,12 @@ class SchedulerProfile:
                 self.scorers.append(p)
             elif isinstance(p, (_RoleFilter, PrefixCacheAffinityFilter)):
                 self.filters.append(p)
-            elif isinstance(p, MaxScorePicker):
+            elif isinstance(p, (MaxScorePicker, RandomPicker, WeightedRandomPicker)):
                 self.picker = p
         return None
 
     def WithPicker(self, picker):
+        assert type(picker) in _PICKER_KIND, "the pickers are MaxScorePicker, RandomPicker and WeightedRandomPicker"
         self.picker = picker
         return self
 
@@ -247,7 +274,8 @@ class SchedulerProfile:
                            [ScorerSpec(ws.scorer.kind, ws.weight, ws.scorer.param, ws.scorer.column, ws.scorer.param2)
                             for ws in self.scorers],
                            AffinityFilterSpec(aff[0].affinityThreshold, aff[0].explorationProbability,
-                                              aff[0].maxTTFTPenaltyMs, aff[0].ttft_column) if aff else None)
+                                              aff[0].maxTTFTPenaltyMs, aff[0].ttft_column) if aff else None,
+                           _PICKER_KIND[type(self.picker)])
 
 
 def NewSchedulerProfile():
