@@ -78,6 +78,9 @@ type Config struct {
 	Encode               *ProfileSpec // non-nil (with Prefill): encode stage for multimodal requests
 	MaxBatch             int          // micro-batcher: requests per flush at most
 	MaxDelayMicros       int          // ... and how long the oldest request of a batch may wait
+	// InFlightLoad runs the inflight-load-producer on the device: every Schedule adds its targets' load, the
+	// InFlightLoadProducer (plugins.go) releases it, and the token-load / active-request scorers read it (Column ignored)
+	InFlightLoad bool
 }
 
 // Engine owns one epp_engine + its micro-batcher and the endpoint-name <-> slot-id table.
@@ -93,6 +96,7 @@ type Engine struct {
 	models map[string]uint32 // TargetModel (+ cache salt) -> epp_model_register id
 
 	inflight sync.WaitGroup // Schedule calls inside epp_submit / epp_wait (Close waits for them)
+	loads    sync.Map       // *scheduling.InferenceRequest -> inflightEntry, with Config.InFlightLoad (plugins.go)
 }
 
 func lastError() error { return errors.New(C.GoString(C.epp_last_error())) }
@@ -146,6 +150,9 @@ func New(cfg Config) (*Engine, error) {
 		c.pick_k = C.int32_t(cfg.PickK)
 	}
 	c.index_commit_interval_us = C.int32_t(cfg.IndexCommitMicros)
+	if cfg.InFlightLoad {
+		c.inflight_load = 1
+	}
 	if err := fillProfile(&c.primary, cfg.Primary); err != nil {
 		return nil, err
 	}
@@ -253,7 +260,8 @@ func roleOf(labels map[string]string) C.uint8_t {
 
 // SetPool replaces the pool-state snapshot (called by the 50 ms scrape loop with Datastore.PodList()).  Endpoints
 // that left the pool lose their slot: their index entries are removed ON THE DEVICE before the slot can be handed
-// to another endpoint (RemovePod, indexer.go:167-182), both under the same lock.
+// to another endpoint (RemovePod, indexer.go:167-182), both under the same lock.  With InFlightLoad their in-flight
+// counters are reset there too (the producer's endpoint-delete event, producer.go:86-97).
 func (e *Engine) SetPool(pods []fwkdl.Endpoint) error {
 	e.mu.Lock()
 	defer e.mu.Unlock()
@@ -265,6 +273,12 @@ func (e *Engine) SetPool(pods []fwkdl.Endpoint) error {
 		if !seen[name] {
 			if rc := C.epp_index_remove_endpoint(e.h, C.uint32_t(slot)); rc != C.EPP_OK {
 				return fmt.Errorf("eppcuda: epp_index_remove_endpoint: %w", lastError())
+			}
+			if e.cfg.InFlightLoad {
+				s := C.uint32_t(slot)
+				if rc := C.epp_inflight_reset(e.h, 1, &s); rc != C.EPP_OK {
+					return fmt.Errorf("eppcuda: epp_inflight_reset: %w", lastError())
+				}
 			}
 			delete(e.slotOf, name)
 			e.nameOf[slot] = types.NamespacedName{}
@@ -319,6 +333,22 @@ type Decision struct {
 }
 
 const NoEndpoint = uint32(C.EPP_NO_ENDPOINT)
+
+// InFlightRelease takes one request and the token estimate of a promptLen-byte prompt off each slot
+// (epp_inflight_release: ResponseBody of the inflight-load-producer).  NoEndpoint entries are skipped.  No CUDA call.
+func (e *Engine) InFlightRelease(slots []uint32, promptLen uint64) error {
+	if len(slots) == 0 {
+		return nil
+	}
+	lens := make([]C.uint64_t, len(slots))
+	for i := range lens {
+		lens[i] = C.uint64_t(promptLen)
+	}
+	if rc := C.epp_inflight_release(e.h, C.int32_t(len(slots)), (*C.uint32_t)(unsafe.Pointer(&slots[0])), &lens[0]); rc != C.EPP_OK {
+		return fmt.Errorf("eppcuda: epp_inflight_release: %w", lastError())
+	}
+	return nil
+}
 
 // schedule = epp_submit + epp_wait for ONE request.  prompt is read during the submit call only (the library copies
 // the bytes it hashes into its pinned staging buffer).

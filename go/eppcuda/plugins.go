@@ -11,6 +11,7 @@ import (
 	"errors"
 	"unsafe"
 
+	fwkdl "github.com/llm-d/llm-d-router/pkg/epp/framework/interface/datalayer"
 	"github.com/llm-d/llm-d-router/pkg/epp/framework/interface/plugin"
 	fwkrc "github.com/llm-d/llm-d-router/pkg/epp/framework/interface/requestcontrol"
 	"github.com/llm-d/llm-d-router/pkg/epp/framework/interface/scheduling"
@@ -50,6 +51,93 @@ func Register(e *Engine) {
 		}
 		return &WeightedScorer{name: name, e: shared, profile: p.Profile, scorer: p.Scorer}, nil
 	})
+	plugin.Register(InFlightLoadProducerType, func(name string, _ json.RawMessage, _ plugin.Handle) (plugin.Plugin, error) {
+		if shared == nil {
+			return nil, errors.New("eppcuda: engine not created")
+		}
+		if !shared.cfg.InFlightLoad {
+			return nil, errors.New("eppcuda: the engine was created without Config.InFlightLoad")
+		}
+		return &InFlightLoadProducer{name: name, e: shared}, nil
+	})
+}
+
+// InFlightLoadProducerType is the reference's plugin type of the in-flight load producer
+// (requestcontrol/dataproducer/inflightload/producer.go).
+const InFlightLoadProducerType = "inflight-load-producer"
+
+// inflightEntry is what Scheduler.Schedule stashes per request for the producer's release: the prefill target, the
+// other targets (decode / primary, encode) and the prompt length the engine's token estimate was made from.
+type inflightEntry struct {
+	promptLen uint64
+	prefill   uint32
+	others    []uint32
+}
+
+// InFlightLoadProducer implements requestcontrol.ResponseBodyProcessor (plugins.go:62-65).  Its PreRequest runs inside
+// the engine (every Schedule adds its targets' load on the device) and its endpoint-delete hook inside Engine.SetPool;
+// ResponseBody releases the load the way producer.go:131-168 does: the prefill target at the first chunk, the others at
+// the end of the stream.  The token estimate reads the prompt length, where the reference reads the request body size.
+type InFlightLoadProducer struct {
+	name string
+	e    *Engine
+}
+
+var _ fwkrc.ResponseBodyProcessor = (*InFlightLoadProducer)(nil)
+
+func (p *InFlightLoadProducer) TypedName() plugin.TypedName {
+	return plugin.TypedName{Type: InFlightLoadProducerType, Name: p.name}
+}
+
+func (p *InFlightLoadProducer) ResponseBody(_ context.Context, request *scheduling.InferenceRequest, resp *fwkrc.Response,
+	_ *fwkdl.EndpointMetadata) {
+	if request == nil || resp == nil {
+		return
+	}
+	v, ok := p.e.loads.Load(request)
+	if !ok {
+		return
+	}
+	ent := v.(inflightEntry)
+	if resp.StartOfStream {
+		_ = p.e.InFlightRelease([]uint32{ent.prefill}, ent.promptLen)
+	}
+	if resp.EndOfStream {
+		p.e.loads.Delete(request)
+		_ = p.e.InFlightRelease(ent.others, ent.promptLen)
+	}
+}
+
+// TokenLoadScorer turns the parameters of a "token-load-scorer" entry (tokenload.Config: queueThresholdTokens, <= 0
+// means 4194304) into the engine's scorer.  With Config.InFlightLoad it reads the engine's counters.
+func TokenLoadScorer(weight float64, params json.RawMessage) (ScorerSpec, error) {
+	var p struct {
+		QueueThresholdTokens int64 `json:"queueThresholdTokens"`
+	}
+	if len(params) > 0 {
+		if err := json.Unmarshal(params, &p); err != nil {
+			return ScorerSpec{}, err
+		}
+	}
+	return ScorerSpec{Kind: int(C.EPP_SCORER_TOKEN_LOAD), Weight: weight, Param: float64(p.QueueThresholdTokens)}, nil
+}
+
+// ActiveRequestScorer turns the parameters of an "active-request-scorer" entry (activerequest.Parameters: idleThreshold,
+// maxBusyScore with default 1.0; requestTimeout is accepted and ignored, the producer's release ends a request) into the
+// engine's scorer.  With Config.InFlightLoad it reads the engine's counters.
+func ActiveRequestScorer(weight float64, params json.RawMessage) (ScorerSpec, error) {
+	p := struct {
+		RequestTimeout string  `json:"requestTimeout"`
+		IdleThreshold  int     `json:"idleThreshold"`
+		MaxBusyScore   float64 `json:"maxBusyScore"`
+	}{MaxBusyScore: 1.0}
+	if len(params) > 0 {
+		if err := json.Unmarshal(params, &p); err != nil {
+			return ScorerSpec{}, err
+		}
+	}
+	return ScorerSpec{Kind: int(C.EPP_SCORER_ACTIVE_REQUEST), Weight: weight, Param: p.MaxBusyScore,
+		Param2: float64(p.IdleThreshold)}, nil
 }
 
 // NoHitLRUType is the reference's plugin type of the no-hit-lru scorer (scorer/nohitlru/no_hit_lru.go).

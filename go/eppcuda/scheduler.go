@@ -103,6 +103,12 @@ func (s *Scheduler) Schedule(ctx context.Context, request *scheduling.InferenceR
 	put(s.Names.Primary, d.Pick, d.Primary)
 	put(s.Names.Prefill, d.PrefillPick, d.Prefill)
 	put(s.Names.Encode, d.EncodePick, d.Encode)
+	if s.Engine.cfg.InFlightLoad {
+		// the engine already added the load of every target (PreRequest); the InFlightLoadProducer releases these
+		// slots when the response comes back
+		s.Engine.loads.Store(request, inflightEntry{promptLen: uint64(len(prompt)), prefill: d.PrefillPick,
+			others: []uint32{d.Pick, d.EncodePick}})
+	}
 	if _, ok := res.ProfileResults[s.Names.Primary]; !ok {
 		return nil, errors.New("failed to find available decode workers") // the pick left the pool since the snapshot
 	}

@@ -29,7 +29,23 @@
  * are applied between batches.  The same holds for the no-hit-lru scorer's LRU: every scheduling call (epp_schedule[_topk],
  * epp_schedule_with_match[_topk], the micro-batcher's flushes) scores against the LRU as it stood when the call started
  * and then applies its cold requests' Adds in request order (on the device, in enqueue order for async batches), so cold
- * requests inside one batch do not rotate; epp_score, epp_prefix_match and epp_hash_prompts never update it.
+ * requests inside one batch do not rotate; epp_score, epp_prefix_match and epp_hash_prompts never update it.  The same
+ * holds for the in-flight counters of the inflight-load producer (below).
+ *
+ * In-flight load (epp_config.inflight_load = 1; the inflight-load-producer, requestcontrol/dataproducer/inflightload/
+ * producer.go): the engine keeps per slot the InFlightLoad{Requests, Tokens} that the token-load and active-request
+ * scorers read, as int64 counters on the device.  Negative counts are kept (a release on a slot reset since its add).
+ *   PreRequest (:110-129): every scheduling call, after its last pick, adds for every request with status 0 one request
+ *       and est(L) tokens to each stage that ran and found an endpoint: pick, prefill_pick and the encode pick (only
+ *       entry 0 of a first-k list; the same slot picked by two stages counts twice).  Status -1 requests add nothing.
+ *       The call scores against the counters as they stood when it started (frozen snapshot, like the no-hit-lru LRU);
+ *       async batches apply their adds in enqueue order.
+ *   est(L) = i + round(1.5 i), i = max(floor(L / 4), 1), halves away from zero (SimpleTokenEstimator, token_estimator.go
+ *       :55-56, 70-71), with L = the request's true prompt length in bytes (lengths[r] / the row length; input_len_bytes[r]
+ *       for epp_schedule_with_match, 0 when NULL).  The reference feeds it the whole HTTP body size.
+ *   ResponseBody (:131-168): epp_inflight_release; endpoint deletion (:86-97): epp_inflight_reset.  Both are folded on the
+ *       host, cost no CUDA call and take effect in call order, before the next scheduling call or epp_inflight_get.
+ * Not available in the endpoint-sharded and peer-memory modes.
  *
  * Tie rule: the reference's max-score picker shuffles with math/rand before its stable sort, i.e. it returns a
  * uniformly random member of the arg-max set (picker/maxscore/picker.go:91-102).  The engine always returns the bit
@@ -118,9 +134,11 @@ typedef enum {
                                   side keep any other Scorer (lora-affinity, session-affinity, ...) */
     EPP_SCORER_RUNNING = 5,    /* "running-requests-size-scorer" scorer/runningrequests/runningrequest.go:78-108 */
     EPP_SCORER_TOKEN_LOAD = 6, /* "token-load-scorer"            scorer/tokenload/token_load.go:84-112; column = ext column
-                                  holding InFlightLoad.Tokens, param = queueThresholdTokens (<= 0: 4194304)       */
+                                  holding InFlightLoad.Tokens (ignored with inflight_load: the engine's counters),
+                                  param = queueThresholdTokens (<= 0: 4194304)                                    */
     EPP_SCORER_ACTIVE_REQUEST = 7, /* "active-request-scorer"    scorer/activerequest/active_request.go:140-173; column = ext
-                                  column holding InFlightLoad.Requests, param = maxBusyScore (outside [0,1]: 1.0),
+                                  column holding InFlightLoad.Requests (ignored with inflight_load: the engine's
+                                  counters), param = maxBusyScore (outside [0,1]: 1.0),
                                   param2 = idleThreshold (< 0: 0)                                                 */
     EPP_SCORER_LORA_AFFINITY = 8, /* "lora-affinity-scorer"      scorer/loraaffinity/lora_affinity.go:76-100; the adapter is the
                                   request's model id; residency comes from epp_pool_set_lora                     */
@@ -226,7 +244,11 @@ typedef struct {
                                       ago, i.e. picks become visible to later requests with a bounded delay, like the
                                       reference's asynchronous PreRequest (approximateprefix/plugin.go:189-194).
                                       epp_index_commit / epp_index_get always commit.                              */
-    uint64_t reserved1[2];
+    int32_t inflight_load;         /* 1: the inflight-load producer runs on the device (see "In-flight load" above) and
+                                      every TOKEN_LOAD / ACTIVE_REQUEST scorer reads its counters (`column` ignored);
+                                      0: off (default)                                                              */
+    uint32_t reserved0;
+    uint64_t reserved1;
 } epp_config;
 
 /* One routing decision (32 bytes).  status: 0 = ok, -1 = no endpoint available for the primary profile
@@ -288,7 +310,8 @@ typedef struct {
     uint64_t device_bytes;
     /* device-pointer batches only: CUDA-event time of each kernel of the last batch on the launch stream.
      * [0] prompt lengths  [1] block digests (dominant: reads every token once)  [2] chain  [3] match+score+pick
-     * [4] the no-hit-lru update after the picks (engines with that scorer; 0 otherwise) */
+     * [4] the no-hit-lru update after the picks (engines with that scorer; 0 otherwise)
+     * [5] the in-flight counters' update after the picks (engines with inflight_load; 0 otherwise) */
     double last_kernel_ms[8];
     /* algorithmic work of the last batch (SURVEY.md 8(d)): table probes P = sum_r min(stop_r+1, B_r) and
      * postings consumed M = sum_r sum_{i<stop_r} |servers(h_i)| */
@@ -418,6 +441,18 @@ EPP_API int32_t epp_index_add_picked(epp_engine *h);
 /* The no-hit-lru scorer's LRU, oldest first (golang-lru Cache.Keys): *out_n = its length, the first min(cap, *out_n)
  * slot ids go to out_eps.  Waits for the batches in flight.  EPP_ERR_STATE when no profile has the scorer. */
 EPP_API int32_t epp_nohit_lru_get(epp_engine *h, uint32_t *out_eps, int32_t cap, int32_t *out_n);
+
+/* ResponseBody of the inflight-load producer (producer.go:131-168): entry i takes 1 request and est(prompt_lens[i]) tokens
+ * off slot eps[i] (the prefill target at the first chunk, the other targets at the end of the stream).  EPP_NO_ENDPOINT
+ * entries are skipped; a slot >= max_endpoints fails the whole call with EPP_ERR_INVALID.  EPP_ERR_STATE when the engine
+ * was created without inflight_load.  No CUDA call: applied before the next scheduling call or epp_inflight_get. */
+EPP_API int32_t epp_inflight_release(epp_engine *h, int32_t n, const uint32_t *eps, const uint64_t *prompt_lens);
+/* Endpoint deletion (producer.go:86-97, 189-192): both counters of slots ids[0 .. n) become 0, after every earlier
+ * release and before every later one.  Call it before a slot id is given to another endpoint. */
+EPP_API int32_t epp_inflight_reset(epp_engine *h, int32_t n, const uint32_t *ids);
+/* The counters of the first min(cap, max_endpoints) slots (InFlightLoad.Requests / .Tokens).  Applies the pending
+ * releases and resets and waits for the batches in flight.  EPP_ERR_STATE without inflight_load. */
+EPP_API int32_t epp_inflight_get(epp_engine *h, int32_t cap, int64_t *out_requests, int64_t *out_tokens);
 
 EPP_API int32_t epp_get_stats(epp_engine *h, epp_stats *out);
 

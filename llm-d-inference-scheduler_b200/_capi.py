@@ -43,7 +43,8 @@ class Config(C.Structure):
                 ("lru_capacity_per_server", C.c_int32), ("handler", C.c_int32), ("always_disagg", C.c_int32),
                 ("non_cached_tokens", C.c_int64), ("n_ext_cols", C.c_int32), ("pick_k", C.c_int32),
                 ("primary", ProfileCfg), ("prefill", ProfileCfg), ("encode", ProfileCfg), ("tie_seed", C.c_uint64),
-                ("encode_enabled", C.c_int32), ("index_commit_interval_us", C.c_int32), ("reserved1", C.c_uint64 * 2)]
+                ("encode_enabled", C.c_int32), ("index_commit_interval_us", C.c_int32), ("inflight_load", C.c_int32),
+                ("reserved0", C.c_uint32), ("reserved1", C.c_uint64)]
 
 
 class Decision(C.Structure):
@@ -130,6 +131,9 @@ SIGNATURES = {
                                                  C.c_int32, C.c_void_p, C.c_void_p, C.c_uint32, C.POINTER(TopkOut)]),
     "epp_index_add_picked": (C.c_int32, [C.c_void_p]),
     "epp_nohit_lru_get": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(C.c_int32)]),
+    "epp_inflight_release": (C.c_int32, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
+    "epp_inflight_reset": (C.c_int32, [C.c_void_p, C.c_int32, C.c_void_p]),
+    "epp_inflight_get": (C.c_int32, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "epp_get_stats": (C.c_int32, [C.c_void_p, C.POINTER(Stats)]),
     "epp_synchronize": (C.c_int32, [C.c_void_p]),
     "epp_event_record": (C.c_int32, [C.c_void_p, C.c_int32]),

@@ -17,6 +17,7 @@
 #include <memory>
 #include <mutex>
 #include <string>
+#include <unordered_map>
 #include <vector>
 
 #include "devbuf.h"
@@ -80,7 +81,7 @@ struct epp_engine {
     size_t max_smem_optin = 0;
 
     Slot slot[2];
-    cudaEvent_t ev[8] = {};
+    cudaEvent_t ev[9] = {};
     cudaEvent_t user_ev[2] = {};    // epp_event_record / epp_event_elapsed_ms
     unsigned long long *wc_host = nullptr;   // pinned: work counters of an async batch
     bool async_pending = false;     // an EPP_BATCH_ASYNC batch whose stats have not been read back yet
@@ -110,6 +111,21 @@ struct epp_engine {
     ProfileState prof_cold[kMaxProfiles];   // cold sets: base / order / groups with the LRU column
     DevBuf nh_last_seq, nh_pos, nh_misc, nh_sort_key, nh_order, nh_cold, nh_col[kMaxProfiles];
     DevBuf nh_prof;                 // ProfileDev[kMaxProfiles] of the cold sets (NoHitView::cold)
+    // inflight-load producer (inflight.cu), allocated only with cfg.inflight_load
+    bool inflight = false;
+    int inflight_mask = 0;          // bit pi: profile pi lists a token-load or active-request scorer (they read the counters)
+    int32_t n_ext_total = 0;        // the caller's ext columns, then (with inflight) the token and request count columns
+    bool inflight_timed = false;    // ev[7] / ev[8] bracket the update of the device batch in flight
+    DevBuf if_req, if_tok;
+    std::mutex if_mu;               // guards if_pending only: releases and resets never wait for a batch
+    std::unordered_map<uint32_t, InflightDelta> if_pending;   // folded releases / resets not applied yet
+    // two staging sets for the folded deltas: a set is refilled once the apply kernel that read it has run (if_ev)
+    InflightDelta *if_host[2] = {};
+    size_t if_host_cap[2] = {};
+    DevBuf if_dev[2];
+    cudaEvent_t if_ev[2] = {};
+    int if_flip = 0;
+    epp_config cfg_user;            // the configuration as given (cfg has the counter columns filled in)
 
     // index
     std::unique_ptr<IndexStore> store;          // write side: LRU bookkeeping in HBM (index_store.cu)
@@ -232,14 +248,15 @@ extern "C" void epp_config_default(epp_config *cfg) {
     cfg->primary.ttft_column = cfg->prefill.ttft_column = cfg->encode.ttft_column = -1;   // no affinity filter, no TTFT column
 }
 
-static int32_t validate_profile(const epp_profile_cfg &p, int n_ext, const char *name) {
+// inflight: the token-load / active-request scorers read the engine's counters, whatever their column.
+static int32_t validate_profile(const epp_profile_cfg &p, int n_ext, bool inflight, const char *name) {
     if (p.filter < EPP_FILTER_NONE || p.filter > EPP_FILTER_ENCODE) return fail(EPP_ERR_INVALID, "%s: bad filter %d", name, p.filter);
     if (p.n_scorers < 0 || p.n_scorers > EPP_MAX_SCORERS) return fail(EPP_ERR_INVALID, "%s: n_scorers %d out of range", name, p.n_scorers);
     for (int s = 0; s < p.n_scorers; s++) {
         const epp_scorer_cfg &sc = p.scorers[s];
         if (sc.kind < EPP_SCORER_PREFIX || sc.kind > EPP_SCORER_NO_HIT_LRU) return fail(EPP_ERR_INVALID, "%s: scorer %d has unknown kind %d", name, s, sc.kind);
         if (!std::isfinite(sc.weight)) return fail(EPP_ERR_INVALID, "%s: scorer %d weight is not finite", name, s);
-        if ((sc.kind == EPP_SCORER_TOKEN_LOAD || sc.kind == EPP_SCORER_ACTIVE_REQUEST) && (sc.column < 0 || sc.column >= n_ext))
+        if (!inflight && (sc.kind == EPP_SCORER_TOKEN_LOAD || sc.kind == EPP_SCORER_ACTIVE_REQUEST) && (sc.column < 0 || sc.column >= n_ext))
             return fail(EPP_ERR_INVALID, "%s: scorer %d reads ext column %d, out of range [0,%d)", name, s, sc.column, n_ext);
         if (sc.kind == EPP_SCORER_EXTERNAL && (sc.param < 0 || sc.param >= n_ext)) return fail(EPP_ERR_INVALID, "%s: scorer %d external column %g out of range [0,%d)", name, s, sc.param, n_ext);
     }
@@ -293,11 +310,13 @@ extern "C" int32_t epp_engine_create(const epp_config *cfg, epp_engine **out) {
     if (cfg->handler != EPP_HANDLER_SINGLE && cfg->handler != EPP_HANDLER_DISAGG) return fail(EPP_ERR_INVALID, "bad handler %d", cfg->handler);
     if (cfg->n_ext_cols < 0 || cfg->n_ext_cols > 64) return fail(EPP_ERR_INVALID, "n_ext_cols %d out of range", cfg->n_ext_cols);
     if (cfg->non_cached_tokens < 0) return fail(EPP_ERR_INVALID, "non_cached_tokens must be >= 0");
-    EPP_TRY(validate_profile(cfg->primary, cfg->n_ext_cols, "primary profile"));
-    if (cfg->handler == EPP_HANDLER_DISAGG) EPP_TRY(validate_profile(cfg->prefill, cfg->n_ext_cols, "prefill profile"));
+    if (cfg->inflight_load != 0 && cfg->inflight_load != 1) return fail(EPP_ERR_INVALID, "inflight_load %d must be 0 or 1", cfg->inflight_load);
+    const bool inflight = cfg->inflight_load != 0;
+    EPP_TRY(validate_profile(cfg->primary, cfg->n_ext_cols, inflight, "primary profile"));
+    if (cfg->handler == EPP_HANDLER_DISAGG) EPP_TRY(validate_profile(cfg->prefill, cfg->n_ext_cols, inflight, "prefill profile"));
     if (cfg->encode_enabled) {
         if (cfg->handler != EPP_HANDLER_DISAGG) return fail(EPP_ERR_INVALID, "encode_enabled needs the disagg handler");
-        EPP_TRY(validate_profile(cfg->encode, cfg->n_ext_cols, "encode profile"));
+        EPP_TRY(validate_profile(cfg->encode, cfg->n_ext_cols, inflight, "encode profile"));
     }
     if (cfg->index_commit_interval_us < 0) return fail(EPP_ERR_INVALID, "index_commit_interval_us must be >= 0");
     if (cfg->pick_k < 0 || cfg->pick_k > 64) return fail(EPP_ERR_INVALID, "pick_k %d out of range [0,64]", cfg->pick_k);
@@ -310,8 +329,25 @@ extern "C" int32_t epp_engine_create(const epp_config *cfg, epp_engine **out) {
 
     std::unique_ptr<epp_engine> e(new epp_engine());
     e->cfg = *cfg;
+    e->cfg_user = *cfg;
     e->n_profiles = cfg->handler == EPP_HANDLER_DISAGG ? 2 : 1;
     e->n_alloc_profiles = cfg->encode_enabled ? 3 : e->n_profiles;
+    e->n_ext_total = cfg->n_ext_cols;
+    if (inflight) {
+        // the counters live in two engine-owned ext columns behind the caller's: every kernel that reads a token-load /
+        // active-request column reads them unchanged
+        e->inflight = true;
+        e->n_ext_total = cfg->n_ext_cols + 2;
+        for (int pi = 0; pi < e->n_alloc_profiles; pi++) {
+            epp_profile_cfg &pc = pi == 0 ? e->cfg.primary : (pi == 1 ? e->cfg.prefill : e->cfg.encode);
+            for (int si = 0; si < pc.n_scorers; si++) {
+                if (pc.scorers[si].kind == EPP_SCORER_TOKEN_LOAD) pc.scorers[si].column = cfg->n_ext_cols;
+                else if (pc.scorers[si].kind == EPP_SCORER_ACTIVE_REQUEST) pc.scorers[si].column = cfg->n_ext_cols + 1;
+                else continue;
+                e->inflight_mask |= 1 << pi;
+            }
+        }
+    }
     CUDA_TRY(cudaSetDevice(cfg->device));
     cudaDeviceProp prop;
     CUDA_TRY(cudaGetDeviceProperties(&prop, cfg->device));
@@ -335,7 +371,15 @@ extern "C" int32_t epp_engine_create(const epp_config *cfg, epp_engine **out) {
     CUDA_TRY(e->kv.reserve(sizeof(double) * E, &e->dev_bytes));
     CUDA_TRY(e->waiting.reserve(sizeof(int32_t) * E, &e->dev_bytes));
     CUDA_TRY(e->running.reserve(sizeof(int32_t) * E, &e->dev_bytes));
-    if (cfg->n_ext_cols) CUDA_TRY(e->ext.reserve(sizeof(double) * E * (size_t)cfg->n_ext_cols, &e->dev_bytes));
+    if (e->n_ext_total) CUDA_TRY(e->ext.reserve(sizeof(double) * E * (size_t)e->n_ext_total, &e->dev_bytes));
+    if (e->inflight) {
+        CUDA_TRY(e->if_req.reserve(sizeof(int64_t) * E, &e->dev_bytes));
+        CUDA_TRY(e->if_tok.reserve(sizeof(int64_t) * E, &e->dev_bytes));
+        CUDA_TRY(cudaMemset(e->if_req.p, 0, sizeof(int64_t) * E));
+        CUDA_TRY(cudaMemset(e->if_tok.p, 0, sizeof(int64_t) * E));
+        CUDA_TRY(cudaMemset(e->ext.as<double>() + E * (size_t)cfg->n_ext_cols, 0, sizeof(double) * E * 2));
+        for (auto &ev : e->if_ev) CUDA_TRY(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+    }
     for (int p = 0; p < e->n_alloc_profiles; p++) EPP_TRY(alloc_profile(e.get(), e->prof[p], profile_cfg(e.get(), p).picker != 0));
     CUDA_TRY(e->idx_cursor.reserve(sizeof(uint32_t) * 4, &e->dev_bytes));
     CUDA_TRY(e->idx_special.reserve(sizeof(IndexSlot), &e->dev_bytes));
@@ -444,6 +488,10 @@ extern "C" int32_t epp_engine_destroy(epp_engine *h) {
     if (h->wc_host) cudaFreeHost(h->wc_host);
     if (h->small_host) cudaFreeHost(h->small_host);
     if (h->small_epoch_host) cudaFreeHost(h->small_epoch_host);
+    for (int i = 0; i < 2; i++) {
+        if (h->if_host[i]) cudaFreeHost(h->if_host[i]);
+        if (h->if_ev[i]) cudaEventDestroy(h->if_ev[i]);
+    }
     for (int g = 0; g < (int)h->p2p_peer.size(); g++)
         if (h->p2p_ipc && g != h->p2p_rank && h->p2p_peer[g]) cudaIpcCloseMemHandle(h->p2p_peer[g]);
     if (h->p2p_buf) cudaFree(h->p2p_buf);
@@ -516,7 +564,7 @@ static LoraDev lora_dev(epp_engine *h) {
 static PoolArrays pool_arrays(epp_engine *h) {
     PoolArrays pa;
     pa.E = h->cfg.max_endpoints;
-    pa.n_ext_cols = h->cfg.n_ext_cols;
+    pa.n_ext_cols = h->n_ext_total;
     pa.role = h->role.as<uint8_t>();
     pa.kv_usage = h->kv.as<double>();
     pa.waiting = h->waiting.as<int32_t>();
@@ -631,27 +679,105 @@ static NoHitView nohit_view(epp_engine *h, int64_t r0) {
     return v;
 }
 
-// Request-independent scorer terms of every profile from the current pool (+ LoRA) snapshot, on the device.
+// Request-independent scorer terms of profile p from the current pool (+ LoRA) snapshot, on the device.
+static int32_t derive_profile(epp_engine *h, int p, cudaStream_t s, int *launches) {
+    ProfileDerived d{};
+    d.cand = h->prof[p].cand.as<uint8_t>();
+    d.contrib = h->prof[p].contrib.as<double>();
+    d.cands = h->prof[p].cands.as<uint32_t>();
+    d.wcum = h->prof[p].wcum.as<double>();
+    d.icum = h->prof[p].icum.as<uint32_t>();
+    d.base = h->prof[p].base.as<double>();
+    d.order = h->prof[p].order.as<uint32_t>();
+    d.grp_size = h->prof[p].grp_size.as<uint32_t>();
+    d.sort_key = h->prof[p].sort_key.as<uint64_t>();
+    d.n_cand = h->prof[p].n_cand.as<int32_t>();
+    d.qminmax = h->prof[p].qminmax.as<int64_t>();
+    CUDA_TRY(launch_pool_prepare(pool_arrays(h), profile_cfg(h, p), d, h->Epad, h->shard_begin, h->shard_end, s, launches));
+    return EPP_OK;
+}
+
 static int32_t derive_pool(epp_engine *h) {
     cudaStream_t s = h->slot[0].stream;
-    PoolArrays pa = pool_arrays(h);
     int launches = 0;
-    for (int p = 0; p < h->n_alloc_profiles; p++) {
-        ProfileDerived d{};
-        d.cand = h->prof[p].cand.as<uint8_t>();
-        d.contrib = h->prof[p].contrib.as<double>();
-        d.cands = h->prof[p].cands.as<uint32_t>();
-        d.wcum = h->prof[p].wcum.as<double>();
-        d.icum = h->prof[p].icum.as<uint32_t>();
-        d.base = h->prof[p].base.as<double>();
-        d.order = h->prof[p].order.as<uint32_t>();
-        d.grp_size = h->prof[p].grp_size.as<uint32_t>();
-        d.sort_key = h->prof[p].sort_key.as<uint64_t>();
-        d.n_cand = h->prof[p].n_cand.as<int32_t>();
-        d.qminmax = h->prof[p].qminmax.as<int64_t>();
-        CUDA_TRY(launch_pool_prepare(pa, p == 0 ? h->cfg.primary : (p == 1 ? h->cfg.prefill : h->cfg.encode), d, h->Epad, h->shard_begin, h->shard_end, s, &launches));
-    }
+    for (int p = 0; p < h->n_alloc_profiles; p++) EPP_TRY(derive_profile(h, p, s, &launches));
     return nohit_derive(h, s, false, &launches);
+}
+
+// ---- inflight-load producer (inflight.cu) ---------------------------------------------------------------------------
+static InflightState inflight_state(epp_engine *h) {
+    InflightState st;
+    const size_t E = (size_t)h->cfg.max_endpoints;
+    st.req = h->if_req.as<int64_t>();
+    st.tok = h->if_tok.as<int64_t>();
+    st.col_tok = h->ext.as<double>() + E * (size_t)h->cfg.n_ext_cols;
+    st.col_req = st.col_tok + E;
+    st.E = h->cfg.max_endpoints;
+    return st;
+}
+
+// After the counters changed: their columns, and every term derived from them -- the profiles that list a token-load or
+// active-request scorer (launch_pool_prepare, random pickers' cumulative arrays included) and the no-hit-lru cold sets,
+// which are built on those profiles' candidates and load maxima.
+static int32_t inflight_rederive(epp_engine *h, cudaStream_t s, int *launches) {
+    if (!h->inflight_mask) return EPP_OK;
+    CUDA_TRY(launch_inflight_columns(inflight_state(h), s, launches));
+    for (int p = 0; p < h->n_alloc_profiles; p++)
+        if (h->inflight_mask & (1 << p)) EPP_TRY(derive_profile(h, p, s, launches));
+    if (h->inflight_mask & h->nohit_mask) EPP_TRY(nohit_derive(h, s, false, launches));
+    return EPP_OK;
+}
+
+// PreRequest of the producer for one scheduling call (producer.go:110-129), enqueued on s behind the call's last pick
+// kernel.  dec / det / in_len hold the call's R requests (det, in_len may be nullptr).
+static int32_t inflight_update(epp_engine *h, const epp_decision *dec, const epp_decision_detail *det, const int64_t *in_len,
+                               int64_t R, cudaStream_t s, int *launches) {
+    if (!h->inflight || R <= 0) return EPP_OK;
+    CUDA_TRY(launch_inflight_add(inflight_state(h), dec, det, in_len, R, s, launches));
+    return inflight_rederive(h, s, launches);
+}
+
+// The same on stream 0 of a device batch, bracketed by ev[7] / ev[8] (epp_stats.last_kernel_ms[5]).
+static int32_t inflight_update_timed(epp_engine *h, const epp_decision *dec, const epp_decision_detail *det, int64_t R,
+                                     int *launches) {
+    if (!h->inflight) return EPP_OK;
+    cudaStream_t s0 = h->slot[0].stream;
+    CUDA_TRY(cudaEventRecord(h->ev[7], s0));
+    EPP_TRY(inflight_update(h, dec, det, h->in_len.as<int64_t>(), R, s0, launches));
+    CUDA_TRY(cudaEventRecord(h->ev[8], s0));
+    h->inflight_timed = true;
+    return EPP_OK;
+}
+
+// Applies the releases and resets folded since the last time (one copy + one kernel on s), then re-derives.
+static int32_t inflight_flush(epp_engine *h, cudaStream_t s, int *launches) {
+    if (!h->inflight) return EPP_OK;
+    std::vector<InflightDelta> d;
+    {
+        std::lock_guard<std::mutex> lk(h->if_mu);
+        if (h->if_pending.empty()) return EPP_OK;
+        d.reserve(h->if_pending.size());
+        for (const auto &kv : h->if_pending) d.push_back(kv.second);
+        h->if_pending.clear();
+    }
+    const int k = h->if_flip;
+    h->if_flip ^= 1;
+    CUDA_TRY(cudaEventSynchronize(h->if_ev[k]));      // the apply kernel that last read staging set k has run
+    const size_t bytes = sizeof(InflightDelta) * d.size();
+    if (h->if_host_cap[k] < bytes) {
+        if (h->if_host[k]) CUDA_TRY(cudaFreeHost(h->if_host[k]));
+        h->if_host[k] = nullptr;
+        h->if_host_cap[k] = 0;
+        const size_t cap = std::max<size_t>(bytes * 2, 4096);
+        CUDA_TRY(cudaHostAlloc(reinterpret_cast<void **>(&h->if_host[k]), cap, cudaHostAllocDefault));
+        h->if_host_cap[k] = cap;
+    }
+    memcpy(h->if_host[k], d.data(), bytes);
+    CUDA_TRY(h->if_dev[k].reserve(bytes, &h->dev_bytes));
+    CUDA_TRY(cudaMemcpyAsync(h->if_dev[k].p, h->if_host[k], bytes, cudaMemcpyHostToDevice, s));
+    CUDA_TRY(launch_inflight_apply(inflight_state(h), h->if_dev[k].as<InflightDelta>(), (int32_t)d.size(), s, launches));
+    CUDA_TRY(cudaEventRecord(h->if_ev[k], s));
+    return inflight_rederive(h, s, launches);
 }
 
 extern "C" int32_t epp_pool_set(epp_engine *h, int32_t n, const uint32_t *ids, const uint8_t *role,
@@ -1293,6 +1419,12 @@ static int32_t finish_async(epp_engine *h) {
         h->stats.last_kernel_ms[4] = tn;
         h->nohit_timed = false;
     }
+    if (h->inflight_timed) {
+        float ti = 0;
+        cudaEventElapsedTime(&ti, h->ev[7], h->ev[8]);
+        h->stats.last_kernel_ms[5] = ti;
+        h->inflight_timed = false;
+    }
     return EPP_OK;
 }
 
@@ -1467,6 +1599,7 @@ static int32_t run_small(epp_engine *h, const BatchView &v, int mode, const uint
         CUDA_TRY(cudaStreamSynchronize(s0));
     }
     EPP_TRY(nohit_update(h, h->small_dec, R, s0, &launches));   // reads the decisions from the pinned copy (UVA)
+    EPP_TRY(inflight_update(h, h->small_dec, h->small_det, h->in_len.as<int64_t>(), R, s0, &launches));
     memcpy(out_dec, h->small_dec, sizeof(epp_decision) * (size_t)R);
     if (out_detail) memcpy(out_detail, h->small_det, sizeof(epp_decision_detail) * (size_t)R);
     h->small_stats_pending = true;
@@ -1528,6 +1661,12 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
     EPP_TRY(reserve_batch(h, R));
     int launches = 0;
     cudaStream_t s0 = h->slot[0].stream;
+    // releases / resets since the last call, on stream 0 before any pick kernel (a pipelined batch's stream 1 waits
+    // for stream 0 below)
+    if (mode == Mode::Schedule) EPP_TRY(inflight_flush(h, s0, &launches));
+    // the stage records reach the producer's add kernel even when the caller asked for none
+    epp_decision_detail *det_out = (mode == Mode::Schedule && !out_detail && h->inflight) ? h->details.as<epp_decision_detail>()
+                                                                                         : out_detail;
 
     if (v.device) {
         uint64_t or_bits = 0;
@@ -1546,7 +1685,7 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
             const int64_t C = std::min<int64_t>(h->dev_chunks, R / min_chunk);
             const int64_t per = ((R + C - 1) / C + 31) & ~(int64_t)31;
             cudaStream_t s1 = h->slot[1].stream;
-            if (h->s1_unjoined && (h->pipe_R != R || h->pipe_per != per)) EPP_TRY(join_streams(h));
+            if (h->s1_unjoined && (h->inflight || h->pipe_R != R || h->pipe_per != per)) EPP_TRY(join_streams(h));
             for (int i = 0; i < 4; i++) CUDA_TRY(cudaEventRecord(h->ev[i], s0));
             if (!h->s1_unjoined) {
                 CUDA_TRY(cudaEventRecord(h->slot[0].done, s0));
@@ -1558,7 +1697,7 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
                 const int64_t r1 = std::min(R, r0 + per);
                 Work w{r0, r1, v.offsets ? v.data : v.data + (uint64_t)r0 * v.uniform_len, v.offsets, v.lengths, v.uniform_len,
                        v.model_ids, or_bits, h->hashes.as<uint64_t>() + (size_t)r0 * B, h->nblocks.as<int32_t>() + r0, v.multimodal};
-                PickParams pp = pick_params(h, w, dec_base + r0, out_detail ? out_detail + r0 : nullptr, nullptr);
+                PickParams pp = pick_params(h, w, dec_base + r0, det_out ? det_out + r0 : nullptr, nullptr);
                 if (tk) attach_topk(h, pp.gen, tk_picks, tk_scores, r0);
                 Slot &sl = h->slot[k & 1];
                 HashParams hp = hash_params(h, w, sl);
@@ -1567,8 +1706,8 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
             }
             h->s1_unjoined = true;
             // the next call's picks must see both chunks' Adds: join the chunks on stream 0 for the update (below), and the
-            // next call's stream-1 chunk waits for stream 0 again (engines without the scorer stay unjoined)
-            if (h->nohit_mask) EPP_TRY(join_streams(h));
+            // next call's stream-1 chunk waits for stream 0 again (engines without the scorer or the producer stay unjoined)
+            if (h->nohit_mask || h->inflight) EPP_TRY(join_streams(h));
             h->pipe_R = R;
             h->pipe_per = per;
         } else if (mode == Mode::HashOnly) {
@@ -1577,7 +1716,7 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
             CUDA_TRY(launch_hash_prompts(hp, s0, &launches, h->ev));
         } else {
             epp_decision *dec = (mode == Mode::Schedule && out_dec) ? out_dec : h->decisions.as<epp_decision>();
-            PickParams pp = pick_params(h, w, dec, mode == Mode::Schedule ? out_detail : nullptr, mode == Mode::Match ? out_match : nullptr);
+            PickParams pp = pick_params(h, w, dec, mode == Mode::Schedule ? det_out : nullptr, mode == Mode::Match ? out_match : nullptr);
             pp.work_counters = h->work_counters.as<unsigned long long>();
             if (tk) attach_topk(h, pp.gen, tk_picks, tk_scores, 0);
             HashParams hp = hash_params(h, w, h->slot[0]);
@@ -1587,8 +1726,11 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
             EPP_TRY(launch_cycle(h, h->slot[0], hp, pp, &launches, h->ev));
         }
         CUDA_TRY(cudaEventRecord(h->ev[4], s0));
-        if (mode == Mode::Schedule)                // after ev[4]: last_kernel_ms[3] stays the match + pick time
-            EPP_TRY(nohit_update_timed(h, out_dec ? out_dec : h->decisions.as<epp_decision>(), R, &launches));
+        if (mode == Mode::Schedule) {              // after ev[4]: last_kernel_ms[3] stays the match + pick time
+            epp_decision *dec = out_dec ? out_dec : h->decisions.as<epp_decision>();
+            EPP_TRY(nohit_update_timed(h, dec, R, &launches));
+            EPP_TRY(inflight_update_timed(h, dec, det_out, R, &launches));
+        }
         CUDA_TRY(cudaMemcpyAsync(h->wc_host, h->work_counters.p, sizeof(unsigned long long) * 4, cudaMemcpyDeviceToHost, s0));
         h->async_pending = true;
         h->async_launches = launches;
@@ -1699,7 +1841,11 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
         }
     }
     CUDA_TRY(cudaStreamSynchronize(h->slot[1].stream));
-    if (mode == Mode::Schedule) EPP_TRY(nohit_update(h, h->decisions.as<epp_decision>(), R, s0, &launches));
+    if (mode == Mode::Schedule) {
+        EPP_TRY(nohit_update(h, h->decisions.as<epp_decision>(), R, s0, &launches));
+        EPP_TRY(inflight_update(h, h->decisions.as<epp_decision>(), h->details.as<epp_decision_detail>(), h->in_len.as<int64_t>(),
+                                R, s0, &launches));
+    }
     CUDA_TRY(cudaEventRecord(h->ev[1], s0));
     CUDA_TRY(cudaStreamSynchronize(s0));
     float t_all = 0;
@@ -1867,6 +2013,8 @@ static int32_t with_match_impl(epp_engine *h, int64_t n_requests, const int32_t 
     const size_t E = (size_t)h->cfg.max_endpoints, n = (size_t)n_requests * E, R = (size_t)n_requests;
     cudaStream_t s = h->slot[0].stream;
     const bool dev = (flags & EPP_BATCH_DEVICE_PTRS) != 0;
+    int launches = 0;
+    EPP_TRY(inflight_flush(h, s, &launches));
     DensePickParams p;
     p.R = n_requests;
     p.E = h->cfg.max_endpoints;
@@ -1926,9 +2074,9 @@ static int32_t with_match_impl(epp_engine *h, int64_t n_requests, const int32_t 
         p.out = h->decisions.as<epp_decision>();
         p.detail = h->details.as<epp_decision_detail>();
     }
-    int launches = 0;
     CUDA_TRY(launch_dense_pick(p, s, &launches));
     EPP_TRY(nohit_update(h, p.out, n_requests, s, &launches));
+    EPP_TRY(inflight_update(h, p.out, p.detail, p.in_len, n_requests, s, &launches));
     if (!dev) {
         CUDA_TRY(cudaMemcpyAsync(out, p.out, sizeof(epp_decision) * R, cudaMemcpyDeviceToHost, s));
         if (detail) CUDA_TRY(cudaMemcpyAsync(detail, p.detail, sizeof(epp_decision_detail) * R, cudaMemcpyDeviceToHost, s));
@@ -1973,10 +2121,61 @@ extern "C" int32_t epp_nohit_lru_get(epp_engine *h, uint32_t *out_eps, int32_t c
     return EPP_OK;
 }
 
+// The producer's token estimate of a prompt of L bytes (the device copy is inflight_est in inflight.cu).
+static int64_t inflight_est_host(int64_t L) {
+    const int64_t i = L < 8 ? 1 : L / 4;
+    return 2 * i + (i + 1) / 2;
+}
+
+extern "C" int32_t epp_inflight_release(epp_engine *h, int32_t n, const uint32_t *eps, const uint64_t *prompt_lens) {
+    if (!h || n < 0 || (n > 0 && (!eps || !prompt_lens))) return fail(EPP_ERR_INVALID, "bad arguments");
+    if (!h->inflight) return fail(EPP_ERR_STATE, "the engine was created without inflight_load");
+    for (int32_t i = 0; i < n; i++)
+        if (eps[i] != EPP_NO_ENDPOINT && eps[i] >= (uint32_t)h->cfg.max_endpoints)
+            return fail(EPP_ERR_INVALID, "entry %d: slot id %u >= max_endpoints %d", i, eps[i], h->cfg.max_endpoints);
+    std::lock_guard<std::mutex> lk(h->if_mu);
+    for (int32_t i = 0; i < n; i++) {
+        if (eps[i] == EPP_NO_ENDPOINT) continue;
+        InflightDelta &d = h->if_pending.try_emplace(eps[i], InflightDelta{eps[i], 0, 0, 0}).first->second;
+        d.req -= 1;
+        d.tok -= inflight_est_host((int64_t)std::min<uint64_t>(prompt_lens[i], (uint64_t)INT64_MAX));
+    }
+    return EPP_OK;
+}
+
+extern "C" int32_t epp_inflight_reset(epp_engine *h, int32_t n, const uint32_t *ids) {
+    if (!h || n < 0 || (n > 0 && !ids)) return fail(EPP_ERR_INVALID, "bad arguments");
+    if (!h->inflight) return fail(EPP_ERR_STATE, "the engine was created without inflight_load");
+    for (int32_t i = 0; i < n; i++)
+        if (ids[i] >= (uint32_t)h->cfg.max_endpoints)
+            return fail(EPP_ERR_INVALID, "entry %d: slot id %u >= max_endpoints %d", i, ids[i], h->cfg.max_endpoints);
+    std::lock_guard<std::mutex> lk(h->if_mu);
+    for (int32_t i = 0; i < n; i++) h->if_pending[ids[i]] = InflightDelta{ids[i], 1, 0, 0};   // drops earlier pending releases
+    return EPP_OK;
+}
+
+extern "C" int32_t epp_inflight_get(epp_engine *h, int32_t cap, int64_t *out_requests, int64_t *out_tokens) {
+    if (!h || cap < 0 || (cap > 0 && (!out_requests || !out_tokens))) return fail(EPP_ERR_INVALID, "bad arguments");
+    std::lock_guard<std::mutex> lk(h->mu);
+    if (!h->inflight) return fail(EPP_ERR_STATE, "the engine was created without inflight_load");
+    EPP_TRY(set_device(h));
+    EPP_TRY(finish_async(h));
+    cudaStream_t s = h->slot[0].stream;
+    int launches = 0;
+    EPP_TRY(inflight_flush(h, s, &launches));
+    const size_t n = (size_t)std::min<int32_t>(cap, h->cfg.max_endpoints);
+    if (n) {
+        CUDA_TRY(cudaMemcpyAsync(out_requests, h->if_req.p, sizeof(int64_t) * n, cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(cudaMemcpyAsync(out_tokens, h->if_tok.p, sizeof(int64_t) * n, cudaMemcpyDeviceToHost, s));
+    }
+    CUDA_TRY(cudaStreamSynchronize(s));
+    return EPP_OK;
+}
+
 extern "C" int32_t epp_get_config(epp_engine *h, epp_config *out) {
     if (!h || !out) return fail(EPP_ERR_INVALID, "NULL argument");
     std::lock_guard<std::mutex> lk(h->mu);
-    *out = h->cfg;
+    *out = h->cfg_user;
     return EPP_OK;
 }
 
@@ -2039,6 +2238,7 @@ extern "C" int32_t epp_shard_set(epp_engine *h, uint32_t ep_begin, uint32_t ep_e
     if (h->general) return fail(EPP_ERR_INVALID, "endpoint-sharded mode supports neither pick_k > 1 nor the prefix-cache-affinity-filter (both need every candidate's score on one rank)");
     if (h->nohit_mask) return fail(EPP_ERR_INVALID, "endpoint-sharded mode does not support the no-hit-lru scorer (coldness needs every rank's match)");
     if (any_random_picker(h)) return fail(EPP_ERR_INVALID, "endpoint-sharded mode does not support the random pickers (a weighted draw needs every rank's scores)");
+    if (h->inflight) return fail(EPP_ERR_INVALID, "endpoint-sharded mode does not support the inflight-load producer");
     h->shard_begin = ep_begin;
     h->shard_end = ep_end;
     h->pool_ready = false;          // candidates are derived per shard: epp_pool_set must follow
@@ -2144,6 +2344,7 @@ extern "C" int32_t epp_shard_p2p_connect(epp_engine *h, int32_t n_ranks, int32_t
     std::lock_guard<std::mutex> lk(h->mu);
     if (h->nohit_mask) return fail(EPP_ERR_INVALID, "endpoint-sharded mode does not support the no-hit-lru scorer (coldness needs every rank's match)");
     if (any_random_picker(h)) return fail(EPP_ERR_INVALID, "endpoint-sharded mode does not support the random pickers (a weighted draw needs every rank's scores)");
+    if (h->inflight) return fail(EPP_ERR_INVALID, "endpoint-sharded mode does not support the inflight-load producer");
     EPP_TRY(set_device(h));
     EPP_TRY(join_streams(h));
     if (!h->p2p_buf) return fail(EPP_ERR_STATE, "epp_shard_p2p_export has not been called");

@@ -175,6 +175,30 @@ cudaError_t launch_nohit_cold_rows(int64_t R, int32_t E, const uint8_t *cand, co
                                    cudaStream_t s, int *launches);
 
 // ------------------------------------------------------------------------------------------------
+// inflight-load producer (inflight.cu): per-slot in-flight request and token counts
+// ------------------------------------------------------------------------------------------------
+struct InflightState {
+    int64_t *req;              // [E] InFlightLoad.Requests
+    int64_t *tok;              // [E] InFlightLoad.Tokens
+    double *col_tok;           // [E] the ext column the token-load scorers read
+    double *col_req;           // [E] the ext column the active-request scorers read
+    int32_t E;
+};
+// Releases and resets of one slot folded on the host: set != 0 replaces the counters, else adds to them.
+struct InflightDelta {
+    uint32_t slot;
+    uint32_t set;
+    int64_t req, tok;
+};
+// PreRequest of one scheduling call: for every request with status 0, +1 request and +est(in_len[r]) tokens on its
+// pick, its prefill pick and (det != nullptr) its encode pick, each that is not EPP_NO_ENDPOINT.  in_len == nullptr: 0.
+cudaError_t launch_inflight_add(const InflightState &st, const epp_decision *dec, const epp_decision_detail *det,
+                                const int64_t *in_len, int64_t R, cudaStream_t s, int *launches);
+cudaError_t launch_inflight_apply(const InflightState &st, const InflightDelta *d, int32_t n, cudaStream_t s, int *launches);
+// col_tok / col_req <- the counters.
+cudaError_t launch_inflight_columns(const InflightState &st, cudaStream_t s, int *launches);
+
+// ------------------------------------------------------------------------------------------------
 // match + score + pick (a3-a14)
 // ------------------------------------------------------------------------------------------------
 struct ProfileDev {            // what the pick kernels read (device pointers + config by value)

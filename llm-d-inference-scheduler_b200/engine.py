@@ -93,7 +93,7 @@ class Engine:
                  *, device: int = 0, block_size_tokens: int = 16, max_prefix_blocks: int = 256,
                  lru_capacity_per_server: int = 31250, non_cached_tokens: int = 0, always_disagg: bool = False,
                  n_ext_cols: int = 0, tie_seed: int = 0, encode: ProfileSpec | None = None, pick_k: int = 0,
-                 index_commit_interval_us: int = 0):
+                 index_commit_interval_us: int = 0, inflight_load: bool = False):
         self._lib = capi.load()
         cfg = capi.Config()
         self._lib.epp_config_default(C.byref(cfg))
@@ -116,6 +116,7 @@ class Engine:
         cfg.tie_seed = tie_seed
         cfg.pick_k = pick_k
         cfg.index_commit_interval_us = index_commit_interval_us
+        cfg.inflight_load = int(inflight_load)
         self.cfg = cfg
         self.E = max_endpoints
         self.B = max_prefix_blocks
@@ -202,6 +203,27 @@ class Engine:
         n = C.c_int32()
         self._check(self._lib.epp_nohit_lru_get(self._h, _ptr(out), out.shape[0], C.byref(n)))
         return [int(x) for x in out[:min(n.value, out.shape[0])]]
+
+    # ---- inflight-load producer (engines created with inflight_load=True) ----
+    def inflight_release(self, eps, prompt_lens):
+        """ResponseBody (producer.go:131-168): 1 request and est(prompt_lens[i]) tokens off slot eps[i] each;
+        EPP_NO_ENDPOINT entries are skipped."""
+        e = np.ascontiguousarray(eps, dtype=np.uint32).reshape(-1)
+        ln = np.ascontiguousarray(prompt_lens, dtype=np.uint64).reshape(-1)
+        assert e.shape == ln.shape
+        self._check(self._lib.epp_inflight_release(self._h, e.shape[0], _ptr(e), _ptr(ln)))
+
+    def inflight_reset(self, ids):
+        """Endpoint deletion (producer.go:86-97): both counters of the slots become 0."""
+        a = np.ascontiguousarray(ids, dtype=np.uint32).reshape(-1)
+        self._check(self._lib.epp_inflight_reset(self._h, a.shape[0], _ptr(a)))
+
+    def inflight_get(self):
+        """-> (requests int64[E], tokens int64[E]): InFlightLoad per slot, after every call made so far."""
+        req = np.zeros(self.E, dtype=np.int64)
+        tok = np.zeros(self.E, dtype=np.int64)
+        self._check(self._lib.epp_inflight_get(self._h, self.E, _ptr(req), _ptr(tok)))
+        return req, tok
 
     # ---- batches ----
     def _batch(self, data, offsets=None, uniform_len=None, model_ids=None, n_requests=None, lengths=None, multimodal=None):

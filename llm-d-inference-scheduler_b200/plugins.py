@@ -134,14 +134,15 @@ def NewLoadAware(queueThreshold: int = 128):     # loadaware.NewLoadAware, load_
     return _Scorer(capi.SCORER_LOAD_AWARE, float(queueThreshold), "load-aware-scorer")
 
 
-def TokenLoadScorer(column: int, queueThresholdTokens: int = 4194304):
-    """ "token-load-scorer" (scorer/tokenload/token_load.go:84-112); `column` = ext column holding InFlightLoad.Tokens."""
+def TokenLoadScorer(column: int = 0, queueThresholdTokens: int = 4194304):
+    """ "token-load-scorer" (scorer/tokenload/token_load.go:84-112); `column` = ext column holding InFlightLoad.Tokens,
+    not needed (ignored) when the Scheduler runs the InFlightLoadProducer."""
     return _Scorer(capi.SCORER_TOKEN_LOAD, float(queueThresholdTokens), "token-load-scorer", column)
 
 
-def NewActiveRequest(column: int, idleThreshold: int = 0, maxBusyScore: float = 1.0):
+def NewActiveRequest(column: int = 0, idleThreshold: int = 0, maxBusyScore: float = 1.0):
     """ "active-request-scorer" (scorer/activerequest/active_request.go:72-101, 140-173); `column` = ext column holding
-    InFlightLoad.Requests."""
+    InFlightLoad.Requests, not needed (ignored) when the Scheduler runs the InFlightLoadProducer."""
     return _Scorer(capi.SCORER_ACTIVE_REQUEST, float(maxBusyScore), "active-request-scorer", column, float(idleThreshold))
 
 
@@ -309,6 +310,7 @@ class ProfileRunResult:
     TargetEndpoints: list
     Score: float = 0.0
     TieCount: int = 1
+    TargetSlots: list = field(default_factory=list)   # engine slot ids of TargetEndpoints
 
 
 @dataclass
@@ -323,6 +325,7 @@ class InferenceRequest:
     TargetModel: str = ""
     Prompt: bytes = b""                          # Body.Completions.Prompt.Raw as bytes
     CacheSalt: str = ""
+    SchedulingResult: object = None              # set by the caller after Schedule (read by ResponseBody processors)
 
 
 class Scheduler:
@@ -333,7 +336,10 @@ class Scheduler:
     tests do (disagg/scheduler_test.go:264-268); otherwise pass match info via `produce`."""
 
     def __init__(self, profileHandler, profiles: dict, *, max_endpoints: int = 64, block_size_tokens: int = 16,
-                 max_prefix_blocks: int = 256, ext_columns: int = 0, device: int = 0, tie_seed: int = 0):
+                 max_prefix_blocks: int = 256, ext_columns: int = 0, device: int = 0, tie_seed: int = 0,
+                 inflight_load: bool = False):
+        """inflight_load: the engine runs the inflight-load producer's counters (InFlightLoadProducer) and the token-load /
+        active-request scorers read them."""
         self.handler = profileHandler
         self.profiles = profiles
         if isinstance(profileHandler, DisaggProfileHandler):
@@ -355,7 +361,7 @@ class Scheduler:
         self.pick_k = ks.pop()
         self.engine = Engine(max_endpoints, primary, prefill, device=device, block_size_tokens=block_size_tokens,
                              max_prefix_blocks=max_prefix_blocks, non_cached_tokens=nct, always_disagg=always,
-                             n_ext_cols=ext_columns, tie_seed=tie_seed, pick_k=self.pick_k)
+                             n_ext_cols=ext_columns, tie_seed=tie_seed, pick_k=self.pick_k, inflight_load=inflight_load)
         self.block_size_tokens = block_size_tokens
 
     def _push_pool(self, endpoints, ext=None):
@@ -395,12 +401,47 @@ class Scheduler:
         if d["status"] != 0:
             raise SchedulingError("failed to find available decode workers" if self.prefill_name
                                   else "no endpoints available for the given request")
-        targets = lambda row: [eps[int(s)] for s in row if int(s) != capi.EPP_NO_ENDPOINT]     # picker order, k at most
-        res = {self.primary_name: ProfileRunResult(targets(primary), float(d["score"]), int(d["tie_count"]))}
+        slots = lambda row: [int(s) for s in row if int(s) != capi.EPP_NO_ENDPOINT]            # picker order, k at most
+        res = {self.primary_name: ProfileRunResult([eps[s] for s in slots(primary)], float(d["score"]), int(d["tie_count"]),
+                                                   slots(primary))}
         if self.prefill_name and d["prefill_pick"] != capi.EPP_NO_ENDPOINT:
-            res[self.prefill_name] = ProfileRunResult(targets(prefill), float(dd["prefill_score"]),
-                                                      int(dd["prefill_tie_count"]))
+            res[self.prefill_name] = ProfileRunResult([eps[s] for s in slots(prefill)], float(dd["prefill_score"]),
+                                                      int(dd["prefill_tie_count"]), slots(prefill))
         return SchedulingResult(res, self.primary_name)
+
+
+class InFlightLoadProducer:
+    """ "inflight-load-producer" (requestcontrol/dataproducer/inflightload/producer.go) on a Scheduler created with
+    inflight_load=True.  PreRequest (:110-129) runs on the device inside every Schedule call; this object carries the
+    other two hooks.  The token estimate reads the request's prompt length in bytes (include/epp_engine.h "In-flight
+    load"), where the reference reads the HTTP body size."""
+
+    def __init__(self, scheduler: Scheduler):
+        self.engine = scheduler.engine
+        self.prefill_name = scheduler.prefill_name
+
+    def ResponseBody(self, request: InferenceRequest, start_of_stream: bool = False, end_of_stream: bool = False):
+        """producer.go:131-168: the prefill target is released at the first chunk, every other target at the end."""
+        result = request.SchedulingResult
+        if result is None:
+            return
+        eps = []
+        for name, pr in result.ProfileResults.items():
+            if not pr.TargetSlots:
+                continue
+            if (start_of_stream and name == self.prefill_name) or (end_of_stream and name != self.prefill_name):
+                eps.append(pr.TargetSlots[0])
+        if eps:
+            self.engine.inflight_release(eps, [len(request.Prompt)] * len(eps))
+
+    def DeleteEndpoint(self, slot: int):
+        """producer.go:189-192 (endpoint-delete event): the slot's counters become 0."""
+        self.engine.inflight_reset([slot])
+
+    def Get(self, slot: int):
+        """InFlightLoad{Requests, Tokens} of a slot as the scorers see it now."""
+        req, tok = self.engine.inflight_get()
+        return int(req[slot]), int(tok[slot])
 
 
 class ApproxPrefixCacheProducer:
