@@ -82,6 +82,9 @@ struct epp_engine {
 
     Slot slot[2];
     cudaEvent_t ev[9] = {};
+    // post-pick update u (0 = no-hit-lru, 1 = inflight) of the device batch in flight is bracketed by ev[5 + 2u] /
+    // ev[6 + 2u]: epp_stats.last_kernel_ms[4 + u]
+    bool post_pick_timed[2] = {};
     cudaEvent_t user_ev[2] = {};    // epp_event_record / epp_event_elapsed_ms
     unsigned long long *wc_host = nullptr;   // pinned: work counters of an async batch
     bool async_pending = false;     // an EPP_BATCH_ASYNC batch whose stats have not been read back yet
@@ -107,7 +110,6 @@ struct epp_engine {
     int nohit_mask = 0;             // bit pi: profile pi has the scorer
     int32_t nohit_lru = 0;          // lruSize
     uint64_t nohit_seq = 1;         // sequence number of the next call's first Add (0 = not in the LRU)
-    bool nohit_timed = false;       // ev[5] / ev[6] bracket the update of the device batch in flight
     ProfileState prof_cold[kMaxProfiles];   // cold sets: base / order / groups with the LRU column
     DevBuf nh_last_seq, nh_pos, nh_misc, nh_sort_key, nh_order, nh_cold, nh_col[kMaxProfiles];
     DevBuf nh_prof;                 // ProfileDev[kMaxProfiles] of the cold sets (NoHitView::cold)
@@ -115,7 +117,6 @@ struct epp_engine {
     bool inflight = false;
     int inflight_mask = 0;          // bit pi: profile pi lists a token-load or active-request scorer (they read the counters)
     int32_t n_ext_total = 0;        // the caller's ext columns, then (with inflight) the token and request count columns
-    bool inflight_timed = false;    // ev[7] / ev[8] bracket the update of the device batch in flight
     DevBuf if_req, if_tok;
     std::mutex if_mu;               // guards if_pending only: releases and resets never wait for a batch
     std::unordered_map<uint32_t, InflightDelta> if_pending;   // folded releases / resets not applied yet
@@ -288,10 +289,11 @@ static int32_t alloc_profile(epp_engine *e, ProfileState &ps, bool random_picker
 }
 
 static int32_t rebuild_presence(epp_engine *h);
-static ProfileDev cold_profile_dev(epp_engine *h, int p);
-static const epp_profile_cfg &profile_cfg(const epp_engine *h, int p) {
+static ProfileDev profile_dev(epp_engine *h, int p, bool cold = false);
+static epp_profile_cfg &profile_cfg(epp_engine *h, int p) {
     return p == 0 ? h->cfg.primary : (p == 1 ? h->cfg.prefill : h->cfg.encode);
 }
+static const epp_profile_cfg &profile_cfg(const epp_engine *h, int p) { return profile_cfg(const_cast<epp_engine *>(h), p); }
 // Does any profile of the handler use a random picker?
 static bool any_random_picker(const epp_engine *h) {
     for (int p = 0; p < h->n_alloc_profiles; p++)
@@ -339,7 +341,7 @@ extern "C" int32_t epp_engine_create(const epp_config *cfg, epp_engine **out) {
         e->inflight = true;
         e->n_ext_total = cfg->n_ext_cols + 2;
         for (int pi = 0; pi < e->n_alloc_profiles; pi++) {
-            epp_profile_cfg &pc = pi == 0 ? e->cfg.primary : (pi == 1 ? e->cfg.prefill : e->cfg.encode);
+            epp_profile_cfg &pc = profile_cfg(e.get(), pi);
             for (int si = 0; si < pc.n_scorers; si++) {
                 if (pc.scorers[si].kind == EPP_SCORER_TOKEN_LOAD) pc.scorers[si].column = cfg->n_ext_cols;
                 else if (pc.scorers[si].kind == EPP_SCORER_ACTIVE_REQUEST) pc.scorers[si].column = cfg->n_ext_cols + 1;
@@ -389,11 +391,11 @@ extern "C" int32_t epp_engine_create(const epp_config *cfg, epp_engine **out) {
     memset(&e->idx_special_host, 0, sizeof(IndexSlot));
     e->idx_special_host.key = kEmptyKey;
     for (int pi = 0; pi < e->n_alloc_profiles; pi++) {
-        const epp_profile_cfg &pc = pi == 0 ? cfg->primary : (pi == 1 ? cfg->prefill : cfg->encode);
+        const epp_profile_cfg &pc = profile_cfg(e.get(), pi);
         for (int si = 0; si < pc.n_scorers; si++) if (pc.scorers[si].kind == EPP_SCORER_LORA_AFFINITY) e->lora_enabled = true;
     }
     for (int pi = 0; pi < e->n_alloc_profiles; pi++) {
-        const epp_profile_cfg &pc = pi == 0 ? cfg->primary : (pi == 1 ? cfg->prefill : cfg->encode);
+        const epp_profile_cfg &pc = profile_cfg(e.get(), pi);
         for (int si = 0; si < pc.n_scorers; si++) {
             if (pc.scorers[si].kind != EPP_SCORER_NO_HIT_LRU) continue;
             if (e->nohit_mask & (1 << pi)) return fail(EPP_ERR_INVALID, "profile %d lists the no-hit-lru scorer twice", pi);
@@ -423,10 +425,8 @@ extern "C" int32_t epp_engine_create(const epp_config *cfg, epp_engine **out) {
             }
     }
     e->general = cfg->pick_k > 1;
-    for (int pi = 0; pi < e->n_alloc_profiles; pi++) {
-        const epp_profile_cfg &pc = pi == 0 ? cfg->primary : (pi == 1 ? cfg->prefill : cfg->encode);
-        if (pc.affinity_threshold > 0.0) e->general = true;
-    }
+    for (int pi = 0; pi < e->n_alloc_profiles; pi++)
+        if (profile_cfg(e.get(), pi).affinity_threshold > 0.0) e->general = true;
     e->store.reset(new IndexStore((uint32_t)cfg->max_endpoints, cfg->lru_capacity_per_server, e->sm_count));
     { const char *v1 = getenv("EPP_INDEX_PATCH"); e->patch_enabled = v1 ? atoi(v1) : 1; }
     { const char *v1 = getenv("EPP_INDEX_LOAD"); e->index_load = v1 ? std::max(2, atoi(v1)) : 0; }
@@ -451,7 +451,7 @@ extern "C" int32_t epp_engine_create(const epp_config *cfg, epp_engine **out) {
         ProfileDev cold[kMaxProfiles];
         memset(cold, 0, sizeof cold);
         for (int pi = 0; pi < e->n_alloc_profiles; pi++)
-            if (e->nohit_mask & (1 << pi)) cold[pi] = cold_profile_dev(e.get(), pi);
+            if (e->nohit_mask & (1 << pi)) cold[pi] = profile_dev(e.get(), pi, true);
         CUDA_TRY(e->nh_prof.reserve(sizeof cold, &e->dev_bytes));
         CUDA_TRY(cudaMemcpy(e->nh_prof.p, cold, sizeof cold, cudaMemcpyHostToDevice));
     }
@@ -574,18 +574,39 @@ static PoolArrays pool_arrays(epp_engine *h) {
     return pa;
 }
 
-static ProfileDev profile_dev(epp_engine *h, int p) {
+// Profile p's warm set, or (cold) its no-hit-lru cold set: the cold set has the warm set's candidates (cand / n_cand /
+// qminmax) and its own contributions, base sums, order, groups and random-picker arrays.
+static ProfileDerived profile_derived(epp_engine *h, int p, bool cold) {
+    const ProfileState &w = h->prof[p], &x = cold ? h->prof_cold[p] : w;
+    ProfileDerived d{};
+    d.cand = w.cand.as<uint8_t>();
+    d.n_cand = w.n_cand.as<int32_t>();
+    d.qminmax = w.qminmax.as<int64_t>();
+    d.contrib = x.contrib.as<double>();
+    d.base = x.base.as<double>();
+    d.order = x.order.as<uint32_t>();
+    d.grp_size = x.grp_size.as<uint32_t>();
+    d.sort_key = x.sort_key.as<uint64_t>();
+    d.cands = x.cands.as<uint32_t>();
+    d.wcum = x.wcum.as<double>();
+    d.icum = x.icum.as<uint32_t>();
+    return d;
+}
+
+// What the pick kernels read of the same set.
+static ProfileDev profile_dev(epp_engine *h, int p, bool cold) {
+    const ProfileDerived d = profile_derived(h, p, cold);
     ProfileDev pd;
-    pd.cfg = p == 0 ? h->cfg.primary : (p == 1 ? h->cfg.prefill : h->cfg.encode);
-    pd.cand = h->prof[p].cand.as<uint8_t>();
-    pd.contrib = h->prof[p].contrib.as<double>();
-    pd.base = h->prof[p].base.as<double>();
-    pd.order = h->prof[p].order.as<uint32_t>();
-    pd.grp_size = h->prof[p].grp_size.as<uint32_t>();
-    pd.n_cand = h->prof[p].n_cand.as<int32_t>();
-    pd.cands = h->prof[p].cands.as<uint32_t>();
-    pd.wcum = h->prof[p].wcum.as<double>();
-    pd.icum = h->prof[p].icum.as<uint32_t>();
+    pd.cfg = profile_cfg(h, p);
+    pd.cand = d.cand;
+    pd.contrib = d.contrib;
+    pd.base = d.base;
+    pd.order = d.order;
+    pd.grp_size = d.grp_size;
+    pd.n_cand = d.n_cand;
+    pd.cands = d.cands;
+    pd.wcum = d.wcum;
+    pd.icum = d.icum;
     return pd;
 }
 
@@ -609,22 +630,10 @@ static int32_t nohit_derive(epp_engine *h, cudaStream_t s, bool gated, int *laun
     PoolArrays pa = pool_arrays(h);
     for (int p = 0; p < h->n_alloc_profiles; p++) {
         if (!(h->nohit_mask & (1 << p))) continue;
-        ProfileDerived d{};
-        d.cand = h->prof[p].cand.as<uint8_t>();
-        d.n_cand = h->prof[p].n_cand.as<int32_t>();
-        d.cands = h->prof_cold[p].cands.as<uint32_t>();
-        d.wcum = h->prof_cold[p].wcum.as<double>();
-        d.icum = h->prof_cold[p].icum.as<uint32_t>();
-        d.qminmax = h->prof[p].qminmax.as<int64_t>();
-        d.contrib = h->prof_cold[p].contrib.as<double>();
-        d.base = h->prof_cold[p].base.as<double>();
-        d.order = h->prof_cold[p].order.as<uint32_t>();
-        d.grp_size = h->prof_cold[p].grp_size.as<uint32_t>();
-        d.sort_key = h->prof_cold[p].sort_key.as<uint64_t>();
+        const ProfileDerived d = profile_derived(h, p, true);
         double *col = h->nh_col[p].as<double>();
         CUDA_TRY(launch_nohit_column(st, h->cfg.max_endpoints, d.cand, d.n_cand, col, gated, s, launches));
-        CUDA_TRY(launch_pool_order(pa, p == 0 ? h->cfg.primary : (p == 1 ? h->cfg.prefill : h->cfg.encode), d, h->Epad, col,
-                                   gated ? st.dirty : nullptr, s, launches));
+        CUDA_TRY(launch_pool_order(pa, profile_cfg(h, p), d, h->Epad, col, gated ? st.dirty : nullptr, s, launches));
     }
     return EPP_OK;
 }
@@ -644,30 +653,6 @@ static int32_t nohit_update(epp_engine *h, const epp_decision *dec, int64_t R, c
     return EPP_OK;
 }
 
-// The same on stream 0 of a device batch, bracketed by ev[5] / ev[6] (epp_stats.last_kernel_ms[4]).
-static int32_t nohit_update_timed(epp_engine *h, const epp_decision *dec, int64_t R, int *launches) {
-    if (!h->nohit_mask) return EPP_OK;
-    cudaStream_t s0 = h->slot[0].stream;
-    CUDA_TRY(cudaEventRecord(h->ev[5], s0));
-    EPP_TRY(nohit_update(h, dec, R, s0, launches));
-    CUDA_TRY(cudaEventRecord(h->ev[6], s0));
-    h->nohit_timed = true;
-    return EPP_OK;
-}
-
-// Profile p's cold set: its candidates, with the cold base / order / groups / contributions.
-static ProfileDev cold_profile_dev(epp_engine *h, int p) {
-    ProfileDev c = profile_dev(h, p);
-    c.contrib = h->prof_cold[p].contrib.as<double>();
-    c.base = h->prof_cold[p].base.as<double>();
-    c.order = h->prof_cold[p].order.as<uint32_t>();
-    c.grp_size = h->prof_cold[p].grp_size.as<uint32_t>();
-    c.cands = h->prof_cold[p].cands.as<uint32_t>();
-    c.wcum = h->prof_cold[p].wcum.as<double>();
-    c.icum = h->prof_cold[p].icum.as<uint32_t>();
-    return c;
-}
-
 // The no-hit-lru view of a pick launch whose first request is r0.
 static NoHitView nohit_view(epp_engine *h, int64_t r0) {
     NoHitView v;
@@ -681,19 +666,8 @@ static NoHitView nohit_view(epp_engine *h, int64_t r0) {
 
 // Request-independent scorer terms of profile p from the current pool (+ LoRA) snapshot, on the device.
 static int32_t derive_profile(epp_engine *h, int p, cudaStream_t s, int *launches) {
-    ProfileDerived d{};
-    d.cand = h->prof[p].cand.as<uint8_t>();
-    d.contrib = h->prof[p].contrib.as<double>();
-    d.cands = h->prof[p].cands.as<uint32_t>();
-    d.wcum = h->prof[p].wcum.as<double>();
-    d.icum = h->prof[p].icum.as<uint32_t>();
-    d.base = h->prof[p].base.as<double>();
-    d.order = h->prof[p].order.as<uint32_t>();
-    d.grp_size = h->prof[p].grp_size.as<uint32_t>();
-    d.sort_key = h->prof[p].sort_key.as<uint64_t>();
-    d.n_cand = h->prof[p].n_cand.as<int32_t>();
-    d.qminmax = h->prof[p].qminmax.as<int64_t>();
-    CUDA_TRY(launch_pool_prepare(pool_arrays(h), profile_cfg(h, p), d, h->Epad, h->shard_begin, h->shard_end, s, launches));
+    CUDA_TRY(launch_pool_prepare(pool_arrays(h), profile_cfg(h, p), profile_derived(h, p, false), h->Epad, h->shard_begin,
+                                 h->shard_end, s, launches));
     return EPP_OK;
 }
 
@@ -737,15 +711,22 @@ static int32_t inflight_update(epp_engine *h, const epp_decision *dec, const epp
     return inflight_rederive(h, s, launches);
 }
 
-// The same on stream 0 of a device batch, bracketed by ev[7] / ev[8] (epp_stats.last_kernel_ms[5]).
-static int32_t inflight_update_timed(epp_engine *h, const epp_decision *dec, const epp_decision_detail *det, int64_t R,
-                                     int *launches) {
-    if (!h->inflight) return EPP_OK;
-    cudaStream_t s0 = h->slot[0].stream;
-    CUDA_TRY(cudaEventRecord(h->ev[7], s0));
-    EPP_TRY(inflight_update(h, dec, det, h->in_len.as<int64_t>(), R, s0, launches));
-    CUDA_TRY(cudaEventRecord(h->ev[8], s0));
-    h->inflight_timed = true;
+// Everything a scheduling call updates behind its last pick kernel, in this order: the no-hit-lru LRU, then the in-flight
+// counters.  Per-call state that a pick changes is updated here and only here, so that every scheduling path carries it
+// alike.  timed (the device batch in flight): each update that is on is bracketed by its event pair for finish_async
+// (post_pick_timed).
+static int32_t after_picks(epp_engine *h, const epp_decision *dec, const epp_decision_detail *det, const int64_t *in_len,
+                           int64_t R, cudaStream_t s, int *launches, bool timed) {
+    if (h->nohit_mask) {
+        if (timed) CUDA_TRY(cudaEventRecord(h->ev[5], s));
+        EPP_TRY(nohit_update(h, dec, R, s, launches));
+        if (timed) { CUDA_TRY(cudaEventRecord(h->ev[6], s)); h->post_pick_timed[0] = true; }
+    }
+    if (h->inflight) {
+        if (timed) CUDA_TRY(cudaEventRecord(h->ev[7], s));
+        EPP_TRY(inflight_update(h, dec, det, in_len, R, s, launches));
+        if (timed) { CUDA_TRY(cudaEventRecord(h->ev[8], s)); h->post_pick_timed[1] = true; }
+    }
     return EPP_OK;
 }
 
@@ -1292,27 +1273,75 @@ static void attach_topk(epp_engine *h, GenView &g, uint32_t *const picks[kMaxPro
     g.topk_scores = scores ? scores + (size_t)r0 * (size_t)k : nullptr;
 }
 
-static PickParams pick_params(epp_engine *h, const Work &w, epp_decision *out, epp_decision_detail *detail,
-                              int32_t *out_match) {
-    PickParams p;
-    p.R = w.r1 - w.r0;
+// The top-k lists of a scheduling call: the caller's arrays (dst), and the device rows the pick kernels write (picks /
+// scores) -- the caller's own arrays for a device batch, engine staging for a host batch.
+struct TopkRows {
+    bool on = false;
+    uint32_t *dst[kMaxProfiles] = {};
+    double *dst_scores = nullptr;
+    uint32_t *picks[kMaxProfiles] = {};
+    double *scores = nullptr;
+};
+
+static int32_t topk_rows(epp_engine *h, const epp_topk_out *out, bool device, int64_t R, TopkRows &t) {
+    if (!out) return EPP_OK;
+    const size_t n = (size_t)R * (size_t)h->cfg.pick_k;
+    t.on = true;
+    t.dst[0] = out->primary; t.dst[1] = out->prefill; t.dst[2] = out->encode;
+    t.dst_scores = out->primary_scores;
+    for (int i = 0; i < kMaxProfiles; i++) {
+        t.picks[i] = t.dst[i];
+        if (!device && t.dst[i]) {
+            CUDA_TRY(h->topk_picks[i].reserve(sizeof(uint32_t) * n, &h->dev_bytes));
+            t.picks[i] = h->topk_picks[i].as<uint32_t>();
+        }
+    }
+    t.scores = t.dst_scores;
+    if (!device && t.scores) {
+        CUDA_TRY(h->topk_scores.reserve(sizeof(double) * n, &h->dev_bytes));
+        t.scores = h->topk_scores.as<double>();
+    }
+    return EPP_OK;
+}
+
+// Copies rows [r0, r0 + n) of a host batch's lists from the staging to the caller's arrays on s.
+static int32_t topk_copy_back(epp_engine *h, const TopkRows &t, int64_t r0, int64_t n, cudaStream_t s) {
+    const size_t K = (size_t)h->cfg.pick_k, o = (size_t)r0 * K, m = (size_t)n * K;
+    for (int i = 0; i < kMaxProfiles; i++)
+        if (t.dst[i]) CUDA_TRY(cudaMemcpyAsync(t.dst[i] + o, t.picks[i] + o, sizeof(uint32_t) * m, cudaMemcpyDeviceToHost, s));
+    if (t.scores) CUDA_TRY(cudaMemcpyAsync(t.dst_scores + o, t.scores + o, sizeof(double) * m, cudaMemcpyDeviceToHost, s));
+    return EPP_OK;
+}
+
+// The decision fields that every pick launch (PickParams, DensePickParams) fills alike, for a launch whose first request
+// is r0.  Each caller sets the rest, and may override block_size_tokens.
+template <class P> static void fill_decision_fields(epp_engine *h, P &p, int64_t r0) {
     p.E = h->cfg.max_endpoints;
-    p.max_blocks = h->cfg.max_prefix_blocks;
     p.block_size_tokens = h->cfg.block_size_tokens;
     p.n_profiles = h->n_profiles;
-    p.encode_on = h->cfg.encode_enabled ? 1 : 0;
-    p.multimodal = w.multimodal_dev ? w.multimodal_dev + w.r0 : nullptr;
     p.always_disagg = h->cfg.always_disagg;
     p.non_cached_tokens = h->cfg.non_cached_tokens;
     for (int i = 0; i < h->n_alloc_profiles; i++) p.prof[i] = profile_dev(h, i);
+    p.lora = lora_dev(h);
+    p.tie_base = h->stats.n_decisions + (uint64_t)r0;
+    p.gen = gen_view(h);
+    p.nohit = nohit_view(h, r0);
+}
+
+static PickParams pick_params(epp_engine *h, const Work &w, epp_decision *out, epp_decision_detail *detail,
+                              int32_t *out_match) {
+    PickParams p;
+    fill_decision_fields(h, p, w.r0);
+    p.R = w.r1 - w.r0;
+    p.max_blocks = h->cfg.max_prefix_blocks;
+    p.encode_on = h->cfg.encode_enabled ? 1 : 0;
+    p.multimodal = w.multimodal_dev ? w.multimodal_dev + w.r0 : nullptr;
     p.tie_seed = h->shard_end != 0xFFFFFFFFu || h->shard_begin != 0 ? 0 : h->cfg.tie_seed;      // sharded mode: lowest slot
-    p.tie_base = h->stats.n_decisions + (uint64_t)w.r0;
     p.hashes = w.hashes_out;
     p.nblocks = w.nblocks_out;
     p.bound = nullptr;
     p.in_len = h->in_len.as<int64_t>() + w.r0;
     p.model_ids = w.model_ids_dev ? w.model_ids_dev + w.r0 : nullptr;
-    p.lora = lora_dev(h);
     p.index = index_view(h);
     p.out = out;
     p.detail = detail;
@@ -1326,8 +1355,6 @@ static PickParams pick_params(epp_engine *h, const Work &w, epp_decision *out, e
     p.overflow_list = nullptr;
     p.overflow_n = nullptr;
     p.req_next = nullptr;
-    p.gen = gen_view(h);
-    p.nohit = nohit_view(h, w.r0);
     return p;
 }
 
@@ -1413,17 +1440,12 @@ static int32_t finish_async(epp_engine *h) {
     h->stats.last_hash_bytes_stored = h->wc_host[2];
     h->stats.last_prompt_bytes_read = h->wc_host[3];
     h->stats.last_kernel_launches = (uint64_t)h->async_launches;
-    if (h->nohit_timed) {
-        float tn = 0;
-        cudaEventElapsedTime(&tn, h->ev[5], h->ev[6]);
-        h->stats.last_kernel_ms[4] = tn;
-        h->nohit_timed = false;
-    }
-    if (h->inflight_timed) {
-        float ti = 0;
-        cudaEventElapsedTime(&ti, h->ev[7], h->ev[8]);
-        h->stats.last_kernel_ms[5] = ti;
-        h->inflight_timed = false;
+    for (int u = 0; u < 2; u++) {
+        if (!h->post_pick_timed[u]) continue;
+        float tu = 0;
+        cudaEventElapsedTime(&tu, h->ev[5 + 2 * u], h->ev[6 + 2 * u]);
+        h->stats.last_kernel_ms[4 + u] = tu;
+        h->post_pick_timed[u] = false;
     }
     return EPP_OK;
 }
@@ -1598,8 +1620,8 @@ static int32_t run_small(epp_engine *h, const BatchView &v, int mode, const uint
         CUDA_TRY(cudaMemcpyAsync(h->small_det, h->details.p, sizeof(epp_decision_detail) * (size_t)R, cudaMemcpyDeviceToHost, s0));
         CUDA_TRY(cudaStreamSynchronize(s0));
     }
-    EPP_TRY(nohit_update(h, h->small_dec, R, s0, &launches));   // reads the decisions from the pinned copy (UVA)
-    EPP_TRY(inflight_update(h, h->small_dec, h->small_det, h->in_len.as<int64_t>(), R, s0, &launches));
+    // reads the decisions from the pinned copies (UVA)
+    EPP_TRY(after_picks(h, h->small_dec, h->small_det, h->in_len.as<int64_t>(), R, s0, &launches, false));
     memcpy(out_dec, h->small_dec, sizeof(epp_decision) * (size_t)R);
     if (out_detail) memcpy(out_detail, h->small_det, sizeof(epp_decision_detail) * (size_t)R);
     h->small_stats_pending = true;
@@ -1631,29 +1653,8 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
         }
     }
     if (h->async_pending && !(v.device && v.async)) EPP_TRY(finish_async(h));
-    // top-k lists of the call in progress: the caller's device arrays, or device staging for a host batch
-    const epp_topk_out *tk = mode == Mode::Schedule ? h->cur_topk : nullptr;
-    const size_t K = (size_t)h->cfg.pick_k;
-    uint32_t *tk_picks[kMaxProfiles] = {nullptr, nullptr, nullptr};
-    uint32_t *tk_host[kMaxProfiles] = {nullptr, nullptr, nullptr};
-    double *tk_scores = nullptr;
-    if (tk) {
-        tk_host[0] = tk->primary; tk_host[1] = tk->prefill; tk_host[2] = tk->encode;
-        if (v.device) {
-            for (int i = 0; i < kMaxProfiles; i++) tk_picks[i] = tk_host[i];
-            tk_scores = tk->primary_scores;
-        } else {
-            for (int i = 0; i < kMaxProfiles; i++)
-                if (tk_host[i]) {
-                    CUDA_TRY(h->topk_picks[i].reserve(sizeof(uint32_t) * (size_t)R * K, &h->dev_bytes));
-                    tk_picks[i] = h->topk_picks[i].as<uint32_t>();
-                }
-            if (tk->primary_scores) {
-                CUDA_TRY(h->topk_scores.reserve(sizeof(double) * (size_t)R * K, &h->dev_bytes));
-                tk_scores = h->topk_scores.as<double>();
-            }
-        }
-    }
+    TopkRows tk;
+    EPP_TRY(topk_rows(h, mode == Mode::Schedule ? h->cur_topk : nullptr, v.device, R, tk));
     const bool pipelined = v.device && v.async && mode == Mode::Schedule && h->dev_chunks > 1 && R >= 2 * 4096 && !h->pick_global;
     // the endpoint-sharded mode's local table is not the global one: its rows stay whole
     const bool trim = mode == Mode::Schedule && !keep_hashes && h->hash_trim && h->shard_begin == 0 && h->shard_end == 0xFFFFFFFFu;
@@ -1698,7 +1699,7 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
                 Work w{r0, r1, v.offsets ? v.data : v.data + (uint64_t)r0 * v.uniform_len, v.offsets, v.lengths, v.uniform_len,
                        v.model_ids, or_bits, h->hashes.as<uint64_t>() + (size_t)r0 * B, h->nblocks.as<int32_t>() + r0, v.multimodal};
                 PickParams pp = pick_params(h, w, dec_base + r0, det_out ? det_out + r0 : nullptr, nullptr);
-                if (tk) attach_topk(h, pp.gen, tk_picks, tk_scores, r0);
+                if (tk.on) attach_topk(h, pp.gen, tk.picks, tk.scores, r0);
                 Slot &sl = h->slot[k & 1];
                 HashParams hp = hash_params(h, w, sl);
                 if (trim) trim_rows(h, w, hp, pp);
@@ -1718,7 +1719,7 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
             epp_decision *dec = (mode == Mode::Schedule && out_dec) ? out_dec : h->decisions.as<epp_decision>();
             PickParams pp = pick_params(h, w, dec, mode == Mode::Schedule ? det_out : nullptr, mode == Mode::Match ? out_match : nullptr);
             pp.work_counters = h->work_counters.as<unsigned long long>();
-            if (tk) attach_topk(h, pp.gen, tk_picks, tk_scores, 0);
+            if (tk.on) attach_topk(h, pp.gen, tk.picks, tk.scores, 0);
             HashParams hp = hash_params(h, w, h->slot[0]);
             hp.stored = h->work_counters.as<unsigned long long>() + 2;
             hp.read = h->work_counters.as<unsigned long long>() + 3;
@@ -1726,11 +1727,9 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
             EPP_TRY(launch_cycle(h, h->slot[0], hp, pp, &launches, h->ev));
         }
         CUDA_TRY(cudaEventRecord(h->ev[4], s0));
-        if (mode == Mode::Schedule) {              // after ev[4]: last_kernel_ms[3] stays the match + pick time
-            epp_decision *dec = out_dec ? out_dec : h->decisions.as<epp_decision>();
-            EPP_TRY(nohit_update_timed(h, dec, R, &launches));
-            EPP_TRY(inflight_update_timed(h, dec, det_out, R, &launches));
-        }
+        if (mode == Mode::Schedule)                // after ev[4]: last_kernel_ms[3] stays the match + pick time
+            EPP_TRY(after_picks(h, out_dec ? out_dec : h->decisions.as<epp_decision>(), det_out, h->in_len.as<int64_t>(), R,
+                                s0, &launches, true));
         CUDA_TRY(cudaMemcpyAsync(h->wc_host, h->work_counters.p, sizeof(unsigned long long) * 4, cudaMemcpyDeviceToHost, s0));
         h->async_pending = true;
         h->async_launches = launches;
@@ -1740,7 +1739,7 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
     }
 
     // ---- small host batch in pinned memory: one zero-copy launch, no copy engine, no stream synchronisation
-    if (mode == Mode::Schedule && !tk && out_dec) {
+    if (mode == Mode::Schedule && !tk.on && out_dec) {
         const uint8_t *data_dev = nullptr;
         const int sm = small_batch_mode(h, v, &data_dev);
         if (sm) return run_small(h, v, sm, data_dev, out_dec, out_detail);
@@ -1821,19 +1820,14 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
             epp_decision *dec = h->decisions.as<epp_decision>() + c.r0;
             epp_decision_detail *det = h->details.as<epp_decision_detail>() + c.r0;
             PickParams pp = pick_params(h, w, dec, det, dm);
-            if (tk) attach_topk(h, pp.gen, tk_picks, tk_scores, c.r0);
+            if (tk.on) attach_topk(h, pp.gen, tk.picks, tk.scores, c.r0);
             HashParams hp = hash_params(h, w, sl);
             if (trim) trim_rows(h, w, hp, pp);
             EPP_TRY(launch_cycle(h, sl, hp, pp, &launches, nullptr));
             if (mode == Mode::Schedule) {
                 if (out_dec) CUDA_TRY(cudaMemcpyAsync(out_dec + c.r0, dec, sizeof(epp_decision) * nreq, cudaMemcpyDeviceToHost, s));
                 if (out_detail) CUDA_TRY(cudaMemcpyAsync(out_detail + c.r0, det, sizeof(epp_decision_detail) * nreq, cudaMemcpyDeviceToHost, s));
-                if (tk) {
-                    const size_t o = (size_t)c.r0 * K;
-                    for (int i = 0; i < kMaxProfiles; i++)
-                        if (tk_host[i]) CUDA_TRY(cudaMemcpyAsync(tk_host[i] + o, tk_picks[i] + o, sizeof(uint32_t) * nreq * K, cudaMemcpyDeviceToHost, s));
-                    if (tk_scores) CUDA_TRY(cudaMemcpyAsync(tk->primary_scores + o, tk_scores + o, sizeof(double) * nreq * K, cudaMemcpyDeviceToHost, s));
-                }
+                if (tk.on) EPP_TRY(topk_copy_back(h, tk, c.r0, (int64_t)nreq, s));
             } else {
                 if (out_match) CUDA_TRY(cudaMemcpyAsync(out_match + (size_t)c.r0 * E, dm, sizeof(int32_t) * nreq * E, cudaMemcpyDeviceToHost, s));
                 if (out_total) CUDA_TRY(cudaMemcpyAsync(out_total + c.r0, w.nblocks_out, sizeof(int32_t) * nreq, cudaMemcpyDeviceToHost, s));
@@ -1841,11 +1835,9 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
         }
     }
     CUDA_TRY(cudaStreamSynchronize(h->slot[1].stream));
-    if (mode == Mode::Schedule) {
-        EPP_TRY(nohit_update(h, h->decisions.as<epp_decision>(), R, s0, &launches));
-        EPP_TRY(inflight_update(h, h->decisions.as<epp_decision>(), h->details.as<epp_decision_detail>(), h->in_len.as<int64_t>(),
-                                R, s0, &launches));
-    }
+    if (mode == Mode::Schedule)
+        EPP_TRY(after_picks(h, h->decisions.as<epp_decision>(), h->details.as<epp_decision_detail>(), h->in_len.as<int64_t>(), R,
+                            s0, &launches, false));
     CUDA_TRY(cudaEventRecord(h->ev[1], s0));
     CUDA_TRY(cudaStreamSynchronize(s0));
     float t_all = 0;
@@ -1949,6 +1941,32 @@ extern "C" int32_t epp_index_add_picked(epp_engine *h) {
 // ------------------------------------------------------------------------------------------------
 // plugin-parity entry points on injected match info
 // ------------------------------------------------------------------------------------------------
+struct MatchRows {
+    const int32_t *match, *total;
+    const uint32_t *model_ids;
+};
+
+// The injected rows of a call (match [R][E], total [R], model_ids [R] or nullptr) on the device: a host call's are
+// copied to engine buffers on s, a device call's are used as they are.
+static int32_t match_rows(epp_engine *h, int64_t R, const int32_t *match, const int32_t *total, const uint32_t *model_ids,
+                          bool dev, cudaStream_t s, MatchRows &m) {
+    m = {match, total, model_ids};
+    if (dev) return EPP_OK;
+    const size_t n = (size_t)R * (size_t)h->cfg.max_endpoints;
+    CUDA_TRY(h->dense_match.reserve(sizeof(int32_t) * n, &h->dev_bytes));
+    CUDA_TRY(h->dense_total.reserve(sizeof(int32_t) * (size_t)R, &h->dev_bytes));
+    CUDA_TRY(cudaMemcpyAsync(h->dense_match.p, match, sizeof(int32_t) * n, cudaMemcpyHostToDevice, s));
+    CUDA_TRY(cudaMemcpyAsync(h->dense_total.p, total, sizeof(int32_t) * (size_t)R, cudaMemcpyHostToDevice, s));
+    m.match = h->dense_match.as<int32_t>();
+    m.total = h->dense_total.as<int32_t>();
+    if (model_ids) {
+        CUDA_TRY(h->score_models.reserve(sizeof(uint32_t) * (size_t)R, &h->dev_bytes));
+        CUDA_TRY(cudaMemcpyAsync(h->score_models.p, model_ids, sizeof(uint32_t) * (size_t)R, cudaMemcpyHostToDevice, s));
+        m.model_ids = h->score_models.as<uint32_t>();
+    }
+    return EPP_OK;
+}
+
 extern "C" int32_t epp_score(epp_engine *h, int64_t n_requests, const int32_t *match, const int32_t *total,
                              const uint32_t *model_ids, int32_t profile, int32_t scorer_index, double *out_scores,
                              uint32_t flags) {
@@ -1958,29 +1976,17 @@ extern "C" int32_t epp_score(epp_engine *h, int64_t n_requests, const int32_t *m
     EPP_TRY(join_streams(h));
     if (!h->pool_ready) return fail(EPP_ERR_STATE, "epp_pool_set has not been called");
     if (profile < 0 || profile >= h->n_alloc_profiles) return fail(EPP_ERR_INVALID, "profile %d out of range", profile);
-    const epp_profile_cfg &pc = profile == 0 ? h->cfg.primary : (profile == 1 ? h->cfg.prefill : h->cfg.encode);
-    if (scorer_index < -1 || scorer_index >= pc.n_scorers) return fail(EPP_ERR_INVALID, "scorer_index %d out of range", scorer_index);
+    if (scorer_index < -1 || scorer_index >= profile_cfg(h, profile).n_scorers) return fail(EPP_ERR_INVALID, "scorer_index %d out of range", scorer_index);
     if (n_requests == 0) return EPP_OK;
     const size_t E = (size_t)h->cfg.max_endpoints, n = (size_t)n_requests * E;
     cudaStream_t s = h->slot[0].stream;
     const bool dev = (flags & EPP_BATCH_DEVICE_PTRS) != 0;
-    const int32_t *d_match = match, *d_total = total;
+    MatchRows m;
+    EPP_TRY(match_rows(h, n_requests, match, total, model_ids, dev, s, m));
     double *d_out = out_scores;
     if (!dev) {
-        CUDA_TRY(h->dense_match.reserve(sizeof(int32_t) * n, &h->dev_bytes));
-        CUDA_TRY(h->dense_total.reserve(sizeof(int32_t) * (size_t)n_requests, &h->dev_bytes));
         CUDA_TRY(h->dense_scores.reserve(sizeof(double) * n, &h->dev_bytes));
-        CUDA_TRY(cudaMemcpyAsync(h->dense_match.p, match, sizeof(int32_t) * n, cudaMemcpyHostToDevice, s));
-        CUDA_TRY(cudaMemcpyAsync(h->dense_total.p, total, sizeof(int32_t) * (size_t)n_requests, cudaMemcpyHostToDevice, s));
-        d_match = h->dense_match.as<int32_t>();
-        d_total = h->dense_total.as<int32_t>();
         d_out = h->dense_scores.as<double>();
-    }
-    const uint32_t *d_models = model_ids;
-    if (!dev && model_ids) {
-        CUDA_TRY(h->score_models.reserve(sizeof(uint32_t) * (size_t)n_requests, &h->dev_bytes));
-        CUDA_TRY(cudaMemcpyAsync(h->score_models.p, model_ids, sizeof(uint32_t) * (size_t)n_requests, cudaMemcpyHostToDevice, s));
-        d_models = h->score_models.as<uint32_t>();
     }
     int launches = 0;
     // no-hit-lru: each request's cold bit for this profile selects its cold set (no_hit_lru.go:259-275)
@@ -1990,11 +1996,12 @@ extern "C" int32_t epp_score(epp_engine *h, int64_t n_requests, const int32_t *m
     if (nh) {
         CUDA_TRY(h->nh_cold.reserve((size_t)n_requests, &h->dev_bytes));
         cold = h->nh_cold.as<uint8_t>();
-        CUDA_TRY(launch_nohit_cold_rows(n_requests, h->cfg.max_endpoints, pw.cand, d_match, cold, s, &launches));
+        CUDA_TRY(launch_nohit_cold_rows(n_requests, h->cfg.max_endpoints, pw.cand, m.match, cold, s, &launches));
     }
-    CUDA_TRY(launch_score_dense(n_requests, h->cfg.max_endpoints, pw, nh ? cold_profile_dev(h, profile) : pw, cold,
+    CUDA_TRY(launch_score_dense(n_requests, h->cfg.max_endpoints, pw, nh ? profile_dev(h, profile, true) : pw, cold,
                                 nh ? h->nh_col[profile].as<double>() : nullptr, pool_arrays(h),
-                                h->prof[profile].qminmax.as<int64_t>(), d_match, d_total, d_models, scorer_index, d_out, s, &launches));
+                                h->prof[profile].qminmax.as<int64_t>(), m.match, m.total, m.model_ids, scorer_index, d_out, s,
+                                &launches));
     if (!dev) CUDA_TRY(cudaMemcpyAsync(out_scores, d_out, sizeof(double) * n, cudaMemcpyDeviceToHost, s));
     CUDA_TRY(cudaStreamSynchronize(s));
     return EPP_OK;
@@ -2010,79 +2017,46 @@ static int32_t with_match_impl(epp_engine *h, int64_t n_requests, const int32_t 
     EPP_TRY(join_streams(h));
     if (!h->pool_ready) return fail(EPP_ERR_STATE, "epp_pool_set has not been called");
     if (n_requests == 0) return EPP_OK;
-    const size_t E = (size_t)h->cfg.max_endpoints, n = (size_t)n_requests * E, R = (size_t)n_requests;
+    const size_t R = (size_t)n_requests;
     cudaStream_t s = h->slot[0].stream;
     const bool dev = (flags & EPP_BATCH_DEVICE_PTRS) != 0;
     int launches = 0;
     EPP_TRY(inflight_flush(h, s, &launches));
     DensePickParams p;
+    fill_decision_fields(h, p, 0);
     p.R = n_requests;
-    p.E = h->cfg.max_endpoints;
-    p.block_size_tokens = block_size_tokens > 0 ? block_size_tokens : h->cfg.block_size_tokens;
-    p.n_profiles = h->n_profiles;
+    if (block_size_tokens > 0) p.block_size_tokens = block_size_tokens;
     p.encode_on = 0;                              // the injected-match entry point has no multimodal flags
     p.multimodal = nullptr;
-    p.always_disagg = h->cfg.always_disagg;
-    p.non_cached_tokens = h->cfg.non_cached_tokens;
-    for (int i = 0; i < h->n_alloc_profiles; i++) p.prof[i] = profile_dev(h, i);
-    p.lora = lora_dev(h);
-    p.model_ids = model_ids;
     p.tie_seed = h->cfg.tie_seed;
-    p.tie_base = h->stats.n_decisions;
-    p.gen = gen_view(h);
-    p.nohit = nohit_view(h, 0);
-    if (h->nohit_mask) CUDA_TRY(h->nh_cold.reserve(R, &h->dev_bytes));
-    p.nohit.cold_out = h->nohit_mask ? h->nh_cold.as<uint8_t>() : nullptr;
-    const size_t K = (size_t)h->cfg.pick_k;
-    uint32_t *tk_host[kMaxProfiles] = {nullptr, nullptr, nullptr};
-    uint32_t *tk_picks[kMaxProfiles] = {nullptr, nullptr, nullptr};
-    double *tk_scores = nullptr;
-    if (topk) {
-        tk_host[0] = topk->primary; tk_host[1] = topk->prefill; tk_host[2] = topk->encode;
-        for (int i = 0; i < kMaxProfiles; i++) {
-            tk_picks[i] = tk_host[i];
-            if (!dev && tk_host[i]) {
-                CUDA_TRY(h->topk_picks[i].reserve(sizeof(uint32_t) * R * K, &h->dev_bytes));
-                tk_picks[i] = h->topk_picks[i].as<uint32_t>();
-            }
-        }
-        tk_scores = topk->primary_scores;
-        if (!dev && tk_scores) {
-            CUDA_TRY(h->topk_scores.reserve(sizeof(double) * R * K, &h->dev_bytes));
-            tk_scores = h->topk_scores.as<double>();
-        }
-        attach_topk(h, p.gen, tk_picks, tk_scores, 0);
+    if (h->nohit_mask) {
+        CUDA_TRY(h->nh_cold.reserve(R, &h->dev_bytes));
+        p.nohit.cold_out = h->nh_cold.as<uint8_t>();
     }
+    TopkRows tk;
+    EPP_TRY(topk_rows(h, topk, dev, n_requests, tk));
+    if (tk.on) attach_topk(h, p.gen, tk.picks, tk.scores, 0);
+    if (!dev) EPP_TRY(reserve_batch(h, n_requests));
+    MatchRows m;
+    EPP_TRY(match_rows(h, n_requests, match, total, model_ids, dev, s, m));
+    p.match = m.match;
+    p.total = m.total;
+    p.model_ids = m.model_ids;
     if (dev) {
-        p.match = match; p.total = total; p.in_len = input_len_bytes; p.out = out; p.detail = detail;
+        p.in_len = input_len_bytes; p.out = out; p.detail = detail;
     } else {
-        if (model_ids) {
-            CUDA_TRY(h->score_models.reserve(sizeof(uint32_t) * R, &h->dev_bytes));
-            CUDA_TRY(cudaMemcpyAsync(h->score_models.p, model_ids, sizeof(uint32_t) * R, cudaMemcpyHostToDevice, s));
-            p.model_ids = h->score_models.as<uint32_t>();
-        }
-        EPP_TRY(reserve_batch(h, n_requests));
-        CUDA_TRY(h->dense_match.reserve(sizeof(int32_t) * n, &h->dev_bytes));
-        CUDA_TRY(h->dense_total.reserve(sizeof(int32_t) * R, &h->dev_bytes));
-        CUDA_TRY(cudaMemcpyAsync(h->dense_match.p, match, sizeof(int32_t) * n, cudaMemcpyHostToDevice, s));
-        CUDA_TRY(cudaMemcpyAsync(h->dense_total.p, total, sizeof(int32_t) * R, cudaMemcpyHostToDevice, s));
         if (input_len_bytes) CUDA_TRY(cudaMemcpyAsync(h->in_len.p, input_len_bytes, sizeof(int64_t) * R, cudaMemcpyHostToDevice, s));
         else CUDA_TRY(cudaMemsetAsync(h->in_len.p, 0, sizeof(int64_t) * R, s));
-        p.match = h->dense_match.as<int32_t>();
-        p.total = h->dense_total.as<int32_t>();
         p.in_len = h->in_len.as<int64_t>();
         p.out = h->decisions.as<epp_decision>();
         p.detail = h->details.as<epp_decision_detail>();
     }
     CUDA_TRY(launch_dense_pick(p, s, &launches));
-    EPP_TRY(nohit_update(h, p.out, n_requests, s, &launches));
-    EPP_TRY(inflight_update(h, p.out, p.detail, p.in_len, n_requests, s, &launches));
+    EPP_TRY(after_picks(h, p.out, p.detail, p.in_len, n_requests, s, &launches, false));
     if (!dev) {
         CUDA_TRY(cudaMemcpyAsync(out, p.out, sizeof(epp_decision) * R, cudaMemcpyDeviceToHost, s));
         if (detail) CUDA_TRY(cudaMemcpyAsync(detail, p.detail, sizeof(epp_decision_detail) * R, cudaMemcpyDeviceToHost, s));
-        for (int i = 0; i < kMaxProfiles; i++)
-            if (tk_host[i]) CUDA_TRY(cudaMemcpyAsync(tk_host[i], tk_picks[i], sizeof(uint32_t) * R * K, cudaMemcpyDeviceToHost, s));
-        if (topk && topk->primary_scores) CUDA_TRY(cudaMemcpyAsync(topk->primary_scores, tk_scores, sizeof(double) * R * K, cudaMemcpyDeviceToHost, s));
+        if (tk.on) EPP_TRY(topk_copy_back(h, tk, 0, n_requests, s));
     }
     CUDA_TRY(cudaStreamSynchronize(s));
     h->kept_R = 0;
@@ -2231,14 +2205,20 @@ extern "C" int32_t epp_event_elapsed_ms(epp_engine *h, double *out_ms) {
 // ------------------------------------------------------------------------------------------------
 // endpoint-sharded mode (kernels: pick_kernels.cu k_shard_*, shard_p2p.cu)
 // ------------------------------------------------------------------------------------------------
+// Per-call state that no rank can keep from its own shard alone.
+static int32_t check_shardable(const epp_engine *h) {
+    if (h->nohit_mask) return fail(EPP_ERR_INVALID, "endpoint-sharded mode does not support the no-hit-lru scorer (coldness needs every rank's match)");
+    if (any_random_picker(h)) return fail(EPP_ERR_INVALID, "endpoint-sharded mode does not support the random pickers (a weighted draw needs every rank's scores)");
+    if (h->inflight) return fail(EPP_ERR_INVALID, "endpoint-sharded mode does not support the inflight-load producer");
+    return EPP_OK;
+}
+
 extern "C" int32_t epp_shard_set(epp_engine *h, uint32_t ep_begin, uint32_t ep_end) {
     if (!h || ep_begin > ep_end) return fail(EPP_ERR_INVALID, "bad shard range");
     std::lock_guard<std::mutex> lk(h->mu);
     if (h->cfg.handler != EPP_HANDLER_SINGLE) return fail(EPP_ERR_INVALID, "endpoint-sharded mode supports the single-profile handler only");
     if (h->general) return fail(EPP_ERR_INVALID, "endpoint-sharded mode supports neither pick_k > 1 nor the prefix-cache-affinity-filter (both need every candidate's score on one rank)");
-    if (h->nohit_mask) return fail(EPP_ERR_INVALID, "endpoint-sharded mode does not support the no-hit-lru scorer (coldness needs every rank's match)");
-    if (any_random_picker(h)) return fail(EPP_ERR_INVALID, "endpoint-sharded mode does not support the random pickers (a weighted draw needs every rank's scores)");
-    if (h->inflight) return fail(EPP_ERR_INVALID, "endpoint-sharded mode does not support the inflight-load producer");
+    EPP_TRY(check_shardable(h));
     h->shard_begin = ep_begin;
     h->shard_end = ep_end;
     h->pool_ready = false;          // candidates are derived per shard: epp_pool_set must follow
@@ -2342,9 +2322,7 @@ extern "C" int32_t epp_shard_p2p_export(epp_engine *h, int64_t max_requests, uin
 extern "C" int32_t epp_shard_p2p_connect(epp_engine *h, int32_t n_ranks, int32_t rank, const void *peers, int32_t ipc_handles) {
     if (!h || n_ranks <= 0 || n_ranks > 64 || rank < 0 || rank >= n_ranks || !peers) return fail(EPP_ERR_INVALID, "bad arguments");
     std::lock_guard<std::mutex> lk(h->mu);
-    if (h->nohit_mask) return fail(EPP_ERR_INVALID, "endpoint-sharded mode does not support the no-hit-lru scorer (coldness needs every rank's match)");
-    if (any_random_picker(h)) return fail(EPP_ERR_INVALID, "endpoint-sharded mode does not support the random pickers (a weighted draw needs every rank's scores)");
-    if (h->inflight) return fail(EPP_ERR_INVALID, "endpoint-sharded mode does not support the inflight-load producer");
+    EPP_TRY(check_shardable(h));
     EPP_TRY(set_device(h));
     EPP_TRY(join_streams(h));
     if (!h->p2p_buf) return fail(EPP_ERR_STATE, "epp_shard_p2p_export has not been called");

@@ -282,8 +282,14 @@ cudaError_t launch_match_pick(const PickParams &p, uint32_t *gscratch, int grid,
 // overflows it are appended to p.overflow_list for the dense-counter kernel).  8 warps per CTA, 6-8 CTAs per SM;
 // ctas = 6 bounds the one-profile lowest-slot build to 40 registers instead of 32 (the engine's EPP_MATCH_CTAS).
 cudaError_t launch_match_pick_sparse(const PickParams &p, int sm_count, int ctas, cudaStream_t s, int *launches);
-// Does some profile of the launch have a random picker?  Then the sparse and small-batch paths launch their _rand builds.
-bool any_random_picker(const PickParams &p);
+// Does some profile of the launch (PickParams, DensePickParams) have a random picker?  Then the sparse, small-batch,
+// dense-counter and injected-match paths launch their _rand builds.
+template <class Params> inline bool any_random_picker(const Params &p) {
+    const int np = p.encode_on ? 3 : (p.n_profiles >= 2 ? 2 : 1);
+    for (int i = 0; i < np; i++)
+        if (p.prof[i].cfg.picker) return true;
+    return false;
+}
 // cycle_small.cu: a1-a14 of a small host batch in ONE launch, one CTA per request, prompts read from and decisions
 // written to PINNED HOST memory (zero-copy); flags[r] = epoch (| 0x80000000 when the request overflowed the sparse map and
 // was appended to pp.overflow_list instead of being decided) is written last, after a system-scope fence.

@@ -86,13 +86,6 @@ cudaError_t launch_nohit(const PickParams &p, int sm_count, cudaStream_t s) {
 }
 }  // namespace
 
-bool any_random_picker(const PickParams &p) {
-    const int np = p.encode_on ? 3 : (p.n_profiles >= 2 ? 2 : 1);
-    for (int i = 0; i < np; i++)
-        if (p.prof[i].cfg.picker) return true;
-    return false;
-}
-
 cudaError_t launch_match_pick_sparse(const PickParams &p, int sm_count, int ctas, cudaStream_t s, int *launches) {
     if (p.R <= 0) return cudaSuccess;
     if (!p.req_next || p.R > INT32_MAX) return cudaErrorInvalidValue;

@@ -576,10 +576,7 @@ __global__ void __launch_bounds__(256) k_dense_pick_rand(DensePickParams p) { de
 cudaError_t launch_dense_pick(const DensePickParams &p, cudaStream_t s, int *launches) {
     if (p.R <= 0) return cudaSuccess;
     int64_t threads = p.R * 32;
-    const int np = p.encode_on ? 3 : (p.n_profiles >= 2 ? 2 : 1);
-    bool rand = false;
-    for (int i = 0; i < np; i++) rand |= p.prof[i].cfg.picker != EPP_PICKER_MAX_SCORE;
-    if (rand) k_dense_pick_rand<<<(unsigned)((threads + 255) / 256), 256, 0, s>>>(p);
+    if (any_random_picker(p)) k_dense_pick_rand<<<(unsigned)((threads + 255) / 256), 256, 0, s>>>(p);
     else k_dense_pick<<<(unsigned)((threads + 255) / 256), 256, 0, s>>>(p);
     if (launches) *launches += 1;
     return cudaGetLastError();
