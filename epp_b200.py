@@ -24,4 +24,5 @@ DECISION_DTYPE = _pkg.DECISION_DTYPE
 DETAIL_DTYPE = _pkg.DETAIL_DTYPE
 SHARD_BEST_DTYPE = _pkg.SHARD_BEST_DTYPE
 decisions_from_torch = _pkg.decisions_from_torch
+pack_subsets = _pkg.pack_subsets
 Batcher = _pkg.Batcher

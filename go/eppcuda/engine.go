@@ -353,6 +353,12 @@ func (e *Engine) InFlightRelease(slots []uint32, promptLen uint64) error {
 // schedule = epp_submit + epp_wait for ONE request.  prompt is read during the submit call only (the library copies
 // the bytes it hashes into its pinned staging buffer).
 func (e *Engine) schedule(model uint32, prompt []byte, multimodal bool) (Decision, error) {
+	return e.scheduleSubset(model, prompt, multimodal, nil)
+}
+
+// scheduleSubset = schedule for a request whose candidates are the endpoints of `slots` (sorted; the gateway's endpoint
+// subset, epp_submit_subset), or the whole pool when slots is nil.  At most C.EPP_SUBSET_MAX_SLOTS slots.
+func (e *Engine) scheduleSubset(model uint32, prompt []byte, multimodal bool, slots []uint32) (Decision, error) {
 	e.inflight.Add(1)
 	defer e.inflight.Done()
 	var ticket C.uint64_t
@@ -364,7 +370,17 @@ func (e *Engine) schedule(model uint32, prompt []byte, multimodal bool) (Decisio
 	if multimodal {
 		mm = 1
 	}
-	if rc := C.epp_submit(e.b, C.uint32_t(model), p, C.uint64_t(len(prompt)), mm, &ticket); rc != C.EPP_OK {
+	var rc C.int32_t
+	if slots == nil {
+		rc = C.epp_submit(e.b, C.uint32_t(model), p, C.uint64_t(len(prompt)), mm, &ticket)
+	} else {
+		var sp *C.uint32_t
+		if len(slots) > 0 {
+			sp = (*C.uint32_t)(unsafe.Pointer(&slots[0]))
+		}
+		rc = C.epp_submit_subset(e.b, C.uint32_t(model), p, C.uint64_t(len(prompt)), mm, C.uint32_t(len(slots)), sp, &ticket)
+	}
+	if rc != C.EPP_OK {
 		return Decision{}, errors.New(C.GoString(C.epp_batcher_last_error()))
 	}
 	var d C.epp_decision

@@ -1,8 +1,12 @@
 package eppcuda
 
+// #include "epp_engine.h"
+import "C"
+
 import (
 	"context"
 	"errors"
+	"sort"
 
 	"k8s.io/apimachinery/pkg/types"
 
@@ -27,7 +31,9 @@ type ProfileNames struct{ Primary, Prefill, Encode string }
 type Scheduler struct {
 	Engine   *Engine
 	Names    ProfileNames
-	Fallback requestcontrol.Scheduler // the reference scheduler: used when the director passes a SUBSET of the pool
+	// the reference scheduler: used only for a candidate the engine has no slot for (not in its pool snapshot yet), or a
+	// subset of more than EPP_SUBSET_MAX_SLOTS endpoints
+	Fallback requestcontrol.Scheduler
 }
 
 var _ requestcontrol.Scheduler = (*Scheduler)(nil)
@@ -44,16 +50,34 @@ func (s *Scheduler) Schedule(ctx context.Context, request *scheduling.InferenceR
 	for _, ep := range candidates {
 		byName[ep.GetMetadata().NamespacedName] = ep
 	}
-	// the engine scores its whole pool snapshot; a director-side subset (candidates.Locate with subsetting metadata)
-	// is the reference scheduler's job
+	if len(byName) == 0 { // an empty subset decides nothing (the director answers ServiceUnavailable before this)
+		return nil, errors.New("failed to find available decode workers")
+	}
+	// A director-side subset (candidates.Locate with x-gateway-destination-endpoint-subset metadata, director.go:222-243)
+	// goes to the engine as the sorted slots of the candidates (epp_submit_subset); the whole pool as no subset.
 	s.Engine.mu.RLock()
-	whole := len(byName) == len(s.Engine.slotOf)
+	slots := make([]uint32, 0, len(byName)) // non-nil: no candidates is an empty subset (status -1), never the whole pool
+	known := true
+	for name := range byName {
+		slot, ok := s.Engine.slotOf[name]
+		if !ok {
+			known = false
+			break
+		}
+		slots = append(slots, slot)
+	}
+	whole := known && len(slots) == len(s.Engine.slotOf)
 	s.Engine.mu.RUnlock()
-	if !whole {
+	if !known || (!whole && len(slots) > int(C.EPP_SUBSET_MAX_SLOTS)) {
 		if s.Fallback != nil {
 			return s.Fallback.Schedule(ctx, request, candidates)
 		}
-		return nil, errors.New("eppcuda: candidate list is not the engine's pool snapshot and no fallback scheduler is set")
+		return nil, errors.New("eppcuda: a candidate is not in the engine's pool snapshot (or the subset is too large) and no fallback scheduler is set")
+	}
+	if whole {
+		slots = nil
+	} else {
+		sort.Slice(slots, func(i, j int) bool { return slots[i] < slots[j] })
 	}
 	prompt, err := UserInputBytes(request)
 	if err != nil {
@@ -68,7 +92,7 @@ func (s *Scheduler) Schedule(ctx context.Context, request *scheduling.InferenceR
 		return nil, err
 	}
 	mm := HasMultimodalContent != nil && HasMultimodalContent(request)
-	d, err := s.Engine.schedule(model, prompt, mm)
+	d, err := s.Engine.scheduleSubset(model, prompt, mm, slots)
 	if err != nil {
 		return nil, err
 	}

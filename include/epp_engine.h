@@ -434,6 +434,45 @@ EPP_API int32_t epp_schedule_with_match_topk(epp_engine *h, int64_t n_requests, 
                                      epp_decision *out, epp_decision_detail *detail, uint32_t flags,
                                      const epp_topk_out *topk);
 
+/* ---- Endpoint subsets (requestcontrol/candidates.go:98-167, director.go:222-243) -------------------------------------
+ * When Envoy attaches x-gateway-destination-endpoint-subset metadata, Scheduler.Schedule receives only that subset's
+ * endpoints.  A request with a subset is decided exactly as the reference decides it when Schedule is called with the
+ * subset's endpoints:
+ *   - Candidates: every profile's candidates are the subset's slots that are in the pool and pass the profile's role
+ *     filter; the affinity filter, scorers and picker run over those.  Subset slots not in the pool are ignored.
+ *   - Everything normalised over "the candidates" uses the narrowed set: the queue / running min-max, the active-request
+ *     max, the no-hit-lru cold test (no SUBSET candidate holds a block) and its cold ranks (never-used index in slot
+ *     order, neverUsedCount + the position in the engine's one LRU, over totalEndpoints = |candidates|), the affinity
+ *     filter's len(endpoints) <= 1 gate and its sticky / TTFT sets, tie_count, the tie rank, the first-k ranks and the
+ *     random pickers' population.
+ *   - The prefix match is NOT narrowed (matchLongestPrefix walks the whole index, approximateprefix/plugin.go:214-230):
+ *     totalBlocks, the global stop (the first block no endpoint holds) and each member's matchBlocks are those of the
+ *     whole pool.  The P/D decider reads the pick's match count, as without a subset.
+ *   - Random pickers: every subset candidate is an EXPLICIT item (no gaps; wcum is not read), the rule stated above for a
+ *     set narrowed by the affinity filter.  W is the left fold of s+ in ascending slot order; the +inf and 2^-128 rules are
+ *     unchanged.  So an explicit subset listing the whole pool gives the max-score decisions of no subset; under the
+ *     weighted-random picker its W may differ from the gap fold's in the last bits (a different summation order).
+ *   - Ordinal, tie key (4 * ordinal + profile index) and the after-pick updates (no-hit-lru Adds, in-flight adds,
+ *     epp_index_add_picked) read subset picks like any other.
+ *   - An empty subset (counts[r] == 0) gives status -1 (the director answers ServiceUnavailable before Schedule).
+ * The subset arrays are HOST memory for every batch kind (EPP_BATCH_DEVICE_PTRS / EPP_BATCH_ASYNC included), validated and
+ * copied before the call returns.  A slot >= max_endpoints, a slot list that is not strictly ascending or a wrong
+ * struct_size fails the call with EPP_ERR_INVALID before anything is launched and before any LRU, counter or ordinal state
+ * changes; so does any subset call on an endpoint-sharded or peer-memory engine.  EPP_SUBSET_ALL rows are decided exactly as
+ * by epp_schedule; a batch without a restricted row IS epp_schedule.  Restricted rows are re-decided by a kernel of their
+ * own after the batch's match kernels (so such batches never take the small-batch single-launch path); its device time is
+ * epp_stats.last_kernel_ms[6] on device-pointer batches (0 otherwise). */
+#define EPP_SUBSET_ALL 0xFFFFFFFFu
+typedef struct {
+    uint32_t struct_size;          /* sizeof(epp_subset)                                                                 */
+    uint32_t reserved;
+    const uint32_t *counts;        /* [R] slots of request r, or EPP_SUBSET_ALL = the whole pool (decided as by epp_schedule) */
+    const uint64_t *offsets;       /* [R] request r's slots are slots[offsets[r] .. offsets[r] + counts[r])             */
+    const uint32_t *slots;         /* strictly ascending within a request, each < max_endpoints                          */
+} epp_subset;
+EPP_API int32_t epp_schedule_subset(epp_engine *h, const epp_batch *batch, const epp_subset *subset, epp_decision *out,
+                                    epp_decision_detail *detail, int32_t keep_hashes, const epp_topk_out *topk /* or NULL */);
+
 /* PreRequest (approximateprefix/plugin.go:164-200): index the hashes of the LAST epp_schedule batch
  * (keep_hashes=1) for each request's primary pick and prefill pick. */
 EPP_API int32_t epp_index_add_picked(epp_engine *h);
@@ -533,6 +572,13 @@ EPP_API int32_t epp_batcher_destroy(epp_batcher *b);     /* flushes what is pend
  * Neither call takes a lock: a submit is one compare-and-swap + the copy, a wait polls / sleeps on the flush counter. */
 EPP_API int32_t epp_submit(epp_batcher *b, uint32_t model_id, const void *prompt, uint64_t prompt_len,
                            uint32_t multimodal, uint64_t *out_ticket);
+/* epp_submit for a request whose candidates are the n_slots endpoints slots[0 .. n_slots) (see "Endpoint subsets"; any
+ * order, duplicates allowed: the batcher sorts and deduplicates them).  Up to EPP_SUBSET_MAX_SLOTS slots, kept in the
+ * batcher's staging next to the prompt; more is EPP_ERR_CAPACITY, a slot >= max_endpoints EPP_ERR_INVALID.  A flush
+ * holding a request submitted this way runs epp_schedule_subset, every other flush epp_schedule. */
+#define EPP_SUBSET_MAX_SLOTS 1024
+EPP_API int32_t epp_submit_subset(epp_batcher *b, uint32_t model_id, const void *prompt, uint64_t prompt_len,
+                                  uint32_t multimodal, uint32_t n_slots, const uint32_t *slots, uint64_t *out_ticket);
 EPP_API int32_t epp_wait(epp_batcher *b, uint64_t ticket, epp_decision *out, epp_decision_detail *out_detail);
 /* The same on an engine created with pick_k > 1, plus the request's first-k lists (ProfileRunResult.TargetEndpoints of
  * each profile, see epp_topk_out): primary / prefill / encode receive pick_k slot ids each (EPP_NO_ENDPOINT padded); any

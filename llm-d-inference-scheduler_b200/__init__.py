@@ -10,7 +10,7 @@ The directory name is not a Python identifier; import it with importlib (see epp
 """
 from . import _capi as capi
 from .engine import (DECISION_DTYPE, DETAIL_DTYPE, SHARD_BEST_DTYPE, AffinityFilterSpec, Batcher, Engine, EngineError, PinnedBuffer, ProfileSpec,
-                     ScorerSpec, decisions_from_torch)
+                     ScorerSpec, decisions_from_torch, pack_subsets)
 
 __all__ = ["capi", "Engine", "Batcher", "EngineError", "ProfileSpec", "ScorerSpec", "AffinityFilterSpec", "PinnedBuffer", "DECISION_DTYPE", "DETAIL_DTYPE",
-           "SHARD_BEST_DTYPE", "decisions_from_torch"]
+           "SHARD_BEST_DTYPE", "decisions_from_torch", "pack_subsets"]

@@ -80,6 +80,15 @@ class TopkOut(C.Structure):
                 ("prefill", C.c_void_p), ("encode", C.c_void_p)]
 
 
+EPP_SUBSET_ALL = 0xFFFFFFFF
+EPP_SUBSET_MAX_SLOTS = 1024
+
+
+class Subset(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("reserved", C.c_uint32), ("counts", C.c_void_p), ("offsets", C.c_void_p),
+                ("slots", C.c_void_p)]
+
+
 class BatcherCfg(C.Structure):
     _fields_ = [("struct_size", C.c_uint32), ("max_batch", C.c_int32), ("max_delay_us", C.c_int32),
                 ("index_picks", C.c_int32)]
@@ -129,6 +138,8 @@ SIGNATURES = {
     "epp_schedule_topk": (C.c_int32, [C.c_void_p, C.POINTER(Batch), C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(TopkOut)]),
     "epp_schedule_with_match_topk": (C.c_int32, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                                  C.c_int32, C.c_void_p, C.c_void_p, C.c_uint32, C.POINTER(TopkOut)]),
+    "epp_schedule_subset": (C.c_int32, [C.c_void_p, C.POINTER(Batch), C.POINTER(Subset), C.c_void_p, C.c_void_p, C.c_int32,
+                                        C.POINTER(TopkOut)]),
     "epp_index_add_picked": (C.c_int32, [C.c_void_p]),
     "epp_nohit_lru_get": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(C.c_int32)]),
     "epp_inflight_release": (C.c_int32, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
@@ -150,6 +161,8 @@ SIGNATURES = {
     "epp_batcher_create": (C.c_int32, [C.c_void_p, C.POINTER(BatcherCfg), C.POINTER(C.c_void_p)]),
     "epp_batcher_destroy": (C.c_int32, [C.c_void_p]),
     "epp_submit": (C.c_int32, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_uint32, C.POINTER(C.c_uint64)]),
+    "epp_submit_subset": (C.c_int32, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_uint32, C.c_uint32, C.c_void_p,
+                                      C.POINTER(C.c_uint64)]),
     "epp_wait": (C.c_int32, [C.c_void_p, C.c_uint64, C.POINTER(Decision), C.POINTER(DecisionDetail)]),
     "epp_wait_topk": (C.c_int32, [C.c_void_p, C.c_uint64, C.POINTER(Decision), C.POINTER(DecisionDetail), C.c_void_p,
                                   C.c_void_p, C.c_void_p]),

@@ -65,6 +65,11 @@ struct Staging {
     epp_decision *dec = nullptr;
     epp_decision_detail *det = nullptr;
     uint32_t *topk[3] = {nullptr, nullptr, nullptr};   // [max_batch][pick_k] primary / prefill / encode lists (pick_k > 1)
+    // endpoint subsets (epp_submit_subset): per row EPP_SUBSET_ALL or its slot count, its slots at row * EPP_SUBSET_MAX_SLOTS
+    std::vector<uint32_t> sub_counts;          // [max_batch]
+    std::vector<uint64_t> sub_offsets;         // [max_batch]
+    std::vector<uint32_t> sub_slots;           // [max_batch][EPP_SUBSET_MAX_SLOTS], allocated by the first subset submit
+    std::atomic<int32_t> any_subset{0};        // some row of the batch using this buffer has a subset
     std::atomic<int32_t> ready{0};             // rows of the batch using this buffer whose copy is complete
     std::atomic<int64_t> first_arrival_ns{0};  // when row 0 of that batch was reserved
 };
@@ -86,6 +91,9 @@ struct epp_batcher {
     epp_batcher_cfg cfg{};
     uint64_t row_cap = 0;                      // bytes of a prompt that hashPrompt can read (hashing.go:63-66)
     int32_t pick_k = 0;                        // the engine's maxNumOfEndpoints (> 1: flushes also fetch the first-k lists)
+    uint32_t max_endpoints = 0;
+    std::once_flag sub_once;                   // the subset slot staging of every buffer, allocated on first use
+    bool sub_alloc_failed = false;
     Staging buf[kBufs];
     std::vector<Result> results;
     std::atomic<uint64_t> fill{0};             // (sequence number of the batch being filled << 20) | rows reserved in it
@@ -154,12 +162,21 @@ static void flusher_main(epp_batcher *b) {
         batch.multimodal = st.multimodal;
         batch.flags = EPP_BATCH_LENGTHS_EXCEED_ROWS;
         int32_t rc;
-        if (b->pick_k > 1) {
-            epp_topk_out tk;
-            memset(&tk, 0, sizeof tk);
-            tk.struct_size = sizeof tk;
-            tk.k = b->pick_k;
-            tk.primary = st.topk[0]; tk.prefill = st.topk[1]; tk.encode = st.topk[2];
+        epp_topk_out tk;
+        memset(&tk, 0, sizeof tk);
+        tk.struct_size = sizeof tk;
+        tk.k = b->pick_k;
+        tk.primary = st.topk[0]; tk.prefill = st.topk[1]; tk.encode = st.topk[2];
+        if (st.any_subset.load(std::memory_order_acquire)) {
+            epp_subset sub;
+            memset(&sub, 0, sizeof sub);
+            sub.struct_size = sizeof sub;
+            sub.counts = st.sub_counts.data();
+            sub.offsets = st.sub_offsets.data();
+            sub.slots = st.sub_slots.data();
+            rc = epp_schedule_subset(b->eng, &batch, &sub, st.dec, st.det, b->cfg.index_picks ? 1 : 0, b->pick_k > 1 ? &tk : nullptr);
+            st.any_subset.store(0, std::memory_order_relaxed);
+        } else if (b->pick_k > 1) {
             rc = epp_schedule_topk(b->eng, &batch, st.dec, st.det, b->cfg.index_picks ? 1 : 0, &tk);
         } else {
             rc = epp_schedule(b->eng, &batch, st.dec, st.det, b->cfg.index_picks ? 1 : 0);
@@ -224,6 +241,7 @@ extern "C" int32_t epp_batcher_create(epp_engine *h, const epp_batcher_cfg *cfg,
     // rows start on 32-byte boundaries (selects the aligned hash kernels)
     b->row_cap = ((uint64_t)ec.max_prefix_blocks * (uint64_t)ec.block_size_tokens * 4 + 31) & ~31ull;
     b->pick_k = ec.pick_k;
+    b->max_endpoints = (uint32_t)ec.max_endpoints;
     b->results = std::vector<Result>(kResults);
     const size_t mb = (size_t)cfg->max_batch;
     for (int i = 0; i < kBufs; i++) {
@@ -243,6 +261,9 @@ extern "C" int32_t epp_batcher_create(epp_engine *h, const epp_batcher_cfg *cfg,
             *dst[k] = p;
         }
         for (size_t r = 0; r <= mb; r++) st.offsets[r] = (uint64_t)r * b->row_cap;
+        st.sub_counts.assign(mb, EPP_SUBSET_ALL);
+        st.sub_offsets.resize(mb);
+        for (size_t r = 0; r < mb; r++) st.sub_offsets[r] = (uint64_t)r * EPP_SUBSET_MAX_SLOTS;
         if (b->pick_k > 1)
             for (int q = 0; q < 3; q++) {
                 rc = epp_host_alloc(sizeof(uint32_t) * mb * (size_t)b->pick_k, &p);
@@ -275,9 +296,9 @@ extern "C" int32_t epp_batcher_destroy(epp_batcher *b) {
     return EPP_OK;
 }
 
-extern "C" int32_t epp_submit(epp_batcher *b, uint32_t model_id, const void *prompt, uint64_t prompt_len,
-                              uint32_t multimodal, uint64_t *out_ticket) {
-    if (!b || !out_ticket || (prompt_len && !prompt)) return bfail(EPP_ERR_INVALID, "NULL argument");
+// sub: the request's slots, sorted and deduplicated, or nullptr (the whole pool)
+static int32_t submit_impl(epp_batcher *b, uint32_t model_id, const void *prompt, uint64_t prompt_len, uint32_t multimodal,
+                           const std::vector<uint32_t> *sub, uint64_t *out_ticket) {
     const uint64_t max_batch = (uint64_t)b->cfg.max_batch;
     uint64_t seq, idx;
     for (int spin = 0;; spin++) {
@@ -312,9 +333,42 @@ extern "C" int32_t epp_submit(epp_batcher *b, uint32_t model_id, const void *pro
     st.multimodal[idx] = multimodal ? 1 : 0;
     const uint64_t n_copy = prompt_len < b->row_cap ? prompt_len : b->row_cap;
     if (n_copy) memcpy(st.data + (size_t)idx * b->row_cap, prompt, n_copy);
+    if (sub) {
+        if (!sub->empty()) memcpy(st.sub_slots.data() + (size_t)idx * EPP_SUBSET_MAX_SLOTS, sub->data(), sizeof(uint32_t) * sub->size());
+        st.sub_counts[idx] = (uint32_t)sub->size();
+        st.any_subset.store(1, std::memory_order_relaxed);         // published by the release below
+    } else {
+        st.sub_counts[idx] = EPP_SUBSET_ALL;
+    }
     st.ready.fetch_add(1, std::memory_order_release);              // the flusher waits for this before it reads the row
     *out_ticket = (seq << 20) | idx;
     return EPP_OK;
+}
+
+extern "C" int32_t epp_submit(epp_batcher *b, uint32_t model_id, const void *prompt, uint64_t prompt_len,
+                              uint32_t multimodal, uint64_t *out_ticket) {
+    if (!b || !out_ticket || (prompt_len && !prompt)) return bfail(EPP_ERR_INVALID, "NULL argument");
+    return submit_impl(b, model_id, prompt, prompt_len, multimodal, nullptr, out_ticket);
+}
+
+extern "C" int32_t epp_submit_subset(epp_batcher *b, uint32_t model_id, const void *prompt, uint64_t prompt_len,
+                                     uint32_t multimodal, uint32_t n_slots, const uint32_t *slots, uint64_t *out_ticket) {
+    if (!b || !out_ticket || (prompt_len && !prompt) || (n_slots && !slots)) return bfail(EPP_ERR_INVALID, "NULL argument");
+    if (n_slots > EPP_SUBSET_MAX_SLOTS) return bfail(EPP_ERR_CAPACITY, "more than EPP_SUBSET_MAX_SLOTS slots in one subset");
+    std::vector<uint32_t> sub(slots, slots + n_slots);
+    for (uint32_t e : sub)
+        if (e >= b->max_endpoints) return bfail(EPP_ERR_INVALID, "subset slot >= max_endpoints");
+    std::sort(sub.begin(), sub.end());
+    sub.erase(std::unique(sub.begin(), sub.end()), sub.end());
+    std::call_once(b->sub_once, [b] {
+        try {
+            for (int i = 0; i < kBufs; i++) b->buf[i].sub_slots.resize((size_t)b->cfg.max_batch * EPP_SUBSET_MAX_SLOTS);
+        } catch (...) {
+            b->sub_alloc_failed = true;
+        }
+    });
+    if (b->sub_alloc_failed) return bfail(EPP_ERR_CAPACITY, "cannot allocate the batcher's subset staging");
+    return submit_impl(b, model_id, prompt, prompt_len, multimodal, &sub, out_ticket);
 }
 
 extern "C" int32_t epp_wait(epp_batcher *b, uint64_t ticket, epp_decision *out, epp_decision_detail *out_detail) {

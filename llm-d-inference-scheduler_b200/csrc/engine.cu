@@ -188,6 +188,15 @@ struct epp_engine {
     bool general = false;           // a profile configures the prefix-cache-affinity-filter or pick_k > 1: every batch takes
                                     // the dense-counter kernel with the full-scan evaluation of pick_general.cuh
     const epp_topk_out *cur_topk = nullptr;   // top-k destination of the call in progress (under mu)
+    // endpoint subsets of the call in progress (epp_schedule_subset, subset_pick.cu): its restricted requests in ascending
+    // order, or nullptr; their rows and slot lists were validated on the host and copied to sub_rows / sub_slots
+    const std::vector<SubsetRow> *cur_sub = nullptr;
+    DevBuf sub_rows, sub_slots, sub_hits, sub_scratch;
+    std::vector<cudaEvent_t> sub_ev;    // pairs bracketing the subset launches of the device batch in flight
+    int sub_ev_used = 0;                // events of sub_ev recorded for it (last_kernel_ms[6])
+    void *sub_host = nullptr;           // pinned staging of the rows and slots being uploaded
+    size_t sub_host_cap = 0;
+    cudaEvent_t sub_up_ev = nullptr;    // behind the last upload from sub_host
     DevBuf topk_picks[kMaxProfiles], topk_scores;   // device staging of the lists for host batches
     int64_t kept_R = 0;             // rows of `hashes` valid for epp_index_add_picked
     int64_t shard_R = 0;            // rows of `hashes` valid for epp_shard_pick / epp_shard_merge
@@ -485,6 +494,9 @@ extern "C" int32_t epp_engine_destroy(epp_engine *h) {
     }
     for (auto &ev : h->ev) if (ev) cudaEventDestroy(ev);
     for (auto &ev : h->user_ev) if (ev) cudaEventDestroy(ev);
+    for (auto &ev : h->sub_ev) cudaEventDestroy(ev);
+    if (h->sub_up_ev) cudaEventDestroy(h->sub_up_ev);
+    if (h->sub_host) cudaFreeHost(h->sub_host);
     if (h->wc_host) cudaFreeHost(h->wc_host);
     if (h->small_host) cudaFreeHost(h->small_host);
     if (h->small_epoch_host) cudaFreeHost(h->small_epoch_host);
@@ -1447,6 +1459,48 @@ static int32_t finish_async(epp_engine *h) {
         h->stats.last_kernel_ms[4 + u] = tu;
         h->post_pick_timed[u] = false;
     }
+    double ts = 0.0;
+    for (int i = 0; i + 1 < h->sub_ev_used; i += 2) {
+        float t1 = 0;
+        cudaEventElapsedTime(&t1, h->sub_ev[i], h->sub_ev[i + 1]);
+        ts += t1;
+    }
+    h->stats.last_kernel_ms[6] = ts;
+    h->sub_ev_used = 0;
+    return EPP_OK;
+}
+
+// The restricted requests among rows [r0, r1) of a Schedule batch, re-decided on s by the subset kernel after the match
+// kernels of the same rows (pp: their PickParams, trimmed rows included).  timed: bracket it for last_kernel_ms[6].
+static int32_t launch_subset(epp_engine *h, const PickParams &pp, int64_t r0, int64_t r1, cudaStream_t s, int *launches,
+                             bool timed) {
+    if (!h->cur_sub) return EPP_OK;
+    const std::vector<SubsetRow> &rows = *h->cur_sub;
+    auto below = [](const SubsetRow &a, int64_t r) { return (int64_t)a.row < r; };
+    const size_t lo = std::lower_bound(rows.begin(), rows.end(), r0, below) - rows.begin();
+    const size_t hi = std::lower_bound(rows.begin(), rows.end(), r1, below) - rows.begin();
+    if (lo == hi) return EPP_OK;
+    SubsetView sv;
+    sv.rows = h->sub_rows.as<SubsetRow>() + lo;
+    sv.n_rows = (int32_t)(hi - lo);
+    sv.r0 = r0;
+    sv.slots = h->sub_slots.as<uint32_t>();
+    sv.hits = h->sub_hits.as<int32_t>();
+    sv.scratch = h->sub_scratch.as<int32_t>();
+    sv.nohit_pos = h->nohit_mask ? h->nh_pos.as<int32_t>() : nullptr;
+    if (timed) {
+        while ((int)h->sub_ev.size() < h->sub_ev_used + 2) {
+            cudaEvent_t ev;
+            CUDA_TRY(cudaEventCreate(&ev));
+            h->sub_ev.push_back(ev);
+        }
+        CUDA_TRY(cudaEventRecord(h->sub_ev[h->sub_ev_used], s));
+    }
+    CUDA_TRY(launch_subset_pick(pp, sv, s, launches));
+    if (timed) {
+        CUDA_TRY(cudaEventRecord(h->sub_ev[h->sub_ev_used + 1], s));
+        h->sub_ev_used += 2;
+    }
     return EPP_OK;
 }
 
@@ -1678,6 +1732,9 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
                v.multimodal};
         CUDA_TRY(cudaMemsetAsync(h->work_counters.p, 0, sizeof(unsigned long long) * 4, s0));
         const int64_t min_chunk = 4096;
+        h->sub_ev_used = 0;
+        PickParams sub_pp;                         // the one-pass launch's rows, for its subset launch behind ev[4]
+        bool sub_pending = false;
         if (pipelined) {
             // Throughput mode: the batch runs as C chunks alternating between the engine's two streams, so the hash
             // kernel of one chunk (HBM / integer bound) shares the SMs with the match kernel of another (latency bound).
@@ -1704,6 +1761,7 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
                 HashParams hp = hash_params(h, w, sl);
                 if (trim) trim_rows(h, w, hp, pp);
                 EPP_TRY(launch_cycle(h, sl, hp, pp, &launches, nullptr));
+                EPP_TRY(launch_subset(h, pp, r0, r1, sl.stream, &launches, true));
             }
             h->s1_unjoined = true;
             // the next call's picks must see both chunks' Adds: join the chunks on stream 0 for the update (below), and the
@@ -1725,8 +1783,11 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
             hp.read = h->work_counters.as<unsigned long long>() + 3;
             if (trim) trim_rows(h, w, hp, pp);
             EPP_TRY(launch_cycle(h, h->slot[0], hp, pp, &launches, h->ev));
+            sub_pp = pp;
+            sub_pending = mode == Mode::Schedule;
         }
         CUDA_TRY(cudaEventRecord(h->ev[4], s0));
+        if (sub_pending) EPP_TRY(launch_subset(h, sub_pp, 0, R, s0, &launches, true));   // after ev[4]: [3] stays match + pick
         if (mode == Mode::Schedule)                // after ev[4]: last_kernel_ms[3] stays the match + pick time
             EPP_TRY(after_picks(h, out_dec ? out_dec : h->decisions.as<epp_decision>(), det_out, h->in_len.as<int64_t>(), R,
                                 s0, &launches, true));
@@ -1739,7 +1800,9 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
     }
 
     // ---- small host batch in pinned memory: one zero-copy launch, no copy engine, no stream synchronisation
-    if (mode == Mode::Schedule && !tk.on && out_dec) {
+    // (not for a batch with restricted requests: the kernel hands the decisions to the host before a subset launch could
+    // rewrite them)
+    if (mode == Mode::Schedule && !tk.on && out_dec && !h->cur_sub) {
         const uint8_t *data_dev = nullptr;
         const int sm = small_batch_mode(h, v, &data_dev);
         if (sm) return run_small(h, v, sm, data_dev, out_dec, out_detail);
@@ -1825,6 +1888,7 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
             if (trim) trim_rows(h, w, hp, pp);
             EPP_TRY(launch_cycle(h, sl, hp, pp, &launches, nullptr));
             if (mode == Mode::Schedule) {
+                EPP_TRY(launch_subset(h, pp, c.r0, c.r1, s, &launches, false));
                 if (out_dec) CUDA_TRY(cudaMemcpyAsync(out_dec + c.r0, dec, sizeof(epp_decision) * nreq, cudaMemcpyDeviceToHost, s));
                 if (out_detail) CUDA_TRY(cudaMemcpyAsync(out_detail + c.r0, det, sizeof(epp_decision_detail) * nreq, cudaMemcpyDeviceToHost, s));
                 if (tk.on) EPP_TRY(topk_copy_back(h, tk, c.r0, (int64_t)nreq, s));
@@ -1843,6 +1907,7 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
     float t_all = 0;
     cudaEventElapsedTime(&t_all, h->ev[0], h->ev[1]);
     h->stats.last_kernels_ms = t_all;
+    h->stats.last_kernel_ms[6] = 0.0;              // the subset kernel is timed on device batches only
     h->stats.last_hash_ms = h->stats.last_match_pick_ms = 0;
     h->stats.last_kernel_launches = (uint64_t)launches;
     return EPP_OK;
@@ -1878,8 +1943,73 @@ static int32_t check_topk(epp_engine *h, const epp_topk_out *topk) {
     return EPP_OK;
 }
 
+// Validates the subsets of a batch of R requests on the host and lists the restricted ones in ascending request order,
+// each with its offset in the packed slot array (*n_slots entries in all).  Nothing of the engine changes.
+static int32_t check_subset(const epp_engine *h, int64_t R, const epp_subset *s, std::vector<SubsetRow> &rows,
+                            uint64_t *n_slots) {
+    if (s->struct_size != sizeof(epp_subset)) return fail(EPP_ERR_INVALID, "epp_subset.struct_size %u != %zu", s->struct_size, sizeof(epp_subset));
+    if (h->shard_begin != 0 || h->shard_end != 0xFFFFFFFFu || h->p2p_buf)
+        return fail(EPP_ERR_INVALID, "endpoint subsets are not available in the endpoint-sharded and peer-memory modes");
+    if (R > 0 && !s->counts) return fail(EPP_ERR_INVALID, "epp_subset.counts is NULL");
+    const uint32_t E = (uint32_t)h->cfg.max_endpoints;
+    int64_t n_rows = 0;
+    for (int64_t r = 0; r < R; r++) n_rows += s->counts[r] != EPP_SUBSET_ALL;
+    rows.reserve((size_t)n_rows);
+    uint64_t total = 0;
+    for (int64_t r = 0; r < R; r++) {
+        const uint32_t n = s->counts[r];
+        if (n == EPP_SUBSET_ALL) continue;
+        if (n > E) return fail(EPP_ERR_INVALID, "request %lld: %u slots, more than max_endpoints %u", (long long)r, n, E);
+        if (n) {
+            if (!s->offsets || !s->slots) return fail(EPP_ERR_INVALID, "epp_subset.offsets / slots is NULL");
+            const uint32_t *src = s->slots + s->offsets[r];
+            for (uint32_t i = 0; i < n; i++) {
+                if (src[i] >= E) return fail(EPP_ERR_INVALID, "request %lld: slot %u >= max_endpoints %u", (long long)r, src[i], E);
+                if (i && src[i] <= src[i - 1]) return fail(EPP_ERR_INVALID, "request %lld: slots not strictly ascending at entry %u", (long long)r, i);
+            }
+        }
+        rows.push_back({total, (uint32_t)r, n});
+        total += n;
+    }
+    *n_slots = total;
+    return EPP_OK;
+}
+
+// The restricted rows and their slots to the device on stream 0, behind everything enqueued so far (a pipelined batch's
+// stream 1 joins first), through the engine's pinned staging: the slots are packed into it straight from the caller's
+// arrays and copied asynchronously.  The staging is refilled only once the previous call's copy has run (sub_up_ev).
+static int32_t upload_subset(epp_engine *h, const std::vector<SubsetRow> &rows, const epp_subset *s, uint64_t n_slots) {
+    cudaStream_t s0 = h->slot[0].stream;
+    EPP_TRY(join_streams(h));
+    const size_t ns = (size_t)std::max<uint64_t>(n_slots, 1);
+    CUDA_TRY(h->sub_rows.reserve(sizeof(SubsetRow) * rows.size(), &h->dev_bytes));
+    CUDA_TRY(h->sub_slots.reserve(sizeof(uint32_t) * ns, &h->dev_bytes));
+    CUDA_TRY(h->sub_hits.reserve(sizeof(int32_t) * ns, &h->dev_bytes));
+    CUDA_TRY(h->sub_scratch.reserve(sizeof(int32_t) * ns, &h->dev_bytes));
+    if (!h->sub_up_ev) CUDA_TRY(cudaEventCreateWithFlags(&h->sub_up_ev, cudaEventDisableTiming));
+    else CUDA_TRY(cudaEventSynchronize(h->sub_up_ev));
+    const size_t rows_bytes = (sizeof(SubsetRow) * rows.size() + 15) & ~(size_t)15;
+    const size_t need = rows_bytes + sizeof(uint32_t) * (size_t)n_slots;
+    if (need > h->sub_host_cap) {
+        if (h->sub_host) CUDA_TRY(cudaFreeHost(h->sub_host));
+        h->sub_host = nullptr;
+        h->sub_host_cap = 0;
+        CUDA_TRY(cudaHostAlloc(&h->sub_host, need, cudaHostAllocDefault));
+        h->sub_host_cap = need;
+    }
+    uint8_t *stage = static_cast<uint8_t *>(h->sub_host);
+    memcpy(stage, rows.data(), sizeof(SubsetRow) * rows.size());
+    uint32_t *dst = reinterpret_cast<uint32_t *>(stage + rows_bytes);
+    for (const SubsetRow &row : rows)
+        if (row.n) memcpy(dst + row.off, s->slots + s->offsets[row.row], sizeof(uint32_t) * row.n);
+    CUDA_TRY(cudaMemcpyAsync(h->sub_rows.p, stage, sizeof(SubsetRow) * rows.size(), cudaMemcpyHostToDevice, s0));
+    if (n_slots) CUDA_TRY(cudaMemcpyAsync(h->sub_slots.p, dst, sizeof(uint32_t) * (size_t)n_slots, cudaMemcpyHostToDevice, s0));
+    CUDA_TRY(cudaEventRecord(h->sub_up_ev, s0));
+    return EPP_OK;
+}
+
 static int32_t schedule_impl(epp_engine *h, const epp_batch *batch, epp_decision *out, epp_decision_detail *detail,
-                             int32_t keep_hashes, const epp_topk_out *topk) {
+                             int32_t keep_hashes, const epp_topk_out *topk, const epp_subset *subset = nullptr) {
     if (!h) return fail(EPP_ERR_INVALID, "NULL engine");
     if (!out) return fail(EPP_ERR_INVALID, "out is NULL");
     std::lock_guard<std::mutex> lk(h->mu);
@@ -1888,10 +2018,19 @@ static int32_t schedule_impl(epp_engine *h, const epp_batch *batch, epp_decision
     EPP_TRY(check_batch(h, batch, v));
     if (topk) EPP_TRY(check_topk(h, topk));
     if (h->cfg.encode_enabled && v.multimodal && !detail) return fail(EPP_ERR_INVALID, "an encode profile is configured and the batch flags multimodal requests: `detail` (which carries the encode pick) must not be NULL");
+    std::vector<SubsetRow> sub_rows;
+    uint64_t sub_n_slots = 0;
+    if (subset) EPP_TRY(check_subset(h, v.R, subset, sub_rows, &sub_n_slots));
+    if (!sub_rows.empty()) {
+        if (!h->pool_ready) return fail(EPP_ERR_STATE, "epp_pool_set has not been called");
+        EPP_TRY(upload_subset(h, sub_rows, subset, sub_n_slots));
+    }
     h->kept_R = 0;
     h->cur_topk = topk;
+    h->cur_sub = sub_rows.empty() ? nullptr : &sub_rows;
     const int32_t rc = run_batch(h, v, Mode::Schedule, nullptr, nullptr, out, detail, nullptr, nullptr, keep_hashes != 0);
     h->cur_topk = nullptr;
+    h->cur_sub = nullptr;
     EPP_TRY(rc);
     h->stats.n_batches++;
     h->stats.n_decisions += (uint64_t)v.R;
@@ -1917,6 +2056,12 @@ extern "C" int32_t epp_schedule_topk(epp_engine *h, const epp_batch *batch, epp_
                                      int32_t keep_hashes, const epp_topk_out *topk) {
     if (!topk) return fail(EPP_ERR_INVALID, "topk is NULL");
     return schedule_impl(h, batch, out, detail, keep_hashes, topk);
+}
+
+extern "C" int32_t epp_schedule_subset(epp_engine *h, const epp_batch *batch, const epp_subset *subset, epp_decision *out,
+                                       epp_decision_detail *detail, int32_t keep_hashes, const epp_topk_out *topk) {
+    if (!subset) return fail(EPP_ERR_INVALID, "subset is NULL");
+    return schedule_impl(h, batch, out, detail, keep_hashes, topk, subset);
 }
 
 // PreRequest: approximateprefix/plugin.go:164-200 (primary target + "prefill" profile target).

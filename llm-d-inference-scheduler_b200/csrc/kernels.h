@@ -331,6 +331,25 @@ struct DensePickParams {
     NoHitView nohit;
 };
 cudaError_t launch_dense_pick(const DensePickParams &p, cudaStream_t s, int *launches);
+// subset_pick.cu: per-request endpoint subsets (include/epp_engine.h, "Endpoint subsets").  One warp re-decides one
+// restricted request of a launch whose ordinary match kernel has run: it walks the request's stored hash row up to the
+// global stop counting only the listed holders, then evaluates every profile over the listed slots (full evaluation:
+// affinity filter, scorer normalisation, no-hit-lru cold ranks, first-k and random draws over the narrowed set).
+struct SubsetRow {
+    uint64_t off;              // the request's slots are slots[off .. off + n), ascending
+    uint32_t row;              // absolute request index in the batch
+    uint32_t n;
+};
+struct SubsetView {
+    const SubsetRow *rows;     // [n_rows] restricted requests of this launch
+    int32_t n_rows;
+    int64_t r0;                // the PickParams rows start at request r0
+    const uint32_t *slots;
+    int32_t *hits;             // parallel to slots: the request's matchBlocks on each listed slot (written here)
+    int32_t *scratch;          // parallel to slots: no-hit-lru cold ranks (written here)
+    const int32_t *nohit_pos;  // [E] position in the no-hit-lru LRU (oldest 0, -1 = never used), or nullptr
+};
+cudaError_t launch_subset_pick(const PickParams &p, const SubsetView &sv, cudaStream_t s, int *launches);
 // Scorer.Score parity: out[R][E].  scorer_index -1 => weighted ordered sum (-1.0 for non-candidates).
 // cold != nullptr (the profile has a no-hit-lru scorer): cold[r] selects prof_cold and the raw cold column nohit_col
 // for request r.

@@ -88,6 +88,27 @@ def _ptr(x):
     return x.ctypes.data_as(C.c_void_p)
 
 
+def pack_subsets(subsets):
+    """Per-request endpoint subsets -> the host arrays of epp_subset: (counts u32 [R], offsets u64 [R], slots u32 [...]).
+    Entry r is None (the whole pool: EPP_SUBSET_ALL) or a sequence of slot ids, sorted and deduplicated here."""
+    R = len(subsets)
+    counts = np.full(R, capi.EPP_SUBSET_ALL, dtype=np.uint32)
+    offsets = np.zeros(R, dtype=np.uint64)
+    parts, n = [], 0
+    for r, s in enumerate(subsets):
+        if s is None:
+            continue
+        u = np.unique(np.asarray(s, dtype=np.int64))
+        if u.size and (u[0] < 0 or u[-1] > 0xFFFFFFFE):
+            raise ValueError(f"request {r}: slot id out of range")
+        counts[r] = u.size
+        offsets[r] = n
+        parts.append(u.astype(np.uint32))
+        n += u.size
+    slots = np.concatenate(parts) if parts else np.zeros(0, dtype=np.uint32)
+    return counts, offsets, np.ascontiguousarray(slots, dtype=np.uint32)
+
+
 class Engine:
     def __init__(self, max_endpoints: int, primary: ProfileSpec | None = None, prefill: ProfileSpec | None = None,
                  *, device: int = 0, block_size_tokens: int = 16, max_prefix_blocks: int = 256,
@@ -323,11 +344,13 @@ class Engine:
                                                 _ptr(mep), _ptr(mmo), _ptr(mst)))
 
     def schedule(self, data, offsets=None, uniform_len=None, model_ids=None, n_requests=None, keep_hashes=False,
-                 detail=True, out=None, lengths=None, asynchronous=False, multimodal=None, topk=False):
+                 detail=True, out=None, lengths=None, asynchronous=False, multimodal=None, topk=False, subsets=None):
         """a1-a14 Scheduler.Schedule for a batch -> (decisions, details).  asynchronous=True (CUDA tensors only)
         enqueues the batch and returns; the outputs are complete after synchronize().  topk=True (engines created with
         pick_k > 1) also returns the dict of the pickers' first-k lists (maxscore/picker.go:104-115): "primary",
-        "primary_scores", "prefill", "encode", each [R][pick_k], padded with EPP_NO_ENDPOINT / 0."""
+        "primary_scores", "prefill", "encode", each [R][pick_k], padded with EPP_NO_ENDPOINT / 0.
+        subsets: None, or a list of R entries, each None (the whole pool) or a sequence of slot ids: the request's
+        candidates (the gateway's endpoint subset, include/epp_engine.h "Endpoint subsets"); epp_schedule_subset."""
         b, R, dev, keep = self._batch(data, offsets, uniform_len, model_ids, n_requests, lengths, multimodal)
         if asynchronous:
             b.flags |= capi.EPP_BATCH_ASYNC
@@ -338,12 +361,21 @@ class Engine:
         else:
             dec = np.zeros(R, dtype=DECISION_DTYPE) if out is None else out
             det = np.zeros(R, dtype=DETAIL_DTYPE) if detail else None
-        if not topk:
+        lists, tk = self._topk_out(R, data.device if dev else None) if topk else (None, None)
+        if subsets is not None:
+            if len(subsets) != R:
+                raise ValueError(f"subsets has {len(subsets)} entries for {R} requests")
+            packed = pack_subsets(subsets)              # host arrays, kept alive until the call returns
+            sub = capi.Subset()
+            sub.struct_size = C.sizeof(capi.Subset)
+            sub.counts, sub.offsets, sub.slots = (_ptr(a) for a in packed)
+            self._check(self._lib.epp_schedule_subset(self._h, C.byref(b), C.byref(sub), _ptr(dec), _ptr(det),
+                                                      int(keep_hashes), C.byref(tk) if topk else None))
+        elif not topk:
             self._check(self._lib.epp_schedule(self._h, C.byref(b), _ptr(dec), _ptr(det), int(keep_hashes)))
-            return dec, det
-        lists, tk = self._topk_out(R, data.device if dev else None)
-        self._check(self._lib.epp_schedule_topk(self._h, C.byref(b), _ptr(dec), _ptr(det), int(keep_hashes), C.byref(tk)))
-        return dec, det, lists
+        else:
+            self._check(self._lib.epp_schedule_topk(self._h, C.byref(b), _ptr(dec), _ptr(det), int(keep_hashes), C.byref(tk)))
+        return (dec, det, lists) if topk else (dec, det)
 
     def _topk_out(self, R: int, device=None):
         """Destination arrays of the pickers' first-k lists (numpy, or torch on `device`) + the epp_topk_out record."""
@@ -461,12 +493,18 @@ class Batcher:
         if rc != 0:
             raise EngineError(rc, (self._lib.epp_batcher_last_error() or b"").decode())
 
-    def submit(self, prompt, model_id: int = 0, multimodal: bool = False) -> int:
+    def submit(self, prompt, model_id: int = 0, multimodal: bool = False, subset=None) -> int:
+        """subset: None (the whole pool) or a sequence of slot ids, the request's candidates (epp_submit_subset)."""
         buf = np.ascontiguousarray(prompt).view(np.uint8).reshape(-1) if not isinstance(prompt, (bytes, bytearray)) else prompt
         n = len(buf)
         ptr = buf.ctypes.data_as(C.c_void_p) if isinstance(buf, np.ndarray) else C.cast(C.c_char_p(bytes(buf)), C.c_void_p)
         t = C.c_uint64()
-        self._check(self._lib.epp_submit(self._b, model_id, ptr, n, int(multimodal), C.byref(t)))
+        if subset is None:
+            self._check(self._lib.epp_submit(self._b, model_id, ptr, n, int(multimodal), C.byref(t)))
+        else:
+            sl = np.ascontiguousarray(np.asarray(subset, dtype=np.uint32).reshape(-1))
+            self._check(self._lib.epp_submit_subset(self._b, model_id, ptr, n, int(multimodal), sl.shape[0], _ptr(sl),
+                                                    C.byref(t)))
         return t.value
 
     def wait(self, ticket: int):
