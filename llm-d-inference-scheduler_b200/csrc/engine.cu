@@ -882,7 +882,7 @@ extern "C" int32_t epp_pool_set_lora(epp_engine *h, int32_t n, const uint32_t *i
 // Clears the presence bitmap and sets the bits of every key the read table holds.  16 bits per table slot, which is
 // >= 26 per distinct key at the load factors the build and the patches allow, up to 2^26 bits (8 MiB, L2-resident) while
 // the table fits its L2 budget.  A larger table is read from DRAM anyway: its bitmap may grow to 2^30 bits (128 MiB), as
-// 2^26 bits over 1.3e8 keys would be mostly set and prove few misses (the lookup's latency hides behind a window).
+// 2^26 bits over 1.3e8 keys would be mostly set and prove few misses (the lookup's latency hides behind its window).
 static int32_t rebuild_presence(epp_engine *h) {
     const int cap = h->idx_capacity * sizeof(IndexSlot) > h->l2_table_bytes ? 30 : 26;
     int l = 6;

@@ -22,8 +22,8 @@
 //   (digest -> chain), empty (chain -> digest).  With each empty hand-over the chain assigns the stage kStages ahead
 //   (block 0 of a window and its number of full blocks per slot); once every request is taken and done it names the
 //   last stage, and both sides leave the ring there.
-//   A request closed at window c (block c*W proven absent) is known only after window c+1 has been chained, and one
-//   more window is assigned by then: it reads at most kStages windows past its closing window.
+//   A request closed at window c (block c*W proven absent) is known once window c has been chained; window c+1 is
+//   assigned by then: it reads at most kStages - 1 windows past its closing window.
 #include "hash_blocks.cuh"
 #include "index.cuh"
 
@@ -64,9 +64,9 @@ __device__ __forceinline__ void request_lengths(const HashParams &p, int64_t r, 
 }
 
 // Per-lane stop bound of the chain warp: the first window whose leading block reads as absent in the presence bitmap
-// (one lookup per window of W blocks).  The word is loaded right after the window is chained and examined only once the
-// NEXT window has been chained, so the L2 latency hides behind that work instead of stalling the ring; a window is
-// stored while no earlier one has been proven absent, so a row may run up to W - 1 hashes past its bound (never read).
+// (one lookup per window of W blocks).  The word is loaded as soon as the window's leading hash is chained and examined
+// once its other W - 1 hashes are, so the L2 latency hides behind them; a window proven absent is neither stored nor
+// followed by more than the one window the ring has already assigned, and a row ends at its bound.
 struct StopBound {
     int32_t bnd = INT32_MAX;        // a block proven absent (bound >= the global stop); INT32_MAX while none is
     int32_t pending = -1;           // block whose presence word is in flight, or -1
@@ -99,8 +99,9 @@ __device__ __forceinline__ uint64_t chain_window(const uint64_t *sm, const HashP
     for (int j = 0; j < W; j++) {
         if (j < n_here) prev = xxh_chain_step32(sm[j], lenp8, prev);
         hv[j] = prev;
+        if (j == 0 && p.presence) sb.issue(p, k * W, prev);    // the window's leading block: looked up at once
     }
-    if (sb.pending >= 0) sb.resolve();                         // the previous window's word has had this window's time
+    if (sb.pending >= 0) sb.resolve();                         // its word has had the window's other W - 1 steps
     const int32_t n_store = min(n_here, sb.bnd - k * W);
     if (n_store <= 0) return prev;
     n_stored += (uint32_t)n_store;
@@ -114,7 +115,6 @@ __device__ __forceinline__ uint64_t chain_window(const uint64_t *sm, const HashP
         for (int j = 0; j < W; j++)
             if (j < n_store) dst[j] = hv[j];
     }
-    if (p.presence && sb.bnd == INT32_MAX) sb.issue(p, k * W, hv[0]);        // closed requests issue no loads
     return prev;
 }
 }  // namespace

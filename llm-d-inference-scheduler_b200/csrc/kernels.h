@@ -29,7 +29,7 @@ struct HashParams {
     int32_t staged;             // hash_staged.cu (cp.async-staged, warp-per-task) kernel: 0 off, 1 default shape, else a launch shape (A/B)
     // k_hash_fused only: presence != nullptr trims the rows to the read table's reach.  bound[r] = the first block at a
     // window start (every 8th block is looked up) whose presence bit is clear (index.cuh), else nblocks[r]: the global
-    // stop is <= bound[r].  Hashes [0, bound[r]) are stored, plus at most the rest of bound's window.
+    // stop is <= bound[r].  Hashes [0, bound[r]) are stored.
     const uint32_t *presence;
     int32_t presence_shift;
     int32_t *bound;             // [R]
