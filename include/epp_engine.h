@@ -517,6 +517,8 @@ typedef struct {
 } epp_shard_best;              /* 24 bytes */
 EPP_API int32_t epp_shard_set(epp_engine *h, uint32_t ep_begin, uint32_t ep_end);
 EPP_API int32_t epp_shard_probe(epp_engine *h, const epp_batch *batch, uint32_t *out_masks);
+/* Scores the batch of the last epp_shard_probe.  Its per-request model ids (the lora-affinity scorer's adapters) are the
+ * engine's own copy, taken by epp_shard_probe: the caller's model_ids array need not outlive that call. */
 EPP_API int32_t epp_shard_pick(epp_engine *h, int64_t n_requests, const uint32_t *global_masks, epp_shard_best *out_best);
 EPP_API int32_t epp_shard_merge(epp_engine *h, int64_t n_requests, int32_t n_ranks, const epp_shard_best *all_best,
                         epp_decision *out);

@@ -200,6 +200,7 @@ struct epp_engine {
     DevBuf topk_picks[kMaxProfiles], topk_scores;   // device staging of the lists for host batches
     int64_t kept_R = 0;             // rows of `hashes` valid for epp_index_add_picked
     int64_t shard_R = 0;            // rows of `hashes` valid for epp_shard_pick / epp_shard_merge
+    bool shard_models = false;      // the probed batch had model ids: its copy in `model_ids` feeds epp_shard_pick
     // endpoint-sharded mode over NVLink peer memory (shard_p2p.cu)
     void *p2p_buf = nullptr;        // this rank's exchange buffer {flags, masks, records} (cudaMalloc, IPC-exported)
     size_t p2p_bytes = 0, p2p_masks_off = 0, p2p_best_off = 0;
@@ -2382,14 +2383,19 @@ extern "C" int32_t epp_shard_probe(epp_engine *h, const epp_batch *batch, uint32
     if (!v.device) return fail(EPP_ERR_INVALID, "epp_shard_probe takes device-pointer batches (EPP_BATCH_DEVICE_PTRS)");
     h->kept_R = 0;
     h->shard_R = 0;
+    h->shard_models = false;
     EPP_TRY(commit_locked(h));
     EPP_TRY(run_batch(h, v, Mode::HashOnly, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr));
     int launches = 0;
     cudaStream_t s = h->slot[0].stream;
+    // the pick (a later call) scores lora-affinity with the batch's adapters: keep a copy, the caller's ids may be gone
+    if (v.model_ids && v.R)
+        CUDA_TRY(cudaMemcpyAsync(h->model_ids.p, v.model_ids, sizeof(uint32_t) * (size_t)v.R, cudaMemcpyDeviceToDevice, s));
     CUDA_TRY(launch_shard_probe(v.R, h->cfg.max_prefix_blocks, h->hashes.as<uint64_t>(), h->nblocks.as<int32_t>(),
                                 index_view(h), out_masks, mask_words_of(h), s, &launches));
     CUDA_TRY(cudaStreamSynchronize(s));
     h->shard_R = v.R;
+    h->shard_models = v.model_ids != nullptr;
     return EPP_OK;
 }
 
@@ -2401,7 +2407,8 @@ extern "C" int32_t epp_shard_pick(epp_engine *h, int64_t n_requests, const uint3
     if (!h->pool_ready) return fail(EPP_ERR_STATE, "epp_pool_set has not been called (after epp_shard_set)");
     if (n_requests != h->shard_R) return fail(EPP_ERR_STATE, "epp_shard_pick: n_requests %lld does not match the probed batch (%lld)", (long long)n_requests, (long long)h->shard_R);
     if (n_requests == 0) return EPP_OK;
-    Work w{0, n_requests, nullptr, nullptr, nullptr, 0, nullptr, 0, h->hashes.as<uint64_t>(), h->nblocks.as<int32_t>()};
+    Work w{0, n_requests, nullptr, nullptr, nullptr, 0, h->shard_models ? h->model_ids.as<uint32_t>() : nullptr, 0,
+           h->hashes.as<uint64_t>(), h->nblocks.as<int32_t>()};
     PickParams pp = pick_params(h, w, h->decisions.as<epp_decision>(), nullptr, nullptr);
     pp.global_masks = global_masks;
     pp.mask_words = mask_words_of(h);
