@@ -53,12 +53,16 @@ type AffinitySpec struct {
 	TTFTColumn             int // ext column carrying LatencyPredictionInfo.TTFT; -1 = attribute absent
 }
 
-// ProfileSpec mirrors epp_profile_cfg: role filter -> [prefix-cache-affinity-filter] -> scorers in order -> picker.
+// ProfileSpec mirrors epp_profile_cfg: role filter and label filters -> [prefix-cache-affinity-filter] -> scorers in
+// order -> picker.
 type ProfileSpec struct {
 	Filter   int // C.EPP_FILTER_*
 	Scorers  []ScorerSpec
 	Affinity *AffinitySpec
 	Picker   int // C.EPP_PICKER_* (0 = max-score-picker); see RandomPicker / WeightedRandomPicker
+	// Labels: the requirements of the profile's label filters (ProfileLabels of its LabelFilter plugins, labels.go),
+	// all ANDed with Filter; epp_label_filters_set
+	Labels []LabelReq
 }
 
 // Config mirrors epp_config (EndpointPickerConfig fields that define this path).
@@ -94,6 +98,7 @@ type Engine struct {
 	nameOf []types.NamespacedName // by slot; zero value = free
 	free   []uint32
 	models map[string]uint32 // TargetModel (+ cache salt) -> epp_model_register id
+	keys   map[string]bool   // label keys some profile's label filter references (SetPool sends only these)
 
 	inflight sync.WaitGroup // Schedule calls inside epp_submit / epp_wait (Close waits for them)
 	loads    sync.Map       // *scheduling.InferenceRequest -> inflightEntry, with Config.InFlightLoad (plugins.go)
@@ -169,12 +174,21 @@ func New(cfg Config) (*Engine, error) {
 		}
 	}
 	e := &Engine{cfg: cfg, slotOf: map[types.NamespacedName]uint32{}, models: map[string]uint32{},
-		nameOf: make([]types.NamespacedName, cfg.MaxEndpoints)}
+		nameOf: make([]types.NamespacedName, cfg.MaxEndpoints), keys: labelKeys(cfg)}
 	for s := cfg.MaxEndpoints - 1; s >= 0; s-- {
 		e.free = append(e.free, uint32(s))
 	}
 	if rc := C.epp_engine_create(&c, &e.h); rc != C.EPP_OK {
 		return nil, fmt.Errorf("eppcuda: epp_engine_create: %w", lastError())
+	}
+	for i, p := range []*ProfileSpec{&cfg.Primary, cfg.Prefill, cfg.Encode} {
+		if p == nil || (i == 2 && cfg.Prefill == nil) {
+			continue
+		}
+		if err := e.setLabelFilters(i, p.Labels); err != nil {
+			C.epp_engine_destroy(e.h)
+			return nil, err
+		}
 	}
 	var bc C.epp_batcher_cfg
 	bc.struct_size = C.uint32_t(unsafe.Sizeof(bc))
@@ -288,8 +302,13 @@ func (e *Engine) SetPool(pods []fwkdl.Endpoint) error {
 	n := len(pods)
 	if n == 0 {
 		C.epp_pool_set(e.h, 0, nil, nil, nil, nil, nil, nil)
+		if len(e.keys) > 0 {
+			C.epp_pool_set_labels(e.h, 0, nil, nil, nil)
+		}
 		return nil
 	}
+	var text []byte
+	offsets := make([]C.uint64_t, n+1)
 	ids := make([]C.uint32_t, n)
 	role := make([]C.uint8_t, n)
 	kv := make([]C.double, n)
@@ -310,12 +329,22 @@ func (e *Engine) SetPool(pods []fwkdl.Endpoint) error {
 		m := p.GetMetrics()
 		ids[i] = C.uint32_t(slot)
 		role[i] = roleOf(p.GetMetadata().Labels)
+		if len(e.keys) > 0 {
+			var err error
+			if text, err = appendLabels(text, p.GetMetadata().Labels, e.keys); err != nil {
+				return err
+			}
+			offsets[i+1] = C.uint64_t(len(text))
+		}
 		kv[i] = C.double(m.KVCacheUsagePercent)
 		waiting[i] = C.int32_t(m.WaitingQueueSize)
 		running[i] = C.int32_t(m.RunningRequestsSize)
 	}
 	if rc := C.epp_pool_set(e.h, C.int32_t(n), &ids[0], &role[0], &kv[0], &waiting[0], &running[0], nil); rc != C.EPP_OK {
 		return fmt.Errorf("eppcuda: epp_pool_set: %w", lastError())
+	}
+	if len(e.keys) > 0 {
+		return e.setPoolLabels(ids, text, offsets)
 	}
 	return nil
 }

@@ -29,9 +29,11 @@ const (
 var shared *Engine // set by Register
 
 // Register installs the factories (plugin.Register, registry.go:25-30).  Call it next to RegisterAllPlugins
-// (cmd/epp/main.go:59) after the engine has been created.
+// (cmd/epp/main.go:59) after the engine has been created.  It also replaces the factories of label-selector-filter,
+// by-label-selector and by-label with ones whose plugins carry the engine's compiled requirements (labels.go).
 func Register(e *Engine) {
 	shared = e
+	registerLabelFilters()
 	plugin.Register(PrefixProducerType, func(name string, _ json.RawMessage, _ plugin.Handle) (plugin.Plugin, error) {
 		if shared == nil {
 			return nil, errors.New("eppcuda: engine not created")

@@ -367,6 +367,55 @@ EPP_API int32_t epp_pool_set_lora(epp_engine *h, int32_t n, const uint32_t *ids,
                           const int32_t *n_models_loaded, int64_t n_members, const uint32_t *member_ep,
                           const uint32_t *member_model, const uint8_t *member_state);
 
+/* ---- Label filters (filter/bylabel/selector.go:34-101 "label-selector-filter" / deprecated "by-label-selector", and
+ * filter/bylabel/filter.go:34-117 "by-label") ---------------------------------------------------------------------------
+ * Each profile may hold label requirements besides its role filter.  A slot is a candidate of the profile when it is in
+ * the pool, passes the role filter and matches EVERY requirement (AND; an empty list keeps everything).  The chain is
+ * [role and label filters, any order] [prefix-cache-affinity-filter]: label and role filters are pure per-endpoint
+ * predicates, so their order does not matter; a label filter after the affinity filter is not supported.  Labels are the
+ * endpoint's EndpointMetadata.Labels; a requirement on key k reads labels[k]:
+ *   EPP_LABEL_IN            k present and its value among `values` (an absent key never matches, even with "" listed)
+ *   EPP_LABEL_NOT_IN        k absent, or its value not among `values` (an absent key always matches)
+ *   EPP_LABEL_EXISTS        k present (any value, "" included)
+ *   EPP_LABEL_DOES_NOT_EXIST k absent
+ *   EPP_LABEL_BY_LABEL      by-label with allowsNoLabel = false: labels[k] among `values`, where an ABSENT key reads as ""
+ *                           (filter.go:108-111), so "" among `values` also admits slots without the key
+ *   EPP_LABEL_BY_LABEL_OR_ABSENT  by-label with allowsNoLabel = true: k absent, or labels[k] among `values`
+ * matchLabels {k: v} is k In [v].  IN / NOT_IN / BY_LABEL need at least one value, EXISTS / DOES_NOT_EXIST take none,
+ * BY_LABEL_OR_ABSENT any number.  The IN / NOT_IN rules for absent keys and the key / value syntax come from
+ * k8s.io/apimachinery's Requirement.Matches and validation, which the reference does not pin in its own tests; this
+ * engine states them as its contract.  The C side checks structure only (a key is non-empty and holds no '=' or newline,
+ * a value holds no newline); the shims validate label syntax as LabelSelectorAsSelector does.
+ * Caps: EPP_LABEL_MAX_REQS requirements per profile, 16 distinct keys over all profiles, 62 distinct named values per key.
+ * Over a cap is EPP_ERR_INVALID.  Every rejected call changes no state.
+ * Cost: the filters are decided when the pool kernels derive each profile's candidates (per snapshot), not per request. */
+#define EPP_LABEL_MAX_REQS 32
+typedef enum {
+    EPP_LABEL_IN = 0,
+    EPP_LABEL_NOT_IN = 1,
+    EPP_LABEL_EXISTS = 2,
+    EPP_LABEL_DOES_NOT_EXIST = 3,
+    EPP_LABEL_BY_LABEL = 4,            /* by-label, allowsNoLabel = false: value in the set, an absent key reads "" */
+    EPP_LABEL_BY_LABEL_OR_ABSENT = 5   /* by-label, allowsNoLabel = true                                          */
+} epp_label_op;
+typedef struct {
+    const char *key;                   /* NUL-terminated                                                           */
+    int32_t op;                        /* epp_label_op                                                             */
+    int32_t n_values;
+    const char *const *values;         /* [n_values] NUL-terminated; duplicates allowed                            */
+} epp_label_req;
+/* profile: 0 primary / decode, 1 prefill, 2 encode (a profile the configuration has).  Replaces that profile's label
+ * requirements.  Only before the engine's first successful epp_pool_set / epp_pool_set_labels (EPP_ERR_STATE after). */
+EPP_API int32_t epp_label_filters_set(epp_engine *h, int32_t profile, int32_t n, const epp_label_req *reqs);
+/* EndpointMetadata.Labels of the listed slots: text[offsets[i] .. offsets[i+1]) holds entry i's labels as "key=value\n"
+ * lines (each split at its first '=').  offsets: [n + 1], non-decreasing.  Replaces every slot's labels (slots not listed
+ * have none) and re-derives every profile, as epp_pool_set does; batches enqueued before the call decide on the labels
+ * they were enqueued under, and epp_pool_set alone keeps the labels.  Rejected: a NULL array, a slot id >= max_endpoints
+ * or listed twice, a line without '=' or newline, an empty key, a key repeated within one slot.  On an engine without
+ * label requirements the call only validates: nothing on the device reads labels. */
+EPP_API int32_t epp_pool_set_labels(epp_engine *h, int32_t n, const uint32_t *ids, const uint64_t *offsets,
+                                    const uint8_t *text);
+
 /* ---- prefix index write side (approximateprefix/indexer.go:52-83, 105-115, 167-182; plugin.go:164-211) --
  * The LRU bookkeeping lives in HBM (index_store.cu): epp_index_add calls are queued and applied as ONE device batch,
  * in call order, by the next commit / lookup / remove; epp_index_add_picked never leaves the device.  The read table

@@ -89,6 +89,14 @@ class Subset(C.Structure):
                 ("slots", C.c_void_p)]
 
 
+EPP_LABEL_MAX_REQS = 32
+LABEL_IN, LABEL_NOT_IN, LABEL_EXISTS, LABEL_DOES_NOT_EXIST, LABEL_BY_LABEL, LABEL_BY_LABEL_OR_ABSENT = range(6)
+
+
+class LabelReq(C.Structure):
+    _fields_ = [("key", C.c_char_p), ("op", C.c_int32), ("n_values", C.c_int32), ("values", C.POINTER(C.c_char_p))]
+
+
 class BatcherCfg(C.Structure):
     _fields_ = [("struct_size", C.c_uint32), ("max_batch", C.c_int32), ("max_delay_us", C.c_int32),
                 ("index_picks", C.c_int32)]
@@ -130,6 +138,8 @@ SIGNATURES = {
     "epp_prefix_match": (C.c_int32, [C.c_void_p, C.POINTER(Batch), C.c_void_p, C.c_void_p]),
     "epp_pool_set_lora": (C.c_int32, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
                                       C.c_void_p, C.c_void_p]),
+    "epp_label_filters_set": (C.c_int32, [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(LabelReq)]),
+    "epp_pool_set_labels": (C.c_int32, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "epp_score": (C.c_int32, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p,
                               C.c_uint32]),
     "epp_schedule": (C.c_int32, [C.c_void_p, C.POINTER(Batch), C.c_void_p, C.c_void_p, C.c_int32]),

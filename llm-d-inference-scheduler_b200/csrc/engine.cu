@@ -59,6 +59,19 @@ struct ProfileState {
     DevBuf cands, wcum, icum;       // random pickers only (ProfileDerived)
 };
 
+struct LabelReq {                   // one epp_label_req, copied
+    std::string key;
+    int32_t op;
+    std::vector<std::string> values;
+};
+// Every profile's label requirements compiled against one interning of keys and values (epp_label_filters_set).
+struct LabelPlan {
+    std::vector<std::string> keys;                                  // row k of lcode
+    std::vector<std::unordered_map<std::string, uint8_t>> codes;    // per key: named value -> code 1..62
+    LabelFilterDev dev[kMaxProfiles] = {};                          // lcode filled in by label_dev
+};
+static constexpr int kMaxLabelKeys = 16, kMaxLabelValues = 62;
+
 struct Slot {                       // per-stream staging for host-pointer batches
     cudaStream_t stream = nullptr;
     DevBuf data;
@@ -105,6 +118,11 @@ struct epp_engine {
     DevBuf lora_max, lora_cnt, lora_ptr, lora_ep, lora_state, score_models;   // LoRA residency (epp_pool_set_lora)
     bool lora_set = false, lora_enabled = false;
     int32_t lora_models = 0;
+    // label filters: the requirements of each profile, their compiled form and the interned labels of every slot
+    std::vector<LabelReq> label_reqs[kMaxProfiles];
+    LabelPlan labels;
+    DevBuf lcode;                   // uint8 [labels.keys.size()][E] (LabelFilterDev)
+    bool pool_called = false;       // epp_pool_set / epp_pool_set_labels succeeded once: the label filters are fixed
     ProfileState prof[kMaxProfiles];
     // no-hit-lru scorer (nohit_lru.cu), allocated only when a profile lists it
     int nohit_mask = 0;             // bit pi: profile pi has the scorer
@@ -677,10 +695,16 @@ static NoHitView nohit_view(epp_engine *h, int64_t r0) {
     return v;
 }
 
-// Request-independent scorer terms of profile p from the current pool (+ LoRA) snapshot, on the device.
+static LabelFilterDev label_dev(epp_engine *h, int p) {
+    LabelFilterDev d = h->labels.dev[p];
+    d.lcode = h->lcode.as<uint8_t>();
+    return d;
+}
+
+// Request-independent scorer terms of profile p from the current pool (+ LoRA, + labels) snapshot, on the device.
 static int32_t derive_profile(epp_engine *h, int p, cudaStream_t s, int *launches) {
-    CUDA_TRY(launch_pool_prepare(pool_arrays(h), profile_cfg(h, p), profile_derived(h, p, false), h->Epad, h->shard_begin,
-                                 h->shard_end, s, launches));
+    CUDA_TRY(launch_pool_prepare(pool_arrays(h), profile_cfg(h, p), label_dev(h, p), profile_derived(h, p, false), h->Epad,
+                                 h->shard_begin, h->shard_end, s, launches));
     return EPP_OK;
 }
 
@@ -814,6 +838,7 @@ extern "C" int32_t epp_pool_set(epp_engine *h, int32_t n, const uint32_t *ids, c
     EPP_TRY(derive_pool(h));
     CUDA_TRY(cudaStreamSynchronize(s));
     h->pool_ready = true;
+    h->pool_called = true;
     return EPP_OK;
 }
 
@@ -872,6 +897,144 @@ extern "C" int32_t epp_pool_set_lora(epp_engine *h, int32_t n, const uint32_t *i
     }
     h->lora_models = n_models;
     h->lora_set = true;
+    if (h->pool_ready) EPP_TRY(derive_pool(h));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    return EPP_OK;
+}
+
+// ---- label filters ----------------------------------------------------------------------------------------------------
+// Interns the keys and named values of every profile's requirements and compiles each requirement to one mask of the
+// codes it admits (include/epp_engine.h "Label filters").  Fails on a cap; `out` is then unusable.
+static int32_t compile_labels(const std::vector<LabelReq> (&reqs)[kMaxProfiles], LabelPlan &out) {
+    out = LabelPlan{};
+    for (int p = 0; p < kMaxProfiles; p++) {
+        LabelFilterDev &d = out.dev[p];
+        d.n = (int32_t)reqs[p].size();
+        for (int i = 0; i < d.n; i++) {
+            const LabelReq &q = reqs[p][i];
+            size_t k = std::find(out.keys.begin(), out.keys.end(), q.key) - out.keys.begin();
+            if (k == out.keys.size()) {
+                if ((int)k == kMaxLabelKeys) return fail(EPP_ERR_INVALID, "label filters reference more than %d distinct keys", kMaxLabelKeys);
+                out.keys.push_back(q.key);
+                out.codes.emplace_back();
+            }
+            auto &codes = out.codes[k];
+            uint64_t named = 0;
+            bool empty_named = false;
+            for (const std::string &v : q.values) {
+                auto it = codes.find(v);
+                if (it == codes.end()) {
+                    if ((int)codes.size() == kMaxLabelValues)
+                        return fail(EPP_ERR_INVALID, "label key \"%s\": more than %d distinct values named", q.key.c_str(), kMaxLabelValues);
+                    it = codes.emplace(v, (uint8_t)(codes.size() + 1)).first;
+                }
+                named |= 1ull << it->second;
+                empty_named |= v.empty();
+            }
+            const uint64_t absent = 1ull, all = ~0ull;
+            uint64_t m = 0;
+            switch (q.op) {
+                case EPP_LABEL_IN: m = named; break;                                 // absent never matches
+                case EPP_LABEL_NOT_IN: m = all & ~named; break;                      // absent always matches
+                case EPP_LABEL_EXISTS: m = all & ~absent; break;
+                case EPP_LABEL_DOES_NOT_EXIST: m = absent; break;
+                case EPP_LABEL_BY_LABEL: m = named | (empty_named ? absent : 0); break;   // absent reads ""
+                case EPP_LABEL_BY_LABEL_OR_ABSENT: m = named | absent; break;
+            }
+            d.key[i] = (uint8_t)k;
+            d.mask[i] = m;
+        }
+    }
+    return EPP_OK;
+}
+
+extern "C" int32_t epp_label_filters_set(epp_engine *h, int32_t profile, int32_t n, const epp_label_req *reqs) {
+    if (!h) return fail(EPP_ERR_INVALID, "NULL engine");
+    if (profile < 0 || profile >= h->n_alloc_profiles) return fail(EPP_ERR_INVALID, "profile %d is not configured", profile);
+    if (n < 0 || n > EPP_LABEL_MAX_REQS) return fail(EPP_ERR_INVALID, "%d label requirements, out of range [0,%d]", n, EPP_LABEL_MAX_REQS);
+    if (n > 0 && !reqs) return fail(EPP_ERR_INVALID, "NULL requirements");
+    std::vector<LabelReq> mine;
+    for (int32_t i = 0; i < n; i++) {
+        const epp_label_req &r = reqs[i];
+        if (!r.key || !r.key[0]) return fail(EPP_ERR_INVALID, "requirement %d: empty key", i);
+        if (strpbrk(r.key, "=\n")) return fail(EPP_ERR_INVALID, "requirement %d: key holds '=' or a newline", i);
+        if (r.op < EPP_LABEL_IN || r.op > EPP_LABEL_BY_LABEL_OR_ABSENT) return fail(EPP_ERR_INVALID, "requirement %d: unknown op %d", i, r.op);
+        const bool takes = r.op != EPP_LABEL_EXISTS && r.op != EPP_LABEL_DOES_NOT_EXIST;
+        const bool needs = r.op == EPP_LABEL_IN || r.op == EPP_LABEL_NOT_IN || r.op == EPP_LABEL_BY_LABEL;
+        if (r.n_values < 0 || (!takes && r.n_values != 0) || (needs && r.n_values == 0))
+            return fail(EPP_ERR_INVALID, "requirement %d: %d values do not fit op %d", i, r.n_values, r.op);
+        if (r.n_values > 0 && !r.values) return fail(EPP_ERR_INVALID, "requirement %d: NULL values", i);
+        LabelReq q{r.key, r.op, {}};
+        for (int32_t j = 0; j < r.n_values; j++) {
+            if (!r.values[j]) return fail(EPP_ERR_INVALID, "requirement %d: value %d is NULL", i, j);
+            if (strchr(r.values[j], '\n')) return fail(EPP_ERR_INVALID, "requirement %d: value %d holds a newline", i, j);
+            q.values.emplace_back(r.values[j]);
+        }
+        mine.push_back(std::move(q));
+    }
+    std::lock_guard<std::mutex> lk(h->mu);
+    if (h->pool_called) return fail(EPP_ERR_STATE, "label filters are fixed once the pool has been set");
+    std::vector<LabelReq> all[kMaxProfiles];
+    for (int p = 0; p < kMaxProfiles; p++) all[p] = p == profile ? mine : h->label_reqs[p];
+    LabelPlan plan;
+    EPP_TRY(compile_labels(all, plan));
+    EPP_TRY(set_device(h));
+    const size_t bytes = plan.keys.size() * (size_t)h->cfg.max_endpoints;
+    if (bytes) {
+        CUDA_TRY(h->lcode.reserve(bytes, &h->dev_bytes));
+        cudaStream_t s = h->slot[0].stream;                      // the stream every later upload and derive runs on
+        CUDA_TRY(cudaMemsetAsync(h->lcode.p, 0, bytes, s));      // no labels yet: every key absent
+        CUDA_TRY(cudaStreamSynchronize(s));
+    }
+    h->label_reqs[profile] = std::move(mine);
+    h->labels = std::move(plan);
+    return EPP_OK;
+}
+
+extern "C" int32_t epp_pool_set_labels(epp_engine *h, int32_t n, const uint32_t *ids, const uint64_t *offsets,
+                                       const uint8_t *text) {
+    if (!h) return fail(EPP_ERR_INVALID, "NULL engine");
+    if (n < 0 || (n > 0 && (!ids || !offsets || !text))) return fail(EPP_ERR_INVALID, "NULL label arrays");
+    std::lock_guard<std::mutex> lk(h->mu);
+    const uint32_t E = (uint32_t)h->cfg.max_endpoints;
+    const size_t K = h->labels.keys.size();
+    std::vector<uint8_t> seen(E, 0), lc(K * (size_t)E, 0);
+    std::unordered_map<std::string, size_t> key_row;
+    for (size_t k = 0; k < K; k++) key_row.emplace(h->labels.keys[k], k);
+    std::vector<std::string> slot_keys;
+    for (int32_t i = 0; i < n; i++) {
+        const uint32_t id = ids[i];
+        if (id >= E) return fail(EPP_ERR_INVALID, "label entry %d: slot id %u >= max_endpoints %u", i, id, E);
+        if (seen[id]) return fail(EPP_ERR_INVALID, "label entry %d: duplicate slot id %u", i, id);
+        seen[id] = 1;
+        if (offsets[i + 1] < offsets[i]) return fail(EPP_ERR_INVALID, "label entry %d: offsets decrease", i);
+        slot_keys.clear();
+        const char *p = reinterpret_cast<const char *>(text) + offsets[i], *end = reinterpret_cast<const char *>(text) + offsets[i + 1];
+        while (p < end) {
+            const char *nl = static_cast<const char *>(memchr(p, '\n', (size_t)(end - p)));
+            if (!nl) return fail(EPP_ERR_INVALID, "label entry %d: a label is not terminated by a newline", i);
+            const char *eq = static_cast<const char *>(memchr(p, '=', (size_t)(nl - p)));
+            if (!eq) return fail(EPP_ERR_INVALID, "label entry %d: a label has no '='", i);
+            if (eq == p) return fail(EPP_ERR_INVALID, "label entry %d: a label has an empty key", i);
+            std::string key(p, eq);
+            if (std::find(slot_keys.begin(), slot_keys.end(), key) != slot_keys.end())
+                return fail(EPP_ERR_INVALID, "label entry %d: key \"%s\" repeated", i, key.c_str());
+            slot_keys.push_back(key);
+            auto kr = key_row.find(key);
+            if (kr != key_row.end()) {                     // keys no requirement references are dropped here
+                const auto &codes = h->labels.codes[kr->second];
+                auto c = codes.find(std::string(eq + 1, nl));
+                lc[kr->second * (size_t)E + id] = c == codes.end() ? 63 : c->second;
+            }
+            p = nl + 1;
+        }
+    }
+    h->pool_called = true;
+    if (!K) return EPP_OK;                                 // no label filter: nothing on the device reads labels
+    EPP_TRY(set_device(h));
+    EPP_TRY(join_streams(h));
+    cudaStream_t s = h->slot[0].stream;
+    CUDA_TRY(cudaMemcpyAsync(h->lcode.p, lc.data(), lc.size(), cudaMemcpyHostToDevice, s));
     if (h->pool_ready) EPP_TRY(derive_pool(h));
     CUDA_TRY(cudaStreamSynchronize(s));
     return EPP_OK;

@@ -121,7 +121,7 @@ struct PoolArrays {
 };
 struct ProfileDerived {
     // per profile, device arrays
-    uint8_t *cand;             // [E] 1 = passes the role filter
+    uint8_t *cand;             // [E] 1 = passes the role and label filters
     double *contrib;           // [EPP_MAX_SCORERS][E] clamp(score)*weight of every request-independent scorer
     double *base;              // [E] ordered weighted sum with every prefix term = clamp(0)*w
     uint32_t *order;           // [Epad] candidates sorted by (base desc, slot asc); then non-candidates
@@ -135,10 +135,20 @@ struct ProfileDerived {
     double *wcum;              // [E + 1]
     uint32_t *icum;            // [E + 1]
 };
+// A profile's label filters (include/epp_engine.h "Label filters"), compiled on the host: slot e passes requirement i
+// when bit lcode[key[i]][e] of mask[i] is set.  lcode codes: 0 = key absent, 1..62 = a value some requirement names,
+// 63 = any other value.  n == 0: no label filter (lcode is not read).
+struct LabelFilterDev {
+    const uint8_t *lcode;      // [keys][E]
+    int32_t n;
+    uint8_t key[EPP_LABEL_MAX_REQS];
+    uint64_t mask[EPP_LABEL_MAX_REQS];
+};
 // [shard_begin, shard_end): only these slots become candidates (queue min/max still span the whole pool).
 // A no-hit-lru scorer gets its warm score 0.5 here (the cold set comes from launch_pool_order).
-cudaError_t launch_pool_prepare(const PoolArrays &pool, const epp_profile_cfg &prof, const ProfileDerived &d,
-                                int32_t Epad, uint32_t shard_begin, uint32_t shard_end, cudaStream_t s, int *launches);
+cudaError_t launch_pool_prepare(const PoolArrays &pool, const epp_profile_cfg &prof, const LabelFilterDev &labels,
+                                const ProfileDerived &d, int32_t Epad, uint32_t shard_begin, uint32_t shard_end,
+                                cudaStream_t s, int *launches);
 // The contribution rows, base sums, (base desc, slot asc) order and groups of d over d.cand / d.n_cand / d.qminmax (already
 // derived), with the raw no-hit-lru score of slot e = nohit_col[e] (nullptr: the warm 0.5).  gate != nullptr: every kernel
 // returns at once unless *gate != 0.

@@ -25,15 +25,15 @@ namespace epp {
 // ------------------------------------------------------------------------------------------------
 // pool snapshot -> derived per-profile arrays
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(1024) k_pool_candidates(PoolArrays pool, int filter, uint32_t shard_begin,
-                                                          uint32_t shard_end, uint8_t *cand, int32_t *n_cand,
-                                                          int64_t *qminmax) {
+__global__ void __launch_bounds__(1024) k_pool_candidates(PoolArrays pool, int filter, LabelFilterDev labels,
+                                                          uint32_t shard_begin, uint32_t shard_end, uint8_t *cand,
+                                                          int32_t *n_cand, int64_t *qminmax) {
     __shared__ long long s_mn[2][32], s_mx[2][32];
     __shared__ int s_cnt[32];
     long long mnw = LLONG_MAX, mxw = LLONG_MIN, mnr = LLONG_MAX, mxr = LLONG_MIN;
     int cnt = 0;
     for (int e = threadIdx.x; e < pool.E; e += blockDim.x) {
-        bool k = filter_keeps(filter, pool.role[e]);
+        bool k = profile_keeps(filter, labels, pool, e);
         bool local = k && (uint32_t)e >= shard_begin && (uint32_t)e < shard_end;
         cand[e] = local ? 1 : 0;
         if (k) {      // queue min/max span every candidate of the pool, not only this shard's (queue.go:79-91)
@@ -68,7 +68,8 @@ __global__ void __launch_bounds__(1024) k_pool_candidates(PoolArrays pool, int f
 
 // active-request scorers: max in-flight request count over the profile's candidates (whole pool, like the queue
 // min/max), starting from 0 (active_request.go:144-155) -> qminmax[4 + s].
-__global__ void __launch_bounds__(1024) k_pool_aux(PoolArrays pool, epp_profile_cfg cfg, int filter, int64_t *qminmax) {
+__global__ void __launch_bounds__(1024) k_pool_aux(PoolArrays pool, epp_profile_cfg cfg, int filter, LabelFilterDev labels,
+                                                   int64_t *qminmax) {
     __shared__ long long s_mx[32];
     for (int s = 0; s < cfg.n_scorers; s++) {
         if (cfg.scorers[s].kind != EPP_SCORER_ACTIVE_REQUEST) continue;
@@ -76,7 +77,7 @@ __global__ void __launch_bounds__(1024) k_pool_aux(PoolArrays pool, epp_profile_
         long long mx = 0;
         if (col >= 0 && col < pool.n_ext_cols)
             for (int e = threadIdx.x; e < pool.E; e += blockDim.x)
-                if (filter_keeps(filter, pool.role[e])) mx = max(mx, (long long)pool.ext[(size_t)col * (size_t)pool.E + (size_t)e]);
+                if (profile_keeps(filter, labels, pool, e)) mx = max(mx, (long long)pool.ext[(size_t)col * (size_t)pool.E + (size_t)e]);
         for (int o = 16; o; o >>= 1) mx = max(mx, __shfl_xor_sync(0xffffffffu, mx, o));
         if ((threadIdx.x & 31) == 0) s_mx[threadIdx.x >> 5] = mx;
         __syncthreads();
@@ -226,12 +227,13 @@ cudaError_t launch_pool_order(const PoolArrays &pool, const epp_profile_cfg &pro
     return cudaGetLastError();
 }
 
-cudaError_t launch_pool_prepare(const PoolArrays &pool, const epp_profile_cfg &prof, const ProfileDerived &d,
-                                int32_t Epad, uint32_t shard_begin, uint32_t shard_end, cudaStream_t s, int *launches) {
-    k_pool_candidates<<<1, 1024, 0, s>>>(pool, prof.filter, shard_begin, shard_end, d.cand, d.n_cand, d.qminmax);
+cudaError_t launch_pool_prepare(const PoolArrays &pool, const epp_profile_cfg &prof, const LabelFilterDev &labels,
+                                const ProfileDerived &d, int32_t Epad, uint32_t shard_begin, uint32_t shard_end,
+                                cudaStream_t s, int *launches) {
+    k_pool_candidates<<<1, 1024, 0, s>>>(pool, prof.filter, labels, shard_begin, shard_end, d.cand, d.n_cand, d.qminmax);
     for (int i = 0; i < prof.n_scorers; i++)
         if (prof.scorers[i].kind == EPP_SCORER_ACTIVE_REQUEST) {
-            k_pool_aux<<<1, 1024, 0, s>>>(pool, prof, prof.filter, d.qminmax);
+            k_pool_aux<<<1, 1024, 0, s>>>(pool, prof, prof.filter, labels, d.qminmax);
             if (launches) *launches += 1;
             break;
         }

@@ -30,6 +30,15 @@ __device__ __forceinline__ bool filter_keeps(int filter, uint8_t role) {
     }
 }
 
+// Does the profile keep slot e: its role filter AND every label requirement (one bit test each).  The pool kernels are
+// the only callers: every per-request kernel reads the cand[] they write.
+__device__ __forceinline__ bool profile_keeps(int filter, const LabelFilterDev &lf, const PoolArrays &pool, int32_t e) {
+    if (!filter_keeps(filter, pool.role[e])) return false;
+    for (int i = 0; i < lf.n; i++)
+        if (!((lf.mask[i] >> lf.lcode[(size_t)lf.key[i] * (size_t)pool.E + (size_t)e]) & 1ull)) return false;
+    return true;
+}
+
 // enforceScoreRange, scheduler_profile.go:194-202 (NaN passes through, as in Go)
 __device__ __forceinline__ double clamp01(double s) {
     if (s < 0.0) return 0.0;

@@ -47,12 +47,14 @@ class AffinityFilterSpec:
 
 @dataclass
 class ProfileSpec:
-    """One SchedulerProfile: role filter -> [prefix-cache-affinity-filter] -> scorers in order -> picker
-    (capi.PICKER_MAX_SCORE / PICKER_RANDOM / PICKER_WEIGHTED_RANDOM)."""
+    """One SchedulerProfile: role filter and label filters -> [prefix-cache-affinity-filter] -> scorers in order ->
+    picker (capi.PICKER_MAX_SCORE / PICKER_RANDOM / PICKER_WEIGHTED_RANDOM).  labels: the label requirements
+    [(key, capi.LABEL_* op, [values...]), ...], all ANDed (Engine.label_filters_set)."""
     filter: int = capi.FILTER_NONE
     scorers: list = field(default_factory=list)
     affinity: AffinityFilterSpec | None = None
     picker: int = capi.PICKER_MAX_SCORE
+    labels: list = field(default_factory=list)
 
 
 def _fill_profile(dst: capi.ProfileCfg, spec: ProfileSpec):
@@ -143,6 +145,9 @@ class Engine:
         self.B = max_prefix_blocks
         self._h = C.c_void_p()
         self._check(self._lib.epp_engine_create(C.byref(cfg), C.byref(self._h)))
+        for p, spec in enumerate((primary, prefill, encode)):
+            if spec is not None and spec.labels:
+                self.label_filters_set(p, spec.labels)
 
     # ---- plumbing ----
     def _check(self, rc: int):
@@ -342,6 +347,35 @@ class Engine:
         mst = np.ascontiguousarray(mem[:, 2], dtype=np.uint8)
         self._check(self._lib.epp_pool_set_lora(self._h, ids.shape[0], _ptr(ids), _ptr(mx), _ptr(nl), mem.shape[0],
                                                 _ptr(mep), _ptr(mmo), _ptr(mst)))
+
+    def label_filters_set(self, profile: int, reqs):
+        """The label requirements of profile 0 (primary / decode), 1 (prefill) or 2 (encode), ANDed with its role
+        filter: reqs = [(key, op, [values...]), ...], op one of capi.LABEL_* (include/epp_engine.h "Label filters").
+        Only before the first pool_set / pool_set_labels."""
+        reqs = list(reqs)
+        arr = (capi.LabelReq * max(len(reqs), 1))()
+        keep = []
+        for i, (key, op, values) in enumerate(reqs):
+            vals = [v.encode() if isinstance(v, str) else bytes(v) for v in values]
+            va = (C.c_char_p * max(len(vals), 1))(*vals)
+            keep.append(va)
+            arr[i].key = key.encode() if isinstance(key, str) else bytes(key)
+            arr[i].op = op
+            arr[i].n_values = len(vals)
+            arr[i].values = C.cast(va, C.POINTER(C.c_char_p))
+        self._check(self._lib.epp_label_filters_set(self._h, profile, len(reqs), arr))
+
+    def pool_set_labels(self, ids, labels):
+        """EndpointMetadata.Labels of slots ids[i] = labels[i] (a dict str -> str, or None); other slots have none."""
+        ids = np.ascontiguousarray(ids, dtype=np.uint32)
+        assert len(labels) == ids.shape[0]
+        if any("\n" in k or "=" in k or "\n" in v for lb in labels for k, v in (lb or {}).items()):
+            raise ValueError("a label key holds '=' or a newline, or a value holds a newline")
+        parts = [b"".join(f"{k}={v}\n".encode() for k, v in (lb or {}).items()) for lb in labels]
+        offs = np.zeros(len(parts) + 1, dtype=np.uint64)
+        np.cumsum([len(p) for p in parts], out=offs[1:])
+        text = np.frombuffer(b"".join(parts) or b"\0", dtype=np.uint8)
+        self._check(self._lib.epp_pool_set_labels(self._h, ids.shape[0], _ptr(ids), _ptr(offs), _ptr(text)))
 
     def schedule(self, data, offsets=None, uniform_len=None, model_ids=None, n_requests=None, keep_hashes=False,
                  detail=True, out=None, lengths=None, asynchronous=False, multimodal=None, topk=False, subsets=None):

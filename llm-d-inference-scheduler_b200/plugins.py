@@ -10,10 +10,13 @@ Reference interfaces mirrored (paths relative to the reference root):
   Scheduler.Schedule                                      pkg/epp/scheduling/scheduler.go:54-102
   MaxScorePicker (maxNumOfEndpoints)                      .../picker/maxscore/picker.go:58-115
   prefix-cache-affinity-filter                            .../filter/prefixcacheaffinity/plugin.go:45-151
+  label-selector-filter / by-label-selector / by-label    .../filter/bylabel/selector.go:34-101, filter.go:34-117
   approximateprefix dataProducer Produce / PreRequest     .../approximateprefix/plugin.go:135-200
 """
 from __future__ import annotations
 
+import json
+import re
 from dataclasses import dataclass, field
 
 import numpy as np
@@ -189,6 +192,140 @@ def NewEncodeRole():
     return _RoleFilter(capi.FILTER_ENCODE)
 
 
+# ---- label filters (filter/bylabel/selector.go, filter.go; decided in the pool kernels, include/epp_engine.h) ----
+LabelSelectorFilterType, ByLabelSelectorType, ByLabelType = "label-selector-filter", "by-label-selector", "by-label"
+_NAME_RE = re.compile(r"^([A-Za-z0-9]([-A-Za-z0-9_.]*[A-Za-z0-9])?)?$")
+_DNS1123_RE = re.compile(r"^[a-z0-9]([-a-z0-9]*[a-z0-9])?(\.[a-z0-9]([-a-z0-9]*[a-z0-9])?)*$")
+_OPS = {"In": capi.LABEL_IN, "NotIn": capi.LABEL_NOT_IN, "Exists": capi.LABEL_EXISTS,
+        "DoesNotExist": capi.LABEL_DOES_NOT_EXIST}
+
+
+def _validate_key(k: str):
+    """apimachinery validation.IsQualifiedName: [prefix/]name, prefix a DNS-1123 subdomain <= 253, name <= 63."""
+    if not isinstance(k, str):
+        raise ValueError(f"invalid label key {k!r}")
+    parts = k.split("/")
+    if len(parts) > 2:
+        raise ValueError(f"invalid label key {k!r}: a qualified name must consist of alphanumeric characters, '-', '_' "
+                         "or '.', with an optional DNS subdomain prefix and '/'")
+    name = parts[-1]
+    if len(parts) == 2 and (not parts[0] or len(parts[0]) > 253 or not _DNS1123_RE.match(parts[0])):
+        raise ValueError(f"invalid label key {k!r}: prefix part must be a lowercase RFC 1123 subdomain")
+    if not name or len(name) > 63 or not _NAME_RE.match(name):
+        raise ValueError(f"invalid label key {k!r}: name part must be non-empty, at most 63 characters, alphanumeric, "
+                         "'-', '_' or '.', and start and end with an alphanumeric character")
+
+
+def _validate_value(v: str):
+    """apimachinery validation.IsValidLabelValue: empty, or <= 63 characters of the name form."""
+    if not isinstance(v, str) or len(v) > 63 or not _NAME_RE.match(v):
+        raise ValueError(f"invalid label value: {v!r}: a valid label must be an empty string or consist of alphanumeric "
+                         "characters, '-', '_' or '.', and must start and end with an alphanumeric character")
+
+
+@dataclass
+class _LabelFilter:
+    """A label filter: its typed name and its requirements (key, capi.LABEL_* op, values), all ANDed."""
+    type_name: str
+    name: str
+    reqs: list
+
+    def TypedName(self):
+        return (self.type_name, self.name)
+
+
+def _requirement(key, op_name, values):
+    """labels.NewRequirement: operator, value count, key and value syntax."""
+    if op_name not in _OPS:
+        raise ValueError(f"{op_name!r} is not a valid label selector operator")
+    _validate_key(key)
+    values = list(values or [])
+    op = _OPS[op_name]
+    if op in (capi.LABEL_IN, capi.LABEL_NOT_IN) and not values:
+        raise ValueError("for 'in', 'notin' operators, values set can't be empty")
+    if op in (capi.LABEL_EXISTS, capi.LABEL_DOES_NOT_EXIST) and values:
+        raise ValueError("values set must be empty for exists and does not exist")
+    for v in values:
+        _validate_value(v)
+    return (key, op, values)
+
+
+def _selector_requirements(selector):
+    """metav1.LabelSelectorAsSelector: None = Nothing, {} = Everything, else matchLabels (k In [v]) AND matchExpressions."""
+    if selector is None:
+        # labels.Nothing(): Exists and DoesNotExist on one key, which no endpoint meets together.  The key counts against
+        # the engine's 16 interned keys; llm-d.ai/role is the one a P/D configuration is most likely to name anyway.
+        return [(RoleLabel, capi.LABEL_EXISTS, []), (RoleLabel, capi.LABEL_DOES_NOT_EXIST, [])]
+    if not isinstance(selector, dict):
+        raise ValueError(f"not a label selector: {selector!r}")
+    # fields other than matchLabels / matchExpressions are ignored, as json.Unmarshal ignores them
+    reqs = [_requirement(k, "In", [v]) for k, v in (selector.get("matchLabels") or {}).items()]
+    for ex in selector.get("matchExpressions") or []:
+        reqs.append(_requirement(ex.get("key"), ex.get("operator"), ex.get("values")))
+    return reqs
+
+
+def NewSelector(name: str, selector):
+    """bylabel.NewSelector (selector.go:62-77): selector is a metav1.LabelSelector as a dict."""
+    if name == "":
+        raise ValueError("Selector: missing filter name")
+    return _LabelFilter(LabelSelectorFilterType, name, _selector_requirements(selector))
+
+
+def SelectorFactory(name: str, rawParameters):
+    """ "label-selector-filter" (selector.go:34-42): rawParameters is JSON text, bytes, a dict or None."""
+    params = {}
+    if rawParameters is not None:
+        try:
+            params = json.loads(rawParameters) if isinstance(rawParameters, (str, bytes)) else rawParameters
+        except json.JSONDecodeError as e:
+            raise ValueError(f"failed to parse the parameters of the '{LabelSelectorFilterType}' filter - {e}") from e
+    if params is None:                    # JSON null leaves the empty LabelSelector: Everything, not Nothing
+        params = {}
+    return NewSelector(name, params)
+
+
+LabelSelectorFilterFactory = SelectorFactory
+
+
+def DeprecatedSelectorFactory(name: str, rawParameters):
+    """ "by-label-selector" (selector.go:44-60): SelectorFactory reporting the legacy type."""
+    f = SelectorFactory(name, rawParameters)
+    f.type_name = ByLabelSelectorType
+    return f
+
+
+def NewByLabel(name: str, labelName: str, allowsNoLabel: bool, *validValues):
+    """bylabel.NewByLabel (filter.go:64-77): keeps an endpoint whose label is absent and allowsNoLabel holds, or whose
+    labels[labelName] is among validValues (an absent label reads as "")."""
+    op = capi.LABEL_BY_LABEL_OR_ABSENT if allowsNoLabel else capi.LABEL_BY_LABEL
+    if not validValues and not allowsNoLabel:
+        return _LabelFilter(ByLabelType, name, _selector_requirements(None))      # keeps nothing, as in Go
+    return _LabelFilter(ByLabelType, name, [(labelName, op, list(dict.fromkeys(validValues)))])
+
+
+def ByLabelFactory(name: str, rawParameters):
+    """ "by-label" (filter.go:34-57) with its errors."""
+    params = {}
+    if rawParameters is not None:
+        try:
+            params = json.loads(rawParameters) if isinstance(rawParameters, (str, bytes)) else dict(rawParameters)
+        except json.JSONDecodeError as e:
+            raise ValueError(f"failed to parse the parameters of the '{ByLabelType}' filter - {e}") from e
+    label, values, allows = params.get("label", ""), params.get("validValues") or [], params.get("allowsNoLabel", False)
+    if not isinstance(label, str) or not isinstance(allows, bool) or not isinstance(values, list) or \
+            not all(isinstance(v, str) for v in values):
+        raise ValueError(f"failed to parse the parameters of the '{ByLabelType}' filter")
+    if name == "":
+        raise ValueError(f"invalid configuration for '{ByLabelType}' filter: name cannot be empty")
+    if label == "":
+        raise ValueError(f"invalid configuration for '{ByLabelType}' filter: 'label' must be specified")
+    if not values and not allows:
+        raise ValueError(f"invalid configuration for '{ByLabelType}' filter: either 'validValues' must be non-empty or "
+                         "'allowsNoLabel' must be true")
+    return NewByLabel(name, label, allows, *values)
+
+
 @dataclass
 class PrefixCacheAffinityFilter:                 # filter/prefixcacheaffinity "prefix-cache-affinity-filter"; DefaultConfig :62-66
     affinityThreshold: float = 0.80
@@ -241,11 +378,7 @@ class SchedulerProfile:
         self.picker = MaxScorePicker()
 
     def WithFilters(self, *filters):
-        roles = [f for f in filters if isinstance(f, _RoleFilter)]
-        aff = [f for f in filters if isinstance(f, PrefixCacheAffinityFilter)]
-        assert len(roles) <= 1 and len(aff) <= 1 and len(roles) + len(aff) == len(filters), \
-            "a profile's filter chain is: [one role filter] [one prefix-cache-affinity-filter]"
-        assert not (roles and aff) or filters.index(roles[0]) < filters.index(aff[0]), "the role filter comes first"
+        _check_chain(filters)
         self.filters = list(filters)
         return self
 
@@ -257,7 +390,8 @@ class SchedulerProfile:
         for p in plugins:
             if isinstance(p, WeightedScorer):
                 self.scorers.append(p)
-            elif isinstance(p, (_RoleFilter, PrefixCacheAffinityFilter)):
+            elif isinstance(p, (_RoleFilter, _LabelFilter, PrefixCacheAffinityFilter)):
+                _check_chain(self.filters + [p])
                 self.filters.append(p)
             elif isinstance(p, (MaxScorePicker, RandomPicker, WeightedRandomPicker)):
                 self.picker = p
@@ -276,7 +410,24 @@ class SchedulerProfile:
                             for ws in self.scorers],
                            AffinityFilterSpec(aff[0].affinityThreshold, aff[0].explorationProbability,
                                               aff[0].maxTTFTPenaltyMs, aff[0].ttft_column) if aff else None,
-                           _PICKER_KIND[type(self.picker)])
+                           _PICKER_KIND[type(self.picker)],
+                           [q for f in self.filters if isinstance(f, _LabelFilter) for q in f.reqs])
+
+
+def _check_chain(filters):
+    """A profile's filter chain: label filters (any number) and at most one role filter, in any order (pure per-endpoint
+    predicates, so their order does not matter), then at most one prefix-cache-affinity-filter, last: it depends on
+    the set it receives."""
+    filters = list(filters)
+    roles = [f for f in filters if isinstance(f, _RoleFilter)]
+    aff = [i for i, f in enumerate(filters) if isinstance(f, PrefixCacheAffinityFilter)]
+    assert all(isinstance(f, (_RoleFilter, _LabelFilter, PrefixCacheAffinityFilter)) for f in filters), \
+        "a profile's filters are role filters, label filters and the prefix-cache-affinity-filter"
+    assert len(roles) <= 1, "at most one role filter per profile"
+    assert len(aff) <= 1 and (not aff or aff[0] == len(filters) - 1), \
+        "the prefix-cache-affinity-filter comes last: no filter may follow it"
+    n = sum(len(f.reqs) for f in filters if isinstance(f, _LabelFilter))
+    assert n <= capi.EPP_LABEL_MAX_REQS, f"{n} label requirements, at most {capi.EPP_LABEL_MAX_REQS} per profile"
 
 
 def NewSchedulerProfile():
@@ -363,6 +514,7 @@ class Scheduler:
                              max_prefix_blocks=max_prefix_blocks, non_cached_tokens=nct, always_disagg=always,
                              n_ext_cols=ext_columns, tie_seed=tie_seed, pick_k=self.pick_k, inflight_load=inflight_load)
         self.block_size_tokens = block_size_tokens
+        self.has_labels = any(p.spec().labels for p in profiles.values())
 
     def _push_pool(self, endpoints, ext=None):
         n = len(endpoints)
@@ -370,6 +522,8 @@ class Scheduler:
                              [e.metrics.KVCacheUsagePercent for e in endpoints],
                              [e.metrics.WaitingQueueSize for e in endpoints],
                              [e.metrics.RunningRequestsSize for e in endpoints], ext)
+        if self.has_labels:
+            self.engine.pool_set_labels(np.arange(n, dtype=np.uint32), [e.metadata.Labels for e in endpoints])
 
     def Schedule(self, requests, candidateEndpoints, ext=None):
         single = isinstance(requests, InferenceRequest)
