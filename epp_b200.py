@@ -25,4 +25,6 @@ DETAIL_DTYPE = _pkg.DETAIL_DTYPE
 SHARD_BEST_DTYPE = _pkg.SHARD_BEST_DTYPE
 decisions_from_torch = _pkg.decisions_from_torch
 pack_subsets = _pkg.pack_subsets
+pack_predictions = _pkg.pack_predictions
+PREDICTION_DTYPE = _pkg.PREDICTION_DTYPE
 Batcher = _pkg.Batcher

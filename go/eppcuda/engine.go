@@ -63,6 +63,9 @@ type ProfileSpec struct {
 	// Labels: the requirements of the profile's label filters (ProfileLabels of its LabelFilter plugins, labels.go),
 	// all ANDed with Filter; epp_label_filters_set
 	Labels []LabelReq
+	// Latency: the profile's tier filter, first affinity filter and latency-scorer (ProfilePlacement, latency.go);
+	// epp_latency_profile_set.  nil: none.
+	Latency *LatencySpec
 }
 
 // Config mirrors epp_config (EndpointPickerConfig fields that define this path).
@@ -94,6 +97,7 @@ type Engine struct {
 	cfg Config
 
 	mu     sync.RWMutex
+	latency bool // some profile has a latency piece: Scheduler.Schedule passes each request's predictions
 	slotOf map[types.NamespacedName]uint32
 	nameOf []types.NamespacedName // by slot; zero value = free
 	free   []uint32
@@ -186,6 +190,10 @@ func New(cfg Config) (*Engine, error) {
 			continue
 		}
 		if err := e.setLabelFilters(i, p.Labels); err != nil {
+			C.epp_engine_destroy(e.h)
+			return nil, err
+		}
+		if err := e.setLatency(i, p); err != nil {
 			C.epp_engine_destroy(e.h)
 			return nil, err
 		}
@@ -388,28 +396,32 @@ func (e *Engine) schedule(model uint32, prompt []byte, multimodal bool) (Decisio
 // scheduleSubset = schedule for a request whose candidates are the endpoints of `slots` (sorted; the gateway's endpoint
 // subset, epp_submit_subset), or the whole pool when slots is nil.  At most C.EPP_SUBSET_MAX_SLOTS slots.
 func (e *Engine) scheduleSubset(model uint32, prompt []byte, multimodal bool, slots []uint32) (Decision, error) {
-	e.inflight.Add(1)
-	defer e.inflight.Done()
-	var ticket C.uint64_t
-	var p unsafe.Pointer
-	if len(prompt) > 0 {
-		p = unsafe.Pointer(&prompt[0])
-	}
-	mm := C.uint32_t(0)
-	if multimodal {
-		mm = 1
-	}
-	var rc C.int32_t
-	if slots == nil {
-		rc = C.epp_submit(e.b, C.uint32_t(model), p, C.uint64_t(len(prompt)), mm, &ticket)
-	} else {
+	return e.submitAndWait(func(ticket *C.uint64_t) C.int32_t {
+		var p unsafe.Pointer
+		if len(prompt) > 0 {
+			p = unsafe.Pointer(&prompt[0])
+		}
+		mm := C.uint32_t(0)
+		if multimodal {
+			mm = 1
+		}
+		if slots == nil {
+			return C.epp_submit(e.b, C.uint32_t(model), p, C.uint64_t(len(prompt)), mm, ticket)
+		}
 		var sp *C.uint32_t
 		if len(slots) > 0 {
 			sp = (*C.uint32_t)(unsafe.Pointer(&slots[0]))
 		}
-		rc = C.epp_submit_subset(e.b, C.uint32_t(model), p, C.uint64_t(len(prompt)), mm, C.uint32_t(len(slots)), sp, &ticket)
-	}
-	if rc != C.EPP_OK {
+		return C.epp_submit_subset(e.b, C.uint32_t(model), p, C.uint64_t(len(prompt)), mm, C.uint32_t(len(slots)), sp, ticket)
+	})
+}
+
+// submitAndWait runs one submit call of the batcher, then waits for the request's decision.
+func (e *Engine) submitAndWait(submit func(ticket *C.uint64_t) C.int32_t) (Decision, error) {
+	e.inflight.Add(1)
+	defer e.inflight.Done()
+	var ticket C.uint64_t
+	if rc := submit(&ticket); rc != C.EPP_OK {
 		return Decision{}, errors.New(C.GoString(C.epp_batcher_last_error()))
 	}
 	var d C.epp_decision

@@ -34,6 +34,7 @@ var shared *Engine // set by Register
 func Register(e *Engine) {
 	shared = e
 	registerLabelFilters()
+	registerLatencyPlugins()
 	plugin.Register(PrefixProducerType, func(name string, _ json.RawMessage, _ plugin.Handle) (plugin.Plugin, error) {
 		if shared == nil {
 			return nil, errors.New("eppcuda: engine not created")

@@ -68,7 +68,8 @@ func (s *Scheduler) Schedule(ctx context.Context, request *scheduling.InferenceR
 	}
 	whole := known && len(slots) == len(s.Engine.slotOf)
 	s.Engine.mu.RUnlock()
-	if !known || (!whole && len(slots) > int(C.EPP_SUBSET_MAX_SLOTS)) {
+	// a latency engine takes no subsets: a restricted request goes to the fallback scheduler
+	if !known || (!whole && (s.Engine.latency || len(slots) > int(C.EPP_SUBSET_MAX_SLOTS))) {
 		if s.Fallback != nil {
 			return s.Fallback.Schedule(ctx, request, candidates)
 		}
@@ -92,7 +93,12 @@ func (s *Scheduler) Schedule(ctx context.Context, request *scheduling.InferenceR
 		return nil, err
 	}
 	mm := HasMultimodalContent != nil && HasMultimodalContent(request)
-	d, err := s.Engine.scheduleSubset(model, prompt, mm, slots)
+	var d Decision
+	if s.Engine.latency {
+		d, err = s.Engine.schedulePredicted(model, prompt, mm, s.Engine.predictions(candidates))
+	} else {
+		d, err = s.Engine.scheduleSubset(model, prompt, mm, slots)
+	}
 	if err != nil {
 		return nil, err
 	}

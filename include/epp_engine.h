@@ -142,13 +142,15 @@ typedef enum {
                                   param2 = idleThreshold (< 0: 0)                                                 */
     EPP_SCORER_LORA_AFFINITY = 8, /* "lora-affinity-scorer"      scorer/loraaffinity/lora_affinity.go:76-100; the adapter is the
                                   request's model id; residency comes from epp_pool_set_lora                     */
-    EPP_SCORER_NO_HIT_LRU = 9  /* "no-hit-lru-scorer"            scorer/nohitlru/no_hit_lru.go:259-321; param = lruSize (<= 0:
+    EPP_SCORER_NO_HIT_LRU = 9, /* "no-hit-lru-scorer"          scorer/nohitlru/no_hit_lru.go:259-321; param = lruSize (<= 0:
                                   1024), the same in every profile that lists it (they share ONE LRU).  A request is cold
                                   for a profile when no candidate holds a block of its prompt (the engine's own match is
                                   the producer).  Every scheduling call scores against the LRU as it stood when the call
                                   started and then Adds, for each cold request in request order, its pick and its
                                   prefill pick (PreRequest, :279-321): inside one batch cold requests do not rotate.
                                   Not available in the endpoint-sharded and peer-memory modes.                    */
+    EPP_SCORER_LATENCY = 10    /* "latency-scorer"               scorer/latency/plugin.go:144-395; reads the request's latency
+                                  predictions, configured by epp_latency_profile_set (see "Latency predictions")  */
 } epp_scorer_kind;
 
 /* Value of the llm-d.ai/role label (filter/bylabel/roles.go:25-44). */
@@ -522,6 +524,96 @@ typedef struct {
 EPP_API int32_t epp_schedule_subset(epp_engine *h, const epp_batch *batch, const epp_subset *subset, epp_decision *out,
                                     epp_decision_detail *detail, int32_t keep_hashes, const epp_topk_out *topk /* or NULL */);
 
+/* ---- Latency predictions (datalayer/attribute/latency/data_types.go; filter/sloheadroomtier/plugin.go:84-138;
+ * scorer/latency/plugin.go:144-395) ---------------------------------------------------------------------------------
+ * The predicted-latency producer computes a LatencyPredictionInfo per (request, endpoint): headroom = the request's SLO
+ * minus a prediction that depends on its prompt.  The caller passes those per request:
+ *   - Request r carries entries (slot, ttft, ttft_headroom, tpot_headroom, dispatched): TTFT(), TTFTHeadroom(),
+ *     TPOTHeadroom() and DispatchedRequestCount() of the endpoint in that slot, for that request.  Nothing else of the
+ *     attribute is read by the plugins.  A candidate without an entry has no attribute.  A request without entries, and
+ *     every request of a call without predictions, has no attribute anywhere.  Every profile of the request sees the same
+ *     entries (decode, prefill and encode).  Entries for slots that are not candidates are ignored.
+ *   - A profile has a latency piece when epp_latency_profile_set enables its tier filter or its first affinity filter, or
+ *     when it lists EPP_SCORER_LATENCY (which, without that call, uses the defaults of epp_latency_cfg_default).  Profiles
+ *     without one are decided exactly as on any other engine.
+ * Filter chain of a latency profile:
+ *     [role + label filters] -> [affinity A1] -> [tier filter T] -> [affinity A2] -> scorers in order -> picker
+ *   A1 (the epp_latency_cfg a1_* fields) needs T.  A2 is the profile's own prefix-cache-affinity-filter (epp_profile_cfg
+ *   affinity_*, with today's exploration draw).  Each stage works on the set it receives; everything after the chain uses
+ *   the final set: the len(endpoints) <= 1 gates, the sticky sets, the queue / running min-max, the active-request max,
+ *   the latency scorer's buckets, tie_count, and the random pickers' population, where every candidate is an EXPLICIT item
+ *   (no gaps, as for a set narrowed by the affinity filter).  Both affinity filters read TTFT from the entries: bestTTFT
+ *   skips candidates without one.  ttft_column must be < 0 on a latency profile.
+ * Tier filter: a set of <= 1 is kept.  Else positive = has an entry with both headrooms >= 0, negative = has an entry with
+ *   either headroom < 0, no-prediction = no entry.  No entry anywhere: keep all.  Else the no-prediction endpoints join
+ *   negative; with both tiers non-empty negative is kept when u < epsilon_explore_neg, else positive; otherwise the
+ *   non-empty tier.
+ * Draws: A1 and T each draw u = (mix64((tie_seed ^ D) ^ mix64(key)) >> 11) * 2^-53 with key = 4 * ordinal + profile index
+ *   and D = 0x8EBC6AF09C88C6E3 (A1), 0x589965CC75374CC3 (T).  With tie_seed == 0 neither explores.
+ * Latency scorer (Go amd64 arithmetic: no fused multiply-add):
+ *   - No candidate of the final set has an entry: composite fallback.  Weights divided by their sum ((1, 0, 0) when the sum
+ *     is <= 0); maxQ = the set's largest waiting count (from 0); relQueue = (maxQ - q) / maxQ (1 when maxQ == 0); prefix =
+ *     match / total (0 when total == 0); composite = wkv * (1 - kv) + wq * relQueue + wprefix * prefix, left to right;
+ *     score = int(math.Round(100 * composite)) / 100.
+ *   - Else negative = has an entry with either headroom < 0; positive = every other candidate, those without an entry
+ *     included.  The scored bucket is positive (configured strategy) when non-empty, else the negative candidates with
+ *     dispatched == 0 when there are any, else the first non-empty of TPOT-only-negative, TTFT-only-negative,
+ *     both-negative; negative buckets use "least".  Candidates outside the bucket score 0.
+ *   - In the bucket: alpha, beta = the normalised ttft / tpot weights ((1, 0) when their sum is <= 0); ranges of |headroom|
+ *     per dimension over the bucket; eps = 1e-9; a range <= eps with the other > eps moves all weight to the other;
+ *     n = (|h| - min) / range, or 0.5 when range <= eps; combined = alpha * nT + beta * nP; score =
+ *     float64(int(x * 100) + 1) / 100 with x = combined ("most") or 1 - combined ("least"), int truncating toward zero.
+ *   The latency scorer enters the ordered, clamped weighted sum like every other scorer.  A latency profile may not list
+ *   the no-hit-lru scorer (its cold test over a tier-narrowed set is not built); epp_score rejects a latency scorer index,
+ *   and -1 on a latency profile.
+ * Predictions are HOST memory for every batch kind, validated and copied before the call returns.  A slot list that is not
+ * strictly ascending, a slot >= max_endpoints, a non-finite ttft or headroom, a wrong struct_size, or predictions on an
+ * engine without a latency profile fail the call with EPP_ERR_INVALID before anything is launched and before any LRU,
+ * counter or ordinal state changes.  Endpoint subsets (epp_schedule_subset, epp_submit_subset) and the endpoint-sharded
+ * modes are not available on a latency engine.  Plain epp_schedule* on a latency engine decides every request without predictions. */
+enum { EPP_HEADROOM_LEAST = 0, EPP_HEADROOM_MOST = 1 };
+typedef struct {
+    uint32_t struct_size;              /* sizeof(epp_latency_cfg)                                                      */
+    int32_t tier_filter;               /* 1: the slo-headroom-tier-filter T runs between A1 and A2                     */
+    double epsilon_explore_neg;        /* T's EpsilonExploreNeg, [0, 1] (default 0.01)                                 */
+    double a1_affinity_threshold;      /* > 0: affinity filter A1 before T (needs tier_filter); <= 1                   */
+    double a1_exploration_probability; /* [0, 1]                                                                       */
+    double a1_max_ttft_penalty_ms;     /* >= 0                                                                         */
+    double ttft_weight;                /* latency-scorer TTFTWeight (default 0.8)                                      */
+    double tpot_weight;                /* TPOTWeight (default 0.2)                                                     */
+    int32_t strategy;                  /* EPP_HEADROOM_LEAST (default) or EPP_HEADROOM_MOST                            */
+    int32_t reserved;
+    double composite_kv_weight;        /* CompositeKVWeight / QueueWeight / PrefixWeight (default 1, 1, 1)             */
+    double composite_queue_weight;
+    double composite_prefix_weight;
+} epp_latency_cfg;
+EPP_API void epp_latency_cfg_default(epp_latency_cfg *cfg);
+/* Sets profile's latency configuration (0 = primary / decode, 1 = prefill, 2 = encode).  Only before the engine's first
+ * successful epp_pool_set / epp_pool_set_labels (EPP_ERR_STATE after), and not on an endpoint-sharded engine. */
+EPP_API int32_t epp_latency_profile_set(epp_engine *h, int32_t profile, const epp_latency_cfg *cfg);
+
+typedef struct {                       /* 32 bytes */
+    uint32_t slot;
+    int32_t dispatched;                /* DispatchedRequestCount()                                                     */
+    double ttft;                       /* TTFT()                                                                       */
+    double ttft_headroom;              /* TTFTHeadroom()                                                               */
+    double tpot_headroom;              /* TPOTHeadroom()                                                               */
+} epp_prediction;
+typedef struct {
+    uint32_t struct_size;              /* sizeof(epp_predictions)                                                      */
+    uint32_t reserved;
+    const uint32_t *counts;            /* [R] entries of request r                                                     */
+    const uint64_t *offsets;           /* [R] request r's entries are entries[offsets[r] .. offsets[r] + counts[r])    */
+    const epp_prediction *entries;     /* slots strictly ascending within a request                                    */
+} epp_predictions;
+/* epp_schedule_topk / epp_schedule_with_match_topk with predictions (preds may be NULL: no predictions; topk may be NULL). */
+EPP_API int32_t epp_schedule_predicted(epp_engine *h, const epp_batch *batch, const epp_predictions *preds, epp_decision *out,
+                                       epp_decision_detail *detail, int32_t keep_hashes, const epp_topk_out *topk);
+EPP_API int32_t epp_schedule_with_match_predicted(epp_engine *h, int64_t n_requests, const int32_t *match, const int32_t *total,
+                                                  const uint32_t *model_ids, const int64_t *input_len_bytes,
+                                                  int32_t block_size_tokens, epp_decision *out, epp_decision_detail *detail,
+                                                  uint32_t flags, const epp_topk_out *topk, const epp_predictions *preds);
+
 /* PreRequest (approximateprefix/plugin.go:164-200): index the hashes of the LAST epp_schedule batch
  * (keep_hashes=1) for each request's primary pick and prefill pick. */
 EPP_API int32_t epp_index_add_picked(epp_engine *h);
@@ -630,6 +722,13 @@ EPP_API int32_t epp_submit(epp_batcher *b, uint32_t model_id, const void *prompt
 #define EPP_SUBSET_MAX_SLOTS 1024
 EPP_API int32_t epp_submit_subset(epp_batcher *b, uint32_t model_id, const void *prompt, uint64_t prompt_len,
                                   uint32_t multimodal, uint32_t n_slots, const uint32_t *slots, uint64_t *out_ticket);
+/* epp_submit with the request's latency predictions (include "Latency predictions"): n entries, in any slot order (the
+ * batcher sorts them), staged next to the prompt; a flush that holds such a request runs epp_schedule_predicted.  More
+ * than EPP_PRED_MAX_SLOTS entries is EPP_ERR_CAPACITY; two entries for one slot, a slot >= max_endpoints, a non-finite
+ * value, or an engine without a latency profile is EPP_ERR_INVALID, refused here so that no flush fails for it. */
+#define EPP_PRED_MAX_SLOTS 1024
+EPP_API int32_t epp_submit_predicted(epp_batcher *b, uint32_t model_id, const void *prompt, uint64_t prompt_len,
+                                     uint32_t multimodal, uint32_t n, const epp_prediction *entries, uint64_t *out_ticket);
 EPP_API int32_t epp_wait(epp_batcher *b, uint64_t ticket, epp_decision *out, epp_decision_detail *out_detail);
 /* The same on an engine created with pick_k > 1, plus the request's first-k lists (ProfileRunResult.TargetEndpoints of
  * each profile, see epp_topk_out): primary / prefill / encode receive pick_k slot ids each (EPP_NO_ENDPOINT padded); any

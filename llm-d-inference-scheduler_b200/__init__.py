@@ -9,8 +9,8 @@ build.py     nvcc build (in-tree, sm_90a)
 The directory name is not a Python identifier; import it with importlib (see epp_b200.py at the repo root).
 """
 from . import _capi as capi
-from .engine import (DECISION_DTYPE, DETAIL_DTYPE, SHARD_BEST_DTYPE, AffinityFilterSpec, Batcher, Engine, EngineError, PinnedBuffer, ProfileSpec,
-                     ScorerSpec, decisions_from_torch, pack_subsets)
+from .engine import (DECISION_DTYPE, DETAIL_DTYPE, PREDICTION_DTYPE, SHARD_BEST_DTYPE, AffinityFilterSpec, Batcher, Engine, EngineError, PinnedBuffer, ProfileSpec,
+                     ScorerSpec, decisions_from_torch, pack_predictions, pack_subsets)
 
 __all__ = ["capi", "Engine", "Batcher", "EngineError", "ProfileSpec", "ScorerSpec", "AffinityFilterSpec", "PinnedBuffer", "DECISION_DTYPE", "DETAIL_DTYPE",
-           "SHARD_BEST_DTYPE", "decisions_from_torch", "pack_subsets"]
+           "SHARD_BEST_DTYPE", "PREDICTION_DTYPE", "decisions_from_torch", "pack_predictions", "pack_subsets"]

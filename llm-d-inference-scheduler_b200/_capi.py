@@ -18,7 +18,7 @@ EPP_BATCH_LENGTHS_EXCEED_ROWS = 4
 EPP_OK, EPP_ERR_INVALID, EPP_ERR_CUDA, EPP_ERR_NO_DEVICE, EPP_ERR_CAPACITY, EPP_ERR_STATE, EPP_ERR_NCCL = \
     0, -1, -2, -3, -4, -5, -6
 (SCORER_PREFIX, SCORER_KV_UTIL, SCORER_QUEUE, SCORER_LOAD_AWARE, SCORER_EXTERNAL, SCORER_RUNNING, SCORER_TOKEN_LOAD,
- SCORER_ACTIVE_REQUEST, SCORER_LORA_AFFINITY, SCORER_NO_HIT_LRU) = range(10)
+ SCORER_ACTIVE_REQUEST, SCORER_LORA_AFFINITY, SCORER_NO_HIT_LRU, SCORER_LATENCY) = range(11)
 (ROLE_NONE, ROLE_DECODE, ROLE_PREFILL, ROLE_PREFILL_DECODE, ROLE_BOTH, ROLE_ENCODE, ROLE_ENCODE_PREFILL,
  ROLE_ENCODE_PREFILL_DECODE, ROLE_OTHER) = range(9)
 FILTER_NONE, FILTER_DECODE, FILTER_PREFILL, FILTER_ENCODE = range(4)
@@ -82,11 +82,33 @@ class TopkOut(C.Structure):
 
 EPP_SUBSET_ALL = 0xFFFFFFFF
 EPP_SUBSET_MAX_SLOTS = 1024
+EPP_PRED_MAX_SLOTS = 1024
 
 
 class Subset(C.Structure):
     _fields_ = [("struct_size", C.c_uint32), ("reserved", C.c_uint32), ("counts", C.c_void_p), ("offsets", C.c_void_p),
                 ("slots", C.c_void_p)]
+
+
+HEADROOM_LEAST, HEADROOM_MOST = 0, 1
+
+
+class LatencyCfg(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("tier_filter", C.c_int32), ("epsilon_explore_neg", C.c_double),
+                ("a1_affinity_threshold", C.c_double), ("a1_exploration_probability", C.c_double),
+                ("a1_max_ttft_penalty_ms", C.c_double), ("ttft_weight", C.c_double), ("tpot_weight", C.c_double),
+                ("strategy", C.c_int32), ("reserved", C.c_int32), ("composite_kv_weight", C.c_double),
+                ("composite_queue_weight", C.c_double), ("composite_prefix_weight", C.c_double)]
+
+
+class Prediction(C.Structure):
+    _fields_ = [("slot", C.c_uint32), ("dispatched", C.c_int32), ("ttft", C.c_double), ("ttft_headroom", C.c_double),
+                ("tpot_headroom", C.c_double)]
+
+
+class Predictions(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("reserved", C.c_uint32), ("counts", C.c_void_p), ("offsets", C.c_void_p),
+                ("entries", C.c_void_p)]
 
 
 EPP_LABEL_MAX_REQS = 32
@@ -113,6 +135,7 @@ class ShardBest(C.Structure):
 
 
 assert C.sizeof(Decision) == 32 and C.sizeof(DecisionDetail) == 40 and C.sizeof(ShardBest) == 24
+assert C.sizeof(Prediction) == 32
 
 # name -> (restype, argtypes): every symbol include/epp_engine.h declares
 SIGNATURES = {
@@ -150,6 +173,13 @@ SIGNATURES = {
                                                  C.c_int32, C.c_void_p, C.c_void_p, C.c_uint32, C.POINTER(TopkOut)]),
     "epp_schedule_subset": (C.c_int32, [C.c_void_p, C.POINTER(Batch), C.POINTER(Subset), C.c_void_p, C.c_void_p, C.c_int32,
                                         C.POINTER(TopkOut)]),
+    "epp_latency_cfg_default": (None, [C.POINTER(LatencyCfg)]),
+    "epp_latency_profile_set": (C.c_int32, [C.c_void_p, C.c_int32, C.POINTER(LatencyCfg)]),
+    "epp_schedule_predicted": (C.c_int32, [C.c_void_p, C.POINTER(Batch), C.POINTER(Predictions), C.c_void_p, C.c_void_p,
+                                           C.c_int32, C.POINTER(TopkOut)]),
+    "epp_schedule_with_match_predicted": (C.c_int32, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                      C.c_int32, C.c_void_p, C.c_void_p, C.c_uint32, C.POINTER(TopkOut),
+                                                      C.POINTER(Predictions)]),
     "epp_index_add_picked": (C.c_int32, [C.c_void_p]),
     "epp_nohit_lru_get": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(C.c_int32)]),
     "epp_inflight_release": (C.c_int32, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
@@ -173,6 +203,8 @@ SIGNATURES = {
     "epp_submit": (C.c_int32, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_uint32, C.POINTER(C.c_uint64)]),
     "epp_submit_subset": (C.c_int32, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_uint32, C.c_uint32, C.c_void_p,
                                       C.POINTER(C.c_uint64)]),
+    "epp_submit_predicted": (C.c_int32, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_uint32, C.c_uint32, C.c_void_p,
+                                         C.POINTER(C.c_uint64)]),
     "epp_wait": (C.c_int32, [C.c_void_p, C.c_uint64, C.POINTER(Decision), C.POINTER(DecisionDetail)]),
     "epp_wait_topk": (C.c_int32, [C.c_void_p, C.c_uint64, C.POINTER(Decision), C.POINTER(DecisionDetail), C.c_void_p,
                                   C.c_void_p, C.c_void_p]),

@@ -27,6 +27,7 @@
 #include <atomic>
 #include <chrono>
 #include <climits>
+#include <cmath>
 #include <cstring>
 #include <mutex>
 #include <string>
@@ -34,6 +35,9 @@
 #include <vector>
 
 #include "../../include/epp_engine.h"
+
+// engine.cu: the engine's profiles with a latency piece (0: none)
+int32_t engine_latency_mask(const epp_engine *h);
 
 namespace {
 constexpr int kBufs = 4;                       // staging buffers: batches k .. k+3 can be filling / in flight at once
@@ -70,6 +74,11 @@ struct Staging {
     std::vector<uint64_t> sub_offsets;         // [max_batch]
     std::vector<uint32_t> sub_slots;           // [max_batch][EPP_SUBSET_MAX_SLOTS], allocated by the first subset submit
     std::atomic<int32_t> any_subset{0};        // some row of the batch using this buffer has a subset
+    // latency predictions (epp_submit_predicted): per row its entry count, its entries at row * EPP_PRED_MAX_SLOTS
+    std::vector<uint32_t> pred_counts;         // [max_batch]
+    std::vector<uint64_t> pred_offsets;        // [max_batch]
+    std::vector<epp_prediction> pred_entries;  // [max_batch][EPP_PRED_MAX_SLOTS], allocated by the first predicted submit
+    std::atomic<int32_t> any_pred{0};          // some row of the batch using this buffer has predictions
     std::atomic<int32_t> ready{0};             // rows of the batch using this buffer whose copy is complete
     std::atomic<int64_t> first_arrival_ns{0};  // when row 0 of that batch was reserved
 };
@@ -94,6 +103,8 @@ struct epp_batcher {
     uint32_t max_endpoints = 0;
     std::once_flag sub_once;                   // the subset slot staging of every buffer, allocated on first use
     bool sub_alloc_failed = false;
+    std::once_flag pred_once;                  // the prediction staging of every buffer, allocated on first use
+    bool pred_alloc_failed = false;
     Staging buf[kBufs];
     std::vector<Result> results;
     std::atomic<uint64_t> fill{0};             // (sequence number of the batch being filled << 20) | rows reserved in it
@@ -167,7 +178,17 @@ static void flusher_main(epp_batcher *b) {
         tk.struct_size = sizeof tk;
         tk.k = b->pick_k;
         tk.primary = st.topk[0]; tk.prefill = st.topk[1]; tk.encode = st.topk[2];
-        if (st.any_subset.load(std::memory_order_acquire)) {
+        if (st.any_pred.load(std::memory_order_acquire)) {
+            // a latency engine takes no subsets (epp_submit_subset refuses them), so the two never share a batch
+            epp_predictions pr;
+            memset(&pr, 0, sizeof pr);
+            pr.struct_size = sizeof pr;
+            pr.counts = st.pred_counts.data();
+            pr.offsets = st.pred_offsets.data();
+            pr.entries = st.pred_entries.data();
+            rc = epp_schedule_predicted(b->eng, &batch, &pr, st.dec, st.det, b->cfg.index_picks ? 1 : 0, b->pick_k > 1 ? &tk : nullptr);
+            st.any_pred.store(0, std::memory_order_relaxed);
+        } else if (st.any_subset.load(std::memory_order_acquire)) {
             epp_subset sub;
             memset(&sub, 0, sizeof sub);
             sub.struct_size = sizeof sub;
@@ -264,6 +285,9 @@ extern "C" int32_t epp_batcher_create(epp_engine *h, const epp_batcher_cfg *cfg,
         st.sub_counts.assign(mb, EPP_SUBSET_ALL);
         st.sub_offsets.resize(mb);
         for (size_t r = 0; r < mb; r++) st.sub_offsets[r] = (uint64_t)r * EPP_SUBSET_MAX_SLOTS;
+        st.pred_counts.assign(mb, 0);
+        st.pred_offsets.resize(mb);
+        for (size_t r = 0; r < mb; r++) st.pred_offsets[r] = (uint64_t)r * EPP_PRED_MAX_SLOTS;
         if (b->pick_k > 1)
             for (int q = 0; q < 3; q++) {
                 rc = epp_host_alloc(sizeof(uint32_t) * mb * (size_t)b->pick_k, &p);
@@ -296,9 +320,11 @@ extern "C" int32_t epp_batcher_destroy(epp_batcher *b) {
     return EPP_OK;
 }
 
-// sub: the request's slots, sorted and deduplicated, or nullptr (the whole pool)
+// sub: the request's slots, sorted and deduplicated, or nullptr (the whole pool); pred: its predictions, validated and
+// sorted by slot, or nullptr (none)
 static int32_t submit_impl(epp_batcher *b, uint32_t model_id, const void *prompt, uint64_t prompt_len, uint32_t multimodal,
-                           const std::vector<uint32_t> *sub, uint64_t *out_ticket) {
+                           const std::vector<uint32_t> *sub, uint64_t *out_ticket,
+                           const std::vector<epp_prediction> *pred = nullptr) {
     const uint64_t max_batch = (uint64_t)b->cfg.max_batch;
     uint64_t seq, idx;
     for (int spin = 0;; spin++) {
@@ -340,6 +366,13 @@ static int32_t submit_impl(epp_batcher *b, uint32_t model_id, const void *prompt
     } else {
         st.sub_counts[idx] = EPP_SUBSET_ALL;
     }
+    if (pred && !pred->empty()) {
+        memcpy(st.pred_entries.data() + (size_t)idx * EPP_PRED_MAX_SLOTS, pred->data(), sizeof(epp_prediction) * pred->size());
+        st.pred_counts[idx] = (uint32_t)pred->size();
+        st.any_pred.store(1, std::memory_order_relaxed);           // published by the release below
+    } else {
+        st.pred_counts[idx] = 0;
+    }
     st.ready.fetch_add(1, std::memory_order_release);              // the flusher waits for this before it reads the row
     *out_ticket = (seq << 20) | idx;
     return EPP_OK;
@@ -355,6 +388,8 @@ extern "C" int32_t epp_submit_subset(epp_batcher *b, uint32_t model_id, const vo
                                      uint32_t multimodal, uint32_t n_slots, const uint32_t *slots, uint64_t *out_ticket) {
     if (!b || !out_ticket || (prompt_len && !prompt) || (n_slots && !slots)) return bfail(EPP_ERR_INVALID, "NULL argument");
     if (n_slots > EPP_SUBSET_MAX_SLOTS) return bfail(EPP_ERR_CAPACITY, "more than EPP_SUBSET_MAX_SLOTS slots in one subset");
+    // refused here rather than at the flush, where it would fail every request of the batch
+    if (engine_latency_mask(b->eng)) return bfail(EPP_ERR_INVALID, "endpoint subsets are not available on an engine with latency profiles");
     std::vector<uint32_t> sub(slots, slots + n_slots);
     for (uint32_t e : sub)
         if (e >= b->max_endpoints) return bfail(EPP_ERR_INVALID, "subset slot >= max_endpoints");
@@ -369,6 +404,32 @@ extern "C" int32_t epp_submit_subset(epp_batcher *b, uint32_t model_id, const vo
     });
     if (b->sub_alloc_failed) return bfail(EPP_ERR_CAPACITY, "cannot allocate the batcher's subset staging");
     return submit_impl(b, model_id, prompt, prompt_len, multimodal, &sub, out_ticket);
+}
+
+extern "C" int32_t epp_submit_predicted(epp_batcher *b, uint32_t model_id, const void *prompt, uint64_t prompt_len,
+                                        uint32_t multimodal, uint32_t n, const epp_prediction *entries, uint64_t *out_ticket) {
+    if (!b || !out_ticket || (prompt_len && !prompt) || (n && !entries)) return bfail(EPP_ERR_INVALID, "NULL argument");
+    if (n > EPP_PRED_MAX_SLOTS) return bfail(EPP_ERR_CAPACITY, "more than EPP_PRED_MAX_SLOTS predictions for one request");
+    // every rule epp_schedule_predicted checks, so that one request's predictions never fail its batch
+    if (!engine_latency_mask(b->eng)) return bfail(EPP_ERR_INVALID, "predictions passed to an engine without a latency profile");
+    std::vector<epp_prediction> pred(entries, entries + n);
+    for (const epp_prediction &p : pred) {
+        if (p.slot >= b->max_endpoints) return bfail(EPP_ERR_INVALID, "prediction slot >= max_endpoints");
+        if (!std::isfinite(p.ttft) || !std::isfinite(p.ttft_headroom) || !std::isfinite(p.tpot_headroom))
+            return bfail(EPP_ERR_INVALID, "a prediction is not finite");
+    }
+    std::sort(pred.begin(), pred.end(), [](const epp_prediction &x, const epp_prediction &y) { return x.slot < y.slot; });
+    for (size_t i = 1; i < pred.size(); i++)
+        if (pred[i].slot == pred[i - 1].slot) return bfail(EPP_ERR_INVALID, "two predictions for one slot");
+    std::call_once(b->pred_once, [b] {
+        try {
+            for (int i = 0; i < kBufs; i++) b->buf[i].pred_entries.resize((size_t)b->cfg.max_batch * EPP_PRED_MAX_SLOTS);
+        } catch (...) {
+            b->pred_alloc_failed = true;
+        }
+    });
+    if (b->pred_alloc_failed) return bfail(EPP_ERR_CAPACITY, "cannot allocate the batcher's prediction staging");
+    return submit_impl(b, model_id, prompt, prompt_len, multimodal, nullptr, out_ticket, &pred);
 }
 
 extern "C" int32_t epp_wait(epp_batcher *b, uint64_t ticket, epp_decision *out, epp_decision_detail *out_detail) {

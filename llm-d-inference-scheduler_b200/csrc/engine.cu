@@ -123,6 +123,15 @@ struct epp_engine {
     LabelPlan labels;
     DevBuf lcode;                   // uint8 [labels.keys.size()][E] (LabelFilterDev)
     bool pool_called = false;       // epp_pool_set / epp_pool_set_labels succeeded once: the label filters are fixed
+    // latency predictions (include/epp_engine.h "Latency predictions"): each profile's configuration, the profiles with a
+    // latency piece, and the staged entries of the call in progress (cur_pred: the call passed predictions)
+    epp_latency_cfg lat_cfg[kMaxProfiles] = {};
+    int lat_mask = 0;
+    bool cur_pred = false;
+    DevBuf lat_cnt, lat_off, lat_ent;
+    void *lat_host = nullptr;       // pinned staging of counts, offsets and entries
+    size_t lat_host_cap = 0;
+    cudaEvent_t lat_up_ev = nullptr;    // behind the last upload from lat_host
     ProfileState prof[kMaxProfiles];
     // no-hit-lru scorer (nohit_lru.cu), allocated only when a profile lists it
     int nohit_mask = 0;             // bit pi: profile pi has the scorer
@@ -283,7 +292,7 @@ static int32_t validate_profile(const epp_profile_cfg &p, int n_ext, bool inflig
     if (p.n_scorers < 0 || p.n_scorers > EPP_MAX_SCORERS) return fail(EPP_ERR_INVALID, "%s: n_scorers %d out of range", name, p.n_scorers);
     for (int s = 0; s < p.n_scorers; s++) {
         const epp_scorer_cfg &sc = p.scorers[s];
-        if (sc.kind < EPP_SCORER_PREFIX || sc.kind > EPP_SCORER_NO_HIT_LRU) return fail(EPP_ERR_INVALID, "%s: scorer %d has unknown kind %d", name, s, sc.kind);
+        if (sc.kind < EPP_SCORER_PREFIX || sc.kind > EPP_SCORER_LATENCY) return fail(EPP_ERR_INVALID, "%s: scorer %d has unknown kind %d", name, s, sc.kind);
         if (!std::isfinite(sc.weight)) return fail(EPP_ERR_INVALID, "%s: scorer %d weight is not finite", name, s);
         if (!inflight && (sc.kind == EPP_SCORER_TOKEN_LOAD || sc.kind == EPP_SCORER_ACTIVE_REQUEST) && (sc.column < 0 || sc.column >= n_ext))
             return fail(EPP_ERR_INVALID, "%s: scorer %d reads ext column %d, out of range [0,%d)", name, s, sc.column, n_ext);
@@ -296,6 +305,32 @@ static int32_t validate_profile(const epp_profile_cfg &p, int n_ext, bool inflig
     if (p.affinity_threshold > 0.0 && p.ttft_column >= n_ext) return fail(EPP_ERR_INVALID, "%s: ttft_column %d out of range [0,%d)", name, p.ttft_column, n_ext);
     if (p.picker < EPP_PICKER_MAX_SCORE || p.picker > EPP_PICKER_WEIGHTED_RANDOM) return fail(EPP_ERR_INVALID, "%s: unknown picker %d", name, p.picker);
     return EPP_OK;
+}
+
+static bool lists_scorer(const epp_profile_cfg &p, int kind) {
+    for (int s = 0; s < p.n_scorers; s++)
+        if (p.scorers[s].kind == kind) return true;
+    return false;
+}
+// The rules a profile with a latency piece adds to validate_profile ("Latency predictions").
+static int32_t validate_latency(const epp_profile_cfg &p, const epp_latency_cfg &c, const char *name) {
+    if (c.struct_size != sizeof(epp_latency_cfg)) return fail(EPP_ERR_INVALID, "epp_latency_cfg.struct_size %u != %zu", c.struct_size, sizeof(epp_latency_cfg));
+    if (c.tier_filter != 0 && c.tier_filter != 1) return fail(EPP_ERR_INVALID, "%s: tier_filter %d must be 0 or 1", name, c.tier_filter);
+    if (!(c.epsilon_explore_neg >= 0.0 && c.epsilon_explore_neg <= 1.0)) return fail(EPP_ERR_INVALID, "%s: epsilonExploreNeg must be in [0, 1], got %f", name, c.epsilon_explore_neg);
+    if (std::isnan(c.a1_affinity_threshold) || c.a1_affinity_threshold > 1.0) return fail(EPP_ERR_INVALID, "%s: A1 affinityThreshold must be <= 1.0, got %f", name, c.a1_affinity_threshold);
+    if (!(c.a1_exploration_probability >= 0.0 && c.a1_exploration_probability <= 1.0)) return fail(EPP_ERR_INVALID, "%s: A1 explorationProbability must be in [0, 1], got %f", name, c.a1_exploration_probability);
+    if (!(c.a1_max_ttft_penalty_ms >= 0.0)) return fail(EPP_ERR_INVALID, "%s: A1 maxTTFTPenaltyMs must be >= 0, got %f", name, c.a1_max_ttft_penalty_ms);
+    if (c.a1_affinity_threshold > 0.0 && !c.tier_filter) return fail(EPP_ERR_INVALID, "%s: an affinity filter before the tier filter needs the tier filter", name);
+    if (c.strategy != EPP_HEADROOM_LEAST && c.strategy != EPP_HEADROOM_MOST) return fail(EPP_ERR_INVALID, "%s: unknown headroom strategy %d", name, c.strategy);
+    const double w[5] = {c.ttft_weight, c.tpot_weight, c.composite_kv_weight, c.composite_queue_weight, c.composite_prefix_weight};
+    for (double x : w) if (!std::isfinite(x)) return fail(EPP_ERR_INVALID, "%s: latency-scorer weights must be finite", name);
+    const bool piece = c.tier_filter || c.a1_affinity_threshold > 0.0 || lists_scorer(p, EPP_SCORER_LATENCY);
+    if (piece && lists_scorer(p, EPP_SCORER_NO_HIT_LRU)) return fail(EPP_ERR_INVALID, "%s: the no-hit-lru scorer is not available on a latency profile", name);
+    if (piece && p.ttft_column >= 0) return fail(EPP_ERR_INVALID, "%s: a latency profile reads TTFT from the predictions: ttft_column must be < 0", name);
+    return EPP_OK;
+}
+static bool latency_piece(const epp_profile_cfg &p, const epp_latency_cfg &c) {
+    return c.tier_filter || c.a1_affinity_threshold > 0.0 || lists_scorer(p, EPP_SCORER_LATENCY);
 }
 
 static int32_t alloc_profile(epp_engine *e, ProfileState &ps, bool random_picker) {
@@ -455,6 +490,13 @@ extern "C" int32_t epp_engine_create(const epp_config *cfg, epp_engine **out) {
     e->general = cfg->pick_k > 1;
     for (int pi = 0; pi < e->n_alloc_profiles; pi++)
         if (profile_cfg(e.get(), pi).affinity_threshold > 0.0) e->general = true;
+    for (int pi = 0; pi < e->n_alloc_profiles; pi++) {
+        epp_latency_cfg_default(&e->lat_cfg[pi]);
+        const epp_profile_cfg &pc = profile_cfg(e.get(), pi);
+        EPP_TRY(validate_latency(pc, e->lat_cfg[pi], pi == 0 ? "primary profile" : (pi == 1 ? "prefill profile" : "encode profile")));
+        if (latency_piece(pc, e->lat_cfg[pi])) e->lat_mask |= 1 << pi;
+    }
+    if (e->lat_mask) e->general = true;
     e->store.reset(new IndexStore((uint32_t)cfg->max_endpoints, cfg->lru_capacity_per_server, e->sm_count));
     { const char *v1 = getenv("EPP_INDEX_PATCH"); e->patch_enabled = v1 ? atoi(v1) : 1; }
     { const char *v1 = getenv("EPP_INDEX_LOAD"); e->index_load = v1 ? std::max(2, atoi(v1)) : 0; }
@@ -507,6 +549,8 @@ extern "C" int32_t epp_engine_destroy(epp_engine *h) {
     if (!h) return EPP_OK;
     cudaSetDevice(h->cfg.device);
     cudaDeviceSynchronize();
+    if (h->lat_host) cudaFreeHost(h->lat_host);
+    if (h->lat_up_ev) cudaEventDestroy(h->lat_up_ev);
     for (int i = 0; i < 2; i++) {
         if (h->slot[i].stream) cudaStreamDestroy(h->slot[i].stream);
         if (h->slot[i].done) cudaEventDestroy(h->slot[i].done);
@@ -1562,9 +1606,29 @@ static int32_t launch_overflow_pass(epp_engine *h, Slot &sl, PickParams pp, int 
 
 // Standalone match/pick over hashes already in HBM: warp-per-request sparse kernel + overflow pass (or the dense
 // kernel alone for Produce-parity rows / A-B runs).
-static int32_t launch_match(epp_engine *h, Slot &sl, PickParams pp, int *launches) {
+// The latency view of a launch whose request 0 is row r0 of the call in progress.
+static LatView lat_view(epp_engine *h, int64_t r0) {
+    LatView v;
+    memset(&v, 0, sizeof v);
+    v.mask = h->lat_mask;
+    v.r0 = r0;
+    for (int i = 0; i < kMaxProfiles; i++) v.cfg[i] = h->lat_cfg[i];
+    if (h->cur_pred) {
+        v.cnt = h->lat_cnt.as<uint32_t>();
+        v.off = h->lat_off.as<uint64_t>();
+        v.ent = h->lat_ent.as<epp_prediction>();
+    }
+    return v;
+}
+
+// r0: row of pp's request 0 in the call (reads the call's latency predictions).
+static int32_t launch_match(epp_engine *h, Slot &sl, PickParams pp, int *launches, int64_t r0 = 0) {
     cudaStream_t s = sl.stream;
     uint32_t *gs = h->pick_global ? sl.pick_scratch.as<uint32_t>() : nullptr;
+    if (pp.gen.on && h->lat_mask && !pp.out_match) {
+        CUDA_TRY(launch_match_pick_lat(pp, lat_view(h, r0), gs, h->pick_grid, h->pick_smem, s, launches));
+        return EPP_OK;
+    }
     if (pp.out_match || pp.gen.on) {
         CUDA_TRY(launch_match_pick(pp, gs, h->pick_grid, h->pick_smem, s, launches));
         return EPP_OK;
@@ -1593,9 +1657,10 @@ static void trim_rows(epp_engine *h, const Work &w, HashParams &hp, PickParams &
 
 // The whole cycle for one Work item: hash kernel, then the standalone match / score / pick kernel (every fused or
 // concurrently scheduled arrangement of the two was measured slower).
-static int32_t launch_cycle(epp_engine *h, Slot &sl, const HashParams &hp, PickParams pp, int *launches, cudaEvent_t *ev) {
+static int32_t launch_cycle(epp_engine *h, Slot &sl, const HashParams &hp, PickParams pp, int *launches, cudaEvent_t *ev,
+                            int64_t r0) {
     CUDA_TRY(launch_hash_prompts(hp, sl.stream, launches, ev));
-    return launch_match(h, sl, pp, launches);
+    return launch_match(h, sl, pp, launches, r0);
 }
 
 // Completes the device batch in flight on stream 0 and reads its per-kernel CUDA-event times and work counters.
@@ -1924,7 +1989,7 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
                 Slot &sl = h->slot[k & 1];
                 HashParams hp = hash_params(h, w, sl);
                 if (trim) trim_rows(h, w, hp, pp);
-                EPP_TRY(launch_cycle(h, sl, hp, pp, &launches, nullptr));
+                EPP_TRY(launch_cycle(h, sl, hp, pp, &launches, nullptr, r0));
                 EPP_TRY(launch_subset(h, pp, r0, r1, sl.stream, &launches, true));
             }
             h->s1_unjoined = true;
@@ -1946,7 +2011,7 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
             hp.stored = h->work_counters.as<unsigned long long>() + 2;
             hp.read = h->work_counters.as<unsigned long long>() + 3;
             if (trim) trim_rows(h, w, hp, pp);
-            EPP_TRY(launch_cycle(h, h->slot[0], hp, pp, &launches, h->ev));
+            EPP_TRY(launch_cycle(h, h->slot[0], hp, pp, &launches, h->ev, 0));
             sub_pp = pp;
             sub_pending = mode == Mode::Schedule;
         }
@@ -2050,7 +2115,7 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
             if (tk.on) attach_topk(h, pp.gen, tk.picks, tk.scores, c.r0);
             HashParams hp = hash_params(h, w, sl);
             if (trim) trim_rows(h, w, hp, pp);
-            EPP_TRY(launch_cycle(h, sl, hp, pp, &launches, nullptr));
+            EPP_TRY(launch_cycle(h, sl, hp, pp, &launches, nullptr, c.r0));
             if (mode == Mode::Schedule) {
                 EPP_TRY(launch_subset(h, pp, c.r0, c.r1, s, &launches, false));
                 if (out_dec) CUDA_TRY(cudaMemcpyAsync(out_dec + c.r0, dec, sizeof(epp_decision) * nreq, cudaMemcpyDeviceToHost, s));
@@ -2114,6 +2179,7 @@ static int32_t check_subset(const epp_engine *h, int64_t R, const epp_subset *s,
     if (s->struct_size != sizeof(epp_subset)) return fail(EPP_ERR_INVALID, "epp_subset.struct_size %u != %zu", s->struct_size, sizeof(epp_subset));
     if (h->shard_begin != 0 || h->shard_end != 0xFFFFFFFFu || h->p2p_buf)
         return fail(EPP_ERR_INVALID, "endpoint subsets are not available in the endpoint-sharded and peer-memory modes");
+    if (h->lat_mask) return fail(EPP_ERR_INVALID, "endpoint subsets are not available on an engine with latency profiles");
     if (R > 0 && !s->counts) return fail(EPP_ERR_INVALID, "epp_subset.counts is NULL");
     const uint32_t E = (uint32_t)h->cfg.max_endpoints;
     int64_t n_rows = 0;
@@ -2172,8 +2238,108 @@ static int32_t upload_subset(epp_engine *h, const std::vector<SubsetRow> &rows, 
     return EPP_OK;
 }
 
+// For the batcher (batcher.cu), which refuses subsets and checks predictions at submit time.  The mask is fixed once the
+// pool is set, and no batch is scheduled before that.
+int32_t engine_latency_mask(const epp_engine *h) { return h->lat_mask; }
+
+extern "C" void epp_latency_cfg_default(epp_latency_cfg *cfg) {
+    if (!cfg) return;
+    memset(cfg, 0, sizeof *cfg);
+    cfg->struct_size = sizeof(epp_latency_cfg);
+    cfg->epsilon_explore_neg = 0.01;                  // sloheadroomtier/plugin.go:50-52
+    cfg->a1_affinity_threshold = 0.0;                 // no A1
+    cfg->a1_exploration_probability = 0.01;           // prefixcacheaffinity/plugin.go:62-66
+    cfg->a1_max_ttft_penalty_ms = 5000.0;
+    cfg->ttft_weight = 0.8;                           // scorer/latency/plugin.go:83-90
+    cfg->tpot_weight = 0.2;
+    cfg->strategy = EPP_HEADROOM_LEAST;
+    cfg->composite_kv_weight = cfg->composite_queue_weight = cfg->composite_prefix_weight = 1.0;
+}
+
+extern "C" int32_t epp_latency_profile_set(epp_engine *h, int32_t profile, const epp_latency_cfg *cfg) {
+    if (!h || !cfg) return fail(EPP_ERR_INVALID, "NULL engine or configuration");
+    if (profile < 0 || profile >= h->n_alloc_profiles) return fail(EPP_ERR_INVALID, "profile %d is not configured", profile);
+    std::lock_guard<std::mutex> lk(h->mu);
+    if (h->pool_called) return fail(EPP_ERR_STATE, "latency profiles are fixed once the pool has been set");
+    if (h->shard_begin != 0 || h->shard_end != 0xFFFFFFFFu || h->p2p_buf)
+        return fail(EPP_ERR_INVALID, "endpoint-sharded mode does not support latency profiles");
+    const epp_profile_cfg &pc = profile_cfg(h, profile);
+    EPP_TRY(validate_latency(pc, *cfg, profile == 0 ? "primary profile" : (profile == 1 ? "prefill profile" : "encode profile")));
+    h->lat_cfg[profile] = *cfg;
+    if (latency_piece(pc, *cfg)) h->lat_mask |= 1 << profile;
+    else h->lat_mask &= ~(1 << profile);
+    if (h->lat_mask) h->general = true;
+    return EPP_OK;
+}
+
+// Validates the predictions of a batch of R requests on the host (*n_ent entries in all).  Nothing of the engine changes.
+static int32_t check_predictions(const epp_engine *h, int64_t R, const epp_predictions *p, uint64_t *n_ent) {
+    if (p->struct_size != sizeof(epp_predictions)) return fail(EPP_ERR_INVALID, "epp_predictions.struct_size %u != %zu", p->struct_size, sizeof(epp_predictions));
+    if (!h->lat_mask) return fail(EPP_ERR_INVALID, "predictions passed to an engine without a latency profile");
+    if (R > 0 && !p->counts) return fail(EPP_ERR_INVALID, "epp_predictions.counts is NULL");
+    const uint32_t E = (uint32_t)h->cfg.max_endpoints;
+    uint64_t total = 0;
+    for (int64_t r = 0; r < R; r++) {
+        const uint32_t n = p->counts[r];
+        if (!n) continue;
+        if (n > E) return fail(EPP_ERR_INVALID, "request %lld: %u predictions, more than max_endpoints %u", (long long)r, n, E);
+        if (!p->offsets || !p->entries) return fail(EPP_ERR_INVALID, "epp_predictions.offsets / entries is NULL");
+        const epp_prediction *src = p->entries + p->offsets[r];
+        for (uint32_t i = 0; i < n; i++) {
+            if (src[i].slot >= E) return fail(EPP_ERR_INVALID, "request %lld: slot %u >= max_endpoints %u", (long long)r, src[i].slot, E);
+            if (i && src[i].slot <= src[i - 1].slot) return fail(EPP_ERR_INVALID, "request %lld: prediction slots not strictly ascending at entry %u", (long long)r, i);
+            if (!std::isfinite(src[i].ttft) || !std::isfinite(src[i].ttft_headroom) || !std::isfinite(src[i].tpot_headroom))
+                return fail(EPP_ERR_INVALID, "request %lld: prediction %u is not finite", (long long)r, i);
+        }
+        total += n;
+    }
+    *n_ent = total;
+    return EPP_OK;
+}
+
+// Counts, packed offsets and entries to the device on stream 0, behind everything enqueued so far, through the engine's
+// pinned staging (refilled only once the previous call's copy has run), as upload_subset does.
+static int32_t upload_predictions(epp_engine *h, int64_t R, const epp_predictions *p, uint64_t n_ent) {
+    cudaStream_t s0 = h->slot[0].stream;
+    EPP_TRY(join_streams(h));
+    const size_t nr = (size_t)std::max<int64_t>(R, 1), ne = (size_t)std::max<uint64_t>(n_ent, 1);
+    CUDA_TRY(h->lat_cnt.reserve(sizeof(uint32_t) * nr, &h->dev_bytes));
+    CUDA_TRY(h->lat_off.reserve(sizeof(uint64_t) * nr, &h->dev_bytes));
+    CUDA_TRY(h->lat_ent.reserve(sizeof(epp_prediction) * ne, &h->dev_bytes));
+    if (!h->lat_up_ev) CUDA_TRY(cudaEventCreateWithFlags(&h->lat_up_ev, cudaEventDisableTiming));
+    else CUDA_TRY(cudaEventSynchronize(h->lat_up_ev));
+    const size_t off_at = (sizeof(uint32_t) * nr + 15) & ~(size_t)15;
+    const size_t ent_at = off_at + sizeof(uint64_t) * nr;
+    const size_t need = ent_at + sizeof(epp_prediction) * (size_t)n_ent;
+    if (need > h->lat_host_cap) {
+        if (h->lat_host) CUDA_TRY(cudaFreeHost(h->lat_host));
+        h->lat_host = nullptr;
+        h->lat_host_cap = 0;
+        CUDA_TRY(cudaHostAlloc(&h->lat_host, need, cudaHostAllocDefault));
+        h->lat_host_cap = need;
+    }
+    uint8_t *stage = static_cast<uint8_t *>(h->lat_host);
+    uint32_t *cnt = reinterpret_cast<uint32_t *>(stage);
+    uint64_t *off = reinterpret_cast<uint64_t *>(stage + off_at);
+    epp_prediction *ent = reinterpret_cast<epp_prediction *>(stage + ent_at);
+    uint64_t o = 0;
+    for (int64_t r = 0; r < R; r++) {
+        const uint32_t n = p->counts[r];
+        cnt[r] = n;
+        off[r] = o;
+        if (n) memcpy(ent + o, p->entries + p->offsets[r], sizeof(epp_prediction) * n);
+        o += n;
+    }
+    CUDA_TRY(cudaMemcpyAsync(h->lat_cnt.p, cnt, sizeof(uint32_t) * (size_t)R, cudaMemcpyHostToDevice, s0));
+    CUDA_TRY(cudaMemcpyAsync(h->lat_off.p, off, sizeof(uint64_t) * (size_t)R, cudaMemcpyHostToDevice, s0));
+    if (n_ent) CUDA_TRY(cudaMemcpyAsync(h->lat_ent.p, ent, sizeof(epp_prediction) * (size_t)n_ent, cudaMemcpyHostToDevice, s0));
+    CUDA_TRY(cudaEventRecord(h->lat_up_ev, s0));
+    return EPP_OK;
+}
+
 static int32_t schedule_impl(epp_engine *h, const epp_batch *batch, epp_decision *out, epp_decision_detail *detail,
-                             int32_t keep_hashes, const epp_topk_out *topk, const epp_subset *subset = nullptr) {
+                             int32_t keep_hashes, const epp_topk_out *topk, const epp_subset *subset = nullptr,
+                             const epp_predictions *preds = nullptr) {
     if (!h) return fail(EPP_ERR_INVALID, "NULL engine");
     if (!out) return fail(EPP_ERR_INVALID, "out is NULL");
     std::lock_guard<std::mutex> lk(h->mu);
@@ -2185,16 +2351,21 @@ static int32_t schedule_impl(epp_engine *h, const epp_batch *batch, epp_decision
     std::vector<SubsetRow> sub_rows;
     uint64_t sub_n_slots = 0;
     if (subset) EPP_TRY(check_subset(h, v.R, subset, sub_rows, &sub_n_slots));
-    if (!sub_rows.empty()) {
+    uint64_t n_ent = 0;
+    if (preds) EPP_TRY(check_predictions(h, v.R, preds, &n_ent));
+    if (!sub_rows.empty() || (preds && v.R)) {
         if (!h->pool_ready) return fail(EPP_ERR_STATE, "epp_pool_set has not been called");
-        EPP_TRY(upload_subset(h, sub_rows, subset, sub_n_slots));
     }
+    if (!sub_rows.empty()) EPP_TRY(upload_subset(h, sub_rows, subset, sub_n_slots));
+    if (preds && v.R) EPP_TRY(upload_predictions(h, v.R, preds, n_ent));
     h->kept_R = 0;
     h->cur_topk = topk;
     h->cur_sub = sub_rows.empty() ? nullptr : &sub_rows;
+    h->cur_pred = preds && v.R;
     const int32_t rc = run_batch(h, v, Mode::Schedule, nullptr, nullptr, out, detail, nullptr, nullptr, keep_hashes != 0);
     h->cur_topk = nullptr;
     h->cur_sub = nullptr;
+    h->cur_pred = false;
     EPP_TRY(rc);
     h->stats.n_batches++;
     h->stats.n_decisions += (uint64_t)v.R;
@@ -2220,6 +2391,11 @@ extern "C" int32_t epp_schedule_topk(epp_engine *h, const epp_batch *batch, epp_
                                      int32_t keep_hashes, const epp_topk_out *topk) {
     if (!topk) return fail(EPP_ERR_INVALID, "topk is NULL");
     return schedule_impl(h, batch, out, detail, keep_hashes, topk);
+}
+
+extern "C" int32_t epp_schedule_predicted(epp_engine *h, const epp_batch *batch, const epp_predictions *preds, epp_decision *out,
+                                          epp_decision_detail *detail, int32_t keep_hashes, const epp_topk_out *topk) {
+    return schedule_impl(h, batch, out, detail, keep_hashes, topk, nullptr, preds);
 }
 
 extern "C" int32_t epp_schedule_subset(epp_engine *h, const epp_batch *batch, const epp_subset *subset, epp_decision *out,
@@ -2286,6 +2462,8 @@ extern "C" int32_t epp_score(epp_engine *h, int64_t n_requests, const int32_t *m
     if (!h->pool_ready) return fail(EPP_ERR_STATE, "epp_pool_set has not been called");
     if (profile < 0 || profile >= h->n_alloc_profiles) return fail(EPP_ERR_INVALID, "profile %d out of range", profile);
     if (scorer_index < -1 || scorer_index >= profile_cfg(h, profile).n_scorers) return fail(EPP_ERR_INVALID, "scorer_index %d out of range", scorer_index);
+    if (((h->lat_mask >> profile) & 1) && (scorer_index < 0 || profile_cfg(h, profile).scorers[scorer_index].kind == EPP_SCORER_LATENCY))
+        return fail(EPP_ERR_INVALID, "epp_score does not evaluate latency pieces (the weighted sum of a latency profile, the latency scorer)");
     if (n_requests == 0) return EPP_OK;
     const size_t E = (size_t)h->cfg.max_endpoints, n = (size_t)n_requests * E;
     cudaStream_t s = h->slot[0].stream;
@@ -2318,14 +2496,23 @@ extern "C" int32_t epp_score(epp_engine *h, int64_t n_requests, const int32_t *m
 
 static int32_t with_match_impl(epp_engine *h, int64_t n_requests, const int32_t *match, const int32_t *total,
                                const uint32_t *model_ids, const int64_t *input_len_bytes, int32_t block_size_tokens, epp_decision *out,
-                               epp_decision_detail *detail, uint32_t flags, const epp_topk_out *topk) {
+                               epp_decision_detail *detail, uint32_t flags, const epp_topk_out *topk,
+                               const epp_predictions *preds = nullptr) {
     if (!h || n_requests < 0 || (n_requests && (!match || !total || !out))) return fail(EPP_ERR_INVALID, "bad arguments");
     std::lock_guard<std::mutex> lk(h->mu);
     if (topk) EPP_TRY(check_topk(h, topk));
+    uint64_t n_ent = 0;
+    if (preds) EPP_TRY(check_predictions(h, n_requests, preds, &n_ent));
     EPP_TRY(set_device(h));
     EPP_TRY(join_streams(h));
     if (!h->pool_ready) return fail(EPP_ERR_STATE, "epp_pool_set has not been called");
     if (n_requests == 0) return EPP_OK;
+    if (preds) EPP_TRY(upload_predictions(h, n_requests, preds, n_ent));
+    h->cur_pred = preds != nullptr;
+    struct PredReset {                             // the call's predictions end with it, whichever way it returns
+        epp_engine *h;
+        ~PredReset() { h->cur_pred = false; }
+    } pred_reset{h};
     const size_t R = (size_t)n_requests;
     cudaStream_t s = h->slot[0].stream;
     const bool dev = (flags & EPP_BATCH_DEVICE_PTRS) != 0;
@@ -2360,7 +2547,11 @@ static int32_t with_match_impl(epp_engine *h, int64_t n_requests, const int32_t 
         p.out = h->decisions.as<epp_decision>();
         p.detail = h->details.as<epp_decision_detail>();
     }
-    CUDA_TRY(launch_dense_pick(p, s, &launches));
+    if (h->lat_mask) {
+        CUDA_TRY(launch_dense_pick_lat(p, lat_view(h, 0), s, &launches));
+    } else {
+        CUDA_TRY(launch_dense_pick(p, s, &launches));
+    }
     EPP_TRY(after_picks(h, p.out, p.detail, p.in_len, n_requests, s, &launches, false));
     if (!dev) {
         CUDA_TRY(cudaMemcpyAsync(out, p.out, sizeof(epp_decision) * R, cudaMemcpyDeviceToHost, s));
@@ -2377,6 +2568,13 @@ extern "C" int32_t epp_schedule_with_match(epp_engine *h, int64_t n_requests, co
                                            const uint32_t *model_ids, const int64_t *input_len_bytes, int32_t block_size_tokens, epp_decision *out,
                                            epp_decision_detail *detail, uint32_t flags) {
     return with_match_impl(h, n_requests, match, total, model_ids, input_len_bytes, block_size_tokens, out, detail, flags, nullptr);
+}
+
+extern "C" int32_t epp_schedule_with_match_predicted(epp_engine *h, int64_t n_requests, const int32_t *match, const int32_t *total,
+                                                     const uint32_t *model_ids, const int64_t *input_len_bytes,
+                                                     int32_t block_size_tokens, epp_decision *out, epp_decision_detail *detail,
+                                                     uint32_t flags, const epp_topk_out *topk, const epp_predictions *preds) {
+    return with_match_impl(h, n_requests, match, total, model_ids, input_len_bytes, block_size_tokens, out, detail, flags, topk, preds);
 }
 
 extern "C" int32_t epp_schedule_with_match_topk(epp_engine *h, int64_t n_requests, const int32_t *match, const int32_t *total,
@@ -2516,6 +2714,7 @@ extern "C" int32_t epp_event_elapsed_ms(epp_engine *h, double *out_ms) {
 // ------------------------------------------------------------------------------------------------
 // Per-call state that no rank can keep from its own shard alone.
 static int32_t check_shardable(const epp_engine *h) {
+    if (h->lat_mask) return fail(EPP_ERR_INVALID, "endpoint-sharded mode does not support latency profiles");
     if (h->nohit_mask) return fail(EPP_ERR_INVALID, "endpoint-sharded mode does not support the no-hit-lru scorer (coldness needs every rank's match)");
     if (any_random_picker(h)) return fail(EPP_ERR_INVALID, "endpoint-sharded mode does not support the random pickers (a weighted draw needs every rank's scores)");
     if (h->inflight) return fail(EPP_ERR_INVALID, "endpoint-sharded mode does not support the inflight-load producer");

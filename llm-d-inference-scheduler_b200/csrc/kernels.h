@@ -341,6 +341,21 @@ struct DensePickParams {
     NoHitView nohit;
 };
 cudaError_t launch_dense_pick(const DensePickParams &p, cudaStream_t s, int *launches);
+// Latency predictions (include/epp_engine.h, "Latency predictions"): the general evaluation of pick_latency.cuh for the
+// profiles whose bit is set in `mask`, with request r's entries at ent[off[r0 + r] .. + cnt[r0 + r]) (cnt == nullptr: no
+// request has any).  The _lat builds of the dense-counter and injected-match kernels take it as an extra argument, so
+// the parameters of every other kernel stay as they are.
+struct LatView {
+    const uint32_t *cnt;       // [batch R] absolute request rows
+    const uint64_t *off;
+    const epp_prediction *ent;
+    int64_t r0;                // row of this launch's request 0
+    int32_t mask;              // profiles with a latency piece
+    epp_latency_cfg cfg[kMaxProfiles];
+};
+cudaError_t launch_match_pick_lat(const PickParams &p, const LatView &lv, uint32_t *gscratch, int grid, size_t smem,
+                                  cudaStream_t s, int *launches);
+cudaError_t launch_dense_pick_lat(const DensePickParams &p, const LatView &lv, cudaStream_t s, int *launches);
 // subset_pick.cu: per-request endpoint subsets (include/epp_engine.h, "Endpoint subsets").  One warp re-decides one
 // restricted request of a launch whose ordinary match kernel has run: it walks the request's stored hash row up to the
 // global stop counting only the listed holders, then evaluates every profile over the listed slots (full evaluation:

@@ -17,6 +17,7 @@
 
 #include "index.cuh"
 #include "pick_general.cuh"
+#include "pick_latency.cuh"
 #include "pick_random.cuh"
 #include "score.cuh"
 
@@ -353,9 +354,29 @@ __device__ inline Best gen_eval_profile(const P &p, const ProfileDev &pf, int pi
                      (k > 1 && pi == 0 && p.gen.topk_scores) ? p.gen.topk_scores + r * k : nullptr);
 }
 
+// lat::eval for latency profile pi of request r (the row handling of gen_eval_profile).
+template <bool kRand, typename P, typename CntOf>
+__device__ inline Best lat_eval_profile(const P &p, const LatView &lv, int pi, int64_t r, int32_t total, int lane,
+                                        uint32_t adapter, uint64_t key, CntOf cnt_of) {
+    const int32_t k = p.gen.topk > 1 ? p.gen.topk : 1;
+    if (pi == 0 && k > 1) {
+        for (int q = 0; q < kMaxProfiles; q++)
+            if (p.gen.topk_picks[q]) for (int j = lane; j < k; j += 32) p.gen.topk_picks[q][r * k + j] = EPP_NO_ENDPOINT;
+        __syncwarp();
+    }
+    lat::Req q;
+    q.n = lv.cnt ? lv.cnt[lv.r0 + r] : 0u;
+    q.ent = q.n ? lv.ent + lv.off[lv.r0 + r] : nullptr;
+    return lat::eval<kRand>(p.prof[pi], lv.cfg[pi], p.gen, q, p.E, total, lane, p.lora, adapter, p.tie_seed, key, cnt_of, k,
+                            (k > 1 && p.gen.topk_picks[pi]) ? p.gen.topk_picks[pi] + r * k : nullptr,
+                            (k > 1 && pi == 0 && p.gen.topk_scores) ? p.gen.topk_scores + r * k : nullptr);
+}
+
 // kRand: the engine has a random picker (k_match_pick_rand); the max-score build carries none of its code.
-template <bool kRand>
-__device__ __forceinline__ void match_pick_dense(const PickParams &p, int32_t cnt_words, uint32_t *gscratch) {
+// kLat: the engine has latency profiles (k_match_pick_lat*): those evaluate through lat::eval with the request's entries.
+template <bool kRand, bool kLat = false>
+__device__ __forceinline__ void match_pick_dense(const PickParams &p, int32_t cnt_words, uint32_t *gscratch,
+                                                 const LatView *lv = nullptr) {
     extern __shared__ uint32_t smem[];
     const int lane = threadIdx.x & 31;
     const int warp = threadIdx.x >> 5;
@@ -433,7 +454,14 @@ __device__ __forceinline__ void match_pick_dense(const PickParams &p, int32_t cn
         auto cnt_of = [&](uint32_t e) { return (int32_t)cnt_get(cnt32, e); };
         bool cold = false;
         auto is_cold = [&](const ProfileDev &pf) { return cold_scan(pf, p.E, lane, cnt_of); };
-        if (p.gen.on) {       // affinity filter / top-k: full-scan evaluation (pick_general.cuh)
+        if constexpr (kLat) {
+            decide_stages<3>(p, r, total, p.n_profiles >= 2 ? p.in_len[r] : 0,
+                          [&](int pi, uint64_t key) {
+                              if ((lv->mask >> pi) & 1) return lat_eval_profile<kRand>(p, *lv, pi, r, total, lane, adapter, key, cnt_of);
+                              return gen_eval_profile<kRand>(p, nohit_select(p, pi, cold, is_cold), pi, r, total, lane, adapter, key, cnt_of);
+                          },
+                          cnt_of, d, dd);
+        } else if (p.gen.on) {       // affinity filter / top-k: full-scan evaluation (pick_general.cuh)
             decide_stages<3>(p, r, total, p.n_profiles >= 2 ? p.in_len[r] : 0,
                           [&](int pi, uint64_t key) { return gen_eval_profile<kRand>(p, nohit_select(p, pi, cold, is_cold), pi, r, total, lane, adapter, key, cnt_of); },
                           cnt_of, d, dd);
@@ -490,6 +518,13 @@ __global__ void __launch_bounds__(kPickWarps * 32) k_match_pick_rand(PickParams 
     match_pick_dense<true>(p, cnt_words, gscratch);
 }
 
+__global__ void __launch_bounds__(kPickWarps * 32) k_match_pick_lat(PickParams p, int32_t cnt_words, uint32_t *gscratch, LatView lv) {
+    match_pick_dense<false, true>(p, cnt_words, gscratch, &lv);
+}
+__global__ void __launch_bounds__(kPickWarps * 32) k_match_pick_lat_rand(PickParams p, int32_t cnt_words, uint32_t *gscratch, LatView lv) {
+    match_pick_dense<true, true>(p, cnt_words, gscratch, &lv);
+}
+
 // The engine allocates gscratch when E does not fit in shared memory; see engine.cu.
 size_t match_pick_smem_bytes(int32_t E, bool global_counts) {
     int32_t cnt_words = (E + 1) / 2;
@@ -512,6 +547,24 @@ cudaError_t launch_match_pick(const PickParams &p, uint32_t *gscratch, int grid,
     int32_t cnt_words = (p.E + 1) / 2;
     if (any_random_picker(p)) k_match_pick_rand<<<grid, kPickWarps * 32, smem, s>>>(p, cnt_words, gscratch);
     else k_match_pick<<<grid, kPickWarps * 32, smem, s>>>(p, cnt_words, gscratch);
+    if (launches) *launches += 1;
+    return cudaGetLastError();
+}
+
+cudaError_t launch_match_pick_lat(const PickParams &p, const LatView &lv, uint32_t *gscratch, int grid, size_t smem,
+                                  cudaStream_t s, int *launches) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    static bool attr_set[64] = {};
+    if (!attr_set[dev & 63]) {
+        cudaError_t e = cudaFuncSetAttribute(k_match_pick_lat, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(k_match_pick_lat_rand, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+        if (e != cudaSuccess) return e;
+        attr_set[dev & 63] = true;
+    }
+    int32_t cnt_words = (p.E + 1) / 2;
+    if (any_random_picker(p)) k_match_pick_lat_rand<<<grid, kPickWarps * 32, smem, s>>>(p, cnt_words, gscratch, lv);
+    else k_match_pick_lat<<<grid, kPickWarps * 32, smem, s>>>(p, cnt_words, gscratch, lv);
     if (launches) *launches += 1;
     return cudaGetLastError();
 }
@@ -543,8 +596,8 @@ __device__ inline Best eval_profile_dense(const ProfileDev &pf, int32_t E, const
     return b;
 }
 
-template <bool kRand>
-__device__ __forceinline__ void dense_pick(const DensePickParams &p) {
+template <bool kRand, bool kLat = false>
+__device__ __forceinline__ void dense_pick(const DensePickParams &p, const LatView *lv = nullptr) {
     const int lane = threadIdx.x & 31;
     const int64_t r = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (r >= p.R) return;
@@ -556,7 +609,14 @@ __device__ __forceinline__ void dense_pick(const DensePickParams &p) {
     auto cnt_of = [&](uint32_t e) { return mrow[e]; };
     bool cold = false;
     auto is_cold = [&](const ProfileDev &pf) { return cold_scan(pf, p.E, lane, cnt_of); };
-    if (p.gen.on) {
+    if constexpr (kLat) {
+        decide_stages<3>(p, r, total, p.in_len ? p.in_len[r] : 0,
+                      [&](int pi, uint64_t key) {
+                          if ((lv->mask >> pi) & 1) return lat_eval_profile<kRand>(p, *lv, pi, r, total, lane, adapter, key, cnt_of);
+                          return gen_eval_profile<kRand>(p, nohit_select(p, pi, cold, is_cold), pi, r, total, lane, adapter, key, cnt_of);
+                      },
+                      cnt_of, d, dd);
+    } else if (p.gen.on) {
         decide_stages<3>(p, r, total, p.in_len ? p.in_len[r] : 0,
                       [&](int pi, uint64_t key) { return gen_eval_profile<kRand>(p, nohit_select(p, pi, cold, is_cold), pi, r, total, lane, adapter, key, cnt_of); },
                       cnt_of, d, dd);
@@ -580,6 +640,18 @@ cudaError_t launch_dense_pick(const DensePickParams &p, cudaStream_t s, int *lau
     int64_t threads = p.R * 32;
     if (any_random_picker(p)) k_dense_pick_rand<<<(unsigned)((threads + 255) / 256), 256, 0, s>>>(p);
     else k_dense_pick<<<(unsigned)((threads + 255) / 256), 256, 0, s>>>(p);
+    if (launches) *launches += 1;
+    return cudaGetLastError();
+}
+
+__global__ void __launch_bounds__(256) k_dense_pick_lat(DensePickParams p, LatView lv) { dense_pick<false, true>(p, &lv); }
+__global__ void __launch_bounds__(256) k_dense_pick_lat_rand(DensePickParams p, LatView lv) { dense_pick<true, true>(p, &lv); }
+
+cudaError_t launch_dense_pick_lat(const DensePickParams &p, const LatView &lv, cudaStream_t s, int *launches) {
+    if (p.R <= 0) return cudaSuccess;
+    int64_t threads = p.R * 32;
+    if (any_random_picker(p)) k_dense_pick_lat_rand<<<(unsigned)((threads + 255) / 256), 256, 0, s>>>(p, lv);
+    else k_dense_pick_lat<<<(unsigned)((threads + 255) / 256), 256, 0, s>>>(p, lv);
     if (launches) *launches += 1;
     return cudaGetLastError();
 }

@@ -1,0 +1,373 @@
+// pick_latency.cuh -- the general evaluation of one SchedulerProfile with a latency piece for one request (one warp), as
+// defined in include/epp_engine.h ("Latency predictions"):
+//   [role + label filters] -> [affinity A1] -> [slo-headroom-tier-filter T] -> [affinity A2] -> scorers -> picker,
+// with the latency-scorer (scorer/latency/plugin.go:144-395) among the scorers.  The request-level state (the A1 / T / A2
+// decisions, the scored bucket, its per-dimension min / max, alpha and beta) is computed once per stage by warp
+// reductions; after that a slot's membership and score are per-slot predicates over its entry, which each lane finds by
+// binary search in the request's ascending entry list.
+// Only the _lat builds of the dense-counter and injected-match kernels include this code.
+#pragma once
+#include <cfloat>
+#include <climits>
+
+#include "pick_general.cuh"
+
+namespace epp {
+namespace lat {
+
+constexpr uint64_t kA1Domain = 0x8EBC6AF09C88C6E3ULL;
+constexpr uint64_t kTierDomain = 0x589965CC75374CC3ULL;
+constexpr double kEps = 1e-9;        // scorer/latency/plugin.go:41
+
+__device__ __forceinline__ double draw_u(uint64_t seed, uint64_t dom, uint64_t key) {
+    return (double)(mix64((seed ^ dom) ^ mix64(key)) >> 11) * 0x1.0p-53;
+}
+
+// int(x) of Go on amd64 (CVTTSD2SQ): truncation toward zero, 0x8000000000000000 for NaN and out-of-range values
+__device__ __forceinline__ long long go_int(double x) {
+    if (!(x > -0x1.0p63 && x < 0x1.0p63)) return LLONG_MIN;
+    return (long long)x;
+}
+
+__device__ __forceinline__ uint32_t warp_sum(uint32_t v) {
+    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(gen::kFull, v, o);
+    return v;
+}
+
+// The request's entries, ascending slot.
+struct Req {
+    const epp_prediction *ent;
+    uint32_t n;
+    __device__ __forceinline__ const epp_prediction *find(uint32_t e) const {
+        uint32_t lo = 0, hi = n;
+        while (lo < hi) {
+            const uint32_t mid = (lo + hi) >> 1;
+            if (ent[mid].slot < e) lo = mid + 1; else hi = mid;
+        }
+        return (lo < n && ent[lo].slot == e) ? ent + lo : nullptr;
+    }
+};
+
+// both headrooms >= 0 (sloheadroomtier/plugin.go:102)
+__device__ __forceinline__ bool meets(const epp_prediction *p) { return p->ttft_headroom >= 0.0 && p->tpot_headroom >= 0.0; }
+
+enum { kTierAll = 0, kTierPos = 1, kTierNeg = 2 };
+enum { kBucketPos = 0, kBucketIdle = 1, kBucketTpot = 2, kBucketTtft = 3, kBucketBoth = 4, kComposite = 5 };
+
+// The scored bucket of Score (plugin.go:172-235); p == nullptr: no entry (positive, headrooms 0).
+__device__ __forceinline__ bool in_bucket(int bucket, const epp_prediction *p) {
+    if (!p) return bucket == kBucketPos;
+    const bool tn = p->ttft_headroom < 0.0, pn = p->tpot_headroom < 0.0;
+    switch (bucket) {
+        case kBucketPos: return !tn && !pn;
+        case kBucketIdle: return (tn || pn) && p->dispatched == 0;
+        case kBucketTpot: return !tn && pn;
+        case kBucketTtft: return tn && !pn;
+        case kBucketBoth: return tn && pn;
+        default: return false;
+    }
+}
+
+struct State {
+    bool a1, a2;
+    int tier;
+    gen::Norm nm;                   // normalisation over the final set (nm.sticky / nm.thr unused)
+    bool scorer;                    // the profile lists the latency scorer
+    int bucket;
+    bool most;
+    double alpha, beta, mn_t, rng_t, mn_p, rng_p;
+    long long max_q;
+    double wkv, wq, wpref;
+};
+
+// prefix-cache-affinity-filter (plugin.go:105-151) over the n members of in_set, TTFT from the entries (bestTTFT,
+// :173-184, skips members without one).  True: the set narrows to the sticky members.
+template <typename InSet, typename CntOf>
+__device__ inline bool affinity(double thr, double explore, double penalty, uint64_t dom, uint32_t n, const Req &q,
+                                int32_t E, int32_t total, int lane, uint64_t seed, uint64_t key, InSet in_set, CntOf cnt_of) {
+    if (!(thr > 0.0) || n <= 1) return false;                                           // :108
+    if (seed && draw_u(seed, dom, key) < explore) return false;                         // :113-117
+    uint32_t ns = 0, nn = 0;
+    double bs = DBL_MAX, bn = DBL_MAX;
+    for (uint32_t e = lane; e < (uint32_t)E; e += 32) {
+        if (!in_set(e)) continue;
+        const epp_prediction *p = q.find(e);
+        const double t = p ? p->ttft : DBL_MAX;
+        if (gen::is_sticky(cnt_of(e), total, thr)) { ns++; if (t < bs) bs = t; }
+        else { nn++; if (t < bn) bn = t; }
+    }
+    for (int o = 16; o; o >>= 1) {
+        ns += __shfl_xor_sync(gen::kFull, ns, o);
+        nn += __shfl_xor_sync(gen::kFull, nn, o);
+        const double os = __shfl_xor_sync(gen::kFull, bs, o), on = __shfl_xor_sync(gen::kFull, bn, o);
+        if (os < bs) bs = os;
+        if (on < bn) bn = on;
+    }
+    if (ns == 0) return false;                                                           // :130-134
+    if (penalty > 0.0 && nn > 0 && __dsub_rn(bs, bn) > penalty) return false;            // :137-146
+    return true;
+}
+
+// The latency scorer's raw score of final-set member e (p = its entry or nullptr).
+__device__ __forceinline__ double score_raw(const State &st, const PoolArrays &pool, uint32_t e, const epp_prediction *p,
+                                            int32_t match, int32_t total) {
+    if (st.bucket == kComposite) {                                                       // compositeScores, :323-367
+        const long long q = pool.waiting[e];
+        const double rel = st.max_q > 0 ? __ddiv_rn((double)(st.max_q - q), (double)st.max_q) : 1.0;
+        const double kv_free = __dsub_rn(1.0, pool.kv_usage[e]);
+        const double c = __dadd_rn(__dadd_rn(__dmul_rn(st.wkv, kv_free), __dmul_rn(st.wq, rel)),
+                                   __dmul_rn(st.wpref, prefix_score(match, total)));
+        return __ddiv_rn((double)go_int(round(__dadd_rn(0.0, __dmul_rn(100.0, c)))), 100.0);
+    }
+    if (!in_bucket(st.bucket, p)) return 0.0;
+    const double ht = p ? fabs(p->ttft_headroom) : 0.0, hp = p ? fabs(p->tpot_headroom) : 0.0;   // scoreBucket, :246-318
+    const double nt = st.rng_t > kEps ? __ddiv_rn(__dsub_rn(ht, st.mn_t), st.rng_t) : 0.5;
+    const double np = st.rng_p > kEps ? __ddiv_rn(__dsub_rn(hp, st.mn_p), st.rng_p) : 0.5;
+    const double comb = __dadd_rn(__dmul_rn(st.alpha, nt), __dmul_rn(st.beta, np));
+    const double x = st.most ? comb : __dsub_rn(1.0, comb);
+    return __ddiv_rn((double)(go_int(__dmul_rn(x, 100.0)) + 1), 100.0);
+}
+
+// runScorerPlugins over the final set (weighted_sum_over with the latency scorer).
+__device__ inline double weighted_sum(const ProfileDev &pf, const GenView &g, const State &st, uint32_t e,
+                                      const epp_prediction *p, int32_t match, int32_t total, const LoraDev &L, int lora_st) {
+    double acc = 0.0;
+#pragma unroll 1
+    for (int s = 0; s < pf.cfg.n_scorers; s++) {
+        const epp_scorer_cfg &sc = pf.cfg.scorers[s];
+        double raw;
+        if (sc.kind == EPP_SCORER_PREFIX) raw = prefix_score(match, total);
+        else if (sc.kind == EPP_SCORER_LORA_AFFINITY) raw = lora_score(L, e, lora_st);
+        else if (sc.kind == EPP_SCORER_LATENCY) raw = score_raw(st, g.pool, e, p, match, total);
+        else raw = pool_score(sc, s, g.pool, st.nm.q, (int32_t)e);
+        acc = __dadd_rn(acc, __dmul_rn(clamp01(raw), sc.weight));
+    }
+    return acc;
+}
+
+// The request-level state of the chain and the scorer.  Returns the final set's size.
+template <typename CntOf>
+__device__ inline uint32_t prepare(const ProfileDev &pf, const epp_latency_cfg &lc, const GenView &g, const Req &q,
+                                   int32_t E, int32_t total, int lane, uint64_t seed, uint64_t key, CntOf cnt_of, State &st) {
+    const epp_profile_cfg &c = pf.cfg;
+    st.a1 = st.a2 = false;
+    st.tier = kTierAll;
+    auto in1 = [&](uint32_t e) { return pf.cand[e] && (!st.a1 || gen::is_sticky(cnt_of(e), total, lc.a1_affinity_threshold)); };
+    auto in2 = [&](uint32_t e) {
+        if (!in1(e)) return false;
+        if (st.tier == kTierAll) return true;
+        const epp_prediction *p = q.find(e);
+        return (st.tier == kTierPos) == (p && meets(p));
+    };
+    auto in = [&](uint32_t e) { return in2(e) && (!st.a2 || gen::is_sticky(cnt_of(e), total, c.affinity_threshold)); };
+    // A1 over the filtered candidates
+    if (lc.tier_filter)
+        st.a1 = affinity(lc.a1_affinity_threshold, lc.a1_exploration_probability, lc.a1_max_ttft_penalty_ms, kA1Domain,
+                         (uint32_t)*pf.n_cand, q, E, total, lane, seed, key, in1, cnt_of);
+    // T over A1's set (sloheadroomtier/plugin.go:84-138)
+    uint32_t n1 = 0, npos = 0, nneg = 0;
+    for (uint32_t e = lane; e < (uint32_t)E; e += 32) {
+        if (!in1(e)) continue;
+        n1++;
+        const epp_prediction *p = q.find(e);
+        if (p) { if (meets(p)) npos++; else nneg++; }
+    }
+    n1 = warp_sum(n1); npos = warp_sum(npos); nneg = warp_sum(nneg);
+    uint32_t n2 = n1;
+    if (lc.tier_filter && n1 > 1 && (npos || nneg)) {
+        nneg = n1 - npos;                                                               // + the no-prediction endpoints
+        if (npos && nneg) st.tier = (seed && draw_u(seed, kTierDomain, key) < lc.epsilon_explore_neg) ? kTierNeg : kTierPos;
+        else st.tier = npos ? kTierPos : kTierNeg;
+        n2 = st.tier == kTierPos ? npos : nneg;
+    }
+    // A2: the profile's own affinity filter, today's draw
+    st.a2 = affinity(c.affinity_threshold, c.exploration_probability, c.max_ttft_penalty_ms, gen::kExploreDomain, n2, q,
+                     E, total, lane, seed, key, in2, cnt_of);
+    // normalisation over the final set; the latency scorer's bucket
+    uint32_t n = 0, has = 0, pos = 0, idle = 0, tpot = 0, ttft = 0;
+    long long mnw = LLONG_MAX, mxw = LLONG_MIN, mnr = LLONG_MAX, mxr = LLONG_MIN, mxq = 0;
+    for (uint32_t e = lane; e < (uint32_t)E; e += 32) {
+        if (!in(e)) continue;
+        n++;
+        const long long w = g.pool.waiting[e], r = g.pool.running[e];
+        mnw = min(mnw, w); mxw = max(mxw, w);
+        mnr = min(mnr, r); mxr = max(mxr, r);
+        mxq = max(mxq, w);
+        const epp_prediction *p = q.find(e);
+        if (!p) { pos++; continue; }
+        has++;
+        pos += in_bucket(kBucketPos, p);
+        idle += in_bucket(kBucketIdle, p);
+        tpot += in_bucket(kBucketTpot, p);
+        ttft += in_bucket(kBucketTtft, p);
+    }
+    for (int o = 16; o; o >>= 1) {
+        mnw = min(mnw, __shfl_xor_sync(gen::kFull, mnw, o)); mxw = max(mxw, __shfl_xor_sync(gen::kFull, mxw, o));
+        mnr = min(mnr, __shfl_xor_sync(gen::kFull, mnr, o)); mxr = max(mxr, __shfl_xor_sync(gen::kFull, mxr, o));
+        mxq = max(mxq, __shfl_xor_sync(gen::kFull, mxq, o));
+    }
+    n = warp_sum(n); has = warp_sum(has); pos = warp_sum(pos); idle = warp_sum(idle); tpot = warp_sum(tpot); ttft = warp_sum(ttft);
+    st.nm.sticky = false;
+    st.nm.thr = 0.0;
+    st.nm.q[0] = mnw; st.nm.q[1] = mxw; st.nm.q[2] = mnr; st.nm.q[3] = mxr;
+    st.scorer = false;
+    for (int s = 0; s < c.n_scorers; s++) {
+        st.nm.q[4 + s] = 0;
+        if (c.scorers[s].kind == EPP_SCORER_LATENCY) st.scorer = true;
+        if (c.scorers[s].kind != EPP_SCORER_ACTIVE_REQUEST) continue;
+        const int col = c.scorers[s].column;
+        long long mx = 0;
+        if (col >= 0 && col < g.pool.n_ext_cols)
+            for (uint32_t e = lane; e < (uint32_t)E; e += 32)
+                if (in(e)) mx = max(mx, (long long)g.pool.ext[(size_t)col * (size_t)E + (size_t)e]);
+        for (int o = 16; o; o >>= 1) mx = max(mx, __shfl_xor_sync(gen::kFull, mx, o));
+        st.nm.q[4 + s] = mx;
+    }
+    st.max_q = mxq;
+    st.most = false;
+    if (!st.scorer) { st.bucket = kComposite; return n; }
+    if (!has) {                                                                          // compositeScores weights, :326-334
+        st.bucket = kComposite;
+        double wkv = lc.composite_kv_weight, wq = lc.composite_queue_weight, wp = lc.composite_prefix_weight;
+        double sw = __dadd_rn(__dadd_rn(wkv, wq), wp);
+        if (sw <= 0.0) { wkv = 1.0; wq = 0.0; wp = 0.0; sw = 1.0; }
+        st.wkv = __ddiv_rn(wkv, sw); st.wq = __ddiv_rn(wq, sw); st.wpref = __ddiv_rn(wp, sw);
+        return n;
+    }
+    if (pos) { st.bucket = kBucketPos; st.most = lc.strategy == EPP_HEADROOM_MOST; }
+    else if (idle) st.bucket = kBucketIdle;
+    else if (tpot) st.bucket = kBucketTpot;
+    else if (ttft) st.bucket = kBucketTtft;
+    else st.bucket = kBucketBoth;
+    double mnt = DBL_MAX, mxt = -DBL_MAX, mnp = DBL_MAX, mxp = -DBL_MAX;
+    for (uint32_t e = lane; e < (uint32_t)E; e += 32) {
+        if (!in(e)) continue;
+        const epp_prediction *p = q.find(e);
+        if (!in_bucket(st.bucket, p)) continue;
+        const double ht = p ? fabs(p->ttft_headroom) : 0.0, hp = p ? fabs(p->tpot_headroom) : 0.0;
+        if (ht < mnt) mnt = ht;
+        if (ht > mxt) mxt = ht;
+        if (hp < mnp) mnp = hp;
+        if (hp > mxp) mxp = hp;
+    }
+    for (int o = 16; o; o >>= 1) {
+        mnt = fmin(mnt, __shfl_xor_sync(gen::kFull, mnt, o)); mxt = fmax(mxt, __shfl_xor_sync(gen::kFull, mxt, o));
+        mnp = fmin(mnp, __shfl_xor_sync(gen::kFull, mnp, o)); mxp = fmax(mxp, __shfl_xor_sync(gen::kFull, mxp, o));
+    }
+    st.mn_t = mnt; st.mn_p = mnp;
+    st.rng_t = __dsub_rn(mxt, mnt);
+    st.rng_p = __dsub_rn(mxp, mnp);
+    const double sab = __dadd_rn(lc.ttft_weight, lc.tpot_weight);                        // normalizedWeights, :376-382
+    if (sab <= 0.0) { st.alpha = 1.0; st.beta = 0.0; }
+    else { st.alpha = __ddiv_rn(lc.ttft_weight, sab); st.beta = __ddiv_rn(lc.tpot_weight, sab); }
+    if (st.rng_t <= kEps && st.rng_p > kEps) { st.alpha = 0.0; st.beta = 1.0; }        // :277-281
+    else if (st.rng_p <= kEps && st.rng_t > kEps) { st.alpha = 1.0; st.beta = 0.0; }
+    return n;
+}
+
+// One latency profile for one request: the chain, scores, and the first max(1, k) endpoints in picker order (the
+// contract of gen::eval, over the final set).
+template <bool kRand, typename CntOf>
+__device__ inline Best eval(const ProfileDev &pf, const epp_latency_cfg &lc, const GenView &g, const Req &q, int32_t E,
+                            int32_t total, int lane, const LoraDev &lora, uint32_t adapter, uint64_t seed, uint64_t key,
+                            CntOf cnt_of, int32_t k, uint32_t *picks_row, double *scores_row) {
+    Best first;
+    best_init(first);
+    if (k < 1) k = 1;
+    if (picks_row) for (int j = lane; j < k; j += 32) picks_row[j] = EPP_NO_ENDPOINT;
+    if (scores_row) for (int j = lane; j < k; j += 32) scores_row[j] = 0.0;
+    __syncwarp();
+    if (*pf.n_cand == 0) return first;
+    State st;
+    const uint32_t n = prepare(pf, lc, g, q, E, total, lane, seed, key, cnt_of, st);
+    const bool use_lora = lora.enabled && lora.ptr;
+    auto cand = [&](uint32_t e) {
+        if (!pf.cand[e]) return false;
+        if (st.a1 && !gen::is_sticky(cnt_of(e), total, lc.a1_affinity_threshold)) return false;
+        if (st.tier != kTierAll) {
+            const epp_prediction *p = q.find(e);
+            if ((st.tier == kTierPos) != (p && meets(p))) return false;
+        }
+        return !st.a2 || gen::is_sticky(cnt_of(e), total, pf.cfg.affinity_threshold);
+    };
+    auto score = [&](uint32_t e) {
+        const int ls = use_lora ? lora_lookup(lora, adapter, e) : 0;
+        return weighted_sum(pf, g, st, e, q.find(e), cnt_of(e), total, lora, ls);
+    };
+    if (kRand && pf.cfg.picker) {     // random pickers: every member is an explicit item
+        uint32_t g0 = EPP_NO_ENDPOINT, g1 = EPP_NO_ENDPOINT;
+        for (int32_t j = 0; j < k && (uint32_t)j < n; j++) {
+            auto out_of = [&](uint32_t e) {
+                bool o = false;
+                for (int32_t t = 0; t < j; t++)
+                    o |= e == __shfl_sync(gen::kFull, t < 32 ? g0 : g1, t & 31);
+                return o;
+            };
+            const Best b = rnd::draw_scan(pf, E, lane, false, n - (uint32_t)j, (uint32_t)j, seed + (uint64_t)j * gen::kGolden,
+                                          key, cand, [](uint32_t) { return true; }, score, out_of);
+            if (j == 0) first = b;
+            if (lane == (j & 31)) { if (j < 32) g0 = b.pick; else g1 = b.pick; }
+            if (lane == 0) {
+                if (picks_row) picks_row[j] = b.pick;
+                if (scores_row) scores_row[j] = b.val;
+            }
+        }
+        return first;
+    }
+    double v = 0.0;
+    bool have_v = false;
+    uint32_t n_rem = 0;
+    uint32_t g0 = EPP_NO_ENDPOINT, g1 = EPP_NO_ENDPOINT;
+    uint32_t n_taken = 0;
+    for (int32_t j = 0; j < k; j++) {
+        if (n_rem == 0) {
+            Best b;
+            best_init(b);
+            for (uint32_t e = lane; e < (uint32_t)E; e += 32) {
+                if (!cand(e)) continue;
+                const double sc = score(e);
+                if (!have_v || sc < v) best_add(b, sc, e);
+            }
+            b = best_warp_reduce(b);
+            if (!b.ties) break;
+            v = b.val;
+            have_v = true;
+            n_rem = b.ties;
+            n_taken = 0;
+            g0 = g1 = EPP_NO_ENDPOINT;
+            if (j == 0) first = b;
+        }
+        uint32_t rank = seed ? tie_rank(seed + (uint64_t)j * gen::kGolden, key, n_rem) : 0u;
+        uint32_t pick = EPP_NO_ENDPOINT;
+        for (uint32_t e0 = 0; e0 < (uint32_t)E && pick == EPP_NO_ENDPOINT; e0 += 32) {
+            const uint32_t e = e0 + lane;
+            bool hit = e < (uint32_t)E && cand(e) && score(e) == v;
+            if (n_taken && __any_sync(gen::kFull, hit))
+                for (uint32_t t = 0; t < n_taken; t++) {
+                    const uint32_t te = __shfl_sync(gen::kFull, t < 32 ? g0 : g1, (int)(t & 31));
+                    if (te == e) hit = false;
+                }
+            uint32_t bal = __ballot_sync(gen::kFull, hit);
+            const uint32_t cnt = __popc(bal);
+            if (rank < cnt) {
+                for (uint32_t i = 0; i < rank; i++) bal &= bal - 1;
+                pick = e0 + (uint32_t)__ffs(bal) - 1u;
+            } else {
+                rank -= cnt;
+            }
+        }
+        if (pick == EPP_NO_ENDPOINT) break;
+        if (lane == (int)(n_taken & 31)) { if (n_taken < 32) g0 = pick; else g1 = pick; }
+        n_taken++;
+        n_rem--;
+        if (j == 0) first.pick = pick;
+        if (lane == 0) {
+            if (picks_row) picks_row[j] = pick;
+            if (scores_row) scores_row[j] = v;
+        }
+    }
+    return first;
+}
+
+}  // namespace lat
+}  // namespace epp

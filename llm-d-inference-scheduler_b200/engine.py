@@ -55,6 +55,7 @@ class ProfileSpec:
     affinity: AffinityFilterSpec | None = None
     picker: int = capi.PICKER_MAX_SCORE
     labels: list = field(default_factory=list)
+    latency: dict | None = None      # Engine.latency_profile_set fields of a profile with a latency piece, or None
 
 
 def _fill_profile(dst: capi.ProfileCfg, spec: ProfileSpec):
@@ -111,6 +112,57 @@ def pack_subsets(subsets):
     return counts, offsets, np.ascontiguousarray(slots, dtype=np.uint32)
 
 
+PREDICTION_DTYPE = np.dtype([("slot", "<u4"), ("dispatched", "<i4"), ("ttft", "<f8"), ("ttft_headroom", "<f8"),
+                             ("tpot_headroom", "<f8")])
+assert PREDICTION_DTYPE.itemsize == C.sizeof(capi.Prediction)
+
+
+def pack_predictions(predictions):
+    """Per-request latency predictions -> the host arrays of epp_predictions: (counts u32 [R], offsets u64 [R], entries
+    [n] of PREDICTION_DTYPE).  Entry r is None (no predictions) or an iterable of (slot, ttft, ttft_headroom,
+    tpot_headroom, dispatched) -- LatencyPredictionInfo's TTFT(), TTFTHeadroom(), TPOTHeadroom() and
+    DispatchedRequestCount() on that slot for request r, or an array of PREDICTION_DTYPE.  Entries are sorted by slot here;
+    a slot given twice is an error."""
+    R = len(predictions)
+    counts = np.zeros(R, dtype=np.uint32)
+    offsets = np.zeros(R, dtype=np.uint64)
+    parts, n = [], 0
+    for r, p in enumerate(predictions):
+        offsets[r] = n
+        if p is None:
+            continue
+        if isinstance(p, np.ndarray) and p.dtype == PREDICTION_DTYPE:
+            a = np.sort(p, order="slot", kind="stable")
+            if a.size > 1 and (np.diff(a["slot"].astype(np.int64)) == 0).any():
+                raise ValueError(f"request {r}: a slot has two predictions")
+            if a.size and a["slot"][-1] == 0xFFFFFFFF:
+                raise ValueError(f"request {r}: slot id out of range")
+            counts[r] = a.size
+            parts.append(a)
+            n += a.size
+            continue
+        rows = sorted((int(sl), float(t), float(th), float(tp), int(d)) for sl, t, th, tp, d in p)
+        a = np.zeros(len(rows), dtype=PREDICTION_DTYPE)
+        for i, (sl, t, th, tp, d) in enumerate(rows):
+            if sl < 0 or sl > 0xFFFFFFFE:
+                raise ValueError(f"request {r}: slot id {sl} out of range")
+            if i and sl == rows[i - 1][0]:
+                raise ValueError(f"request {r}: slot {sl} has two predictions")
+            a[i] = (sl, d, t, th, tp)
+        counts[r] = len(rows)
+        parts.append(a)
+        n += len(rows)
+    entries = np.concatenate(parts) if parts else np.zeros(0, dtype=PREDICTION_DTYPE)
+    return counts, offsets, np.ascontiguousarray(entries)
+
+
+def _predictions_struct(packed):
+    p = capi.Predictions()
+    p.struct_size = C.sizeof(capi.Predictions)
+    p.counts, p.offsets, p.entries = (_ptr(a) for a in packed)
+    return p
+
+
 class Engine:
     def __init__(self, max_endpoints: int, primary: ProfileSpec | None = None, prefill: ProfileSpec | None = None,
                  *, device: int = 0, block_size_tokens: int = 16, max_prefix_blocks: int = 256,
@@ -148,6 +200,8 @@ class Engine:
         for p, spec in enumerate((primary, prefill, encode)):
             if spec is not None and spec.labels:
                 self.label_filters_set(p, spec.labels)
+            if spec is not None and spec.latency is not None:
+                self.latency_profile_set(p, **spec.latency)
 
     # ---- plumbing ----
     def _check(self, rc: int):
@@ -377,14 +431,32 @@ class Engine:
         text = np.frombuffer(b"".join(parts) or b"\0", dtype=np.uint8)
         self._check(self._lib.epp_pool_set_labels(self._h, ids.shape[0], _ptr(ids), _ptr(offs), _ptr(text)))
 
+    def latency_profile_set(self, profile: int, **fields):
+        """The latency configuration of profile 0 (primary / decode), 1 (prefill) or 2 (encode): the epp_latency_cfg
+        fields given as keywords (tier_filter, epsilon_explore_neg, a1_affinity_threshold, a1_exploration_probability,
+        a1_max_ttft_penalty_ms, ttft_weight, tpot_weight, strategy, composite_kv_weight, composite_queue_weight,
+        composite_prefix_weight), the others at the reference's defaults (include/epp_engine.h "Latency predictions").
+        Only before the first pool_set / pool_set_labels."""
+        cfg = capi.LatencyCfg()
+        self._lib.epp_latency_cfg_default(C.byref(cfg))
+        names = {n for n, _ in capi.LatencyCfg._fields_} - {"struct_size", "reserved"}
+        for k, v in fields.items():
+            if k not in names:
+                raise TypeError(f"unknown latency configuration field {k!r}")
+            setattr(cfg, k, v)
+        self._check(self._lib.epp_latency_profile_set(self._h, profile, C.byref(cfg)))
+
     def schedule(self, data, offsets=None, uniform_len=None, model_ids=None, n_requests=None, keep_hashes=False,
-                 detail=True, out=None, lengths=None, asynchronous=False, multimodal=None, topk=False, subsets=None):
+                 detail=True, out=None, lengths=None, asynchronous=False, multimodal=None, topk=False, subsets=None,
+                 predictions=None):
         """a1-a14 Scheduler.Schedule for a batch -> (decisions, details).  asynchronous=True (CUDA tensors only)
         enqueues the batch and returns; the outputs are complete after synchronize().  topk=True (engines created with
         pick_k > 1) also returns the dict of the pickers' first-k lists (maxscore/picker.go:104-115): "primary",
         "primary_scores", "prefill", "encode", each [R][pick_k], padded with EPP_NO_ENDPOINT / 0.
         subsets: None, or a list of R entries, each None (the whole pool) or a sequence of slot ids: the request's
-        candidates (the gateway's endpoint subset, include/epp_engine.h "Endpoint subsets"); epp_schedule_subset."""
+        candidates (the gateway's endpoint subset, include/epp_engine.h "Endpoint subsets"); epp_schedule_subset.
+        predictions: None, or a list of R entries in the form pack_predictions takes (include/epp_engine.h "Latency
+        predictions"); epp_schedule_predicted."""
         b, R, dev, keep = self._batch(data, offsets, uniform_len, model_ids, n_requests, lengths, multimodal)
         if asynchronous:
             b.flags |= capi.EPP_BATCH_ASYNC
@@ -396,7 +468,16 @@ class Engine:
             dec = np.zeros(R, dtype=DECISION_DTYPE) if out is None else out
             det = np.zeros(R, dtype=DETAIL_DTYPE) if detail else None
         lists, tk = self._topk_out(R, data.device if dev else None) if topk else (None, None)
-        if subsets is not None:
+        if predictions is not None:
+            if len(predictions) != R:
+                raise ValueError(f"predictions has {len(predictions)} entries for {R} requests")
+            if subsets is not None:
+                raise ValueError("subsets and predictions cannot be combined")
+            packed = pack_predictions(predictions)      # host arrays, kept alive until the call returns
+            pr = _predictions_struct(packed)
+            self._check(self._lib.epp_schedule_predicted(self._h, C.byref(b), C.byref(pr), _ptr(dec), _ptr(det),
+                                                         int(keep_hashes), C.byref(tk) if topk else None))
+        elif subsets is not None:
             if len(subsets) != R:
                 raise ValueError(f"subsets has {len(subsets)} entries for {R} requests")
             packed = pack_subsets(subsets)              # host arrays, kept alive until the call returns
@@ -430,7 +511,7 @@ class Engine:
         return lists, tk
 
     def schedule_with_match(self, match, total, input_len_bytes=None, block_size_tokens: int = 0, model_ids=None,
-                            topk=False):
+                            topk=False, predictions=None):
         match = np.ascontiguousarray(match, dtype=np.int32).reshape(-1, self.E)
         total = np.ascontiguousarray(total, dtype=np.int32)
         R = match.shape[0]
@@ -438,6 +519,16 @@ class Engine:
         dec = np.zeros(R, dtype=DECISION_DTYPE)
         det = np.zeros(R, dtype=DETAIL_DTYPE)
         mids = None if model_ids is None else np.ascontiguousarray(model_ids, dtype=np.uint32)
+        if predictions is not None:
+            if len(predictions) != R:
+                raise ValueError(f"predictions has {len(predictions)} entries for {R} requests")
+            packed = pack_predictions(predictions)
+            pr = _predictions_struct(packed)
+            lists, tk = self._topk_out(R) if topk else (None, None)
+            self._check(self._lib.epp_schedule_with_match_predicted(
+                self._h, R, _ptr(match), _ptr(total), _ptr(mids), _ptr(il), block_size_tokens, _ptr(dec), _ptr(det), 0,
+                C.byref(tk) if topk else None, C.byref(pr)))
+            return (dec, det, lists) if topk else (dec, det)
         if not topk:
             self._check(self._lib.epp_schedule_with_match(self._h, R, _ptr(match), _ptr(total), _ptr(mids), _ptr(il),
                                                           block_size_tokens, _ptr(dec), _ptr(det), 0))
@@ -527,13 +618,27 @@ class Batcher:
         if rc != 0:
             raise EngineError(rc, (self._lib.epp_batcher_last_error() or b"").decode())
 
-    def submit(self, prompt, model_id: int = 0, multimodal: bool = False, subset=None) -> int:
-        """subset: None (the whole pool) or a sequence of slot ids, the request's candidates (epp_submit_subset)."""
+    def submit(self, prompt, model_id: int = 0, multimodal: bool = False, subset=None, predictions=None) -> int:
+        """subset: None (the whole pool) or a sequence of slot ids, the request's candidates (epp_submit_subset).
+        predictions: None or the request's entries in the form pack_predictions takes (epp_submit_predicted)."""
         buf = np.ascontiguousarray(prompt).view(np.uint8).reshape(-1) if not isinstance(prompt, (bytes, bytearray)) else prompt
         n = len(buf)
         ptr = buf.ctypes.data_as(C.c_void_p) if isinstance(buf, np.ndarray) else C.cast(C.c_char_p(bytes(buf)), C.c_void_p)
         t = C.c_uint64()
-        if subset is None:
+        if predictions is not None:
+            if subset is not None:
+                raise ValueError("subsets and predictions cannot be combined")
+            if isinstance(predictions, np.ndarray) and predictions.dtype == PREDICTION_DTYPE:
+                ent = np.ascontiguousarray(predictions)
+            else:
+                ent = np.zeros(len(predictions), dtype=PREDICTION_DTYPE)
+            for i, (sl, tt, th, tp, d) in enumerate(() if ent is predictions else predictions):
+                if not 0 <= int(sl) <= 0xFFFFFFFE:
+                    raise ValueError(f"slot id {sl} out of range")
+                ent[i] = (int(sl), int(d), float(tt), float(th), float(tp))
+            self._check(self._lib.epp_submit_predicted(self._b, model_id, ptr, n, int(multimodal), ent.shape[0], _ptr(ent),
+                                                       C.byref(t)))
+        elif subset is None:
             self._check(self._lib.epp_submit(self._b, model_id, ptr, n, int(multimodal), C.byref(t)))
         else:
             sl = np.ascontiguousarray(np.asarray(subset, dtype=np.uint32).reshape(-1))

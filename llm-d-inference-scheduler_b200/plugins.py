@@ -12,6 +12,9 @@ Reference interfaces mirrored (paths relative to the reference root):
   prefix-cache-affinity-filter                            .../filter/prefixcacheaffinity/plugin.go:45-151
   label-selector-filter / by-label-selector / by-label    .../filter/bylabel/selector.go:34-101, filter.go:34-117
   approximateprefix dataProducer Produce / PreRequest     .../approximateprefix/plugin.go:135-200
+  LatencyPredictionInfo (LatencyPredictionInfoKey)        .../datalayer/attribute/latency/data_types.go:23-96
+  slo-headroom-tier-filter                                .../filter/sloheadroomtier/plugin.go:43-73
+  latency-scorer                                          .../scorer/latency/plugin.go:59-125
 """
 from __future__ import annotations
 
@@ -326,6 +329,134 @@ def ByLabelFactory(name: str, rawParameters):
     return NewByLabel(name, label, allows, *values)
 
 
+# ---- latency predictions (include/epp_engine.h "Latency predictions") ----
+LatencyPredictionInfoKey = "LatencyPredictionInfoKey"        # attribute/latency/data_types.go:24
+
+
+class LatencyPredictionInfo:                     # attribute/latency/data_types.go:36-80
+    def __init__(self, ttftValid, tpotValid, ttftHeadroom, tpotHeadroom, ttft, tpot, dispatchedRequestCount):
+        self._ttft_valid, self._tpot_valid = bool(ttftValid), bool(tpotValid)
+        self._ttft_headroom, self._tpot_headroom = float(ttftHeadroom), float(tpotHeadroom)
+        self._ttft, self._tpot = float(ttft), float(tpot)
+        self._dispatched = int(dispatchedRequestCount)
+
+    def TTFTValid(self): return self._ttft_valid
+    def TPOTValid(self): return self._tpot_valid
+    def IsValid(self): return self._ttft_valid and self._tpot_valid
+    def TTFTHeadroom(self): return self._ttft_headroom
+    def TPOTHeadroom(self): return self._tpot_headroom
+    def TTFT(self): return self._ttft
+    def TPOT(self): return self._tpot
+    def DispatchedRequestCount(self): return self._dispatched
+
+    def entry(self, slot: int):
+        """The engine's prediction entry (slot, ttft, ttft_headroom, tpot_headroom, dispatched): the four values the
+        plugins read."""
+        return (slot, self._ttft, self._ttft_headroom, self._tpot_headroom, self._dispatched)
+
+
+def NewLatencyPredictionInfo(ttftValid, tpotValid, ttftHeadroom, tpotHeadroom, ttft, tpot, dispatchedRequestCount):
+    return LatencyPredictionInfo(ttftValid, tpotValid, ttftHeadroom, tpotHeadroom, ttft, tpot, dispatchedRequestCount)
+
+
+def _unmarshal(raw, fields: dict, type_name: str) -> dict:
+    """json.Unmarshal of rawParameters into a Config struct: keys match field names case-insensitively, unknown keys
+    are ignored, null leaves the defaults, a value of the wrong JSON type is an error.  fields: json name -> float / str."""
+    if raw is None:
+        return {}
+    if isinstance(raw, (str, bytes, bytearray)):
+        if len(raw) == 0:
+            return {}
+        try:
+            raw = json.loads(raw)
+        except json.JSONDecodeError as e:
+            raise ValueError(f"failed to unmarshal config: {e}") from e
+    if raw is None:
+        return {}
+    if not isinstance(raw, dict):
+        raise ValueError(f"failed to unmarshal config: json: cannot unmarshal {type(raw).__name__} into Go value of type "
+                         f"{type_name}")
+    out = {}
+    lower = {k.lower(): k for k in fields}
+    for k, v in raw.items():
+        name = lower.get(k.lower())
+        if name is None or v is None:
+            continue
+        want = fields[name]
+        ok = isinstance(v, str) if want is str else (isinstance(v, (int, float)) and not isinstance(v, bool))
+        if not ok:
+            raise ValueError(f"failed to unmarshal config: json: cannot unmarshal {type(v).__name__} into Go struct field "
+                             f"Config.{name} of type {'string' if want is str else 'float64'}")
+        out[name] = want(v)
+    return out
+
+
+SLOHeadroomTierFilterType = "slo-headroom-tier-filter"
+
+
+@dataclass
+class SLOHeadroomTierFilter:                     # filter/sloheadroomtier; DefaultConfig :50-52
+    epsilonExploreNeg: float = 0.01
+    name: str = SLOHeadroomTierFilterType
+
+
+def SLOHeadroomTierFilterFactory(name: str, rawParameters=None):
+    """ "slo-headroom-tier-filter" (plugin.go:59-73): rawParameters is JSON text, bytes, a dict or None."""
+    cfg = _unmarshal(rawParameters, {"epsilonExploreNeg": float}, "sloheadroomtier.Config")
+    eps = cfg.get("epsilonExploreNeg", 0.01)
+    if eps < 0 or eps > 1.0:
+        raise ValueError(f"epsilonExploreNeg must be in [0, 1], got {eps:f}")
+    return SLOHeadroomTierFilter(eps, name)
+
+
+LatencyScorerType = "latency-scorer"
+
+
+@dataclass
+class LatencyScorerConfig:                       # scorer/latency Config; DefaultConfig :83-90
+    ttftWeight: float = 0.8
+    tpotWeight: float = 0.2
+    headroomSelectionStrategy: str = "least"
+    compositeKVWeight: float = 1.0
+    compositeQueueWeight: float = 1.0
+    compositePrefixWeight: float = 1.0
+
+
+@dataclass
+class _LatencyScorer(_Scorer):
+    config: LatencyScorerConfig = field(default_factory=LatencyScorerConfig)
+
+
+def NewLatencyScorer(config: LatencyScorerConfig | None = None, name: str = LatencyScorerType):    # NewPlugin, :107-112
+    return _LatencyScorer(capi.SCORER_LATENCY, 0.0, name, config=config or LatencyScorerConfig())
+
+
+def LatencyScorerFactory(name: str, rawParameters=None):
+    """ "latency-scorer" (plugin.go:114-125).  A strategy other than "most" scores as "least" (the switch's default,
+    :303-310)."""
+    cfg = _unmarshal(rawParameters, {"ttftWeight": float, "tpotWeight": float, "headroomSelectionStrategy": str,
+                                     "compositeKVWeight": float, "compositeQueueWeight": float,
+                                     "compositePrefixWeight": float}, "latency.Config")
+    return NewLatencyScorer(LatencyScorerConfig(**cfg), name)
+
+
+def _latency_fields(tier, a1, scorer) -> dict:
+    """Engine.latency_profile_set fields of a profile's tier filter, first affinity filter and latency scorer."""
+    f = {}
+    if tier is not None:
+        f.update(tier_filter=1, epsilon_explore_neg=tier.epsilonExploreNeg)
+    if a1 is not None:
+        f.update(a1_affinity_threshold=a1.affinityThreshold, a1_exploration_probability=a1.explorationProbability,
+                 a1_max_ttft_penalty_ms=a1.maxTTFTPenaltyMs)
+    if scorer is not None:
+        c = scorer.config
+        f.update(ttft_weight=c.ttftWeight, tpot_weight=c.tpotWeight,
+                 strategy=capi.HEADROOM_MOST if c.headroomSelectionStrategy == "most" else capi.HEADROOM_LEAST,
+                 composite_kv_weight=c.compositeKVWeight, composite_queue_weight=c.compositeQueueWeight,
+                 composite_prefix_weight=c.compositePrefixWeight)
+    return f
+
+
 @dataclass
 class PrefixCacheAffinityFilter:                 # filter/prefixcacheaffinity "prefix-cache-affinity-filter"; DefaultConfig :62-66
     affinityThreshold: float = 0.80
@@ -390,7 +521,7 @@ class SchedulerProfile:
         for p in plugins:
             if isinstance(p, WeightedScorer):
                 self.scorers.append(p)
-            elif isinstance(p, (_RoleFilter, _LabelFilter, PrefixCacheAffinityFilter)):
+            elif isinstance(p, (_RoleFilter, _LabelFilter, PrefixCacheAffinityFilter, SLOHeadroomTierFilter)):
                 _check_chain(self.filters + [p])
                 self.filters.append(p)
             elif isinstance(p, (MaxScorePicker, RandomPicker, WeightedRandomPicker)):
@@ -403,29 +534,60 @@ class SchedulerProfile:
         return self
 
     def spec(self) -> ProfileSpec:
+        """The engine profile: the affinity filter after the tier filter (or the only one) is the profile's own; one
+        before the tier filter, the tier filter and a latency scorer go into ProfileSpec.latency."""
         roles = [f for f in self.filters if isinstance(f, _RoleFilter)]
-        aff = [f for f in self.filters if isinstance(f, PrefixCacheAffinityFilter)]
+        tier_at = [i for i, f in enumerate(self.filters) if isinstance(f, SLOHeadroomTierFilter)]
+        affs = [(i, f) for i, f in enumerate(self.filters) if isinstance(f, PrefixCacheAffinityFilter)]
+        a1 = next((f for i, f in affs if tier_at and i < tier_at[0]), None)
+        a2 = [f for i, f in affs if not tier_at or i > tier_at[0]]
+        lat_scorers = [ws.scorer for ws in self.scorers if isinstance(ws.scorer, _LatencyScorer)]
+        assert len(lat_scorers) <= 1, "at most one latency-scorer per profile"
+        tier = self.filters[tier_at[0]] if tier_at else None
+        latency = None
+        if tier is not None or lat_scorers:
+            latency = _latency_fields(tier, a1, lat_scorers[0] if lat_scorers else None)
+            if a2:
+                assert a2[0].ttft_column < 0, "a latency profile reads TTFT from the predictions, not from an ext column"
         return ProfileSpec(roles[0].kind if roles else capi.FILTER_NONE,
                            [ScorerSpec(ws.scorer.kind, ws.weight, ws.scorer.param, ws.scorer.column, ws.scorer.param2)
                             for ws in self.scorers],
-                           AffinityFilterSpec(aff[0].affinityThreshold, aff[0].explorationProbability,
-                                              aff[0].maxTTFTPenaltyMs, aff[0].ttft_column) if aff else None,
+                           AffinityFilterSpec(a2[0].affinityThreshold, a2[0].explorationProbability,
+                                              a2[0].maxTTFTPenaltyMs, a2[0].ttft_column) if a2 else None,
                            _PICKER_KIND[type(self.picker)],
-                           [q for f in self.filters if isinstance(f, _LabelFilter) for q in f.reqs])
+                           [q for f in self.filters if isinstance(f, _LabelFilter) for q in f.reqs],
+                           latency)
 
 
 def _check_chain(filters):
     """A profile's filter chain: label filters (any number) and at most one role filter, in any order (pure per-endpoint
     predicates, so their order does not matter), then at most one prefix-cache-affinity-filter, last: it depends on
-    the set it receives."""
+    the set it receives.  With a slo-headroom-tier-filter the chain is [role + labels] -> [affinity] -> tier ->
+    [affinity] (include/epp_engine.h "Latency predictions")."""
     filters = list(filters)
     roles = [f for f in filters if isinstance(f, _RoleFilter)]
     aff = [i for i, f in enumerate(filters) if isinstance(f, PrefixCacheAffinityFilter)]
-    assert all(isinstance(f, (_RoleFilter, _LabelFilter, PrefixCacheAffinityFilter)) for f in filters), \
-        "a profile's filters are role filters, label filters and the prefix-cache-affinity-filter"
+    tier = [i for i, f in enumerate(filters) if isinstance(f, SLOHeadroomTierFilter)]
+    assert all(isinstance(f, (_RoleFilter, _LabelFilter, PrefixCacheAffinityFilter, SLOHeadroomTierFilter))
+               for f in filters), \
+        "a profile's filters are role filters, label filters, the prefix-cache-affinity-filter and the " \
+        "slo-headroom-tier-filter"
     assert len(roles) <= 1, "at most one role filter per profile"
-    assert len(aff) <= 1 and (not aff or aff[0] == len(filters) - 1), \
-        "the prefix-cache-affinity-filter comes last: no filter may follow it"
+    assert len(tier) <= 1, "at most one slo-headroom-tier-filter per profile"
+    if tier:
+        t = tier[0]
+        before = [i for i in aff if i < t]
+        after = [i for i in aff if i > t]
+        assert len(before) <= 1 and (not before or before[0] == t - 1), \
+            "an affinity filter before the slo-headroom-tier-filter comes right before it"
+        assert all(isinstance(f, (_RoleFilter, _LabelFilter)) for f in filters[:t - len(before)]), \
+            "role and label filters come before the affinity and tier filters"
+        assert len(after) <= 1 and (not after or after[0] == len(filters) - 1) and \
+            all(i in after for i in range(t + 1, len(filters))), \
+            "only one prefix-cache-affinity-filter may follow the slo-headroom-tier-filter"
+    else:
+        assert len(aff) <= 1 and (not aff or aff[0] == len(filters) - 1), \
+            "the prefix-cache-affinity-filter comes last: no filter may follow it"
     n = sum(len(f.reqs) for f in filters if isinstance(f, _LabelFilter))
     assert n <= capi.EPP_LABEL_MAX_REQS, f"{n} label requirements, at most {capi.EPP_LABEL_MAX_REQS} per profile"
 
@@ -515,6 +677,7 @@ class Scheduler:
                              n_ext_cols=ext_columns, tie_seed=tie_seed, pick_k=self.pick_k, inflight_load=inflight_load)
         self.block_size_tokens = block_size_tokens
         self.has_labels = any(p.spec().labels for p in profiles.values())
+        self.has_latency = any(p.spec().latency is not None for p in profiles.values())
 
     def _push_pool(self, endpoints, ext=None):
         n = len(endpoints)
@@ -525,7 +688,9 @@ class Scheduler:
         if self.has_labels:
             self.engine.pool_set_labels(np.arange(n, dtype=np.uint32), [e.metadata.Labels for e in endpoints])
 
-    def Schedule(self, requests, candidateEndpoints, ext=None):
+    def Schedule(self, requests, candidateEndpoints, ext=None, predictions=None):
+        """predictions: None (each endpoint's LatencyPredictionInfoKey attribute, the same for every request), or one
+        entry per request, each a dict endpoint index -> LatencyPredictionInfo (the producer's per-request output)."""
         single = isinstance(requests, InferenceRequest)
         reqs = [requests] if single else list(requests)
         eps = list(candidateEndpoints)
@@ -543,10 +708,22 @@ class Scheduler:
                 total[:] = info.TotalBlocks()
                 bst = info.BlockSizeTokens()
         in_len = np.array([len(r.Prompt) for r in reqs], dtype=np.int64)
+        preds = None
+        if predictions is not None:
+            if single:
+                predictions = [predictions]
+            assert len(predictions) == len(reqs), "one predictions entry per request"
+            preds = [None if p is None else [info.entry(i) for i, info in sorted(p.items())] for p in predictions]
+        elif self.has_latency:
+            attrs = [(i, ep.Get(LatencyPredictionInfoKey)) for i, ep in enumerate(eps)]
+            row = [info.entry(i) for i, (info, ok) in attrs if ok and info is not None]
+            preds = [row] * len(reqs)
+        if preds is not None and not self.has_latency:
+            raise SchedulingError("latency predictions need a profile with a latency-scorer or slo-headroom-tier-filter")
         if self.pick_k > 1:
-            dec, det, lists = self.engine.schedule_with_match(match, total, in_len, bst, topk=True)
+            dec, det, lists = self.engine.schedule_with_match(match, total, in_len, bst, topk=True, predictions=preds)
         else:
-            dec, det = self.engine.schedule_with_match(match, total, in_len, bst)
+            dec, det = self.engine.schedule_with_match(match, total, in_len, bst, predictions=preds)
             lists = {"primary": dec["pick"].reshape(-1, 1), "prefill": dec["prefill_pick"].reshape(-1, 1)}
         out = [self._result(dec[i], det[i], eps, lists["primary"][i], lists["prefill"][i]) for i in range(len(reqs))]
         return out[0] if single else out
