@@ -664,6 +664,32 @@ EPP_API int32_t epp_shard_pick(epp_engine *h, int64_t n_requests, const uint32_t
 EPP_API int32_t epp_shard_merge(epp_engine *h, int64_t n_requests, int32_t n_ranks, const epp_shard_best *all_best,
                         epp_decision *out);
 
+/* Staged records: the disagg profile handler (decode -> P/D decider -> prefill, with the optional encode stage) in the
+ * endpoint-sharded mode, with the same three phases and two exchanges.  epp_shard_set_staged does what epp_shard_set does,
+ * also accepts EPP_HANDLER_DISAGG (with or without encode_enabled) and returns S in *out_stages: 1 for the single-profile
+ * handler, 2 for decode + prefill, 3 with the encode profile.  Every other refusal of epp_shard_set stays.
+ * epp_shard_pick then writes S records per request, request-major ([R][S]: stage 0 decode, 1 prefill, 2 encode), so the
+ * all-gather yields [n_ranks][R][S] and epp_shard_merge(_detail) reads that.  For request r on one rank:
+ *   stage 0  the local best decode record (as with one stage);
+ *   stage 1  the local best prefill record whenever the P/D decider can still say yes, i.e. always_disagg, or
+ *            non_cached_tokens != 0 and (request bytes / 4) >= non_cached_tokens -- whether it runs depends on the merged
+ *            decode pick's match_blocks, which no rank knows yet; it is evaluated even when this rank has no decode
+ *            candidate; status -1 otherwise;
+ *   stage 2  the local best encode record for multimodal requests, status -1 otherwise.
+ * The merge reduces each stage alone (max score, lowest slot id among equals, ties summed), then applies the handler as
+ * epp_schedule does: no decode pick anywhere -> status -1 and no other stage; encode_ran = multimodal[r]; prefill_ran =
+ * always_disagg || the P/D decider on the merged decode pick's match_blocks; the stage fields come from the reduced
+ * records (EPP_NO_ENDPOINT when no rank has one).  The request lengths (lengths[r] when given, the decider's input) and
+ * multimodal flags are the engine's own copies, kept by epp_shard_probe.  On a peer-memory engine epp_shard_set_staged
+ * must come before epp_shard_p2p_export: the buffer holds max_requests * S records, and a call after an export made for
+ * another S is EPP_ERR_STATE.
+ * out_detail ([R] device, or NULL) receives the prefill and encode fields; with an encode profile and a batch that flags
+ * multimodal requests it must not be NULL (EPP_ERR_INVALID), as in epp_schedule.  epp_shard_merge, epp_shard_schedule_p2p
+ * and epp_shard_p2p_phase are these calls with out_detail = NULL. */
+EPP_API int32_t epp_shard_set_staged(epp_engine *h, uint32_t ep_begin, uint32_t ep_end, int32_t *out_stages);
+EPP_API int32_t epp_shard_merge_detail(epp_engine *h, int64_t n_requests, int32_t n_ranks, const epp_shard_best *all_best,
+                                       epp_decision *out, epp_decision_detail *out_detail);
+
 /* The same protocol with both exchanges done by the ranks' own kernels over NVLink PEER MEMORY (no NCCL): every rank
  * exports one exchange buffer (CUDA IPC handle, 64 bytes; out_ptr is the raw device pointer for ranks that share a
  * process), connects to all peers' buffers (peers: n_ranks x 64-byte handles when ipc_handles != 0, else n_ranks
@@ -680,6 +706,12 @@ EPP_API int32_t epp_shard_schedule_p2p(epp_engine *h, const epp_batch *batch, ep
  * A peer that times out (or whose flags are poisoned) breaks the exchange for good: every later call fails with
  * EPP_ERR_STATE until epp_shard_p2p_export / _connect are called again on every rank. */
 EPP_API int32_t epp_shard_p2p_phase(epp_engine *h, const epp_batch *batch, epp_decision *out, int32_t phase);
+/* The two calls above with the detail of the staged records (see "Staged records"); the batch's multimodal flags are a
+ * device array. */
+EPP_API int32_t epp_shard_schedule_p2p_detail(epp_engine *h, const epp_batch *batch, epp_decision *out,
+                                              epp_decision_detail *out_detail);
+EPP_API int32_t epp_shard_p2p_phase_detail(epp_engine *h, const epp_batch *batch, epp_decision *out,
+                                           epp_decision_detail *out_detail, int32_t phase);
 
 /* The configuration the engine was created with. */
 EPP_API int32_t epp_get_config(epp_engine *h, epp_config *out);

@@ -228,10 +228,13 @@ struct epp_engine {
     int64_t kept_R = 0;             // rows of `hashes` valid for epp_index_add_picked
     int64_t shard_R = 0;            // rows of `hashes` valid for epp_shard_pick / epp_shard_merge
     bool shard_models = false;      // the probed batch had model ids: its copy in `model_ids` feeds epp_shard_pick
+    bool shard_mm = false;          // the probed batch had multimodal flags: its copy in `multimodal` feeds pick and merge
+    int32_t shard_stages = 1;       // records per request of the sharded protocol (epp_shard_set_staged)
     // endpoint-sharded mode over NVLink peer memory (shard_p2p.cu)
     void *p2p_buf = nullptr;        // this rank's exchange buffer {flags, masks, records} (cudaMalloc, IPC-exported)
     size_t p2p_bytes = 0, p2p_masks_off = 0, p2p_best_off = 0;
     int64_t p2p_R = 0;              // requests the buffer was sized for
+    int32_t p2p_stages = 1;         // records per request the buffer was sized for
     int p2p_ranks = 0, p2p_rank = 0;
     bool p2p_ipc = false;
     std::vector<void *> p2p_peer;   // peers' buffers in this process's address space (own buffer at [p2p_rank])
@@ -2721,16 +2724,31 @@ static int32_t check_shardable(const epp_engine *h) {
     return EPP_OK;
 }
 
-extern "C" int32_t epp_shard_set(epp_engine *h, uint32_t ep_begin, uint32_t ep_end) {
+// epp_shard_set (staged == false: the single-profile handler only) and epp_shard_set_staged.
+static int32_t shard_set(epp_engine *h, uint32_t ep_begin, uint32_t ep_end, bool staged, int32_t *out_stages) {
     if (!h || ep_begin > ep_end) return fail(EPP_ERR_INVALID, "bad shard range");
     std::lock_guard<std::mutex> lk(h->mu);
-    if (h->cfg.handler != EPP_HANDLER_SINGLE) return fail(EPP_ERR_INVALID, "endpoint-sharded mode supports the single-profile handler only");
+    if (!staged && h->cfg.handler != EPP_HANDLER_SINGLE) return fail(EPP_ERR_INVALID, "endpoint-sharded mode supports the single-profile handler only");
     if (h->general) return fail(EPP_ERR_INVALID, "endpoint-sharded mode supports neither pick_k > 1 nor the prefix-cache-affinity-filter (both need every candidate's score on one rank)");
     EPP_TRY(check_shardable(h));
+    // the kernels write handler_stages records (kernels.h); the same count from the configuration
+    const int32_t stages = h->cfg.encode_enabled ? 3 : h->n_profiles;
+    if (h->p2p_buf && h->p2p_stages != stages)
+        return fail(EPP_ERR_STATE, "the exchange buffer was exported for %d record(s) per request, this handler needs %d: call epp_shard_set_staged before epp_shard_p2p_export", (int)h->p2p_stages, (int)stages);
     h->shard_begin = ep_begin;
     h->shard_end = ep_end;
+    h->shard_stages = stages;
     h->pool_ready = false;          // candidates are derived per shard: epp_pool_set must follow
+    if (out_stages) *out_stages = stages;
     return EPP_OK;
+}
+
+extern "C" int32_t epp_shard_set(epp_engine *h, uint32_t ep_begin, uint32_t ep_end) {
+    return shard_set(h, ep_begin, ep_end, false, nullptr);
+}
+extern "C" int32_t epp_shard_set_staged(epp_engine *h, uint32_t ep_begin, uint32_t ep_end, int32_t *out_stages) {
+    if (!out_stages) return fail(EPP_ERR_INVALID, "NULL argument");
+    return shard_set(h, ep_begin, ep_end, true, out_stages);
 }
 
 static int32_t mask_words_of(const epp_engine *h) { return (h->cfg.max_prefix_blocks + 31) / 32; }
@@ -2746,18 +2764,52 @@ extern "C" int32_t epp_shard_probe(epp_engine *h, const epp_batch *batch, uint32
     h->kept_R = 0;
     h->shard_R = 0;
     h->shard_models = false;
+    h->shard_mm = false;
     EPP_TRY(commit_locked(h));
     EPP_TRY(run_batch(h, v, Mode::HashOnly, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr));
     int launches = 0;
     cudaStream_t s = h->slot[0].stream;
-    // the pick (a later call) scores lora-affinity with the batch's adapters: keep a copy, the caller's ids may be gone
+    // the pick (a later call) scores lora-affinity with the batch's adapters: keep a copy, the caller's ids may be gone.
+    // Likewise the multimodal flags (encode stage); the request lengths (P/D decider) stay in `in_len` from the hashing.
     if (v.model_ids && v.R)
         CUDA_TRY(cudaMemcpyAsync(h->model_ids.p, v.model_ids, sizeof(uint32_t) * (size_t)v.R, cudaMemcpyDeviceToDevice, s));
+    if (v.multimodal && v.R) {
+        CUDA_TRY(h->multimodal.reserve((size_t)v.R, &h->dev_bytes));
+        CUDA_TRY(cudaMemcpyAsync(h->multimodal.p, v.multimodal, (size_t)v.R, cudaMemcpyDeviceToDevice, s));
+    }
     CUDA_TRY(launch_shard_probe(v.R, h->cfg.max_prefix_blocks, h->hashes.as<uint64_t>(), h->nblocks.as<int32_t>(),
                                 index_view(h), out_masks, mask_words_of(h), s, &launches));
     CUDA_TRY(cudaStreamSynchronize(s));
     h->shard_R = v.R;
     h->shard_models = v.model_ids != nullptr;
+    h->shard_mm = v.multimodal != nullptr;
+    return EPP_OK;
+}
+
+// The merge of rows [r0, r0 + R) of the batch in progress, whose lengths are in_len[r0 ..] and flags multimodal (absolute
+// rows, or nullptr).
+static ShardMergeParams shard_merge_params(epp_engine *h, int64_t r0, int64_t R, int32_t n_ranks, const epp_shard_best *all_best,
+                                           const uint8_t *multimodal, epp_decision *out, epp_decision_detail *detail) {
+    ShardMergeParams p;
+    p.R = R;
+    p.n_ranks = n_ranks;
+    p.stages = h->shard_stages;
+    p.all_best = all_best;
+    p.nblocks = h->nblocks.as<int32_t>() + r0;
+    p.out = out;
+    p.detail = detail;
+    p.always_disagg = h->cfg.always_disagg;
+    p.block_size_tokens = h->cfg.block_size_tokens;
+    p.non_cached_tokens = h->cfg.non_cached_tokens;
+    p.in_len = h->in_len.as<int64_t>() + r0;
+    p.multimodal = multimodal ? multimodal + r0 : nullptr;
+    return p;
+}
+
+// Only the detail carries the encode pick (the rule of epp_schedule).
+static int32_t check_encode_detail(const epp_engine *h, bool multimodal, const epp_decision_detail *detail) {
+    if (h->cfg.encode_enabled && multimodal && !detail)
+        return fail(EPP_ERR_INVALID, "an encode profile is configured and the batch flags multimodal requests: `out_detail` (which carries the encode pick) must not be NULL");
     return EPP_OK;
 }
 
@@ -2770,7 +2822,7 @@ extern "C" int32_t epp_shard_pick(epp_engine *h, int64_t n_requests, const uint3
     if (n_requests != h->shard_R) return fail(EPP_ERR_STATE, "epp_shard_pick: n_requests %lld does not match the probed batch (%lld)", (long long)n_requests, (long long)h->shard_R);
     if (n_requests == 0) return EPP_OK;
     Work w{0, n_requests, nullptr, nullptr, nullptr, 0, h->shard_models ? h->model_ids.as<uint32_t>() : nullptr, 0,
-           h->hashes.as<uint64_t>(), h->nblocks.as<int32_t>()};
+           h->hashes.as<uint64_t>(), h->nblocks.as<int32_t>(), h->shard_mm ? h->multimodal.as<uint8_t>() : nullptr};
     PickParams pp = pick_params(h, w, h->decisions.as<epp_decision>(), nullptr, nullptr);
     pp.global_masks = global_masks;
     pp.mask_words = mask_words_of(h);
@@ -2783,17 +2835,24 @@ extern "C" int32_t epp_shard_pick(epp_engine *h, int64_t n_requests, const uint3
     return EPP_OK;
 }
 
-extern "C" int32_t epp_shard_merge(epp_engine *h, int64_t n_requests, int32_t n_ranks, const epp_shard_best *all_best, epp_decision *out) {
+extern "C" int32_t epp_shard_merge_detail(epp_engine *h, int64_t n_requests, int32_t n_ranks, const epp_shard_best *all_best,
+                                          epp_decision *out, epp_decision_detail *out_detail) {
     if (!h || !all_best || !out || n_ranks <= 0) return fail(EPP_ERR_INVALID, "bad arguments");
     std::lock_guard<std::mutex> lk(h->mu);
     EPP_TRY(set_device(h));
     EPP_TRY(join_streams(h));
     if (n_requests != h->shard_R) return fail(EPP_ERR_STATE, "epp_shard_merge: n_requests does not match the probed batch");
+    EPP_TRY(check_encode_detail(h, h->shard_mm, out_detail));
     int launches = 0;
     cudaStream_t s = h->slot[0].stream;
-    CUDA_TRY(launch_shard_merge(n_requests, n_ranks, all_best, h->nblocks.as<int32_t>(), out, s, &launches));
+    CUDA_TRY(launch_shard_merge(shard_merge_params(h, 0, n_requests, n_ranks, all_best,
+                                                   h->shard_mm ? h->multimodal.as<uint8_t>() : nullptr, out, out_detail),
+                                s, &launches));
     CUDA_TRY(cudaStreamSynchronize(s));
     return EPP_OK;
+}
+extern "C" int32_t epp_shard_merge(epp_engine *h, int64_t n_requests, int32_t n_ranks, const epp_shard_best *all_best, epp_decision *out) {
+    return epp_shard_merge_detail(h, n_requests, n_ranks, all_best, out, nullptr);
 }
 
 // ---- endpoint-sharded mode with the exchanges over NVLink peer memory (shard_p2p.cu) ------------------------------
@@ -2820,11 +2879,12 @@ extern "C" int32_t epp_shard_p2p_export(epp_engine *h, int64_t max_requests, uin
     const size_t W = (size_t)mask_words_of(h);
     h->p2p_masks_off = kP2pHeader;
     h->p2p_best_off = (kP2pHeader + (size_t)max_requests * W * sizeof(uint32_t) + 255) & ~(size_t)255;
-    h->p2p_bytes = (h->p2p_best_off + (size_t)max_requests * sizeof(epp_shard_best) + 255) & ~(size_t)255;
+    h->p2p_bytes = (h->p2p_best_off + (size_t)max_requests * (size_t)h->shard_stages * sizeof(epp_shard_best) + 255) & ~(size_t)255;
     CUDA_TRY(cudaMalloc(&h->p2p_buf, h->p2p_bytes));
     CUDA_TRY(cudaMemset(h->p2p_buf, 0, h->p2p_bytes));
     h->dev_bytes += h->p2p_bytes;
     h->p2p_R = max_requests;
+    h->p2p_stages = h->shard_stages;
     cudaIpcMemHandle_t hd;
     CUDA_TRY(cudaIpcGetMemHandle(&hd, h->p2p_buf));
     static_assert(sizeof(hd) == 64, "cudaIpcMemHandle_t is 64 bytes");
@@ -2863,7 +2923,8 @@ extern "C" int32_t epp_shard_p2p_connect(epp_engine *h, int32_t n_ranks, int32_t
     // while a peer-wait kernel is spinning
     const size_t W = (size_t)mask_words_of(h);
     CUDA_TRY(h->p2p_gmasks.reserve(((size_t)h->p2p_R * W * sizeof(uint32_t) + 15) & ~(size_t)15, &h->dev_bytes));
-    CUDA_TRY(h->p2p_allbest.reserve(sizeof(epp_shard_best) * (size_t)h->p2p_R * (size_t)n_ranks, &h->dev_bytes));
+    CUDA_TRY(h->p2p_allbest.reserve(sizeof(epp_shard_best) * (size_t)h->p2p_R * (size_t)h->p2p_stages * (size_t)n_ranks,
+                                     &h->dev_bytes));
     EPP_TRY(reserve_batch(h, h->p2p_R));
     return EPP_OK;
 }
@@ -2905,10 +2966,11 @@ static int32_t p2p_check(epp_engine *h, cudaStream_t s, unsigned long long epoch
 
 // One phase of the exchange for rows [r0, r1) of the batch (chunk c: its own flag words, stream of slot c).  Phase 0
 // expects ++p2p_epoch and the commit to have happened; the caller checks p2p_err after phase 2 of every chunk.
-static int32_t p2p_phase_rows(epp_engine *h, const BatchView &v, epp_decision *out, int phase, int c, int64_t r0, int64_t r1,
-                              uint64_t or_bits) {
+static int32_t p2p_phase_rows(epp_engine *h, const BatchView &v, epp_decision *out, epp_decision_detail *detail, int phase,
+                              int c, int64_t r0, int64_t r1, uint64_t or_bits) {
     const int64_t R = r1 - r0;
     const int n = h->p2p_ranks;
+    const size_t S = (size_t)h->p2p_stages;
     const size_t W = (size_t)mask_words_of(h), B = (size_t)h->cfg.max_prefix_blocks;
     Slot &sl = h->slot[c];
     cudaStream_t s = sl.stream;
@@ -2917,13 +2979,13 @@ static int32_t p2p_phase_rows(epp_engine *h, const BatchView &v, epp_decision *o
     const size_t flag1 = (size_t)c * kP2pChunkFlags + kP2pFlag1, flag2 = (size_t)c * kP2pChunkFlags + kP2pFlag2;
     const size_t mask_off = h->p2p_masks_off + (size_t)r0 * W * sizeof(uint32_t);
     const size_t mask_bytes = ((size_t)R * W * sizeof(uint32_t) + 15) & ~(size_t)15;
-    const size_t best_off = h->p2p_best_off + (size_t)r0 * sizeof(epp_shard_best);
+    const size_t best_off = h->p2p_best_off + (size_t)r0 * S * sizeof(epp_shard_best);
     const unsigned long long timeout_ns = p2p_timeout_ns();
     const unsigned long long epoch = h->p2p_epoch;
     uint64_t *hashes = h->hashes.as<uint64_t>() + (size_t)r0 * B;
     int32_t *nbs = h->nblocks.as<int32_t>() + r0;
     uint32_t *gmasks = h->p2p_gmasks.as<uint32_t>() + (size_t)r0 * W;
-    epp_shard_best *allbest = h->p2p_allbest.as<epp_shard_best>() + (size_t)r0 * (size_t)n;   // this chunk's own [n][R] matrix
+    epp_shard_best *allbest = h->p2p_allbest.as<epp_shard_best>() + (size_t)r0 * (size_t)n * S;   // this chunk's own [n][R][S] records
     int launches = 0;
     if (phase == 0) {
         // hashes + local presence masks -> own exchange buffer, raise flag 1
@@ -2941,7 +3003,7 @@ static int32_t p2p_phase_rows(epp_engine *h, const BatchView &v, epp_decision *o
         // local best record in the own exchange buffer, raise flag 2
         CUDA_TRY(launch_p2p_wait(peers, n, flag1, epoch, h->p2p_err.as<int>(), timeout_ns, s));
         CUDA_TRY(launch_p2p_or_masks(peers, n, mask_off, mask_bytes, gmasks, s));
-        Work w{r0, r1, nullptr, nullptr, nullptr, 0, nullptr, 0, hashes, nbs};
+        Work w{r0, r1, nullptr, nullptr, nullptr, 0, nullptr, 0, hashes, nbs, v.multimodal};
         PickParams pp = pick_params(h, w, h->decisions.as<epp_decision>() + r0, nullptr, nullptr);
         pp.model_ids = v.model_ids ? v.model_ids + r0 : nullptr;
         pp.global_masks = gmasks;
@@ -2955,8 +3017,9 @@ static int32_t p2p_phase_rows(epp_engine *h, const BatchView &v, epp_decision *o
     }
     // exchange 2: gather every rank's records from the peers and merge
     CUDA_TRY(launch_p2p_wait(peers, n, flag2, epoch, h->p2p_err.as<int>(), timeout_ns, s));
-    CUDA_TRY(launch_p2p_gather(peers, n, best_off, sizeof(epp_shard_best) * (size_t)R, allbest, s));
-    CUDA_TRY(launch_shard_merge(R, n, allbest, nbs, out + r0, s, &launches));
+    CUDA_TRY(launch_p2p_gather(peers, n, best_off, sizeof(epp_shard_best) * S * (size_t)R, allbest, s));
+    CUDA_TRY(launch_shard_merge(shard_merge_params(h, r0, R, n, allbest, v.multimodal, out + r0, detail ? detail + r0 : nullptr),
+                                s, &launches));
     h->p2p_launches += launches + 2;
     return EPP_OK;
 }
@@ -2982,7 +3045,8 @@ static int32_t p2p_end(epp_engine *h, int64_t R) {
     h->stats.n_decisions += (uint64_t)R;
     return EPP_OK;
 }
-static int32_t p2p_prepare(epp_engine *h, const epp_batch *batch, epp_decision *out, BatchView &v) {
+static int32_t p2p_prepare(epp_engine *h, const epp_batch *batch, epp_decision *out, const epp_decision_detail *detail,
+                           BatchView &v) {
     if (!h || !out) return fail(EPP_ERR_INVALID, "NULL argument");
     EPP_TRY(set_device(h));
     EPP_TRY(join_streams(h));
@@ -2993,15 +3057,17 @@ static int32_t p2p_prepare(epp_engine *h, const epp_batch *batch, epp_decision *
     EPP_TRY(check_batch(h, batch, v));
     if (!v.device) return fail(EPP_ERR_INVALID, "the sharded peer-memory entry points take device-pointer batches (EPP_BATCH_DEVICE_PTRS)");
     if (v.R > h->p2p_R) return fail(EPP_ERR_CAPACITY, "batch of %lld requests exceeds the exported exchange buffer (%lld)", (long long)v.R, (long long)h->p2p_R);
+    EPP_TRY(check_encode_detail(h, v.multimodal != nullptr, detail));
     v.async = false;
     return EPP_OK;
 }
 
-extern "C" int32_t epp_shard_schedule_p2p(epp_engine *h, const epp_batch *batch, epp_decision *out) {
+extern "C" int32_t epp_shard_schedule_p2p_detail(epp_engine *h, const epp_batch *batch, epp_decision *out,
+                                                 epp_decision_detail *out_detail) {
     if (!h) return fail(EPP_ERR_INVALID, "NULL argument");
     std::lock_guard<std::mutex> lk(h->mu);
     BatchView v;
-    EPP_TRY(p2p_prepare(h, batch, out, v));
+    EPP_TRY(p2p_prepare(h, batch, out, out_detail, v));
     if (v.R == 0) return EPP_OK;
     uint64_t or_bits = 0;
     EPP_TRY(p2p_begin(h, v, &or_bits));
@@ -3013,8 +3079,8 @@ extern "C" int32_t epp_shard_schedule_p2p(epp_engine *h, const epp_batch *batch,
         CUDA_TRY(cudaStreamWaitEvent(h->slot[1].stream, h->slot[0].done, 0));
     }
     for (int phase = 0; phase < 3; phase++) {
-        EPP_TRY(p2p_phase_rows(h, v, out, phase, 0, 0, half, or_bits));
-        if (split) EPP_TRY(p2p_phase_rows(h, v, out, phase, 1, half, v.R, or_bits));
+        EPP_TRY(p2p_phase_rows(h, v, out, out_detail, phase, 0, 0, half, or_bits));
+        if (split) EPP_TRY(p2p_phase_rows(h, v, out, out_detail, phase, 1, half, v.R, or_bits));
     }
     if (split) {
         h->s1_unjoined = true;
@@ -3022,16 +3088,23 @@ extern "C" int32_t epp_shard_schedule_p2p(epp_engine *h, const epp_batch *batch,
     }
     return p2p_end(h, v.R);
 }
-extern "C" int32_t epp_shard_p2p_phase(epp_engine *h, const epp_batch *batch, epp_decision *out, int32_t phase) {
+extern "C" int32_t epp_shard_schedule_p2p(epp_engine *h, const epp_batch *batch, epp_decision *out) {
+    return epp_shard_schedule_p2p_detail(h, batch, out, nullptr);
+}
+extern "C" int32_t epp_shard_p2p_phase_detail(epp_engine *h, const epp_batch *batch, epp_decision *out,
+                                              epp_decision_detail *out_detail, int32_t phase) {
     if (!h) return fail(EPP_ERR_INVALID, "NULL argument");
     if (phase < 0 || phase > 2) return fail(EPP_ERR_INVALID, "phase %d out of range [0,2]", phase);
     std::lock_guard<std::mutex> lk(h->mu);
     BatchView v;
-    EPP_TRY(p2p_prepare(h, batch, out, v));
+    EPP_TRY(p2p_prepare(h, batch, out, out_detail, v));
     if (v.R == 0) return EPP_OK;
     if (phase == 0) EPP_TRY(p2p_begin(h, v, &h->p2p_or_bits));
-    EPP_TRY(p2p_phase_rows(h, v, out, phase, 0, 0, v.R, h->p2p_or_bits));
+    EPP_TRY(p2p_phase_rows(h, v, out, out_detail, phase, 0, 0, v.R, h->p2p_or_bits));
     if (phase == 2) return p2p_end(h, v.R);
     CUDA_TRY(cudaStreamSynchronize(h->slot[0].stream));
     return EPP_OK;
+}
+extern "C" int32_t epp_shard_p2p_phase(epp_engine *h, const epp_batch *batch, epp_decision *out, int32_t phase) {
+    return epp_shard_p2p_phase_detail(h, batch, out, nullptr, phase);
 }

@@ -266,7 +266,7 @@ struct PickParams {
     // endpoint-sharded mode (nullptr otherwise): the stop rule comes from the OR of all ranks' presence masks
     const uint32_t *global_masks;       // [R][mask_words]
     int32_t mask_words;
-    epp_shard_best *shard_out;          // [R] local best record instead of `out`
+    epp_shard_best *shard_out;          // [R][handler_stages] local best records instead of `out`
     // dense-counter kernel (k_match_pick) only: process the requests listed in req_list[0 .. *req_list_n) (the sparse kernel's overflows)
     const int32_t *req_list;
     const int32_t *req_list_n;
@@ -294,8 +294,13 @@ cudaError_t launch_match_pick(const PickParams &p, uint32_t *gscratch, int grid,
 cudaError_t launch_match_pick_sparse(const PickParams &p, int sm_count, int ctas, cudaStream_t s, int *launches);
 // Does some profile of the launch (PickParams, DensePickParams) have a random picker?  Then the sparse, small-batch,
 // dense-counter and injected-match paths launch their _rand builds.
+// Stages of the handler of a launch (PickParams, DensePickParams): 1 = single profile, 2 = decode + prefill, 3 = + encode.
+// In the endpoint-sharded mode it is also the number of records per request (include/epp_engine.h, "Staged records").
+template <class Params> __host__ __device__ inline int handler_stages(const Params &p) {
+    return p.encode_on ? 3 : (p.n_profiles >= 2 ? 2 : 1);
+}
 template <class Params> inline bool any_random_picker(const Params &p) {
-    const int np = p.encode_on ? 3 : (p.n_profiles >= 2 ? 2 : 1);
+    const int np = handler_stages(p);
     for (int i = 0; i < np; i++)
         if (p.prof[i].cfg.picker) return true;
     return false;
@@ -389,8 +394,24 @@ cudaError_t launch_score_dense(int64_t R, int32_t E, const ProfileDev &prof, con
 cudaError_t launch_shard_probe(int64_t R, int32_t max_blocks, const uint64_t *hashes, const int32_t *nblocks,
                                const IndexView &index, uint32_t *out_masks, int32_t mask_words, cudaStream_t s,
                                int *launches);
-cudaError_t launch_shard_merge(int64_t R, int32_t n_ranks, const epp_shard_best *all_best, const int32_t *nblocks,
-                               epp_decision *out, cudaStream_t s, int *launches);
+// The merge: per stage, max score, lowest slot id among equals, ties summed; then the disagg handler's deciders on the
+// merged decode pick (score.cuh: pd_decide).  stages == 1 is the single-profile handler.
+struct ShardMergeParams {
+    int64_t R;
+    int32_t n_ranks;
+    int32_t stages;                     // records per request and rank
+    const epp_shard_best *all_best;     // [n_ranks][R][stages]
+    const int32_t *nblocks;             // [R]
+    epp_decision *out;                  // [R]
+    epp_decision_detail *detail;        // [R] or nullptr
+    // decider inputs (stages >= 2)
+    int32_t always_disagg;
+    int32_t block_size_tokens;
+    int64_t non_cached_tokens;
+    const int64_t *in_len;              // [R] prompt bytes
+    const uint8_t *multimodal;          // [R] or nullptr (stages == 3)
+};
+cudaError_t launch_shard_merge(const ShardMergeParams &p, cudaStream_t s, int *launches);
 
 // shard_p2p.cu: exchanges of the endpoint-sharded mode over NVLink peer memory (no NCCL)
 cudaError_t launch_p2p_signal(unsigned long long *flag, unsigned long long epoch, cudaStream_t s);

@@ -90,11 +90,16 @@ cudaError_t launch_match_pick_sparse(const PickParams &p, int sm_count, int ctas
     if (p.R <= 0) return cudaSuccess;
     if (!p.req_next || p.R > INT32_MAX) return cudaErrorInvalidValue;
     const bool tie = p.tie_seed != 0;
-    const int stages = p.encode_on ? 3 : (p.n_profiles >= 2 ? 2 : 1);
+    const int stages = handler_stages(p);
     cudaError_t e;
     // the hot configuration (one profile, lowest-slot ties) gets the 32-register build; the variants that carry more
-    // code (stages, tie rule, sharding) keep 40 registers
-    if (p.global_masks) e = launch_one<6, true, false, 1>(p, sm_count, s);
+    // code (stages, tie rule, sharding) keep 40 registers.  The sharded builds write one record per stage and always
+    // take the lowest slot.
+    if (p.global_masks) {
+        if (stages == 1) e = launch_one<6, true, false, 1>(p, sm_count, s);
+        else if (stages == 2) e = launch_one<6, true, false, 2>(p, sm_count, s);
+        else e = launch_one<6, true, false, 3>(p, sm_count, s);
+    }
     else if (any_random_picker(p)) e = launch_kernel<k_match_pick_sparse_rand>(p, sm_count, s);
     else if (p.nohit.mask) {
         if (stages == 1) e = tie ? launch_nohit<true, 1>(p, sm_count, s) : launch_nohit<false, 1>(p, sm_count, s);

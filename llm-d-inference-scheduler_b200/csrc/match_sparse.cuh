@@ -392,6 +392,15 @@ __device__ __forceinline__ bool match_request(const PickParams &p, const uint32_
         return false;
     }
     // ---- a5-a14: the profiles of the handler
+    if constexpr (kSharded && kStages > 1) {
+        // endpoint-sharded disagg handler: one record per stage, each a scoring pass over the same lane map
+        shard_stage_records(p, r, kStages, p.in_len[r],
+                            [&](int pi, uint64_t key) {
+                                return eval_profile_lanes<kTie>(p.prof[pi], p.E, m, total, lane, p.lora, lora_st, p.tie_seed, key);
+                            },
+                            [&](uint32_t e) { return m.n ? (int32_t)map_get(m, e) : 0; }, lane);
+        return true;
+    }
     epp_decision d;
     epp_decision_detail dd;
     bool cold = false;

@@ -454,6 +454,7 @@ __device__ __forceinline__ void match_pick_dense(const PickParams &p, int32_t cn
         auto cnt_of = [&](uint32_t e) { return (int32_t)cnt_get(cnt32, e); };
         bool cold = false;
         auto is_cold = [&](const ProfileDev &pf) { return cold_scan(pf, p.E, lane, cnt_of); };
+        bool staged = false;
         if constexpr (kLat) {
             decide_stages<3>(p, r, total, p.n_profiles >= 2 ? p.in_len[r] : 0,
                           [&](int pi, uint64_t key) {
@@ -466,12 +467,22 @@ __device__ __forceinline__ void match_pick_dense(const PickParams &p, int32_t cn
                           [&](int pi, uint64_t key) { return gen_eval_profile<kRand>(p, nohit_select(p, pi, cold, is_cold), pi, r, total, lane, adapter, key, cnt_of); },
                           cnt_of, d, dd);
         } else {
-            decide_stages<3>(p, r, total, p.n_profiles >= 2 ? p.in_len[r] : 0,
-                          [&](int pi, uint64_t key) { return eval_profile<kRand>(nohit_select(p, pi, cold, is_cold), p.E, cnt32, list, nl, total, lane, p.lora, adapter, p.tie_seed, key); },
-                          cnt_of, d, dd);
+            // endpoint-sharded mode under the disagg handler (never with a random picker or no-hit-lru): one record per stage
+            if constexpr (!kRand) {
+                if (p.shard_out && handler_stages(p) > 1) {
+                    staged = true;
+                    shard_stage_records(p, r, handler_stages(p), p.in_len[r],
+                                        [&](int pi, uint64_t key) { return eval_profile<false>(p.prof[pi], p.E, cnt32, list, nl, total, lane, p.lora, adapter, p.tie_seed, key); },
+                                        cnt_of, lane);
+                }
+            }
+            if (!staged)
+                decide_stages<3>(p, r, total, p.n_profiles >= 2 ? p.in_len[r] : 0,
+                              [&](int pi, uint64_t key) { return eval_profile<kRand>(nohit_select(p, pi, cold, is_cold), p.E, cnt32, list, nl, total, lane, p.lora, adapter, p.tie_seed, key); },
+                              cnt_of, d, dd);
         }
         if (lane == 0 && p.nohit.cold_out) p.nohit.cold_out[r] = cold ? 1 : 0;
-        if (lane == 0) {
+        if (lane == 0 && !staged) {
             if (p.shard_out) {
                 epp_shard_best sb;
                 sb.score = d.score; sb.pick = d.pick; sb.tie_count = d.tie_count;
@@ -732,36 +743,57 @@ cudaError_t launch_shard_probe(int64_t R, int32_t max_blocks, const uint64_t *ha
     return cudaGetLastError();
 }
 
-// all_best is [n_ranks][R]; the winner is the max score, lowest slot id among equals, ties summed.
-__global__ void k_shard_merge(int64_t R, int32_t n_ranks, const epp_shard_best *all_best, const int32_t *nblocks,
-                              epp_decision *out) {
-    int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= R) return;
+// Stage st of request r over every rank's record: the max score, lowest slot id among equals, ties summed; mb = the
+// match_blocks of the winning record.
+__device__ __forceinline__ Best merge_stage(const ShardMergeParams &p, int64_t r, int st, int32_t &mb) {
     Best b;
     best_init(b);
-    int32_t mb = 0;
-    for (int32_t k = 0; k < n_ranks; k++) {
-        epp_shard_best sb = all_best[(int64_t)k * R + r];
+    mb = 0;
+    for (int32_t k = 0; k < p.n_ranks; k++) {
+        epp_shard_best sb = p.all_best[((int64_t)k * p.R + r) * p.stages + st];
         if (sb.status != 0) continue;
         uint32_t before = b.pick;
         best_add(b, sb.score, sb.pick, sb.tie_count);
         if (b.pick != before) mb = sb.match_blocks;
     }
+    return b;
+}
+
+// The decision of request r from the merged stages, as decide_stages makes it from one pool.
+__global__ void k_shard_merge(ShardMergeParams p) {
+    int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= p.R) return;
+    int32_t mb;
+    const Best b = merge_stage(p, r, 0, mb);
     epp_decision d;
     d.status = b.ties ? 0 : -1;
     d.pick = b.ties ? b.pick : EPP_NO_ENDPOINT;
     d.score = b.ties ? b.val : 0.0;
     d.prefill_pick = EPP_NO_ENDPOINT;
     d.tie_count = b.ties;
-    d.total_blocks = nblocks[r];
+    d.total_blocks = p.nblocks[r];
     d.match_blocks = b.ties ? mb : 0;
-    out[r] = d;
+    epp_decision_detail dd;
+    dd.prefill_score = 0.0; dd.prefill_tie_count = 0; dd.prefill_ran = 0;
+    dd.encode_score = 0.0; dd.encode_pick = EPP_NO_ENDPOINT; dd.encode_tie_count = 0; dd.encode_ran = 0; dd.reserved = 0;
+    if (b.ties && p.stages >= 3 && p.multimodal && p.multimodal[r]) {   // no decode pick: no other stage runs
+        dd.encode_ran = 1;
+        const Best b2 = merge_stage(p, r, 2, mb);
+        if (b2.ties) { dd.encode_pick = b2.pick; dd.encode_score = b2.val; dd.encode_tie_count = b2.ties; }
+    }
+    if (b.ties && p.stages >= 2 &&
+        (p.always_disagg || pd_decide(p.non_cached_tokens, p.in_len[r], d.match_blocks, p.block_size_tokens))) {
+        dd.prefill_ran = 1;
+        const Best b1 = merge_stage(p, r, 1, mb);
+        if (b1.ties) { d.prefill_pick = b1.pick; dd.prefill_score = b1.val; dd.prefill_tie_count = b1.ties; }
+    }
+    p.out[r] = d;
+    if (p.detail) p.detail[r] = dd;
 }
 
-cudaError_t launch_shard_merge(int64_t R, int32_t n_ranks, const epp_shard_best *all_best, const int32_t *nblocks,
-                               epp_decision *out, cudaStream_t s, int *launches) {
-    if (R <= 0) return cudaSuccess;
-    k_shard_merge<<<(unsigned)((R + 255) / 256), 256, 0, s>>>(R, n_ranks, all_best, nblocks, out);
+cudaError_t launch_shard_merge(const ShardMergeParams &p, cudaStream_t s, int *launches) {
+    if (p.R <= 0) return cudaSuccess;
+    k_shard_merge<<<(unsigned)((p.R + 255) / 256), 256, 0, s>>>(p);
     if (launches) *launches += 1;
     return cudaGetLastError();
 }

@@ -273,4 +273,31 @@ __device__ __forceinline__ void decide_stages(const P &p, int64_t r, int32_t tot
     }
 }
 
+// Endpoint-sharded mode with the disagg handler (include/epp_engine.h, "Staged records"): this rank's best record of each
+// of the n_stages stages of request r, out[0 .. n_stages).  Whether the prefill stage runs depends on the MERGED decode
+// pick's match_blocks, which no rank knows yet, so a stage is evaluated whenever its decider can still come out true:
+// prefill unless pd_decide is false for every match count (always_disagg, or 0 < non_cached_tokens <= tokens), encode for
+// multimodal requests.  Every stage is evaluated even when this rank has no decode candidate (the decode pick may be
+// another rank's).  A stage that is not evaluated gets status -1.  eval / match_of as in decide_stages; the records go to
+// p.shard_out[r * n_stages ..].
+template <typename P, typename Eval, typename MatchOf>
+__device__ __forceinline__ void shard_stage_records(const P &p, int64_t r, int n_stages, int64_t in_len, Eval eval,
+                                                    MatchOf match_of, int lane) {
+    // decided up front: the request's length and flag need no registers while the stages are scored
+    uint32_t runs = 1u;
+    if (n_stages >= 2 && (p.always_disagg || (p.non_cached_tokens != 0 && in_len / 4 >= p.non_cached_tokens))) runs |= 2u;
+    if (n_stages >= 3 && p.encode_on && p.multimodal && p.multimodal[r]) runs |= 4u;
+#pragma unroll 1
+    for (int st = 0; st < n_stages; st++) {
+        epp_shard_best sb;
+        sb.score = 0.0; sb.pick = EPP_NO_ENDPOINT; sb.tie_count = 0; sb.match_blocks = 0; sb.status = -1;
+        if ((runs >> st) & 1u) {
+            const Best b = eval(st, 4 * (p.tie_base + (uint64_t)r) + (uint64_t)st);
+            const int32_t mb = b.ties ? match_of(b.pick) : 0;
+            if (b.ties) { sb.score = b.val; sb.pick = b.pick; sb.tie_count = b.ties; sb.match_blocks = mb; sb.status = 0; }
+        }
+        if (lane == 0) p.shard_out[r * n_stages + st] = sb;
+    }
+}
+
 }  // namespace epp

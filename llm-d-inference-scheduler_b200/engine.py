@@ -195,6 +195,7 @@ class Engine:
         self.cfg = cfg
         self.E = max_endpoints
         self.B = max_prefix_blocks
+        self.shard_stages = 1           # records per request of the endpoint-sharded protocol (shard_set_staged)
         self._h = C.c_void_p()
         self._check(self._lib.epp_engine_create(C.byref(cfg), C.byref(self._h)))
         for p, spec in enumerate((primary, prefill, encode)):
@@ -560,10 +561,19 @@ class Engine:
     # ---- endpoint-sharded mode (device pointers only) ----
     def shard_set(self, ep_begin: int, ep_end: int):
         self._check(self._lib.epp_shard_set(self._h, ep_begin, ep_end))
+        self.shard_stages = 1
+
+    def shard_set_staged(self, ep_begin: int, ep_end: int) -> int:
+        """shard_set that also takes the disagg handler -> S, the records per request of shard_pick (1 single profile,
+        2 decode + prefill, 3 with encode); shard_pick's out_best is then [R, S * 24] bytes."""
+        s = C.c_int32(0)
+        self._check(self._lib.epp_shard_set_staged(self._h, ep_begin, ep_end, C.byref(s)))
+        self.shard_stages = s.value
+        return s.value
 
     def shard_probe(self, data, out_masks, offsets=None, uniform_len=None, model_ids=None, n_requests=None,
-                    lengths=None):
-        b, R, dev, keep = self._batch(data, offsets, uniform_len, model_ids, n_requests, lengths)
+                    lengths=None, multimodal=None):
+        b, R, dev, keep = self._batch(data, offsets, uniform_len, model_ids, n_requests, lengths, multimodal)
         self._check(self._lib.epp_shard_probe(self._h, C.byref(b), _ptr(out_masks)))
         return R
 
@@ -583,20 +593,23 @@ class Engine:
         self._check(self._lib.epp_shard_p2p_connect(self._h, n_ranks, rank, _ptr(a), int(ipc_handles)))
 
     def shard_schedule_p2p(self, data, out_decisions, offsets=None, uniform_len=None, model_ids=None, n_requests=None,
-                           lengths=None):
-        b, R, dev, keep = self._batch(data, offsets, uniform_len, model_ids, n_requests, lengths)
-        self._check(self._lib.epp_shard_schedule_p2p(self._h, C.byref(b), _ptr(out_decisions)))
+                           lengths=None, multimodal=None, out_detail=None):
+        """out_detail: [R, 40] uint8 CUDA tensor of epp_decision_detail (prefill and encode fields), or None."""
+        b, R, dev, keep = self._batch(data, offsets, uniform_len, model_ids, n_requests, lengths, multimodal)
+        self._check(self._lib.epp_shard_schedule_p2p_detail(self._h, C.byref(b), _ptr(out_decisions), _ptr(out_detail)))
         return R
 
     def shard_p2p_phase(self, data, out_decisions, phase: int, offsets=None, uniform_len=None, model_ids=None,
-                        n_requests=None, lengths=None):
+                        n_requests=None, lengths=None, multimodal=None, out_detail=None):
         """One phase (0, 1, 2) of shard_schedule_p2p, synchronised: for ranks that share a GPU."""
-        b, R, dev, keep = self._batch(data, offsets, uniform_len, model_ids, n_requests, lengths)
-        self._check(self._lib.epp_shard_p2p_phase(self._h, C.byref(b), _ptr(out_decisions), phase))
+        b, R, dev, keep = self._batch(data, offsets, uniform_len, model_ids, n_requests, lengths, multimodal)
+        self._check(self._lib.epp_shard_p2p_phase_detail(self._h, C.byref(b), _ptr(out_decisions), _ptr(out_detail), phase))
         return R
 
-    def shard_merge(self, n_requests, n_ranks, all_best, out_decisions):
-        self._check(self._lib.epp_shard_merge(self._h, n_requests, n_ranks, _ptr(all_best), _ptr(out_decisions)))
+    def shard_merge(self, n_requests, n_ranks, all_best, out_decisions, out_detail=None):
+        """all_best: [n_ranks, R, S * 24] records; out_detail as in shard_schedule_p2p."""
+        self._check(self._lib.epp_shard_merge_detail(self._h, n_requests, n_ranks, _ptr(all_best), _ptr(out_decisions),
+                                                     _ptr(out_detail)))
 
 
 class Batcher:

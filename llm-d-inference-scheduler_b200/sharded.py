@@ -5,9 +5,15 @@ at the first block NO server holds (approximateprefix/plugin.go:219-223), a shar
 
     phase 1  epp_shard_probe   local block-presence masks            [R][W] u32,  W = ceil(max_prefix_blocks / 32)
     exchange all-gather + bitwise OR of the masks (NCCL has no OR reduction)
-    phase 2  epp_shard_pick    global stop applied to local counts -> local best record   [R] x 24 B
+    phase 2  epp_shard_pick    global stop applied to local counts -> local best records  [R][S] x 24 B
     exchange all-gather of the records
-    phase 3  epp_shard_merge   max score, lowest slot id among equals, ties summed
+    phase 3  epp_shard_merge   per stage: max score, lowest slot id among equals, ties summed; then the deciders
+
+S is the engine's number of stages (Engine.shard_set_staged): 1 for the single-profile handler, 2 for the disagg
+handler's decode + prefill, 3 with its encode stage.  The prefill and encode profiles do not depend on the decode pick,
+only whether they run does: every rank publishes its best record of each stage (prefill whenever the P/D decider can
+still say yes, encode for multimodal requests), and the merge applies the deciders to the merged decode pick -- still two
+exchanges.
 
 torch.distributed is the plumbing (NCCL on GPUs, gloo in the CPU tests); the Go shim uses ncclAllGather directly.
 """
@@ -40,7 +46,7 @@ def or_allgather(local_masks, dist=None):
 
 
 def allgather_records(local_best, dist=None):
-    """All-gather the 24-byte best records.  local_best: torch uint8 tensor [R, 24] -> [world, R, 24]."""
+    """All-gather the 24-byte best records.  local_best: torch uint8 tensor [R, S * 24] -> [world, R, S * 24]."""
     import torch
     if dist is None or not dist.is_initialized() or dist.get_world_size() == 1:
         return local_best.unsqueeze(0).clone()
@@ -74,17 +80,61 @@ def merge_records_host(all_best: np.ndarray) -> np.ndarray:
     return out
 
 
-def schedule_sharded(engine, tokens_dev, uniform_len: int, dist=None):
-    """One batch through the sharded protocol on this rank's engine.  tokens_dev: torch CUDA tensor [R, T].
-    Returns a [R, 32] uint8 CUDA tensor of epp_decision records (identical on every rank)."""
+STAGE_DETAIL_DTYPE = np.dtype([("prefill_pick", "<u4"), ("prefill_score", "<f8"), ("prefill_tie_count", "<u4"),
+                               ("prefill_ran", "<u4"), ("encode_pick", "<u4"), ("encode_score", "<f8"),
+                               ("encode_tie_count", "<u4"), ("encode_ran", "<u4")])
+
+
+def pd_decide_host(nct: int, in_len_bytes: int, match_blocks: int, block_size_tokens: int) -> bool:
+    """PrefixBasedPDDecider.disaggregate (prefix_based_pd_decider.go:99-149), as score.cuh pd_decide."""
+    if nct == 0:
+        return False
+    tokens = in_len_bytes // 4
+    return tokens >= nct and tokens - match_blocks * block_size_tokens >= nct
+
+
+def merge_stage_records_host(all_best: np.ndarray, in_len, multimodal=None, *, non_cached_tokens: int = 0,
+                             always_disagg: bool = False, block_size_tokens: int = 16, encode_enabled: bool = False):
+    """Reference semantics of the staged epp_shard_merge on the host, for the CPU tests: all_best [world, R, S] of
+    SHARD_BEST_DTYPE, in_len [R] request bytes, multimodal [R] flags or None -> (decode records [R] as
+    merge_records_host returns them, STAGE_DETAIL_DTYPE [R]).  Each stage is reduced by merge_records_host; the decode
+    pick's match_blocks drives the P/D decider; no decode pick anywhere runs no other stage."""
+    world, R, S = all_best.shape
+    stages = [merge_records_host(all_best[:, :, s]) for s in range(S)]
+    dec = stages[0]
+    det = np.zeros(R, dtype=STAGE_DETAIL_DTYPE)
+    det["prefill_pick"] = NO_ENDPOINT
+    det["encode_pick"] = NO_ENDPOINT
+    for r in range(R):
+        if dec["status"][r] != 0:
+            continue
+        if S >= 3 and encode_enabled and multimodal is not None and multimodal[r]:
+            det["encode_ran"][r] = 1
+            e = stages[2][r]
+            if e["status"] == 0:
+                det["encode_pick"][r], det["encode_score"][r], det["encode_tie_count"][r] = e["pick"], e["score"], e["tie_count"]
+        if S >= 2 and (always_disagg or pd_decide_host(non_cached_tokens, int(in_len[r]), int(dec["match_blocks"][r]),
+                                                       block_size_tokens)):
+            det["prefill_ran"][r] = 1
+            p = stages[1][r]
+            if p["status"] == 0:
+                det["prefill_pick"][r], det["prefill_score"][r], det["prefill_tie_count"][r] = p["pick"], p["score"], p["tie_count"]
+    return dec, det
+
+
+def schedule_sharded(engine, tokens_dev, uniform_len: int, dist=None, detail=None, multimodal=None):
+    """One batch through the sharded protocol on this rank's engine.  tokens_dev: torch CUDA tensor [R, T]; detail: a
+    [R, 40] uint8 CUDA tensor for the epp_decision_detail records (the prefill and encode stages), or None; multimodal:
+    [R] uint8 CUDA tensor or None.  Returns a [R, 32] uint8 CUDA tensor of epp_decision records (identical on every
+    rank)."""
     import torch
     R = tokens_dev.shape[0]
     W = (engine.B + 31) // 32
     dev = tokens_dev.device
     masks = torch.empty((R, W), dtype=torch.int32, device=dev)
-    engine.shard_probe(tokens_dev, masks, uniform_len=uniform_len)
+    engine.shard_probe(tokens_dev, masks, uniform_len=uniform_len, multimodal=multimodal)
     gmasks = or_allgather(masks, dist)
-    best = torch.empty((R, 24), dtype=torch.uint8, device=dev)
+    best = torch.empty((R, 24 * engine.shard_stages), dtype=torch.uint8, device=dev)
     # The engine runs on its own streams and only guarantees that ITS outputs are complete on return; tensors produced
     # by torch / NCCL on the caller's stream must be complete before they are handed over (epp_engine.h, "streams").
     torch.cuda.current_stream(dev).synchronize()
@@ -92,7 +142,7 @@ def schedule_sharded(engine, tokens_dev, uniform_len: int, dist=None):
     allb = allgather_records(best, dist)
     dec = torch.empty((R, 32), dtype=torch.uint8, device=dev)
     torch.cuda.current_stream(dev).synchronize()
-    engine.shard_merge(R, allb.shape[0], allb, dec)
+    engine.shard_merge(R, allb.shape[0], allb, dec, out_detail=detail)
     return dec
 
 
