@@ -186,8 +186,6 @@ struct epp_engine {
                                     // 0 = automatic: 4 while the table stays L2-sized (<= l2_table_bytes), else 2
     uint64_t l2_table_bytes = 24ull << 20;  // half the device's L2: the other half stays for the streamed prompts
     int dev_chunks = 2;             // EPP_DEV_CHUNKS=N: async device batches run as N chunks over both streams (1 = off)
-    int staged = 0;                 // EPP_HASH_STAGED: 0 = hash_fused.cu (default), 1 = hash_staged.cu default shape, else a shape
-    int match_ctas = 8;             // EPP_MATCH_CTAS=6: k_match_pick_sparse's one-profile build bounded to 40 registers, not 32
     int pick_grid = 0;
     bool pick_global = false;
     size_t pick_smem = 0;
@@ -504,11 +502,9 @@ extern "C" int32_t epp_engine_create(const epp_config *cfg, epp_engine **out) {
     { const char *v1 = getenv("EPP_INDEX_PATCH"); e->patch_enabled = v1 ? atoi(v1) : 1; }
     { const char *v1 = getenv("EPP_INDEX_LOAD"); e->index_load = v1 ? std::max(2, atoi(v1)) : 0; }
     { const char *v1 = getenv("EPP_DEV_CHUNKS"); e->dev_chunks = v1 ? std::max(1, atoi(v1)) : 2; }
-    { const char *v1 = getenv("EPP_HASH_STAGED"); e->staged = v1 ? atoi(v1) : 0; }
     { const char *v1 = getenv("EPP_HASH_TRIM"); e->hash_trim = v1 ? atoi(v1) : 1; }
     { const char *v1 = getenv("EPP_HASH_SKIP"); e->hash_skip = v1 ? atoi(v1) : 1; }
     { const char *v1 = getenv("EPP_PRESENCE_LOG2BITS"); e->presence_log2_env = v1 ? std::min(30, std::max(6, atoi(v1))) : 0; }
-    { const char *v1 = getenv("EPP_MATCH_CTAS"); e->match_ctas = (v1 && atoi(v1) == 6) ? 6 : 8; }
     { const char *v1 = getenv("EPP_SMALL_BATCH"); e->small_max = v1 ? std::max(0, atoi(v1)) : 1024; }
     { const char *v1 = getenv("EPP_SMALL_ZEROCOPY"); e->small_zc_max = v1 ? std::max(0, atoi(v1)) : 8; }
     { const char *v1 = getenv("EPP_SMALL_PIPELINE"); e->small_pipe_min = v1 ? std::max(0, atoi(v1)) : 1; }
@@ -1469,7 +1465,6 @@ static HashParams hash_params(epp_engine *h, const Work &w, Slot &sl) {
     p.in_len = h->in_len.as<int64_t>() + w.r0;
     p.offsets_or_bits = w.offsets_or_bits;
     p.sm_count = h->sm_count;
-    p.staged = h->staged;
     p.presence = nullptr;
     p.presence_shift = 0;
     p.bound = nullptr;
@@ -1641,7 +1636,7 @@ static int32_t launch_match(epp_engine *h, Slot &sl, PickParams pp, int *launche
     pp.overflow_list = sl.overflow_list.as<int32_t>();
     pp.overflow_n = sl.overflow_n.as<int32_t>();
     pp.req_next = sl.overflow_n.as<int32_t>() + 1;
-    CUDA_TRY(launch_match_pick_sparse(pp, h->sm_count, h->match_ctas, s, launches));
+    CUDA_TRY(launch_match_pick_sparse(pp, h->sm_count, s, launches));
     return launch_overflow_pass(h, sl, pp, launches);
 }
 

@@ -1,7 +1,6 @@
 // hash_fused.cu -- a1 (hashPrompt, approximateprefix/hashing.go:35-99) as one CTA-cooperative kernel with register-fed
 // 128-bit global loads: the DEFAULT hash kernel of the throughput path (block sizes that are a multiple of 32
-// bytes, 16-byte aligned prompts; everything else takes the generic kernels of hash_kernels.cu).  hash_staged.cu is the
-// cp.async-staged alternative behind EPP_HASH_STAGED=1 (DESIGN.md section 4.1).
+// bytes, 16-byte aligned prompts; everything else takes the generic kernels of hash_kernels.cu; DESIGN.md section 4.1).
 //
 // HBM traffic per request: every prompt byte is read at most once, the 8-byte pre-chain digests never leave the SM
 // (shared-memory ring), the block hashes are written once (the PluginState stash PreRequest needs, plugin.go:150-157)

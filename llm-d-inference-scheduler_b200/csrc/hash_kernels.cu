@@ -1,8 +1,7 @@
 // hash_kernels.cu -- a1: batched chained XXH64 prefix-block hashing (approximateprefix/hashing.go:35-99): the dispatcher
 // and the generic path.
 //   launch_hash_prompts : block sizes that are a multiple of 32 bytes + 16-byte aligned prompts (every BASELINE
-//                         config) -> hash_fused.cu (or, EPP_HASH_STAGED=1 and 64-byte blocks, hash_staged.cu);
-//                         anything else -> the two kernels below
+//                         config) -> hash_fused.cu; anything else -> the two kernels below
 //   k_prompt_lengths    : per request, truncation + block count                     (hashing.go:58-66)
 //   k_hash_generic      : any block size / alignment, one thread per request, fully serial
 //   k_hash_bytes        : XXH64 of one message (the model || salt seed, hashing.go:71-78)
@@ -110,18 +109,15 @@ cudaError_t launch_check_offsets_aligned(const uint64_t *offsets, int64_t n, int
 cudaError_t launch_hash_fused(const HashParams &p, int sm_count, cudaStream_t s, int *launches);
 
 bool hash_fused_selected(const HashParams &p) {
-    return hash_batch_alignment(p) >= 16 && !(p.staged > 0 && hash_staged_supported(p));
+    return hash_batch_alignment(p) >= 16;
 }
 
 // ev (optional, 4 events): recorded around the hash kernel(s): [1]..[2] brackets the kernel that reads the prompt bytes.
 cudaError_t launch_hash_prompts(const HashParams &p, cudaStream_t s, int *launches, cudaEvent_t *ev) {
     if (p.R <= 0) return cudaSuccess;
-    const int align = hash_batch_alignment(p);
-    if (align >= 16) {                          // one kernel: lengths + digests + chain
+    if (hash_fused_selected(p)) {               // one kernel: lengths + digests + chain
         if (ev) { cudaEventRecord(ev[0], s); cudaEventRecord(ev[1], s); }
-        cudaError_t e;
-        if (!hash_fused_selected(p)) e = launch_hash_staged(p, p.staged, s, launches);
-        else e = launch_hash_fused(p, p.sm_count, s, launches);
+        cudaError_t e = launch_hash_fused(p, p.sm_count, s, launches);
         if (ev) { cudaEventRecord(ev[2], s); cudaEventRecord(ev[3], s); }
         return e;
     }

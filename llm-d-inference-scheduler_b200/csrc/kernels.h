@@ -26,7 +26,6 @@ struct HashParams {
     int64_t *in_len;            // [R] untruncated prompt length in bytes (P/D decider), may be nullptr
     uint64_t offsets_or_bits;   // OR of every offsets[r] (low bits decide the common alignment)
     int32_t sm_count;
-    int32_t staged;             // hash_staged.cu (cp.async-staged, warp-per-task) kernel: 0 off, 1 default shape, else a launch shape (A/B)
     // k_hash_fused only: presence != nullptr trims the rows to the read table's reach.  bound[r] = the first block at a
     // window start (every 8th block is looked up) whose presence bit is clear (index.cuh), else nblocks[r]: the global
     // stop is <= bound[r].  Hashes [0, bound[r]) are stored.
@@ -50,11 +49,6 @@ cudaError_t launch_check_offsets_aligned(const uint64_t *offsets, int64_t n, int
 // Whole hashPrompt for a batch.  Returns number of kernels launched via *launches.
 // ev (optional, 4 events): [1]..[2] brackets the kernel(s) that read the prompt bytes.
 cudaError_t launch_hash_prompts(const HashParams &p, cudaStream_t s, int *launches, cudaEvent_t *ev = nullptr);
-
-// hash_staged.cu: a1 with the prompt bytes staged through shared memory by cp.async, one warp per task of 16 / 32
-// requests, no cross-warp synchronisation.  Needs 64-byte blocks and 16-byte aligned prompts.
-bool hash_staged_supported(const HashParams &p);
-cudaError_t launch_hash_staged(const HashParams &p, int shape, cudaStream_t s, int *launches);
 
 // ------------------------------------------------------------------------------------------------
 // prefix index (a2): open-addressed table  hash -> (posting offset, count)
@@ -289,9 +283,8 @@ int match_pick_warps_per_cta();
 cudaError_t launch_match_pick(const PickParams &p, uint32_t *gscratch, int grid, size_t smem, cudaStream_t s,
                               int *launches);
 // The same decision per request with a lane-distributed register map of the matched endpoints (requests whose set
-// overflows it are appended to p.overflow_list for the dense-counter kernel).  8 warps per CTA, 6-8 CTAs per SM;
-// ctas = 6 bounds the one-profile lowest-slot build to 40 registers instead of 32 (the engine's EPP_MATCH_CTAS).
-cudaError_t launch_match_pick_sparse(const PickParams &p, int sm_count, int ctas, cudaStream_t s, int *launches);
+// overflows it are appended to p.overflow_list for the dense-counter kernel).  8 warps per CTA, 6-8 CTAs per SM.
+cudaError_t launch_match_pick_sparse(const PickParams &p, int sm_count, cudaStream_t s, int *launches);
 // Does some profile of the launch (PickParams, DensePickParams) have a random picker?  Then the sparse, small-batch,
 // dense-counter and injected-match paths launch their _rand builds.
 // Stages of the handler of a launch (PickParams, DensePickParams): 1 = single profile, 2 = decode + prefill, 3 = + encode.

@@ -86,7 +86,7 @@ cudaError_t launch_nohit(const PickParams &p, int sm_count, cudaStream_t s) {
 }
 }  // namespace
 
-cudaError_t launch_match_pick_sparse(const PickParams &p, int sm_count, int ctas, cudaStream_t s, int *launches) {
+cudaError_t launch_match_pick_sparse(const PickParams &p, int sm_count, cudaStream_t s, int *launches) {
     if (p.R <= 0) return cudaSuccess;
     if (!p.req_next || p.R > INT32_MAX) return cudaErrorInvalidValue;
     const bool tie = p.tie_seed != 0;
@@ -106,7 +106,7 @@ cudaError_t launch_match_pick_sparse(const PickParams &p, int sm_count, int ctas
         else if (stages == 2) e = tie ? launch_nohit<true, 2>(p, sm_count, s) : launch_nohit<false, 2>(p, sm_count, s);
         else e = tie ? launch_nohit<true, 3>(p, sm_count, s) : launch_nohit<false, 3>(p, sm_count, s);
     }
-    else if (stages == 1 && !tie) e = ctas == 6 ? launch_one<6, false, false, 1>(p, sm_count, s) : launch_one<8, false, false, 1>(p, sm_count, s);
+    else if (stages == 1 && !tie) e = launch_one<8, false, false, 1>(p, sm_count, s);
     else if (stages == 1) e = launch_one<6, false, true, 1>(p, sm_count, s);
     else if (stages == 2) e = tie ? launch_one<6, false, true, 2>(p, sm_count, s) : launch_one<6, false, false, 2>(p, sm_count, s);
     else e = tie ? launch_one<6, false, true, 3>(p, sm_count, s) : launch_one<6, false, false, 3>(p, sm_count, s);

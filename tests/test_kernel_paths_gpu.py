@@ -213,19 +213,17 @@ def _spec(epp, filt, scorers):
 
 
 # ------------------------------------------------------------------------------------------------
-# 2. k_hash_staged (EPP_HASH_STAGED)
+# 2. k_hash_fused: rows at 16 mod 32, one odd-length request per batch
 # ------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("shape,kernel", [("1", "k_hash_staged<16, 4, 4>"), ("1634", "k_hash_staged<16, 3, 4>"),
-                                          ("3244", "k_hash_staged<32, 4, 4>")])
-def test_staged_hash_kernel_vs_oracle_and_default(epp, orc, monkeypatch, shape, kernel):
+@pytest.mark.parametrize("seed", [1, 1634, 3244])
+def test_fused_hash_rows_at_16_vs_oracle(epp, orc, seed):
     """64-byte blocks, rows at 16 mod 32 with `lengths` shorter than the rows: one short request among long ones and one
-    long request among short ones (the unchecked-copy shortcut below the task's shortest request), R not a multiple of
-    16 or 32.  Hashes and decisions against the oracle and against the default kernel."""
+    long request among short ones, R not a multiple of 16 or 32.  Hashes and decisions against the oracle."""
     import torch
     import helpers
     E, bst, maxb = 48, 16, 77
     bb = 4 * bst
-    rng = np.random.default_rng(int(shape))
+    rng = np.random.default_rng(seed)
     fam = _families(rng, 4, bb * (maxb + 2))
     hs_pairs, es_pairs = _family_pairs(orc, rng, fam, b"m", bst, maxb, E, [2, 5, 9, 40])
     kv = rng.integers(0, 3, E) / 3.0
@@ -239,40 +237,26 @@ def test_staged_hash_kernel_vs_oracle_and_default(epp, orc, monkeypatch, shape, 
     for R, odd_one, odd_len, usual_len in ((45, 20, short_n, long_n), (77, 50, long_n, short_n), (100, 99, short_n, long_n)):
         batches.append([_prompt_of_len(rng, fam, odd_len() if r == odd_one else usual_len()) for r in range(R)])
 
-    def run(env):
-        if env is None:
-            monkeypatch.delenv("EPP_HASH_STAGED", raising=False)
-        else:
-            monkeypatch.setenv("EPP_HASH_STAGED", env)
-        out = []
-        with epp.Engine(E, _spec(epp, 0, PRIM), block_size_tokens=bst, max_prefix_blocks=maxb) as eng:
-            eng.register_model(b"m")
-            eng.pool_set(np.arange(E), np.zeros(E, np.uint8), kv, waiting)
-            eng.index_load_snapshot(hs_pairs, es_pairs)
-            for bi, prompts in enumerate(batches):
-                d, o, ln = _aligned(prompts, 16, 3, rng=np.random.default_rng(bi))
-                (hs, nb), names = kernels_launched(lambda: eng.hash_prompts(d, offsets=o, lengths=ln))
-                assert_ran(names, kernel if env else FUSED, ("k_hash_staged<", GENERIC) if env is None else (FUSED, GENERIC),
-                           where=f"EPP_HASH_STAGED={env} batch {bi}")
-                dd, do, dl = _to_dev(d, o, ln)
-                (ddec, ddet), names = kernels_launched(lambda: eng.schedule(dd, offsets=do, lengths=dl))
-                assert_ran(names, kernel if env else FUSED, (GENERIC,), where=f"EPP_HASH_STAGED={env} schedule {bi}")
-                torch.cuda.synchronize()
-                dec = epp.decisions_from_torch(ddec)
-                det = ddet.cpu().numpy().view(epp.DETAIL_DTYPE).reshape(-1)
-                out.append((hs.copy(), nb.copy(), dec, det))
-        return out
-
-    staged, default = run(shape), run(None)
-    for bi, prompts in enumerate(batches):
-        hs, nb, dec, det = staged[bi]
-        _assert_hashes(hs, nb, [orc.hash_prompt(p, b"m", bst, maxb) for p in prompts], f"staged {shape} batch {bi}")
-        pd, po = _pack(prompts)
-        odec, ototal = orc.cycle_batch(b"m", bst, maxb, 0, False, ix, orc.make_profile(0, PRIM), None, pool, pd, po, 4)
-        helpers.assert_decisions_equal(dec, det, odec, ototal, where=f"staged {shape} batch {bi}")
-        for a, b in zip(staged[bi], default[bi]):
-            np.testing.assert_array_equal(a, b)
-        assert (dec["match_blocks"] > 0).any()
+    with epp.Engine(E, _spec(epp, 0, PRIM), block_size_tokens=bst, max_prefix_blocks=maxb) as eng:
+        eng.register_model(b"m")
+        eng.pool_set(np.arange(E), np.zeros(E, np.uint8), kv, waiting)
+        eng.index_load_snapshot(hs_pairs, es_pairs)
+        for bi, prompts in enumerate(batches):
+            where = f"seed {seed} batch {bi}"
+            d, o, ln = _aligned(prompts, 16, 3, rng=np.random.default_rng(bi))
+            (hs, nb), names = kernels_launched(lambda: eng.hash_prompts(d, offsets=o, lengths=ln))
+            assert_ran(names, FUSED, (GENERIC,), where=where)
+            _assert_hashes(hs, nb, [orc.hash_prompt(p, b"m", bst, maxb) for p in prompts], where)
+            dd, do, dl = _to_dev(d, o, ln)
+            (ddec, ddet), names = kernels_launched(lambda: eng.schedule(dd, offsets=do, lengths=dl))
+            assert_ran(names, FUSED, (GENERIC,), where=f"{where} schedule")
+            torch.cuda.synchronize()
+            dec = epp.decisions_from_torch(ddec)
+            det = ddet.cpu().numpy().view(epp.DETAIL_DTYPE).reshape(-1)
+            pd, po = _pack(prompts)
+            odec, ototal = orc.cycle_batch(b"m", bst, maxb, 0, False, ix, orc.make_profile(0, PRIM), None, pool, pd, po, 4)
+            helpers.assert_decisions_equal(dec, det, odec, ototal, where=where)
+            assert (dec["match_blocks"] > 0).any()
 
 
 # ------------------------------------------------------------------------------------------------
@@ -531,15 +515,12 @@ def test_adversarial_read_tables_vs_oracle(epp, orc, monkeypatch, patch):
 # ------------------------------------------------------------------------------------------------
 # 5. every non-sharded instantiation of k_match_pick_sparse
 # ------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("ctas", ["8", "6"])
 @pytest.mark.parametrize("tie_seed", [0, 0x5EED])
 @pytest.mark.parametrize("stages", [1, 2, 3])
-def test_match_kernel_instantiations_vs_oracle(epp, orc, monkeypatch, stages, tie_seed, ctas):
-    """1 / 2 / 3 handler stages x lowest-slot / random tie rule x EPP_MATCH_CTAS 8 / 6, with requests whose holders
-    overflow the sparse map: decisions equal to the oracle's, through the instantiation launch_match_pick_sparse picks.
-    EPP_MATCH_CTAS is an engine setting: an engine created without it in the same process uses the default build."""
+def test_match_kernel_instantiations_vs_oracle(epp, orc, stages, tie_seed):
+    """1 / 2 / 3 handler stages x lowest-slot / random tie rule, with requests whose holders overflow the sparse map:
+    decisions equal to the oracle's, through the instantiation launch_match_pick_sparse picks."""
     import helpers
-    monkeypatch.setenv("EPP_MATCH_CTAS", ctas)
     E, bst, B = 96, 2, 16
     rng = np.random.default_rng(stages * 10 + (tie_seed != 0))
     kv = rng.integers(0, 2, E) / 2.0
@@ -562,7 +543,7 @@ def test_match_kernel_instantiations_vs_oracle(epp, orc, monkeypatch, stages, ti
         kw["non_cached_tokens"] = 4
     if stages == 3:
         kw["encode"] = _spec(epp, 3, ENC)
-    mincta = ctas if stages == 1 and not tie_seed else "6"
+    mincta = 8 if stages == 1 and not tie_seed else 6
     kernel = f"k_match_pick_sparse<{mincta}, false, {'true' if tie_seed else 'false'}, {stages}>"
     with epp.Engine(E, *specs, **kw) as eng:
         eng.register_model(b"m")
@@ -576,12 +557,3 @@ def test_match_kernel_instantiations_vs_oracle(epp, orc, monkeypatch, stages, ti
                                    4, tie_seed=tie_seed, tie_base=0, encode=enc, multimodal=mm)
     helpers.assert_decisions_equal(dec, det, odec, ototal, where=kernel)
     assert (dec["match_blocks"] > 0).sum() > 50 and (dec["tie_count"] > 1).any()
-    if ctas == "6" and stages == 1 and not tie_seed:
-        monkeypatch.delenv("EPP_MATCH_CTAS")
-        with epp.Engine(E, *specs, **kw) as eng:
-            eng.register_model(b"m")
-            eng.pool_set(np.arange(E), role, kv, waiting)
-            eng.index_load_snapshot(hs_pairs, es_pairs)
-            (dec2, _), names = kernels_launched(lambda: eng.schedule(d, offsets=o))
-            assert_ran(names, "k_match_pick_sparse<8, false, false, 1>", where="default engine")
-        np.testing.assert_array_equal(dec2, dec)

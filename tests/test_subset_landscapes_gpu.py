@@ -550,7 +550,7 @@ def check_walk(orc, W, ix, dec, det, prompts, subsets, tie_seed, base, where):
 
 
 @pytest.mark.parametrize("E,variant", [(256, "fused"), (256, "odd-packed"), (256, "EPP_HASH_TRIM=0"),
-                                       (256, "EPP_HASH_SKIP=0"), (256, "EPP_HASH_STAGED=1"), (4096, "fused")])
+                                       (256, "EPP_HASH_SKIP=0"), (4096, "fused")])
 def test_match_walk(epp, orc, monkeypatch, E, variant):
     """Global stops at blocks 0, 31, 32, 33, 63, 64 and the cap, non-contiguous holders, 6 / 33 (/ 1100) holders of a
     block, prompts shorter than a block; aligned rows through the fused kernel (trimmed) or an odd-offset blob through
@@ -569,7 +569,7 @@ def test_match_walk(epp, orc, monkeypatch, E, variant):
     where = f"walk E={E} {variant}"
     assert_subset_ran(names, "device", where)
     if helpers.trace_complete(names):
-        want = {"fused": "k_hash_fused(", "odd-packed": "k_hash_generic(", "EPP_HASH_STAGED=1": "k_hash_staged<"}
+        want = {"fused": "k_hash_fused(", "odd-packed": "k_hash_generic("}
         if variant in want:
             helpers.assert_ran(names, want[variant], where=where)
     check_walk(orc, W, ix, dec, det, prompts, subsets, tie_seed, base, where)

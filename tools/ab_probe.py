@@ -3,7 +3,7 @@
 on ONE GPU and checks that every variant produces identical decisions / hashes.  The engine reads its EPP_* switches
 at epp_engine_create, so each variant is a fresh engine with its own environment.
 
-    python tools/ab_probe.py --variants 'base:;staged:EPP_HASH_STAGED=1;m6:EPP_MATCH_CTAS=6' [--workload config3]
+    python tools/ab_probe.py --variants 'base:;noskip:EPP_HASH_SKIP=0;notrim:EPP_HASH_TRIM=0' [--workload config3]
 
 Prints one JSON line per variant: ms per step of K back-to-back async device batches (CUDA events on the engine's
 stream), the synchronous per-kernel event times, and ms per hash-only pass.  Development tool (not the bench).
@@ -23,7 +23,7 @@ sys.path.insert(0, ROOT)
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--variants", default="base:;staged:EPP_HASH_STAGED=1")
+    ap.add_argument("--variants", default="base:;noskip:EPP_HASH_SKIP=0")
     ap.add_argument("--workload", default="config3")
     ap.add_argument("--requests", type=int, default=0)
     ap.add_argument("--steps", type=int, default=10)

@@ -4,10 +4,10 @@
     # on the GPU box (EPP_DEV_CHUNKS=1: every launch covers the whole batch, like the synchronous pass whose CUDA-event
     # time bench.py divides the bytes by)
     EPP_DEV_CHUNKS=1 ncu --metrics dram__bytes_read.sum,dram__bytes_write.sum,gpu__time_duration.sum --clock-control none \\
-        -k regex:'k_hash_fused|k_hash_staged|k_match_pick_sparse' -s 6 -c 4 --csv --log-file gpurun_out/traffic.csv \\
+        -k regex:'k_hash_fused|k_match_pick_sparse' -s 6 -c 4 --csv --log-file traffic.csv \\
         python bench.py --no-e2e --no-cpu --no-index-write --no-full-index --steps 2 --warmup 3
     # here
-    python tools/ncu_traffic.py gpurun_out/traffic.csv config3
+    python tools/ncu_traffic.py traffic.csv config3
 
 Per kernel the capture's LAST launch is kept (steady state); traffic = dram read + write bytes of that launch."""
 import csv
