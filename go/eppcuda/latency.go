@@ -224,3 +224,32 @@ func (e *Engine) schedulePredicted(model uint32, prompt []byte, multimodal bool,
 		return C.epp_submit_predicted(e.b, C.uint32_t(model), p, C.uint64_t(len(prompt)), mm, C.uint32_t(len(pred)), pp, ticket)
 	})
 }
+
+// scheduleSubsetPredicted = schedulePredicted for a request whose candidates are the endpoints of `slots` (sorted, at
+// most C.EPP_SUBSET_MAX_SLOTS), with the predictions of those candidates (epp_submit_subset_predicted).
+func (e *Engine) scheduleSubsetPredicted(model uint32, prompt []byte, multimodal bool, slots []uint32,
+	pred []C.epp_prediction) (Decision, error) {
+	if len(pred) > int(C.EPP_PRED_MAX_SLOTS) {
+		return Decision{}, fmt.Errorf("eppcuda: %d predictions, more than EPP_PRED_MAX_SLOTS", len(pred))
+	}
+	return e.submitAndWait(func(ticket *C.uint64_t) C.int32_t {
+		var p unsafe.Pointer
+		if len(prompt) > 0 {
+			p = unsafe.Pointer(&prompt[0])
+		}
+		mm := C.uint32_t(0)
+		if multimodal {
+			mm = 1
+		}
+		var sp *C.uint32_t
+		if len(slots) > 0 {
+			sp = (*C.uint32_t)(unsafe.Pointer(&slots[0]))
+		}
+		var pp *C.epp_prediction
+		if len(pred) > 0 {
+			pp = &pred[0]
+		}
+		return C.epp_submit_subset_predicted(e.b, C.uint32_t(model), p, C.uint64_t(len(prompt)), mm, C.uint32_t(len(slots)),
+			sp, C.uint32_t(len(pred)), pp, ticket)
+	})
+}

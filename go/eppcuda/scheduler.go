@@ -54,7 +54,8 @@ func (s *Scheduler) Schedule(ctx context.Context, request *scheduling.InferenceR
 		return nil, errors.New("failed to find available decode workers")
 	}
 	// A director-side subset (candidates.Locate with x-gateway-destination-endpoint-subset metadata, director.go:222-243)
-	// goes to the engine as the sorted slots of the candidates (epp_submit_subset); the whole pool as no subset.
+	// goes to the engine as the sorted slots of the candidates (epp_submit_subset, or epp_submit_subset_predicted on a
+	// latency engine); the whole pool as no subset.
 	s.Engine.mu.RLock()
 	slots := make([]uint32, 0, len(byName)) // non-nil: no candidates is an empty subset (status -1), never the whole pool
 	known := true
@@ -68,8 +69,8 @@ func (s *Scheduler) Schedule(ctx context.Context, request *scheduling.InferenceR
 	}
 	whole := known && len(slots) == len(s.Engine.slotOf)
 	s.Engine.mu.RUnlock()
-	// a latency engine takes no subsets: a restricted request goes to the fallback scheduler
-	if !known || (!whole && (s.Engine.latency || len(slots) > int(C.EPP_SUBSET_MAX_SLOTS))) {
+	// a candidate the snapshot does not know, or a subset too large for the batcher's staging: the fallback scheduler
+	if !known || (!whole && len(slots) > int(C.EPP_SUBSET_MAX_SLOTS)) {
 		if s.Fallback != nil {
 			return s.Fallback.Schedule(ctx, request, candidates)
 		}
@@ -94,8 +95,10 @@ func (s *Scheduler) Schedule(ctx context.Context, request *scheduling.InferenceR
 	}
 	mm := HasMultimodalContent != nil && HasMultimodalContent(request)
 	var d Decision
-	if s.Engine.latency {
+	if s.Engine.latency && slots == nil {
 		d, err = s.Engine.schedulePredicted(model, prompt, mm, s.Engine.predictions(candidates))
+	} else if s.Engine.latency {
+		d, err = s.Engine.scheduleSubsetPredicted(model, prompt, mm, slots, s.Engine.predictions(candidates))
 	} else {
 		d, err = s.Engine.scheduleSubset(model, prompt, mm, slots)
 	}

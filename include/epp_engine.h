@@ -512,7 +512,11 @@ EPP_API int32_t epp_schedule_with_match_topk(epp_engine *h, int64_t n_requests, 
  * changes; so does any subset call on an endpoint-sharded or peer-memory engine.  EPP_SUBSET_ALL rows are decided exactly as
  * by epp_schedule; a batch without a restricted row IS epp_schedule.  Restricted rows are re-decided by a kernel of their
  * own after the batch's match kernels (so such batches never take the small-batch single-launch path); its device time is
- * epp_stats.last_kernel_ms[6] on device-pointer batches (0 otherwise). */
+ * epp_stats.last_kernel_ms[6] on device-pointer batches (0 otherwise).
+ * On an engine with latency profiles ("Latency predictions" below) epp_schedule_subset and epp_submit_subset refuse
+ * subsets with EPP_ERR_INVALID; epp_schedule_subset_predicted and epp_submit_subset_predicted take them, with or without
+ * predictions, and decide a restricted request's latency profiles over its subset candidates (the rules are stated
+ * there).  Non-latency profiles of such an engine follow the rules above. */
 #define EPP_SUBSET_ALL 0xFFFFFFFFu
 typedef struct {
     uint32_t struct_size;          /* sizeof(epp_subset)                                                                 */
@@ -569,8 +573,25 @@ EPP_API int32_t epp_schedule_subset(epp_engine *h, const epp_batch *batch, const
  * Predictions are HOST memory for every batch kind, validated and copied before the call returns.  A slot list that is not
  * strictly ascending, a slot >= max_endpoints, a non-finite ttft or headroom, a wrong struct_size, or predictions on an
  * engine without a latency profile fail the call with EPP_ERR_INVALID before anything is launched and before any LRU,
- * counter or ordinal state changes.  Endpoint subsets (epp_schedule_subset, epp_submit_subset) and the endpoint-sharded
- * modes are not available on a latency engine.  Plain epp_schedule* on a latency engine decides every request without predictions. */
+ * counter or ordinal state changes.  The endpoint-sharded modes are not available on a latency engine, and neither are
+ * epp_schedule_subset and epp_submit_subset: endpoint subsets go through epp_schedule_subset_predicted /
+ * epp_submit_subset_predicted.  Plain epp_schedule* on a latency engine decides every request without predictions.
+ * A restricted request on a latency engine is decided exactly as the reference decides it when Schedule receives the
+ * subset's endpoints and the producer has attached that request's predictions:
+ *   - A profile's candidates are the subset slots that are in the pool and pass its role and label filters; the chain
+ *     [A1] -> [T] -> [A2] -> scorers -> picker runs over those only.  Everything taken "over the set" uses the narrowed set:
+ *     A1's and A2's len(endpoints) <= 1 gates, sticky sets and best-TTFT sets; T's tiers and its "no entry anywhere: keep
+ *     all" rule; the queue / running min-max and the active-request max; the latency scorer's bucket, its |headroom|
+ *     ranges and the composite fallback's maxQ; tie_count, the tie and first-k ranks and the random pickers' population
+ *     (every candidate an explicit item, as on every latency profile).
+ *   - The prefix match is not narrowed: totalBlocks, the global stop and each member's matchBlocks are whole-pool values,
+ *     in the sticky tests and the composite prefix term as everywhere else.
+ *   - Entries for slots outside the subset are ignored; a subset slot without an entry has no attribute.
+ *   - Draw keys and domains are unchanged.  Since latency profiles fold every candidate explicitly in ascending slot order,
+ *     a request whose subset lists the whole pool gets bit-identical decisions to the same request without a subset, for
+ *     all three pickers.
+ *   - An empty subset gives status -1; ordinals, the in-flight adds and epp_index_add_picked read subset picks like any
+ *     other.  No-hit-lru stays refused on latency profiles. */
 enum { EPP_HEADROOM_LEAST = 0, EPP_HEADROOM_MOST = 1 };
 typedef struct {
     uint32_t struct_size;              /* sizeof(epp_latency_cfg)                                                      */
@@ -613,6 +634,13 @@ EPP_API int32_t epp_schedule_with_match_predicted(epp_engine *h, int64_t n_reque
                                                   const uint32_t *model_ids, const int64_t *input_len_bytes,
                                                   int32_t block_size_tokens, epp_decision *out, epp_decision_detail *detail,
                                                   uint32_t flags, const epp_topk_out *topk, const epp_predictions *preds);
+/* Endpoint subsets and predictions in one call.  subset == NULL is exactly epp_schedule_predicted; preds == NULL is
+ * epp_schedule_subset, except that a latency engine is accepted (its restricted requests are then decided without
+ * entries).  Both arrays are validated, with every rule of the two calls, before anything is launched: a rejected call
+ * changes no ordinal, LRU or counter state. */
+EPP_API int32_t epp_schedule_subset_predicted(epp_engine *h, const epp_batch *batch, const epp_subset *subset,
+                                              const epp_predictions *preds, epp_decision *out, epp_decision_detail *detail,
+                                              int32_t keep_hashes, const epp_topk_out *topk /* or NULL */);
 
 /* PreRequest (approximateprefix/plugin.go:164-200): index the hashes of the LAST epp_schedule batch
  * (keep_hashes=1) for each request's primary pick and prefill pick. */
@@ -749,8 +777,9 @@ EPP_API int32_t epp_submit(epp_batcher *b, uint32_t model_id, const void *prompt
                            uint32_t multimodal, uint64_t *out_ticket);
 /* epp_submit for a request whose candidates are the n_slots endpoints slots[0 .. n_slots) (see "Endpoint subsets"; any
  * order, duplicates allowed: the batcher sorts and deduplicates them).  Up to EPP_SUBSET_MAX_SLOTS slots, kept in the
- * batcher's staging next to the prompt; more is EPP_ERR_CAPACITY, a slot >= max_endpoints EPP_ERR_INVALID.  A flush
- * holding a request submitted this way runs epp_schedule_subset, every other flush epp_schedule. */
+ * batcher's staging next to the prompt; more is EPP_ERR_CAPACITY, a slot >= max_endpoints EPP_ERR_INVALID, and so is an
+ * engine with latency profiles (use epp_submit_subset_predicted there).  A flush holding a request submitted this way
+ * runs epp_schedule_subset, every other flush epp_schedule. */
 #define EPP_SUBSET_MAX_SLOTS 1024
 EPP_API int32_t epp_submit_subset(epp_batcher *b, uint32_t model_id, const void *prompt, uint64_t prompt_len,
                                   uint32_t multimodal, uint32_t n_slots, const uint32_t *slots, uint64_t *out_ticket);
@@ -761,6 +790,13 @@ EPP_API int32_t epp_submit_subset(epp_batcher *b, uint32_t model_id, const void 
 #define EPP_PRED_MAX_SLOTS 1024
 EPP_API int32_t epp_submit_predicted(epp_batcher *b, uint32_t model_id, const void *prompt, uint64_t prompt_len,
                                      uint32_t multimodal, uint32_t n, const epp_prediction *entries, uint64_t *out_ticket);
+/* epp_submit for a request on a latency engine with both an endpoint subset (n_slots slots, as for epp_submit_subset) and
+ * its predictions (n_pred entries, as for epp_submit_predicted).  Both lists are checked here with every rule of those two
+ * calls (so a latency engine is required) and staged next to the prompt.  On a latency engine every flush that holds a
+ * subset or a prediction row runs epp_schedule_subset_predicted. */
+EPP_API int32_t epp_submit_subset_predicted(epp_batcher *b, uint32_t model_id, const void *prompt, uint64_t prompt_len,
+                                            uint32_t multimodal, uint32_t n_slots, const uint32_t *slots, uint32_t n_pred,
+                                            const epp_prediction *entries, uint64_t *out_ticket);
 EPP_API int32_t epp_wait(epp_batcher *b, uint64_t ticket, epp_decision *out, epp_decision_detail *out_detail);
 /* The same on an engine created with pick_k > 1, plus the request's first-k lists (ProfileRunResult.TargetEndpoints of
  * each profile, see epp_topk_out): primary / prefill / encode receive pick_k slot ids each (EPP_NO_ENDPOINT padded); any

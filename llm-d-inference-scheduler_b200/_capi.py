@@ -180,6 +180,8 @@ SIGNATURES = {
     "epp_schedule_with_match_predicted": (C.c_int32, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                                       C.c_int32, C.c_void_p, C.c_void_p, C.c_uint32, C.POINTER(TopkOut),
                                                       C.POINTER(Predictions)]),
+    "epp_schedule_subset_predicted": (C.c_int32, [C.c_void_p, C.POINTER(Batch), C.POINTER(Subset), C.POINTER(Predictions),
+                                                  C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(TopkOut)]),
     "epp_index_add_picked": (C.c_int32, [C.c_void_p]),
     "epp_nohit_lru_get": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(C.c_int32)]),
     "epp_inflight_release": (C.c_int32, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
@@ -209,6 +211,8 @@ SIGNATURES = {
                                       C.POINTER(C.c_uint64)]),
     "epp_submit_predicted": (C.c_int32, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_uint32, C.c_uint32, C.c_void_p,
                                          C.POINTER(C.c_uint64)]),
+    "epp_submit_subset_predicted": (C.c_int32, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_uint32, C.c_uint32,
+                                                C.c_void_p, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint64)]),
     "epp_wait": (C.c_int32, [C.c_void_p, C.c_uint64, C.POINTER(Decision), C.POINTER(DecisionDetail)]),
     "epp_wait_topk": (C.c_int32, [C.c_void_p, C.c_uint64, C.POINTER(Decision), C.POINTER(DecisionDetail), C.c_void_p,
                                   C.c_void_p, C.c_void_p]),

@@ -178,24 +178,29 @@ static void flusher_main(epp_batcher *b) {
         tk.struct_size = sizeof tk;
         tk.k = b->pick_k;
         tk.primary = st.topk[0]; tk.prefill = st.topk[1]; tk.encode = st.topk[2];
-        if (st.any_pred.load(std::memory_order_acquire)) {
-            // a latency engine takes no subsets (epp_submit_subset refuses them), so the two never share a batch
+        const bool any_pred = st.any_pred.load(std::memory_order_acquire) != 0;
+        const bool any_sub = st.any_subset.load(std::memory_order_acquire) != 0;
+        if (any_pred || any_sub) {
+            // predictions only reach a latency engine (every predicted submit checks it), where subsets and predictions
+            // may share a batch and even a row: one epp_schedule_subset_predicted decides them all
             epp_predictions pr;
             memset(&pr, 0, sizeof pr);
             pr.struct_size = sizeof pr;
             pr.counts = st.pred_counts.data();
             pr.offsets = st.pred_offsets.data();
             pr.entries = st.pred_entries.data();
-            rc = epp_schedule_predicted(b->eng, &batch, &pr, st.dec, st.det, b->cfg.index_picks ? 1 : 0, b->pick_k > 1 ? &tk : nullptr);
-            st.any_pred.store(0, std::memory_order_relaxed);
-        } else if (st.any_subset.load(std::memory_order_acquire)) {
             epp_subset sub;
             memset(&sub, 0, sizeof sub);
             sub.struct_size = sizeof sub;
             sub.counts = st.sub_counts.data();
             sub.offsets = st.sub_offsets.data();
             sub.slots = st.sub_slots.data();
-            rc = epp_schedule_subset(b->eng, &batch, &sub, st.dec, st.det, b->cfg.index_picks ? 1 : 0, b->pick_k > 1 ? &tk : nullptr);
+            if (engine_latency_mask(b->eng))
+                rc = epp_schedule_subset_predicted(b->eng, &batch, any_sub ? &sub : nullptr, any_pred ? &pr : nullptr, st.dec, st.det,
+                                                   b->cfg.index_picks ? 1 : 0, b->pick_k > 1 ? &tk : nullptr);
+            else
+                rc = epp_schedule_subset(b->eng, &batch, &sub, st.dec, st.det, b->cfg.index_picks ? 1 : 0, b->pick_k > 1 ? &tk : nullptr);
+            st.any_pred.store(0, std::memory_order_relaxed);
             st.any_subset.store(0, std::memory_order_relaxed);
         } else if (b->pick_k > 1) {
             rc = epp_schedule_topk(b->eng, &batch, st.dec, st.det, b->cfg.index_picks ? 1 : 0, &tk);
@@ -384,17 +389,16 @@ extern "C" int32_t epp_submit(epp_batcher *b, uint32_t model_id, const void *pro
     return submit_impl(b, model_id, prompt, prompt_len, multimodal, nullptr, out_ticket);
 }
 
-extern "C" int32_t epp_submit_subset(epp_batcher *b, uint32_t model_id, const void *prompt, uint64_t prompt_len,
-                                     uint32_t multimodal, uint32_t n_slots, const uint32_t *slots, uint64_t *out_ticket) {
-    if (!b || !out_ticket || (prompt_len && !prompt) || (n_slots && !slots)) return bfail(EPP_ERR_INVALID, "NULL argument");
+// A subset's slots checked (every rule epp_schedule_subset applies, bar the engine's kind), sorted and deduplicated into
+// *sub, and the subset staging allocated.  Checked here rather than at the flush, where a bad list would fail every
+// request of the batch.
+static int32_t take_subset(epp_batcher *b, uint32_t n_slots, const uint32_t *slots, std::vector<uint32_t> *sub) {
     if (n_slots > EPP_SUBSET_MAX_SLOTS) return bfail(EPP_ERR_CAPACITY, "more than EPP_SUBSET_MAX_SLOTS slots in one subset");
-    // refused here rather than at the flush, where it would fail every request of the batch
-    if (engine_latency_mask(b->eng)) return bfail(EPP_ERR_INVALID, "endpoint subsets are not available on an engine with latency profiles");
-    std::vector<uint32_t> sub(slots, slots + n_slots);
-    for (uint32_t e : sub)
+    sub->assign(slots, slots + n_slots);
+    for (uint32_t e : *sub)
         if (e >= b->max_endpoints) return bfail(EPP_ERR_INVALID, "subset slot >= max_endpoints");
-    std::sort(sub.begin(), sub.end());
-    sub.erase(std::unique(sub.begin(), sub.end()), sub.end());
+    std::sort(sub->begin(), sub->end());
+    sub->erase(std::unique(sub->begin(), sub->end()), sub->end());
     std::call_once(b->sub_once, [b] {
         try {
             for (int i = 0; i < kBufs; i++) b->buf[i].sub_slots.resize((size_t)b->cfg.max_batch * EPP_SUBSET_MAX_SLOTS);
@@ -403,24 +407,23 @@ extern "C" int32_t epp_submit_subset(epp_batcher *b, uint32_t model_id, const vo
         }
     });
     if (b->sub_alloc_failed) return bfail(EPP_ERR_CAPACITY, "cannot allocate the batcher's subset staging");
-    return submit_impl(b, model_id, prompt, prompt_len, multimodal, &sub, out_ticket);
+    return EPP_OK;
 }
 
-extern "C" int32_t epp_submit_predicted(epp_batcher *b, uint32_t model_id, const void *prompt, uint64_t prompt_len,
-                                        uint32_t multimodal, uint32_t n, const epp_prediction *entries, uint64_t *out_ticket) {
-    if (!b || !out_ticket || (prompt_len && !prompt) || (n && !entries)) return bfail(EPP_ERR_INVALID, "NULL argument");
+// A request's predictions checked with every rule epp_schedule_predicted applies, sorted by slot into *pred, and the
+// prediction staging allocated.
+static int32_t take_predictions(epp_batcher *b, uint32_t n, const epp_prediction *entries, std::vector<epp_prediction> *pred) {
     if (n > EPP_PRED_MAX_SLOTS) return bfail(EPP_ERR_CAPACITY, "more than EPP_PRED_MAX_SLOTS predictions for one request");
-    // every rule epp_schedule_predicted checks, so that one request's predictions never fail its batch
     if (!engine_latency_mask(b->eng)) return bfail(EPP_ERR_INVALID, "predictions passed to an engine without a latency profile");
-    std::vector<epp_prediction> pred(entries, entries + n);
-    for (const epp_prediction &p : pred) {
+    pred->assign(entries, entries + n);
+    for (const epp_prediction &p : *pred) {
         if (p.slot >= b->max_endpoints) return bfail(EPP_ERR_INVALID, "prediction slot >= max_endpoints");
         if (!std::isfinite(p.ttft) || !std::isfinite(p.ttft_headroom) || !std::isfinite(p.tpot_headroom))
             return bfail(EPP_ERR_INVALID, "a prediction is not finite");
     }
-    std::sort(pred.begin(), pred.end(), [](const epp_prediction &x, const epp_prediction &y) { return x.slot < y.slot; });
-    for (size_t i = 1; i < pred.size(); i++)
-        if (pred[i].slot == pred[i - 1].slot) return bfail(EPP_ERR_INVALID, "two predictions for one slot");
+    std::sort(pred->begin(), pred->end(), [](const epp_prediction &x, const epp_prediction &y) { return x.slot < y.slot; });
+    for (size_t i = 1; i < pred->size(); i++)
+        if ((*pred)[i].slot == (*pred)[i - 1].slot) return bfail(EPP_ERR_INVALID, "two predictions for one slot");
     std::call_once(b->pred_once, [b] {
         try {
             for (int i = 0; i < kBufs; i++) b->buf[i].pred_entries.resize((size_t)b->cfg.max_batch * EPP_PRED_MAX_SLOTS);
@@ -429,7 +432,41 @@ extern "C" int32_t epp_submit_predicted(epp_batcher *b, uint32_t model_id, const
         }
     });
     if (b->pred_alloc_failed) return bfail(EPP_ERR_CAPACITY, "cannot allocate the batcher's prediction staging");
+    return EPP_OK;
+}
+
+extern "C" int32_t epp_submit_subset(epp_batcher *b, uint32_t model_id, const void *prompt, uint64_t prompt_len,
+                                     uint32_t multimodal, uint32_t n_slots, const uint32_t *slots, uint64_t *out_ticket) {
+    if (!b || !out_ticket || (prompt_len && !prompt) || (n_slots && !slots)) return bfail(EPP_ERR_INVALID, "NULL argument");
+    if (n_slots > EPP_SUBSET_MAX_SLOTS) return bfail(EPP_ERR_CAPACITY, "more than EPP_SUBSET_MAX_SLOTS slots in one subset");
+    if (engine_latency_mask(b->eng))
+        return bfail(EPP_ERR_INVALID, "endpoint subsets on an engine with latency profiles go through epp_submit_subset_predicted");
+    std::vector<uint32_t> sub;
+    const int32_t rc = take_subset(b, n_slots, slots, &sub);
+    if (rc != EPP_OK) return rc;
+    return submit_impl(b, model_id, prompt, prompt_len, multimodal, &sub, out_ticket);
+}
+
+extern "C" int32_t epp_submit_predicted(epp_batcher *b, uint32_t model_id, const void *prompt, uint64_t prompt_len,
+                                        uint32_t multimodal, uint32_t n, const epp_prediction *entries, uint64_t *out_ticket) {
+    if (!b || !out_ticket || (prompt_len && !prompt) || (n && !entries)) return bfail(EPP_ERR_INVALID, "NULL argument");
+    std::vector<epp_prediction> pred;
+    const int32_t rc = take_predictions(b, n, entries, &pred);
+    if (rc != EPP_OK) return rc;
     return submit_impl(b, model_id, prompt, prompt_len, multimodal, nullptr, out_ticket, &pred);
+}
+
+extern "C" int32_t epp_submit_subset_predicted(epp_batcher *b, uint32_t model_id, const void *prompt, uint64_t prompt_len,
+                                               uint32_t multimodal, uint32_t n_slots, const uint32_t *slots, uint32_t n_pred,
+                                               const epp_prediction *entries, uint64_t *out_ticket) {
+    if (!b || !out_ticket || (prompt_len && !prompt) || (n_slots && !slots) || (n_pred && !entries))
+        return bfail(EPP_ERR_INVALID, "NULL argument");
+    std::vector<uint32_t> sub;
+    std::vector<epp_prediction> pred;
+    int32_t rc = take_subset(b, n_slots, slots, &sub);
+    if (rc == EPP_OK) rc = take_predictions(b, n_pred, entries, &pred);
+    if (rc != EPP_OK) return rc;
+    return submit_impl(b, model_id, prompt, prompt_len, multimodal, &sub, out_ticket, &pred);
 }
 
 extern "C" int32_t epp_wait(epp_batcher *b, uint64_t ticket, epp_decision *out, epp_decision_detail *out_detail) {

@@ -1723,7 +1723,8 @@ static int32_t launch_subset(epp_engine *h, const PickParams &pp, int64_t r0, in
         }
         CUDA_TRY(cudaEventRecord(h->sub_ev[h->sub_ev_used], s));
     }
-    CUDA_TRY(launch_subset_pick(pp, sv, s, launches));
+    const LatView lv = lat_view(h, r0);
+    CUDA_TRY(launch_subset_pick(pp, sv, h->lat_mask ? &lv : nullptr, s, launches));
     if (timed) {
         CUDA_TRY(cudaEventRecord(h->sub_ev[h->sub_ev_used + 1], s));
         h->sub_ev_used += 2;
@@ -2172,12 +2173,14 @@ static int32_t check_topk(epp_engine *h, const epp_topk_out *topk) {
 
 // Validates the subsets of a batch of R requests on the host and lists the restricted ones in ascending request order,
 // each with its offset in the packed slot array (*n_slots entries in all).  Nothing of the engine changes.
+// latency_ok: the call may also carry predictions (epp_schedule_subset_predicted), so a latency engine is accepted.
 static int32_t check_subset(const epp_engine *h, int64_t R, const epp_subset *s, std::vector<SubsetRow> &rows,
-                            uint64_t *n_slots) {
+                            uint64_t *n_slots, bool latency_ok) {
     if (s->struct_size != sizeof(epp_subset)) return fail(EPP_ERR_INVALID, "epp_subset.struct_size %u != %zu", s->struct_size, sizeof(epp_subset));
     if (h->shard_begin != 0 || h->shard_end != 0xFFFFFFFFu || h->p2p_buf)
         return fail(EPP_ERR_INVALID, "endpoint subsets are not available in the endpoint-sharded and peer-memory modes");
-    if (h->lat_mask) return fail(EPP_ERR_INVALID, "endpoint subsets are not available on an engine with latency profiles");
+    if (h->lat_mask && !latency_ok)
+        return fail(EPP_ERR_INVALID, "endpoint subsets on an engine with latency profiles go through epp_schedule_subset_predicted");
     if (R > 0 && !s->counts) return fail(EPP_ERR_INVALID, "epp_subset.counts is NULL");
     const uint32_t E = (uint32_t)h->cfg.max_endpoints;
     int64_t n_rows = 0;
@@ -2337,7 +2340,7 @@ static int32_t upload_predictions(epp_engine *h, int64_t R, const epp_prediction
 
 static int32_t schedule_impl(epp_engine *h, const epp_batch *batch, epp_decision *out, epp_decision_detail *detail,
                              int32_t keep_hashes, const epp_topk_out *topk, const epp_subset *subset = nullptr,
-                             const epp_predictions *preds = nullptr) {
+                             const epp_predictions *preds = nullptr, bool subset_latency_ok = false) {
     if (!h) return fail(EPP_ERR_INVALID, "NULL engine");
     if (!out) return fail(EPP_ERR_INVALID, "out is NULL");
     std::lock_guard<std::mutex> lk(h->mu);
@@ -2348,7 +2351,7 @@ static int32_t schedule_impl(epp_engine *h, const epp_batch *batch, epp_decision
     if (h->cfg.encode_enabled && v.multimodal && !detail) return fail(EPP_ERR_INVALID, "an encode profile is configured and the batch flags multimodal requests: `detail` (which carries the encode pick) must not be NULL");
     std::vector<SubsetRow> sub_rows;
     uint64_t sub_n_slots = 0;
-    if (subset) EPP_TRY(check_subset(h, v.R, subset, sub_rows, &sub_n_slots));
+    if (subset) EPP_TRY(check_subset(h, v.R, subset, sub_rows, &sub_n_slots, subset_latency_ok));
     uint64_t n_ent = 0;
     if (preds) EPP_TRY(check_predictions(h, v.R, preds, &n_ent));
     if (!sub_rows.empty() || (preds && v.R)) {
@@ -2400,6 +2403,12 @@ extern "C" int32_t epp_schedule_subset(epp_engine *h, const epp_batch *batch, co
                                        epp_decision_detail *detail, int32_t keep_hashes, const epp_topk_out *topk) {
     if (!subset) return fail(EPP_ERR_INVALID, "subset is NULL");
     return schedule_impl(h, batch, out, detail, keep_hashes, topk, subset);
+}
+
+extern "C" int32_t epp_schedule_subset_predicted(epp_engine *h, const epp_batch *batch, const epp_subset *subset,
+                                                 const epp_predictions *preds, epp_decision *out, epp_decision_detail *detail,
+                                                 int32_t keep_hashes, const epp_topk_out *topk) {
+    return schedule_impl(h, batch, out, detail, keep_hashes, topk, subset, preds, true);
 }
 
 // PreRequest: approximateprefix/plugin.go:164-200 (primary target + "prefill" profile target).

@@ -341,8 +341,8 @@ struct DensePickParams {
 cudaError_t launch_dense_pick(const DensePickParams &p, cudaStream_t s, int *launches);
 // Latency predictions (include/epp_engine.h, "Latency predictions"): the general evaluation of pick_latency.cuh for the
 // profiles whose bit is set in `mask`, with request r's entries at ent[off[r0 + r] .. + cnt[r0 + r]) (cnt == nullptr: no
-// request has any).  The _lat builds of the dense-counter and injected-match kernels take it as an extra argument, so
-// the parameters of every other kernel stay as they are.
+// request has any).  The _lat builds of the dense-counter, injected-match and subset kernels take it as an extra
+// argument, so the parameters of every other kernel stay as they are.
 struct LatView {
     const uint32_t *cnt;       // [batch R] absolute request rows
     const uint64_t *off;
@@ -358,6 +358,8 @@ cudaError_t launch_dense_pick_lat(const DensePickParams &p, const LatView &lv, c
 // restricted request of a launch whose ordinary match kernel has run: it walks the request's stored hash row up to the
 // global stop counting only the listed holders, then evaluates every profile over the listed slots (full evaluation:
 // affinity filter, scorer normalisation, no-hit-lru cold ranks, first-k and random draws over the narrowed set).
+// lv != nullptr (an engine with latency profiles): k_subset_pick_lat, whose latency profiles run the chain of
+// pick_latency.cuh over the listed slots with the request's predictions.
 struct SubsetRow {
     uint64_t off;              // the request's slots are slots[off .. off + n), ascending
     uint32_t row;              // absolute request index in the batch
@@ -372,7 +374,7 @@ struct SubsetView {
     int32_t *scratch;          // parallel to slots: no-hit-lru cold ranks (written here)
     const int32_t *nohit_pos;  // [E] position in the no-hit-lru LRU (oldest 0, -1 = never used), or nullptr
 };
-cudaError_t launch_subset_pick(const PickParams &p, const SubsetView &sv, cudaStream_t s, int *launches);
+cudaError_t launch_subset_pick(const PickParams &p, const SubsetView &sv, const LatView *lv, cudaStream_t s, int *launches);
 // Scorer.Score parity: out[R][E].  scorer_index -1 => weighted ordered sum (-1.0 for non-candidates).
 // cold != nullptr (the profile has a no-hit-lru scorer): cold[r] selects prof_cold and the raw cold column nohit_col
 // for request r.

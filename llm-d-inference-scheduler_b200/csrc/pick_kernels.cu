@@ -367,7 +367,8 @@ __device__ inline Best lat_eval_profile(const P &p, const LatView &lv, int pi, i
     lat::Req q;
     q.n = lv.cnt ? lv.cnt[lv.r0 + r] : 0u;
     q.ent = q.n ? lv.ent + lv.off[lv.r0 + r] : nullptr;
-    return lat::eval<kRand>(p.prof[pi], lv.cfg[pi], p.gen, q, p.E, total, lane, p.lora, adapter, p.tie_seed, key, cnt_of, k,
+    return lat::eval<kRand>(p.prof[pi], lv.cfg[pi], p.gen, q, p.E, total, lane, p.lora, adapter, p.tie_seed, key,
+                            lat::pool_dom(p.E, cnt_of), k,
                             (k > 1 && p.gen.topk_picks[pi]) ? p.gen.topk_picks[pi] + r * k : nullptr,
                             (k > 1 && pi == 0 && p.gen.topk_scores) ? p.gen.topk_scores + r * k : nullptr);
 }

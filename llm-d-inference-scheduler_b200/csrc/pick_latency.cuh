@@ -5,7 +5,8 @@
 // decisions, the scored bucket, its per-dimension min / max, alpha and beta) is computed once per stage by warp
 // reductions; after that a slot's membership and score are per-slot predicates over its entry, which each lane finds by
 // binary search in the request's ascending entry list.
-// Only the _lat builds of the dense-counter and injected-match kernels include this code.
+// The chain walks an index domain (PoolDom: every slot of the pool; ListDom: a restricted request's listed slots), so
+// the _lat builds of the dense-counter and injected-match kernels and the subset kernel share one evaluation.
 #pragma once
 #include <cfloat>
 #include <climits>
@@ -48,6 +49,32 @@ struct Req {
     }
 };
 
+// The index domain of an evaluation: members i of [0, n), member i is slot at(i) with matchBlocks cnt(i);
+// n_cand(pf) is the number of members that are candidates of profile pf (role and label filters).
+template <typename CntOf>
+struct PoolDom {                   // i -> i over the whole pool
+    uint32_t n;
+    CntOf cnt_of;
+    __device__ __forceinline__ uint32_t at(uint32_t i) const { return i; }
+    __device__ __forceinline__ int32_t cnt(uint32_t i) const { return cnt_of(i); }
+    __device__ __forceinline__ uint32_t n_cand(const ProfileDev &pf, int) const { return (uint32_t)*pf.n_cand; }
+};
+template <typename CntOf>
+__device__ __forceinline__ PoolDom<CntOf> pool_dom(int32_t E, CntOf cnt_of) { return PoolDom<CntOf>{(uint32_t)E, cnt_of}; }
+
+struct ListDom {                   // i -> sl[i] over a restricted request's ascending slot list (endpoint subsets)
+    const uint32_t *sl;
+    const int32_t *hit;            // whole-pool matchBlocks per listed slot
+    uint32_t n;
+    __device__ __forceinline__ uint32_t at(uint32_t i) const { return sl[i]; }
+    __device__ __forceinline__ int32_t cnt(uint32_t i) const { return hit[i]; }
+    __device__ __forceinline__ uint32_t n_cand(const ProfileDev &pf, int lane) const {
+        uint32_t c = 0;
+        for (uint32_t i0 = 0; i0 < n; i0 += 32) c += __popc(__ballot_sync(gen::kFull, i0 + lane < n && pf.cand[sl[i0 + lane]]));
+        return c;
+    }
+};
+
 // both headrooms >= 0 (sloheadroomtier/plugin.go:102)
 __device__ __forceinline__ bool meets(const epp_prediction *p) { return p->ttft_headroom >= 0.0 && p->tpot_headroom >= 0.0; }
 
@@ -82,18 +109,18 @@ struct State {
 
 // prefix-cache-affinity-filter (plugin.go:105-151) over the n members of in_set, TTFT from the entries (bestTTFT,
 // :173-184, skips members without one).  True: the set narrows to the sticky members.
-template <typename InSet, typename CntOf>
+template <typename InSet, typename Dom>
 __device__ inline bool affinity(double thr, double explore, double penalty, uint64_t dom, uint32_t n, const Req &q,
-                                int32_t E, int32_t total, int lane, uint64_t seed, uint64_t key, InSet in_set, CntOf cnt_of) {
+                                int32_t total, int lane, uint64_t seed, uint64_t key, InSet in_set, const Dom &ix) {
     if (!(thr > 0.0) || n <= 1) return false;                                           // :108
     if (seed && draw_u(seed, dom, key) < explore) return false;                         // :113-117
     uint32_t ns = 0, nn = 0;
     double bs = DBL_MAX, bn = DBL_MAX;
-    for (uint32_t e = lane; e < (uint32_t)E; e += 32) {
-        if (!in_set(e)) continue;
-        const epp_prediction *p = q.find(e);
+    for (uint32_t i = lane; i < ix.n; i += 32) {
+        if (!in_set(i)) continue;
+        const epp_prediction *p = q.find(ix.at(i));
         const double t = p ? p->ttft : DBL_MAX;
-        if (gen::is_sticky(cnt_of(e), total, thr)) { ns++; if (t < bs) bs = t; }
+        if (gen::is_sticky(ix.cnt(i), total, thr)) { ns++; if (t < bs) bs = t; }
         else { nn++; if (t < bn) bn = t; }
     }
     for (int o = 16; o; o >>= 1) {
@@ -145,31 +172,32 @@ __device__ inline double weighted_sum(const ProfileDev &pf, const GenView &g, co
     return acc;
 }
 
-// The request-level state of the chain and the scorer.  Returns the final set's size.
-template <typename CntOf>
+// The request-level state of the chain and the scorer over the members of ix (E: the pool's, the stride of its
+// columns).  Returns the final set's size.
+template <typename Dom>
 __device__ inline uint32_t prepare(const ProfileDev &pf, const epp_latency_cfg &lc, const GenView &g, const Req &q,
-                                   int32_t E, int32_t total, int lane, uint64_t seed, uint64_t key, CntOf cnt_of, State &st) {
+                                   int32_t E, int32_t total, int lane, uint64_t seed, uint64_t key, const Dom &ix, State &st) {
     const epp_profile_cfg &c = pf.cfg;
     st.a1 = st.a2 = false;
     st.tier = kTierAll;
-    auto in1 = [&](uint32_t e) { return pf.cand[e] && (!st.a1 || gen::is_sticky(cnt_of(e), total, lc.a1_affinity_threshold)); };
-    auto in2 = [&](uint32_t e) {
-        if (!in1(e)) return false;
+    auto in1 = [&](uint32_t i) { return pf.cand[ix.at(i)] && (!st.a1 || gen::is_sticky(ix.cnt(i), total, lc.a1_affinity_threshold)); };
+    auto in2 = [&](uint32_t i) {
+        if (!in1(i)) return false;
         if (st.tier == kTierAll) return true;
-        const epp_prediction *p = q.find(e);
+        const epp_prediction *p = q.find(ix.at(i));
         return (st.tier == kTierPos) == (p && meets(p));
     };
-    auto in = [&](uint32_t e) { return in2(e) && (!st.a2 || gen::is_sticky(cnt_of(e), total, c.affinity_threshold)); };
+    auto in = [&](uint32_t i) { return in2(i) && (!st.a2 || gen::is_sticky(ix.cnt(i), total, c.affinity_threshold)); };
     // A1 over the filtered candidates
     if (lc.tier_filter)
         st.a1 = affinity(lc.a1_affinity_threshold, lc.a1_exploration_probability, lc.a1_max_ttft_penalty_ms, kA1Domain,
-                         (uint32_t)*pf.n_cand, q, E, total, lane, seed, key, in1, cnt_of);
+                         ix.n_cand(pf, lane), q, total, lane, seed, key, in1, ix);
     // T over A1's set (sloheadroomtier/plugin.go:84-138)
     uint32_t n1 = 0, npos = 0, nneg = 0;
-    for (uint32_t e = lane; e < (uint32_t)E; e += 32) {
-        if (!in1(e)) continue;
+    for (uint32_t i = lane; i < ix.n; i += 32) {
+        if (!in1(i)) continue;
         n1++;
-        const epp_prediction *p = q.find(e);
+        const epp_prediction *p = q.find(ix.at(i));
         if (p) { if (meets(p)) npos++; else nneg++; }
     }
     n1 = warp_sum(n1); npos = warp_sum(npos); nneg = warp_sum(nneg);
@@ -182,12 +210,13 @@ __device__ inline uint32_t prepare(const ProfileDev &pf, const epp_latency_cfg &
     }
     // A2: the profile's own affinity filter, today's draw
     st.a2 = affinity(c.affinity_threshold, c.exploration_probability, c.max_ttft_penalty_ms, gen::kExploreDomain, n2, q,
-                     E, total, lane, seed, key, in2, cnt_of);
+                     total, lane, seed, key, in2, ix);
     // normalisation over the final set; the latency scorer's bucket
     uint32_t n = 0, has = 0, pos = 0, idle = 0, tpot = 0, ttft = 0;
     long long mnw = LLONG_MAX, mxw = LLONG_MIN, mnr = LLONG_MAX, mxr = LLONG_MIN, mxq = 0;
-    for (uint32_t e = lane; e < (uint32_t)E; e += 32) {
-        if (!in(e)) continue;
+    for (uint32_t i = lane; i < ix.n; i += 32) {
+        if (!in(i)) continue;
+        const uint32_t e = ix.at(i);
         n++;
         const long long w = g.pool.waiting[e], r = g.pool.running[e];
         mnw = min(mnw, w); mxw = max(mxw, w);
@@ -218,8 +247,8 @@ __device__ inline uint32_t prepare(const ProfileDev &pf, const epp_latency_cfg &
         const int col = c.scorers[s].column;
         long long mx = 0;
         if (col >= 0 && col < g.pool.n_ext_cols)
-            for (uint32_t e = lane; e < (uint32_t)E; e += 32)
-                if (in(e)) mx = max(mx, (long long)g.pool.ext[(size_t)col * (size_t)E + (size_t)e]);
+            for (uint32_t i = lane; i < ix.n; i += 32)
+                if (in(i)) mx = max(mx, (long long)g.pool.ext[(size_t)col * (size_t)E + (size_t)ix.at(i)]);
         for (int o = 16; o; o >>= 1) mx = max(mx, __shfl_xor_sync(gen::kFull, mx, o));
         st.nm.q[4 + s] = mx;
     }
@@ -240,9 +269,9 @@ __device__ inline uint32_t prepare(const ProfileDev &pf, const epp_latency_cfg &
     else if (ttft) st.bucket = kBucketTtft;
     else st.bucket = kBucketBoth;
     double mnt = DBL_MAX, mxt = -DBL_MAX, mnp = DBL_MAX, mxp = -DBL_MAX;
-    for (uint32_t e = lane; e < (uint32_t)E; e += 32) {
-        if (!in(e)) continue;
-        const epp_prediction *p = q.find(e);
+    for (uint32_t i = lane; i < ix.n; i += 32) {
+        if (!in(i)) continue;
+        const epp_prediction *p = q.find(ix.at(i));
         if (!in_bucket(st.bucket, p)) continue;
         const double ht = p ? fabs(p->ttft_headroom) : 0.0, hp = p ? fabs(p->tpot_headroom) : 0.0;
         if (ht < mnt) mnt = ht;
@@ -266,33 +295,36 @@ __device__ inline uint32_t prepare(const ProfileDev &pf, const epp_latency_cfg &
 }
 
 // One latency profile for one request: the chain, scores, and the first max(1, k) endpoints in picker order (the
-// contract of gen::eval, over the final set).
-template <bool kRand, typename CntOf>
+// contract of gen::eval, over the final set), all over the members of ix: the candidates are its members that pass
+// pf's filters, and every set size, range and draw population is taken over them.  Picks are slots.
+template <bool kRand, typename Dom>
 __device__ inline Best eval(const ProfileDev &pf, const epp_latency_cfg &lc, const GenView &g, const Req &q, int32_t E,
                             int32_t total, int lane, const LoraDev &lora, uint32_t adapter, uint64_t seed, uint64_t key,
-                            CntOf cnt_of, int32_t k, uint32_t *picks_row, double *scores_row) {
+                            const Dom &ix, int32_t k, uint32_t *picks_row, double *scores_row) {
     Best first;
     best_init(first);
     if (k < 1) k = 1;
     if (picks_row) for (int j = lane; j < k; j += 32) picks_row[j] = EPP_NO_ENDPOINT;
     if (scores_row) for (int j = lane; j < k; j += 32) scores_row[j] = 0.0;
     __syncwarp();
-    if (*pf.n_cand == 0) return first;
+    if (ix.n_cand(pf, lane) == 0) return first;
     State st;
-    const uint32_t n = prepare(pf, lc, g, q, E, total, lane, seed, key, cnt_of, st);
+    const uint32_t n = prepare(pf, lc, g, q, E, total, lane, seed, key, ix, st);
     const bool use_lora = lora.enabled && lora.ptr;
-    auto cand = [&](uint32_t e) {
+    auto cand = [&](uint32_t i) {
+        const uint32_t e = ix.at(i);
         if (!pf.cand[e]) return false;
-        if (st.a1 && !gen::is_sticky(cnt_of(e), total, lc.a1_affinity_threshold)) return false;
+        if (st.a1 && !gen::is_sticky(ix.cnt(i), total, lc.a1_affinity_threshold)) return false;
         if (st.tier != kTierAll) {
             const epp_prediction *p = q.find(e);
             if ((st.tier == kTierPos) != (p && meets(p))) return false;
         }
-        return !st.a2 || gen::is_sticky(cnt_of(e), total, pf.cfg.affinity_threshold);
+        return !st.a2 || gen::is_sticky(ix.cnt(i), total, pf.cfg.affinity_threshold);
     };
-    auto score = [&](uint32_t e) {
+    auto score = [&](uint32_t i) {
+        const uint32_t e = ix.at(i);
         const int ls = use_lora ? lora_lookup(lora, adapter, e) : 0;
-        return weighted_sum(pf, g, st, e, q.find(e), cnt_of(e), total, lora, ls);
+        return weighted_sum(pf, g, st, e, q.find(e), ix.cnt(i), total, lora, ls);
     };
     if (kRand && pf.cfg.picker) {     // random pickers: every member is an explicit item
         uint32_t g0 = EPP_NO_ENDPOINT, g1 = EPP_NO_ENDPOINT;
@@ -303,10 +335,11 @@ __device__ inline Best eval(const ProfileDev &pf, const epp_latency_cfg &lc, con
                     o |= e == __shfl_sync(gen::kFull, t < 32 ? g0 : g1, t & 31);
                 return o;
             };
-            const Best b = rnd::draw_scan(pf, E, lane, false, n - (uint32_t)j, (uint32_t)j, seed + (uint64_t)j * gen::kGolden,
-                                          key, cand, [](uint32_t) { return true; }, score, out_of);
+            Best b = rnd::draw_scan(pf, (int32_t)ix.n, lane, false, n - (uint32_t)j, (uint32_t)j, seed + (uint64_t)j * gen::kGolden,
+                                    key, cand, [](uint32_t) { return true; }, score, out_of);
+            if (lane == (j & 31)) { if (j < 32) g0 = b.pick; else g1 = b.pick; }     // members, as out_of compares them
+            b.pick = ix.at(b.pick);
             if (j == 0) first = b;
-            if (lane == (j & 31)) { if (j < 32) g0 = b.pick; else g1 = b.pick; }
             if (lane == 0) {
                 if (picks_row) picks_row[j] = b.pick;
                 if (scores_row) scores_row[j] = b.val;
@@ -323,10 +356,10 @@ __device__ inline Best eval(const ProfileDev &pf, const epp_latency_cfg &lc, con
         if (n_rem == 0) {
             Best b;
             best_init(b);
-            for (uint32_t e = lane; e < (uint32_t)E; e += 32) {
-                if (!cand(e)) continue;
-                const double sc = score(e);
-                if (!have_v || sc < v) best_add(b, sc, e);
+            for (uint32_t i = lane; i < ix.n; i += 32) {
+                if (!cand(i)) continue;
+                const double sc = score(i);
+                if (!have_v || sc < v) best_add(b, sc, i);
             }
             b = best_warp_reduce(b);
             if (!b.ties) break;
@@ -339,19 +372,19 @@ __device__ inline Best eval(const ProfileDev &pf, const epp_latency_cfg &lc, con
         }
         uint32_t rank = seed ? tie_rank(seed + (uint64_t)j * gen::kGolden, key, n_rem) : 0u;
         uint32_t pick = EPP_NO_ENDPOINT;
-        for (uint32_t e0 = 0; e0 < (uint32_t)E && pick == EPP_NO_ENDPOINT; e0 += 32) {
-            const uint32_t e = e0 + lane;
-            bool hit = e < (uint32_t)E && cand(e) && score(e) == v;
+        for (uint32_t i0 = 0; i0 < ix.n && pick == EPP_NO_ENDPOINT; i0 += 32) {
+            const uint32_t i = i0 + lane;
+            bool hit = i < ix.n && cand(i) && score(i) == v;
             if (n_taken && __any_sync(gen::kFull, hit))
                 for (uint32_t t = 0; t < n_taken; t++) {
                     const uint32_t te = __shfl_sync(gen::kFull, t < 32 ? g0 : g1, (int)(t & 31));
-                    if (te == e) hit = false;
+                    if (te == i) hit = false;
                 }
             uint32_t bal = __ballot_sync(gen::kFull, hit);
             const uint32_t cnt = __popc(bal);
             if (rank < cnt) {
                 for (uint32_t i = 0; i < rank; i++) bal &= bal - 1;
-                pick = e0 + (uint32_t)__ffs(bal) - 1u;
+                pick = i0 + (uint32_t)__ffs(bal) - 1u;
             } else {
                 rank -= cnt;
             }
@@ -362,10 +395,11 @@ __device__ inline Best eval(const ProfileDev &pf, const epp_latency_cfg &lc, con
         n_rem--;
         if (j == 0) first.pick = pick;
         if (lane == 0) {
-            if (picks_row) picks_row[j] = pick;
+            if (picks_row) picks_row[j] = ix.at(pick);
             if (scores_row) scores_row[j] = v;
         }
     }
+    if (first.ties) first.pick = ix.at(first.pick);
     return first;
 }
 

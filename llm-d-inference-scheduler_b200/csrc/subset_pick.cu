@@ -12,12 +12,15 @@
 //     arrays, which describe the whole pool).
 // Every step scans the request's list (ascending slot order), so a request costs O(blocks * holders * log S + S) for S
 // listed slots.  The kernels of match_sparse.cuh / pick_kernels.cu are not touched: this one only runs for batches that
-// carry a restricted request.
+// carry a restricted request.  On an engine with latency profiles, k_subset_pick_lat evaluates those profiles with the
+// chain of pick_latency.cuh over the request's list (lat::ListDom) and the request's predictions; its other profiles,
+// the match walk and the rest of the row's handling are k_subset_pick's.
 #include <cfloat>
 #include <climits>
 
 #include "index.cuh"
 #include "pick_general.cuh"
+#include "pick_latency.cuh"
 
 namespace epp {
 namespace {
@@ -303,7 +306,10 @@ __device__ Best eval_subset(const ProfileDev &pf, const PickParams &p, const Sub
     return first;
 }
 
-__global__ void __launch_bounds__(kSubsetWarps * 32) k_subset_pick(PickParams p, SubsetView sv) {
+// One restricted request per warp.  kLat: the engine has latency profiles (lv): those evaluate through lat::eval over
+// the listed slots with the request's predictions (LatView rows are the call's absolute rows, as SubsetRow::row is).
+template <bool kLat>
+__device__ __forceinline__ void subset_pick(const PickParams &p, const SubsetView &sv, const LatView *lv = nullptr) {
     const int lane = threadIdx.x & 31;
     const int32_t j = (int32_t)blockIdx.x * kSubsetWarps + (int32_t)(threadIdx.x >> 5);
     if (j >= sv.n_rows) return;
@@ -358,6 +364,17 @@ __global__ void __launch_bounds__(kSubsetWarps * 32) k_subset_pick(PickParams p,
     }
     bool cold = false;
     auto eval = [&](int pi, uint64_t key) {
+        if constexpr (kLat) {
+            if ((lv->mask >> pi) & 1) {
+                lat::Req lq;
+                lq.n = lv->cnt ? lv->cnt[row.row] : 0u;
+                lq.ent = lq.n ? lv->ent + lv->off[row.row] : nullptr;
+                return lat::eval<true>(p.prof[pi], lv->cfg[pi], p.gen, lq, p.E, total, lane, p.lora, q.adapter, p.tie_seed, key,
+                                       lat::ListDom{q.sl, q.hit, q.n}, k,
+                                       (k > 1 && p.gen.topk_picks[pi]) ? p.gen.topk_picks[pi] + r * k : nullptr,
+                                       (k > 1 && pi == 0 && p.gen.topk_scores) ? p.gen.topk_scores + r * k : nullptr);
+            }
+        }
         return eval_subset(p.prof[pi], p, sv, q, lane, key, (p.nohit.mask >> pi) & 1, &cold, k,
                            (k > 1 && p.gen.topk_picks[pi]) ? p.gen.topk_picks[pi] + r * k : nullptr,
                            (k > 1 && pi == 0 && p.gen.topk_scores) ? p.gen.topk_scores + r * k : nullptr);
@@ -376,12 +393,18 @@ __global__ void __launch_bounds__(kSubsetWarps * 32) k_subset_pick(PickParams p,
     }
 }
 
+__global__ void __launch_bounds__(kSubsetWarps * 32) k_subset_pick(PickParams p, SubsetView sv) { subset_pick<false>(p, sv); }
+__global__ void __launch_bounds__(kSubsetWarps * 32) k_subset_pick_lat(PickParams p, SubsetView sv, LatView lv) {
+    subset_pick<true>(p, sv, &lv);
+}
+
 }  // namespace
 
-cudaError_t launch_subset_pick(const PickParams &p, const SubsetView &sv, cudaStream_t s, int *launches) {
+cudaError_t launch_subset_pick(const PickParams &p, const SubsetView &sv, const LatView *lv, cudaStream_t s, int *launches) {
     if (sv.n_rows <= 0) return cudaSuccess;
     const unsigned grid = (unsigned)((sv.n_rows + kSubsetWarps - 1) / kSubsetWarps);
-    k_subset_pick<<<grid, kSubsetWarps * 32, 0, s>>>(p, sv);
+    if (lv) k_subset_pick_lat<<<grid, kSubsetWarps * 32, 0, s>>>(p, sv, *lv);
+    else k_subset_pick<<<grid, kSubsetWarps * 32, 0, s>>>(p, sv);
     if (launches) *launches += 1;
     return cudaGetLastError();
 }

@@ -457,7 +457,8 @@ class Engine:
         subsets: None, or a list of R entries, each None (the whole pool) or a sequence of slot ids: the request's
         candidates (the gateway's endpoint subset, include/epp_engine.h "Endpoint subsets"); epp_schedule_subset.
         predictions: None, or a list of R entries in the form pack_predictions takes (include/epp_engine.h "Latency
-        predictions"); epp_schedule_predicted."""
+        predictions"); epp_schedule_predicted.  Both together: epp_schedule_subset_predicted (a latency engine's
+        restricted requests decided with their predictions)."""
         b, R, dev, keep = self._batch(data, offsets, uniform_len, model_ids, n_requests, lengths, multimodal)
         if asynchronous:
             b.flags |= capi.EPP_BATCH_ASYNC
@@ -469,22 +470,25 @@ class Engine:
             dec = np.zeros(R, dtype=DECISION_DTYPE) if out is None else out
             det = np.zeros(R, dtype=DETAIL_DTYPE) if detail else None
         lists, tk = self._topk_out(R, data.device if dev else None) if topk else (None, None)
+        if predictions is not None and len(predictions) != R:
+            raise ValueError(f"predictions has {len(predictions)} entries for {R} requests")
+        if subsets is not None and len(subsets) != R:
+            raise ValueError(f"subsets has {len(subsets)} entries for {R} requests")
         if predictions is not None:
-            if len(predictions) != R:
-                raise ValueError(f"predictions has {len(predictions)} entries for {R} requests")
-            if subsets is not None:
-                raise ValueError("subsets and predictions cannot be combined")
-            packed = pack_predictions(predictions)      # host arrays, kept alive until the call returns
-            pr = _predictions_struct(packed)
+            ppacked = pack_predictions(predictions)     # host arrays, kept alive until the call returns
+            pr = _predictions_struct(ppacked)
+        if subsets is not None:
+            spacked = pack_subsets(subsets)             # host arrays, kept alive until the call returns
+            sub = capi.Subset()
+            sub.struct_size = C.sizeof(capi.Subset)
+            sub.counts, sub.offsets, sub.slots = (_ptr(a) for a in spacked)
+        if predictions is not None and subsets is not None:
+            self._check(self._lib.epp_schedule_subset_predicted(self._h, C.byref(b), C.byref(sub), C.byref(pr), _ptr(dec),
+                                                                _ptr(det), int(keep_hashes), C.byref(tk) if topk else None))
+        elif predictions is not None:
             self._check(self._lib.epp_schedule_predicted(self._h, C.byref(b), C.byref(pr), _ptr(dec), _ptr(det),
                                                          int(keep_hashes), C.byref(tk) if topk else None))
         elif subsets is not None:
-            if len(subsets) != R:
-                raise ValueError(f"subsets has {len(subsets)} entries for {R} requests")
-            packed = pack_subsets(subsets)              # host arrays, kept alive until the call returns
-            sub = capi.Subset()
-            sub.struct_size = C.sizeof(capi.Subset)
-            sub.counts, sub.offsets, sub.slots = (_ptr(a) for a in packed)
             self._check(self._lib.epp_schedule_subset(self._h, C.byref(b), C.byref(sub), _ptr(dec), _ptr(det),
                                                       int(keep_hashes), C.byref(tk) if topk else None))
         elif not topk:
@@ -633,14 +637,13 @@ class Batcher:
 
     def submit(self, prompt, model_id: int = 0, multimodal: bool = False, subset=None, predictions=None) -> int:
         """subset: None (the whole pool) or a sequence of slot ids, the request's candidates (epp_submit_subset).
-        predictions: None or the request's entries in the form pack_predictions takes (epp_submit_predicted)."""
+        predictions: None or the request's entries in the form pack_predictions takes (epp_submit_predicted).  Both
+        together: epp_submit_subset_predicted."""
         buf = np.ascontiguousarray(prompt).view(np.uint8).reshape(-1) if not isinstance(prompt, (bytes, bytearray)) else prompt
         n = len(buf)
         ptr = buf.ctypes.data_as(C.c_void_p) if isinstance(buf, np.ndarray) else C.cast(C.c_char_p(bytes(buf)), C.c_void_p)
         t = C.c_uint64()
         if predictions is not None:
-            if subset is not None:
-                raise ValueError("subsets and predictions cannot be combined")
             if isinstance(predictions, np.ndarray) and predictions.dtype == PREDICTION_DTYPE:
                 ent = np.ascontiguousarray(predictions)
             else:
@@ -649,8 +652,13 @@ class Batcher:
                 if not 0 <= int(sl) <= 0xFFFFFFFE:
                     raise ValueError(f"slot id {sl} out of range")
                 ent[i] = (int(sl), int(d), float(tt), float(th), float(tp))
-            self._check(self._lib.epp_submit_predicted(self._b, model_id, ptr, n, int(multimodal), ent.shape[0], _ptr(ent),
-                                                       C.byref(t)))
+            if subset is not None:
+                sl = np.ascontiguousarray(np.asarray(subset, dtype=np.uint32).reshape(-1))
+                self._check(self._lib.epp_submit_subset_predicted(self._b, model_id, ptr, n, int(multimodal), sl.shape[0],
+                                                                  _ptr(sl), ent.shape[0], _ptr(ent), C.byref(t)))
+            else:
+                self._check(self._lib.epp_submit_predicted(self._b, model_id, ptr, n, int(multimodal), ent.shape[0],
+                                                           _ptr(ent), C.byref(t)))
         elif subset is None:
             self._check(self._lib.epp_submit(self._b, model_id, ptr, n, int(multimodal), C.byref(t)))
         else:

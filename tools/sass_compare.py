@@ -21,7 +21,7 @@ def kernels(lib: str) -> dict:
             cur = re.sub(r"_GLOBAL__N__[0-9a-f]+_(\d+)_(\w+?)_cu_[0-9a-f]+", r"_GLOBAL__N_\2", m.group(1))
             fs[cur] = []
         elif cur is not None and "identifier =" not in line:
-            fs[cur].append(line)
+            fs[cur].append(" ".join(line.split()))     # the column padding follows the widest line of the whole module
     return fs
 
 
