@@ -262,6 +262,9 @@ static int32_t join_streams(epp_engine *e) {
     return EPP_OK;
 }
 
+// The endpoint-sharded mode (epp_shard_set): this rank's table and candidates cover a range of the endpoints only.
+static bool sharded(const epp_engine *e) { return e->shard_begin != 0 || e->shard_end != 0xFFFFFFFFu; }
+
 // ------------------------------------------------------------------------------------------------
 // config
 // ------------------------------------------------------------------------------------------------
@@ -1554,7 +1557,7 @@ static PickParams pick_params(epp_engine *h, const Work &w, epp_decision *out, e
     p.max_blocks = h->cfg.max_prefix_blocks;
     p.encode_on = h->cfg.encode_enabled ? 1 : 0;
     p.multimodal = w.multimodal_dev ? w.multimodal_dev + w.r0 : nullptr;
-    p.tie_seed = h->shard_end != 0xFFFFFFFFu || h->shard_begin != 0 ? 0 : h->cfg.tie_seed;      // sharded mode: lowest slot
+    p.tie_seed = sharded(h) ? 0 : h->cfg.tie_seed;      // sharded mode: lowest slot
     p.hashes = w.hashes_out;
     p.nblocks = w.nblocks_out;
     p.bound = nullptr;
@@ -1590,11 +1593,11 @@ static int32_t device_offsets_or_bits(epp_engine *h, const uint64_t *offsets_dev
 enum class Mode { HashOnly, Match, Schedule };
 
 // Dense-counter kernel over the requests a sparse kernel could not finish (their matched-endpoint set overflowed its
-// per-request map).  No host round trip: the kernel reads the list length on the device.
-static int32_t launch_overflow_pass(epp_engine *h, Slot &sl, PickParams pp, int *launches) {
+// per-request map).  No host round trip: the kernel reads the list length on the device, at n.
+static int32_t launch_overflow_pass(epp_engine *h, Slot &sl, PickParams pp, const int32_t *n, int *launches) {
     cudaStream_t s = sl.stream;
     pp.req_list = sl.overflow_list.as<int32_t>();
-    pp.req_list_n = sl.overflow_n.as<int32_t>();
+    pp.req_list_n = n;
     pp.overflow_list = nullptr;
     pp.overflow_n = nullptr;
     pp.work_counters = nullptr;            // already counted by the sparse pass
@@ -1637,7 +1640,7 @@ static int32_t launch_match(epp_engine *h, Slot &sl, PickParams pp, int *launche
     pp.overflow_n = sl.overflow_n.as<int32_t>();
     pp.req_next = sl.overflow_n.as<int32_t>() + 1;
     CUDA_TRY(launch_match_pick_sparse(pp, h->sm_count, s, launches));
-    return launch_overflow_pass(h, sl, pp, launches);
+    return launch_overflow_pass(h, sl, pp, sl.overflow_n.as<int32_t>(), launches);
 }
 
 // A Schedule batch's hash rows are read by nothing but its match kernel, whose global stop never lies beyond the first
@@ -1653,12 +1656,47 @@ static void trim_rows(epp_engine *h, const Work &w, HashParams &hp, PickParams &
     pp.bound = hp.bound;
 }
 
-// The whole cycle for one Work item: hash kernel, then the standalone match / score / pick kernel (every fused or
-// concurrently scheduled arrangement of the two was measured slower).
-static int32_t launch_cycle(epp_engine *h, Slot &sl, const HashParams &hp, PickParams pp, int *launches, cudaEvent_t *ev,
-                            int64_t r0) {
-    CUDA_TRY(launch_hash_prompts(hp, sl.stream, launches, ev));
-    return launch_match(h, sl, pp, launches, r0);
+// What run_batch settles for a call before it takes the device, small or host path.
+struct Call {
+    Mode mode;
+    uint64_t *out_hashes;          // the caller's arrays (nullptr: not asked for)
+    int32_t *out_nblocks, *out_match, *out_total;
+    epp_decision *out_dec;
+    epp_decision_detail *out_detail;
+    epp_decision_detail *det_out;  // out_detail, or the engine's rows when the inflight producer needs the stage records
+    TopkRows tk;
+    bool pipelined = false;        // an async Schedule device batch run as chunks over both streams
+    bool trim = false;             // trim_rows applies
+    int launches = 0;
+};
+
+// Rows [r0, r1) of a device-pointer batch, hashed into the same rows of the engine's buffers.
+static Work device_work(epp_engine *h, const BatchView &v, int64_t r0, int64_t r1, uint64_t or_bits) {
+    return Work{r0, r1, v.offsets ? v.data : v.data + (uint64_t)r0 * v.uniform_len, v.offsets, v.lengths, v.uniform_len,
+                v.model_ids, or_bits, h->hashes.as<uint64_t>() + (size_t)r0 * (size_t)h->cfg.max_prefix_blocks,
+                h->nblocks.as<int32_t>() + r0, v.multimodal};
+}
+
+// The launch sequence of one row range on sl's stream: the hash kernel, then (unless HashOnly) the standalone match /
+// score / pick kernel (every fused or concurrently scheduled arrangement of the two was measured slower), writing dec,
+// det and out_match from row w.r0 on.  counted: the one-pass device launch, which adds to the work counters and brackets
+// the hash kernel with ev[0..3].  pp: the match kernel's parameters, for the subset launch of the same rows.
+static int32_t launch_rows(epp_engine *h, Slot &sl, const Work &w, const Call &call, epp_decision *dec,
+                           epp_decision_detail *det, int32_t *out_match, bool counted, PickParams &pp, int *launches) {
+    unsigned long long *wc = counted ? h->work_counters.as<unsigned long long>() : nullptr;
+    HashParams hp = hash_params(h, w, sl);
+    if (wc) hp.read = wc + 3;
+    if (call.mode != Mode::HashOnly) {
+        pp = pick_params(h, w, dec, det, out_match);
+        if (call.tk.on) attach_topk(h, pp.gen, call.tk.picks, call.tk.scores, w.r0);
+        if (wc) {
+            pp.work_counters = wc;
+            hp.stored = wc + 2;
+        }
+        if (call.trim) trim_rows(h, w, hp, pp);
+    }
+    CUDA_TRY(launch_hash_prompts(hp, sl.stream, launches, counted ? h->ev : nullptr));
+    return call.mode == Mode::HashOnly ? EPP_OK : launch_match(h, sl, pp, launches, w.r0);
 }
 
 // Completes the device batch in flight on stream 0 and reads its per-kernel CUDA-event times and work counters.
@@ -1770,7 +1808,7 @@ static const uint8_t *device_view_of_pinned(const void *p) {
 // reads are slower than the copy engine: beyond a handful of prompts the copy wins).
 static int small_batch_mode(epp_engine *h, const BatchView &v, const uint8_t **data_dev) {
     if (v.device || h->small_max <= 0 || v.R > h->small_max || h->general) return 0;
-    if (h->shard_begin != 0 || h->shard_end != 0xFFFFFFFFu) return 0;
+    if (sharded(h)) return 0;
     const int64_t bs = (int64_t)h->cfg.block_size_tokens * 4;
     if ((bs & 31) || bs > 64 * 1024 || (size_t)h->cfg.max_prefix_blocks > cycle_small_max_blocks()) return 0;
     const uint64_t layout_bits = v.offsets ? v.offsets_or_bits : v.uniform_len;
@@ -1781,7 +1819,7 @@ static int small_batch_mode(epp_engine *h, const BatchView &v, const uint8_t **d
             if ((bits & 15) == 0) return 1;
         }
     }
-    // the staged copy keeps the caller's layout modulo 32 (see run_batch), so only the layout decides the alignment
+    // the staged copy keeps the caller's layout modulo 32 (see run_small), so only the layout decides the alignment
     return (layout_bits & 15) == 0 ? 2 : 0;
 }
 
@@ -1798,6 +1836,31 @@ static StreamWriteValue32 stream_write_value32() {
         return reinterpret_cast<StreamWriteValue32>(p);
     }();
     return fn;
+}
+
+// Waits for the flag word of every request of small batch `epoch` (written after a system-scope fence behind its
+// decision) on the host; *overflowed: some request was left to the overflow pass.
+static int32_t wait_small_flags(epp_engine *h, int64_t R, uint32_t epoch, uint32_t *overflowed) {
+    volatile uint32_t *flags = h->small_flags;
+    uint32_t spins = 0;
+    bool finished_once = false;
+    for (int64_t next = 0; next < R;) {
+        const uint32_t x = flags[next];
+        if ((x & 0x7fffffffu) == epoch) { *overflowed |= x >> 31; next++; continue; }
+#if defined(__x86_64__)
+        __builtin_ia32_pause();
+#endif
+        if ((++spins & 0x3fff) == 0) {             // a faulted launch never raises its flags
+            const cudaError_t q = cudaStreamQuery(h->slot[0].stream);
+            if (q == cudaSuccess) {
+                if (finished_once) return fail(EPP_ERR_CUDA, "small-batch kernel finished without publishing request %lld", (long long)next);
+                finished_once = true;
+            } else if (q != cudaErrorNotReady) {
+                return fail(EPP_ERR_CUDA, "small-batch kernel failed: %s", cudaGetErrorString(q));
+            }
+        }
+    }
+    return EPP_OK;
 }
 
 static int32_t run_small(epp_engine *h, const BatchView &v, int mode, const uint8_t *data_dev, epp_decision *out_dec,
@@ -1846,18 +1909,10 @@ static int32_t run_small(epp_engine *h, const BatchView &v, int mode, const uint
     if (v.lengths) memcpy(h->small_lengths[set], v.lengths, sizeof(uint64_t) * (size_t)R);
     if (v.model_ids) memcpy(h->small_models[set], v.model_ids, sizeof(uint32_t) * (size_t)R);
     if (v.multimodal) memcpy(h->small_mm[set], v.multimodal, (size_t)R);
-    Work w;
-    w.r0 = 0;
-    w.r1 = R;
-    w.data_base = data_dev;
-    w.offsets_dev = v.offsets ? h->small_offsets[set] : nullptr;       // pinned + mapped: host address == device address (UVA)
-    w.lengths_dev = v.lengths ? h->small_lengths[set] : nullptr;
-    w.uniform_len = v.uniform_len;
-    w.model_ids_dev = v.model_ids ? h->small_models[set] : nullptr;
-    w.offsets_or_bits = v.offsets_or_bits;
-    w.hashes_out = h->hashes.as<uint64_t>();
-    w.nblocks_out = h->nblocks.as<int32_t>();
-    w.multimodal_dev = v.multimodal ? h->small_mm[set] : nullptr;
+    // the per-request arrays are pinned + mapped: host address == device address (UVA)
+    const Work w{0, R, data_dev, v.offsets ? h->small_offsets[set] : nullptr, v.lengths ? h->small_lengths[set] : nullptr,
+                 v.uniform_len, v.model_ids ? h->small_models[set] : nullptr, v.offsets_or_bits, h->hashes.as<uint64_t>(),
+                 h->nblocks.as<int32_t>(), v.multimodal ? h->small_mm[set] : nullptr};
     PickParams pp = pick_params(h, w, h->decisions.as<epp_decision>(), h->details.as<epp_decision_detail>(), nullptr);
     pp.overflow_list = h->slot[0].overflow_list.as<int32_t>();
     pp.overflow_n = h->small_overflow_n.as<int32_t>();
@@ -1866,37 +1921,12 @@ static int32_t run_small(epp_engine *h, const BatchView &v, int mode, const uint
     CUDA_TRY(cudaEventRecord(h->ev[0], s0));
     CUDA_TRY(launch_cycle_small(hash_params(h, w, h->slot[0]), pp, so, s0, &launches));
     CUDA_TRY(cudaEventRecord(h->ev[1], s0));
-
-    // wait for the flag word of every request (written after a system-scope fence behind its decision)
-    volatile uint32_t *flags = h->small_flags;
-    uint32_t overflowed = 0, spins = 0;
-    bool finished_once = false;
-    for (int64_t next = 0; next < R;) {
-        const uint32_t x = flags[next];
-        if ((x & 0x7fffffffu) == epoch) { overflowed |= x >> 31; next++; continue; }
-#if defined(__x86_64__)
-        __builtin_ia32_pause();
-#endif
-        if ((++spins & 0x3fff) == 0) {             // a faulted launch never raises its flags
-            const cudaError_t q = cudaStreamQuery(s0);
-            if (q == cudaSuccess) {
-                if (finished_once) return fail(EPP_ERR_CUDA, "small-batch kernel finished without publishing request %lld", (long long)next);
-                finished_once = true;
-            } else if (q != cudaErrorNotReady) {
-                return fail(EPP_ERR_CUDA, "small-batch kernel failed: %s", cudaGetErrorString(q));
-            }
-        }
-    }
+    uint32_t overflowed = 0;
+    EPP_TRY(wait_small_flags(h, R, epoch, &overflowed));
     if (overflowed) {
         // > 32 endpoints hold a part of some prompt: those requests go through the dense-counter kernel, then the whole
         // batch is read back the ordinary way
-        Slot &sl = h->slot[0];
-        PickParams po = pp;
-        po.req_list = sl.overflow_list.as<int32_t>();
-        po.req_list_n = h->small_overflow_n.as<int32_t>();
-        po.overflow_list = nullptr;
-        po.overflow_n = nullptr;
-        CUDA_TRY(launch_match_pick(po, h->pick_global ? sl.pick_scratch.as<uint32_t>() : nullptr, h->pick_grid, h->pick_smem, s0, &launches));
+        EPP_TRY(launch_overflow_pass(h, h->slot[0], pp, h->small_overflow_n.as<int32_t>(), &launches));
         CUDA_TRY(cudaMemsetAsync(h->small_overflow_n.p, 0, sizeof(int32_t), s0));
         CUDA_TRY(cudaMemcpyAsync(h->small_dec, h->decisions.p, sizeof(epp_decision) * (size_t)R, cudaMemcpyDeviceToHost, s0));
         CUDA_TRY(cudaMemcpyAsync(h->small_det, h->details.p, sizeof(epp_decision_detail) * (size_t)R, cudaMemcpyDeviceToHost, s0));
@@ -1912,131 +1942,74 @@ static int32_t run_small(epp_engine *h, const BatchView &v, int mode, const uint
     return EPP_OK;
 }
 
-// Runs hashing (+ match/pick) for a batch.  Host batches are split into chunks whose H2D copy overlaps the
-// kernels of the previous chunk (two streams, two staging buffers); device batches run in one pass.
-// keep_hashes: the hash rows of a Schedule batch stay for epp_index_add_picked (whole rows, no trimming).
-static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t *out_hashes, int32_t *out_nblocks,
-                         epp_decision *out_dec, epp_decision_detail *out_detail, int32_t *out_match,
-                         int32_t *out_total, bool keep_hashes = false) {
+// A device-pointer batch: an async Schedule batch of at least two chunks runs chunk-pipelined over both streams, any other
+// in one pass on stream 0.  An async batch (not Match) returns with its results and stats pending (finish_async).
+static int32_t run_device(epp_engine *h, const BatchView &v, Call &call) {
+    const int64_t R = v.R;
+    cudaStream_t s0 = h->slot[0].stream;
+    uint64_t or_bits = 0;
+    if (v.offsets) EPP_TRY(device_offsets_or_bits(h, v.offsets, R, s0, &or_bits));
+    CUDA_TRY(cudaMemsetAsync(h->work_counters.p, 0, sizeof(unsigned long long) * 4, s0));
+    const int64_t min_chunk = 4096;
+    h->sub_ev_used = 0;
+    epp_decision *dec = call.out_dec ? call.out_dec : h->decisions.as<epp_decision>();
+    PickParams pp;                                 // the rows of the last launch_rows, for their subset launch
+    if (call.pipelined) {
+        // Throughput mode: the batch runs as C chunks alternating between the engine's two streams, so the hash
+        // kernel of one chunk (HBM / integer bound) shares the SMs with the match kernel of another (latency bound).
+        // Consecutive pipelined batches of the same shape are not joined: every row range of the engine's buffers is
+        // only ever touched by one stream, and the next entry point of any other kind joins the streams first.
+        const int64_t C = std::min<int64_t>(h->dev_chunks, R / min_chunk);
+        const int64_t per = ((R + C - 1) / C + 31) & ~(int64_t)31;
+        cudaStream_t s1 = h->slot[1].stream;
+        if (h->s1_unjoined && (h->inflight || h->pipe_R != R || h->pipe_per != per)) EPP_TRY(join_streams(h));
+        for (int i = 0; i < 4; i++) CUDA_TRY(cudaEventRecord(h->ev[i], s0));
+        if (!h->s1_unjoined) {
+            CUDA_TRY(cudaEventRecord(h->slot[0].done, s0));
+            CUDA_TRY(cudaStreamWaitEvent(s1, h->slot[0].done, 0));
+        }
+        int k = 0;
+        for (int64_t r0 = 0; r0 < R; r0 += per, k++) {
+            const int64_t r1 = std::min(R, r0 + per);
+            Slot &sl = h->slot[k & 1];
+            EPP_TRY(launch_rows(h, sl, device_work(h, v, r0, r1, or_bits), call, dec + r0,
+                                call.det_out ? call.det_out + r0 : nullptr, nullptr, false, pp, &call.launches));
+            EPP_TRY(launch_subset(h, pp, r0, r1, sl.stream, &call.launches, true));
+        }
+        h->s1_unjoined = true;
+        // the next call's picks must see both chunks' Adds: join the chunks on stream 0 for the update (below), and the
+        // next call's stream-1 chunk waits for stream 0 again (engines without the scorer or the producer stay unjoined)
+        if (h->nohit_mask || h->inflight) EPP_TRY(join_streams(h));
+        h->pipe_R = R;
+        h->pipe_per = per;
+    } else {
+        Work w = device_work(h, v, 0, R, or_bits);
+        if (call.mode == Mode::HashOnly && call.out_hashes) w.hashes_out = call.out_hashes;
+        if (call.mode == Mode::HashOnly && call.out_nblocks) w.nblocks_out = call.out_nblocks;
+        if (call.mode == Mode::Match && call.out_total) w.nblocks_out = call.out_total;
+        EPP_TRY(launch_rows(h, h->slot[0], w, call, dec, call.mode == Mode::Schedule ? call.det_out : nullptr,
+                            call.mode == Mode::Match ? call.out_match : nullptr, true, pp, &call.launches));
+    }
+    CUDA_TRY(cudaEventRecord(h->ev[4], s0));
+    if (call.mode == Mode::Schedule) {             // after ev[4]: last_kernel_ms[3] stays the match + pick time
+        if (!call.pipelined) EPP_TRY(launch_subset(h, pp, 0, R, s0, &call.launches, true));
+        EPP_TRY(after_picks(h, dec, call.det_out, h->in_len.as<int64_t>(), R, s0, &call.launches, true));
+    }
+    CUDA_TRY(cudaMemcpyAsync(h->wc_host, h->work_counters.p, sizeof(unsigned long long) * 4, cudaMemcpyDeviceToHost, s0));
+    h->async_pending = true;
+    h->async_launches = call.launches;
+    if (v.async && call.mode != Mode::Match) return EPP_OK;    // epp_synchronize() (or the next call that needs the
+                                                               // results on the host) completes it
+    return finish_async(h);
+}
+
+// A host batch: the small per-request arrays are uploaded once, then the prompt bytes go in chunks whose H2D copy
+// overlaps the kernels of the previous chunk (two streams, two staging buffers); each chunk's results are copied back
+// behind its kernels.
+static int32_t run_host(epp_engine *h, const BatchView &v, Call &call) {
     const int64_t R = v.R;
     const size_t B = (size_t)h->cfg.max_prefix_blocks;
-    if (R == 0) return EPP_OK;
-    if (mode != Mode::HashOnly) {
-        if (!h->pool_ready) return fail(EPP_ERR_STATE, "epp_pool_set has not been called");
-        // index updates become visible here -- or, with index_commit_interval_us, at most that much later: the reference
-        // applies PreRequest in a goroutine of its own "to avoid blocking the request path" (approximateprefix/plugin.go:189-194),
-        // so a scheduling cycle may well run against an index that lacks the last few picks
-        const bool due = h->cfg.index_commit_interval_us <= 0 || !h->committed_once ||
-                         ms_since(h->last_commit) * 1000.0 >= (double)h->cfg.index_commit_interval_us;
-        if (due) {
-            EPP_TRY(commit_locked(h));
-            h->last_commit = std::chrono::steady_clock::now();
-            h->committed_once = true;
-        }
-    }
-    if (h->async_pending && !(v.device && v.async)) EPP_TRY(finish_async(h));
-    TopkRows tk;
-    EPP_TRY(topk_rows(h, mode == Mode::Schedule ? h->cur_topk : nullptr, v.device, R, tk));
-    const bool pipelined = v.device && v.async && mode == Mode::Schedule && h->dev_chunks > 1 && R >= 2 * 4096 && !h->pick_global;
-    // the endpoint-sharded mode's local table is not the global one: its rows stay whole
-    const bool trim = mode == Mode::Schedule && !keep_hashes && h->hash_trim && h->shard_begin == 0 && h->shard_end == 0xFFFFFFFFu;
-    if (!pipelined) EPP_TRY(join_streams(h));
-    EPP_TRY(reserve_batch(h, R));
-    int launches = 0;
     cudaStream_t s0 = h->slot[0].stream;
-    // releases / resets since the last call, on stream 0 before any pick kernel (a pipelined batch's stream 1 waits
-    // for stream 0 below)
-    if (mode == Mode::Schedule) EPP_TRY(inflight_flush(h, s0, &launches));
-    // the stage records reach the producer's add kernel even when the caller asked for none
-    epp_decision_detail *det_out = (mode == Mode::Schedule && !out_detail && h->inflight) ? h->details.as<epp_decision_detail>()
-                                                                                         : out_detail;
-
-    if (v.device) {
-        uint64_t or_bits = 0;
-        if (v.offsets) EPP_TRY(device_offsets_or_bits(h, v.offsets, R, s0, &or_bits));
-        Work w{0, R, v.data, v.offsets, v.lengths, v.uniform_len, v.model_ids, or_bits,
-               (mode == Mode::HashOnly && out_hashes) ? out_hashes : h->hashes.as<uint64_t>(),
-               (mode == Mode::HashOnly && out_nblocks) ? out_nblocks : (mode == Mode::Match && out_total ? out_total : h->nblocks.as<int32_t>()),
-               v.multimodal};
-        CUDA_TRY(cudaMemsetAsync(h->work_counters.p, 0, sizeof(unsigned long long) * 4, s0));
-        const int64_t min_chunk = 4096;
-        h->sub_ev_used = 0;
-        PickParams sub_pp;                         // the one-pass launch's rows, for its subset launch behind ev[4]
-        bool sub_pending = false;
-        if (pipelined) {
-            // Throughput mode: the batch runs as C chunks alternating between the engine's two streams, so the hash
-            // kernel of one chunk (HBM / integer bound) shares the SMs with the match kernel of another (latency bound).
-            // Consecutive pipelined batches of the same shape are not joined: every row range of the engine's buffers is
-            // only ever touched by one stream, and the next entry point of any other kind joins the streams first.
-            const int64_t C = std::min<int64_t>(h->dev_chunks, R / min_chunk);
-            const int64_t per = ((R + C - 1) / C + 31) & ~(int64_t)31;
-            cudaStream_t s1 = h->slot[1].stream;
-            if (h->s1_unjoined && (h->inflight || h->pipe_R != R || h->pipe_per != per)) EPP_TRY(join_streams(h));
-            for (int i = 0; i < 4; i++) CUDA_TRY(cudaEventRecord(h->ev[i], s0));
-            if (!h->s1_unjoined) {
-                CUDA_TRY(cudaEventRecord(h->slot[0].done, s0));
-                CUDA_TRY(cudaStreamWaitEvent(s1, h->slot[0].done, 0));
-            }
-            epp_decision *dec_base = out_dec ? out_dec : h->decisions.as<epp_decision>();
-            int k = 0;
-            for (int64_t r0 = 0; r0 < R; r0 += per, k++) {
-                const int64_t r1 = std::min(R, r0 + per);
-                Work w{r0, r1, v.offsets ? v.data : v.data + (uint64_t)r0 * v.uniform_len, v.offsets, v.lengths, v.uniform_len,
-                       v.model_ids, or_bits, h->hashes.as<uint64_t>() + (size_t)r0 * B, h->nblocks.as<int32_t>() + r0, v.multimodal};
-                PickParams pp = pick_params(h, w, dec_base + r0, det_out ? det_out + r0 : nullptr, nullptr);
-                if (tk.on) attach_topk(h, pp.gen, tk.picks, tk.scores, r0);
-                Slot &sl = h->slot[k & 1];
-                HashParams hp = hash_params(h, w, sl);
-                if (trim) trim_rows(h, w, hp, pp);
-                EPP_TRY(launch_cycle(h, sl, hp, pp, &launches, nullptr, r0));
-                EPP_TRY(launch_subset(h, pp, r0, r1, sl.stream, &launches, true));
-            }
-            h->s1_unjoined = true;
-            // the next call's picks must see both chunks' Adds: join the chunks on stream 0 for the update (below), and the
-            // next call's stream-1 chunk waits for stream 0 again (engines without the scorer or the producer stay unjoined)
-            if (h->nohit_mask || h->inflight) EPP_TRY(join_streams(h));
-            h->pipe_R = R;
-            h->pipe_per = per;
-        } else if (mode == Mode::HashOnly) {
-            HashParams hp = hash_params(h, w, h->slot[0]);
-            hp.read = h->work_counters.as<unsigned long long>() + 3;
-            CUDA_TRY(launch_hash_prompts(hp, s0, &launches, h->ev));
-        } else {
-            epp_decision *dec = (mode == Mode::Schedule && out_dec) ? out_dec : h->decisions.as<epp_decision>();
-            PickParams pp = pick_params(h, w, dec, mode == Mode::Schedule ? det_out : nullptr, mode == Mode::Match ? out_match : nullptr);
-            pp.work_counters = h->work_counters.as<unsigned long long>();
-            if (tk.on) attach_topk(h, pp.gen, tk.picks, tk.scores, 0);
-            HashParams hp = hash_params(h, w, h->slot[0]);
-            hp.stored = h->work_counters.as<unsigned long long>() + 2;
-            hp.read = h->work_counters.as<unsigned long long>() + 3;
-            if (trim) trim_rows(h, w, hp, pp);
-            EPP_TRY(launch_cycle(h, h->slot[0], hp, pp, &launches, h->ev, 0));
-            sub_pp = pp;
-            sub_pending = mode == Mode::Schedule;
-        }
-        CUDA_TRY(cudaEventRecord(h->ev[4], s0));
-        if (sub_pending) EPP_TRY(launch_subset(h, sub_pp, 0, R, s0, &launches, true));   // after ev[4]: [3] stays match + pick
-        if (mode == Mode::Schedule)                // after ev[4]: last_kernel_ms[3] stays the match + pick time
-            EPP_TRY(after_picks(h, out_dec ? out_dec : h->decisions.as<epp_decision>(), det_out, h->in_len.as<int64_t>(), R,
-                                s0, &launches, true));
-        CUDA_TRY(cudaMemcpyAsync(h->wc_host, h->work_counters.p, sizeof(unsigned long long) * 4, cudaMemcpyDeviceToHost, s0));
-        h->async_pending = true;
-        h->async_launches = launches;
-        if (v.async && mode != Mode::Match) return EPP_OK;         // epp_synchronize() (or the next call that needs the
-                                                                   // results on the host) completes it
-        return finish_async(h);
-    }
-
-    // ---- small host batch in pinned memory: one zero-copy launch, no copy engine, no stream synchronisation
-    // (not for a batch with restricted requests: the kernel hands the decisions to the host before a subset launch could
-    // rewrite them)
-    if (mode == Mode::Schedule && !tk.on && out_dec && !h->cur_sub) {
-        const uint8_t *data_dev = nullptr;
-        const int sm = small_batch_mode(h, v, &data_dev);
-        if (sm) return run_small(h, v, sm, data_dev, out_dec, out_detail);
-    }
-
-    // ---- host batch: upload the small per-request arrays once, then pipeline the prompt bytes
     if (v.offsets) CUDA_TRY(cudaMemcpyAsync(h->offsets.p, v.offsets, sizeof(uint64_t) * (size_t)(R + 1), cudaMemcpyHostToDevice, s0));
     if (v.lengths) CUDA_TRY(cudaMemcpyAsync(h->lengths.p, v.lengths, sizeof(uint64_t) * (size_t)R, cudaMemcpyHostToDevice, s0));
     if (v.model_ids) CUDA_TRY(cudaMemcpyAsync(h->model_ids.p, v.model_ids, sizeof(uint32_t) * (size_t)R, cudaMemcpyHostToDevice, s0));
@@ -2071,7 +2044,7 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
     }
     for (int i = 0; i < 2; i++) CUDA_TRY(h->slot[i].data.reserve(max_bytes + 64, &h->dev_bytes));
     const size_t E = (size_t)h->cfg.max_endpoints;
-    if (mode == Mode::Match) CUDA_TRY(h->dense_match.reserve(sizeof(int32_t) * (size_t)R * E, &h->dev_bytes));
+    if (call.mode == Mode::Match) CUDA_TRY(h->dense_match.reserve(sizeof(int32_t) * (size_t)R * E, &h->dev_bytes));
 
     CUDA_TRY(cudaEventRecord(h->ev[0], s0));
     for (size_t k = 0; k < chunks.size(); k++) {
@@ -2082,54 +2055,36 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
         // keep the staged copy aligned (mod 32) like the caller's layout
         uint8_t *stage = sl.data.as<uint8_t>() + (c.start & 31);
         if (c.bytes) CUDA_TRY(cudaMemcpyAsync(stage, v.data + c.start, c.bytes, cudaMemcpyHostToDevice, s));
-        Work w;
-        w.r0 = c.r0;
-        w.r1 = c.r1;
-        if (v.offsets) {
-            // the kernels address  data_base + offsets[r]  with ABSOLUTE offsets
-            w.data_base = reinterpret_cast<const uint8_t *>(reinterpret_cast<uintptr_t>(stage) - (uintptr_t)c.start);
-            w.offsets_dev = h->offsets.as<uint64_t>();
-            w.lengths_dev = v.lengths ? h->lengths.as<uint64_t>() : nullptr;
-            w.offsets_or_bits = v.offsets_or_bits;
+        // the kernels address  data_base + offsets[r]  with ABSOLUTE offsets, or  data_base + chunk-local index * uniform_len
+        const uint8_t *base = v.offsets ? reinterpret_cast<const uint8_t *>(reinterpret_cast<uintptr_t>(stage) - (uintptr_t)c.start)
+                                        : stage;
+        const Work w{c.r0, c.r1, base, v.offsets ? h->offsets.as<uint64_t>() : nullptr,
+                     v.offsets && v.lengths ? h->lengths.as<uint64_t>() : nullptr, v.uniform_len,
+                     v.model_ids ? h->model_ids.as<uint32_t>() : nullptr, v.offsets ? v.offsets_or_bits : 0,
+                     h->hashes.as<uint64_t>() + (size_t)c.r0 * B, h->nblocks.as<int32_t>() + c.r0,
+                     v.multimodal ? h->multimodal.as<uint8_t>() : nullptr};
+        int32_t *dm = call.mode == Mode::Match ? h->dense_match.as<int32_t>() + (size_t)c.r0 * E : nullptr;
+        epp_decision *dec = h->decisions.as<epp_decision>() + c.r0;
+        epp_decision_detail *det = h->details.as<epp_decision_detail>() + c.r0;
+        PickParams pp;
+        EPP_TRY(launch_rows(h, sl, w, call, dec, det, dm, false, pp, &call.launches));
+        if (call.mode == Mode::HashOnly) {
+            if (call.out_hashes) CUDA_TRY(cudaMemcpyAsync(call.out_hashes + (size_t)c.r0 * B, w.hashes_out, sizeof(uint64_t) * nreq * B, cudaMemcpyDeviceToHost, s));
+            if (call.out_nblocks) CUDA_TRY(cudaMemcpyAsync(call.out_nblocks + c.r0, w.nblocks_out, sizeof(int32_t) * nreq, cudaMemcpyDeviceToHost, s));
+        } else if (call.mode == Mode::Schedule) {
+            EPP_TRY(launch_subset(h, pp, c.r0, c.r1, s, &call.launches, false));
+            if (call.out_dec) CUDA_TRY(cudaMemcpyAsync(call.out_dec + c.r0, dec, sizeof(epp_decision) * nreq, cudaMemcpyDeviceToHost, s));
+            if (call.out_detail) CUDA_TRY(cudaMemcpyAsync(call.out_detail + c.r0, det, sizeof(epp_decision_detail) * nreq, cudaMemcpyDeviceToHost, s));
+            if (call.tk.on) EPP_TRY(topk_copy_back(h, call.tk, c.r0, (int64_t)nreq, s));
         } else {
-            w.data_base = stage;                    // chunk-local request index * uniform_len
-            w.offsets_dev = nullptr;
-            w.lengths_dev = nullptr;
-            w.offsets_or_bits = 0;
-        }
-        w.uniform_len = v.uniform_len;
-        w.model_ids_dev = v.model_ids ? h->model_ids.as<uint32_t>() : nullptr;
-        w.multimodal_dev = v.multimodal ? h->multimodal.as<uint8_t>() : nullptr;
-        w.hashes_out = h->hashes.as<uint64_t>() + (size_t)c.r0 * B;
-        w.nblocks_out = h->nblocks.as<int32_t>() + c.r0;
-        if (mode == Mode::HashOnly) {
-            CUDA_TRY(launch_hash_prompts(hash_params(h, w, sl), s, &launches));
-            if (out_hashes) CUDA_TRY(cudaMemcpyAsync(out_hashes + (size_t)c.r0 * B, w.hashes_out, sizeof(uint64_t) * nreq * B, cudaMemcpyDeviceToHost, s));
-            if (out_nblocks) CUDA_TRY(cudaMemcpyAsync(out_nblocks + c.r0, w.nblocks_out, sizeof(int32_t) * nreq, cudaMemcpyDeviceToHost, s));
-        } else {
-            int32_t *dm = mode == Mode::Match ? h->dense_match.as<int32_t>() + (size_t)c.r0 * E : nullptr;
-            epp_decision *dec = h->decisions.as<epp_decision>() + c.r0;
-            epp_decision_detail *det = h->details.as<epp_decision_detail>() + c.r0;
-            PickParams pp = pick_params(h, w, dec, det, dm);
-            if (tk.on) attach_topk(h, pp.gen, tk.picks, tk.scores, c.r0);
-            HashParams hp = hash_params(h, w, sl);
-            if (trim) trim_rows(h, w, hp, pp);
-            EPP_TRY(launch_cycle(h, sl, hp, pp, &launches, nullptr, c.r0));
-            if (mode == Mode::Schedule) {
-                EPP_TRY(launch_subset(h, pp, c.r0, c.r1, s, &launches, false));
-                if (out_dec) CUDA_TRY(cudaMemcpyAsync(out_dec + c.r0, dec, sizeof(epp_decision) * nreq, cudaMemcpyDeviceToHost, s));
-                if (out_detail) CUDA_TRY(cudaMemcpyAsync(out_detail + c.r0, det, sizeof(epp_decision_detail) * nreq, cudaMemcpyDeviceToHost, s));
-                if (tk.on) EPP_TRY(topk_copy_back(h, tk, c.r0, (int64_t)nreq, s));
-            } else {
-                if (out_match) CUDA_TRY(cudaMemcpyAsync(out_match + (size_t)c.r0 * E, dm, sizeof(int32_t) * nreq * E, cudaMemcpyDeviceToHost, s));
-                if (out_total) CUDA_TRY(cudaMemcpyAsync(out_total + c.r0, w.nblocks_out, sizeof(int32_t) * nreq, cudaMemcpyDeviceToHost, s));
-            }
+            if (call.out_match) CUDA_TRY(cudaMemcpyAsync(call.out_match + (size_t)c.r0 * E, dm, sizeof(int32_t) * nreq * E, cudaMemcpyDeviceToHost, s));
+            if (call.out_total) CUDA_TRY(cudaMemcpyAsync(call.out_total + c.r0, w.nblocks_out, sizeof(int32_t) * nreq, cudaMemcpyDeviceToHost, s));
         }
     }
     CUDA_TRY(cudaStreamSynchronize(h->slot[1].stream));
-    if (mode == Mode::Schedule)
+    if (call.mode == Mode::Schedule)
         EPP_TRY(after_picks(h, h->decisions.as<epp_decision>(), h->details.as<epp_decision_detail>(), h->in_len.as<int64_t>(), R,
-                            s0, &launches, false));
+                            s0, &call.launches, false));
     CUDA_TRY(cudaEventRecord(h->ev[1], s0));
     CUDA_TRY(cudaStreamSynchronize(s0));
     float t_all = 0;
@@ -2137,8 +2092,54 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
     h->stats.last_kernels_ms = t_all;
     h->stats.last_kernel_ms[6] = 0.0;              // the subset kernel is timed on device batches only
     h->stats.last_hash_ms = h->stats.last_match_pick_ms = 0;
-    h->stats.last_kernel_launches = (uint64_t)launches;
+    h->stats.last_kernel_launches = (uint64_t)call.launches;
     return EPP_OK;
+}
+
+// Runs hashing (+ match/pick) for a batch: device batches in run_device, small host batches in pinned memory in
+// run_small, every other host batch in run_host.
+// keep_hashes: the hash rows of a Schedule batch stay for epp_index_add_picked (whole rows, no trimming).
+static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t *out_hashes, int32_t *out_nblocks,
+                         epp_decision *out_dec, epp_decision_detail *out_detail, int32_t *out_match,
+                         int32_t *out_total, bool keep_hashes = false) {
+    const int64_t R = v.R;
+    if (R == 0) return EPP_OK;
+    if (mode != Mode::HashOnly) {
+        if (!h->pool_ready) return fail(EPP_ERR_STATE, "epp_pool_set has not been called");
+        // index updates become visible here -- or, with index_commit_interval_us, at most that much later: the reference
+        // applies PreRequest in a goroutine of its own "to avoid blocking the request path" (approximateprefix/plugin.go:189-194),
+        // so a scheduling cycle may well run against an index that lacks the last few picks
+        const bool due = h->cfg.index_commit_interval_us <= 0 || !h->committed_once ||
+                         ms_since(h->last_commit) * 1000.0 >= (double)h->cfg.index_commit_interval_us;
+        if (due) {
+            EPP_TRY(commit_locked(h));
+            h->last_commit = std::chrono::steady_clock::now();
+            h->committed_once = true;
+        }
+    }
+    if (h->async_pending && !(v.device && v.async)) EPP_TRY(finish_async(h));
+    Call call{mode, out_hashes, out_nblocks, out_match, out_total, out_dec, out_detail, out_detail};
+    EPP_TRY(topk_rows(h, mode == Mode::Schedule ? h->cur_topk : nullptr, v.device, R, call.tk));
+    call.pipelined = v.device && v.async && mode == Mode::Schedule && h->dev_chunks > 1 && R >= 2 * 4096 && !h->pick_global;
+    // the endpoint-sharded mode's local table is not the global one: its rows stay whole
+    call.trim = mode == Mode::Schedule && !keep_hashes && h->hash_trim && !sharded(h);
+    if (!call.pipelined) EPP_TRY(join_streams(h));
+    EPP_TRY(reserve_batch(h, R));
+    // releases / resets since the last call, on stream 0 before any pick kernel (a pipelined batch's stream 1 waits
+    // for stream 0 in run_device)
+    if (mode == Mode::Schedule) EPP_TRY(inflight_flush(h, h->slot[0].stream, &call.launches));
+    // the stage records reach the producer's add kernel even when the caller asked for none
+    if (mode == Mode::Schedule && !out_detail && h->inflight) call.det_out = h->details.as<epp_decision_detail>();
+    if (v.device) return run_device(h, v, call);
+
+    // small host batch in pinned memory: one zero-copy launch, no copy engine, no stream synchronisation (not for a batch
+    // with restricted requests: the kernel hands the decisions to the host before a subset launch could rewrite them)
+    if (mode == Mode::Schedule && !call.tk.on && out_dec && !h->cur_sub) {
+        const uint8_t *data_dev = nullptr;
+        const int sm = small_batch_mode(h, v, &data_dev);
+        if (sm) return run_small(h, v, sm, data_dev, out_dec, out_detail);
+    }
+    return run_host(h, v, call);
 }
 
 extern "C" int32_t epp_hash_prompts(epp_engine *h, const epp_batch *batch, uint64_t *out_hashes, int32_t *out_nblocks) {
@@ -2177,7 +2178,7 @@ static int32_t check_topk(epp_engine *h, const epp_topk_out *topk) {
 static int32_t check_subset(const epp_engine *h, int64_t R, const epp_subset *s, std::vector<SubsetRow> &rows,
                             uint64_t *n_slots, bool latency_ok) {
     if (s->struct_size != sizeof(epp_subset)) return fail(EPP_ERR_INVALID, "epp_subset.struct_size %u != %zu", s->struct_size, sizeof(epp_subset));
-    if (h->shard_begin != 0 || h->shard_end != 0xFFFFFFFFu || h->p2p_buf)
+    if (sharded(h) || h->p2p_buf)
         return fail(EPP_ERR_INVALID, "endpoint subsets are not available in the endpoint-sharded and peer-memory modes");
     if (h->lat_mask && !latency_ok)
         return fail(EPP_ERR_INVALID, "endpoint subsets on an engine with latency profiles go through epp_schedule_subset_predicted");
@@ -2262,7 +2263,7 @@ extern "C" int32_t epp_latency_profile_set(epp_engine *h, int32_t profile, const
     if (profile < 0 || profile >= h->n_alloc_profiles) return fail(EPP_ERR_INVALID, "profile %d is not configured", profile);
     std::lock_guard<std::mutex> lk(h->mu);
     if (h->pool_called) return fail(EPP_ERR_STATE, "latency profiles are fixed once the pool has been set");
-    if (h->shard_begin != 0 || h->shard_end != 0xFFFFFFFFu || h->p2p_buf)
+    if (sharded(h) || h->p2p_buf)
         return fail(EPP_ERR_INVALID, "endpoint-sharded mode does not support latency profiles");
     const epp_profile_cfg &pc = profile_cfg(h, profile);
     EPP_TRY(validate_latency(pc, *cfg, profile == 0 ? "primary profile" : (profile == 1 ? "prefill profile" : "encode profile")));
@@ -2975,7 +2976,7 @@ static int32_t p2p_phase_rows(epp_engine *h, const BatchView &v, epp_decision *o
     const int64_t R = r1 - r0;
     const int n = h->p2p_ranks;
     const size_t S = (size_t)h->p2p_stages;
-    const size_t W = (size_t)mask_words_of(h), B = (size_t)h->cfg.max_prefix_blocks;
+    const size_t W = (size_t)mask_words_of(h);
     Slot &sl = h->slot[c];
     cudaStream_t s = sl.stream;
     uint8_t *own = static_cast<uint8_t *>(h->p2p_buf);
@@ -2986,17 +2987,14 @@ static int32_t p2p_phase_rows(epp_engine *h, const BatchView &v, epp_decision *o
     const size_t best_off = h->p2p_best_off + (size_t)r0 * S * sizeof(epp_shard_best);
     const unsigned long long timeout_ns = p2p_timeout_ns();
     const unsigned long long epoch = h->p2p_epoch;
-    uint64_t *hashes = h->hashes.as<uint64_t>() + (size_t)r0 * B;
-    int32_t *nbs = h->nblocks.as<int32_t>() + r0;
+    const Work w = device_work(h, v, r0, r1, or_bits);
     uint32_t *gmasks = h->p2p_gmasks.as<uint32_t>() + (size_t)r0 * W;
     epp_shard_best *allbest = h->p2p_allbest.as<epp_shard_best>() + (size_t)r0 * (size_t)n * S;   // this chunk's own [n][R][S] records
     int launches = 0;
     if (phase == 0) {
         // hashes + local presence masks -> own exchange buffer, raise flag 1
-        Work w{r0, r1, v.offsets ? v.data : v.data + (uint64_t)r0 * v.uniform_len, v.offsets, v.lengths, v.uniform_len, v.model_ids,
-               or_bits, hashes, nbs, nullptr};
         CUDA_TRY(launch_hash_prompts(hash_params(h, w, sl), s, &launches));
-        CUDA_TRY(launch_shard_probe(R, h->cfg.max_prefix_blocks, hashes, nbs, index_view(h),
+        CUDA_TRY(launch_shard_probe(R, h->cfg.max_prefix_blocks, w.hashes_out, w.nblocks_out, index_view(h),
                                     reinterpret_cast<uint32_t *>(own + mask_off), (int32_t)W, s, &launches));
         CUDA_TRY(launch_p2p_signal(reinterpret_cast<unsigned long long *>(own + flag1), epoch, s));
         h->p2p_launches += launches + 1;
@@ -3007,9 +3005,7 @@ static int32_t p2p_phase_rows(epp_engine *h, const BatchView &v, epp_decision *o
         // local best record in the own exchange buffer, raise flag 2
         CUDA_TRY(launch_p2p_wait(peers, n, flag1, epoch, h->p2p_err.as<int>(), timeout_ns, s));
         CUDA_TRY(launch_p2p_or_masks(peers, n, mask_off, mask_bytes, gmasks, s));
-        Work w{r0, r1, nullptr, nullptr, nullptr, 0, nullptr, 0, hashes, nbs, v.multimodal};
         PickParams pp = pick_params(h, w, h->decisions.as<epp_decision>() + r0, nullptr, nullptr);
-        pp.model_ids = v.model_ids ? v.model_ids + r0 : nullptr;
         pp.global_masks = gmasks;
         pp.mask_words = (int32_t)W;
         pp.shard_out = reinterpret_cast<epp_shard_best *>(own + best_off);
@@ -3056,7 +3052,7 @@ static int32_t p2p_prepare(epp_engine *h, const epp_batch *batch, epp_decision *
     EPP_TRY(join_streams(h));
     if (h->p2p_peer.empty()) return fail(EPP_ERR_STATE, "epp_shard_p2p_connect has not been called");
     if (h->p2p_broken) return fail(EPP_ERR_STATE, "the sharded exchange is broken (an earlier batch timed out): export and connect the buffers again");
-    if (h->shard_begin == 0 && h->shard_end == 0xFFFFFFFFu) return fail(EPP_ERR_STATE, "epp_shard_set has not been called: every rank would count every endpoint");
+    if (!sharded(h)) return fail(EPP_ERR_STATE, "epp_shard_set has not been called: every rank would count every endpoint");
     if (!h->pool_ready) return fail(EPP_ERR_STATE, "epp_pool_set has not been called (after epp_shard_set)");
     EPP_TRY(check_batch(h, batch, v));
     if (!v.device) return fail(EPP_ERR_INVALID, "the sharded peer-memory entry points take device-pointer batches (EPP_BATCH_DEVICE_PTRS)");
