@@ -66,6 +66,9 @@ type ProfileSpec struct {
 	// Latency: the profile's tier filter, first affinity filter and latency-scorer (ProfilePlacement, latency.go);
 	// epp_latency_profile_set.  nil: none.
 	Latency *LatencySpec
+	// ContextLength: the profile's context-length-aware plugin (ContextLengthPlacement, contextlength.go); it must also
+	// be listed in Scorers as C.EPP_SCORER_CONTEXT_LENGTH with its weight.  epp_context_length_set.  nil: none.
+	ContextLength *ContextLengthSpec
 }
 
 // Config mirrors epp_config (EndpointPickerConfig fields that define this path).
@@ -98,6 +101,7 @@ type Engine struct {
 
 	mu     sync.RWMutex
 	latency bool // some profile has a latency piece: Scheduler.Schedule passes each request's predictions
+	ctxLen  bool // some profile has the context-length-aware plugin: Scheduler.Schedule passes each request's context length
 	slotOf map[types.NamespacedName]uint32
 	nameOf []types.NamespacedName // by slot; zero value = free
 	free   []uint32
@@ -194,6 +198,10 @@ func New(cfg Config) (*Engine, error) {
 			return nil, err
 		}
 		if err := e.setLatency(i, p); err != nil {
+			C.epp_engine_destroy(e.h)
+			return nil, err
+		}
+		if err := e.setContextLength(i, p); err != nil {
 			C.epp_engine_destroy(e.h)
 			return nil, err
 		}

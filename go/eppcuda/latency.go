@@ -91,8 +91,9 @@ func registerLatencyPlugins() {
 // ChainStage is one filter of a profile in order, as ProfilePlacement reads it: a TierFilter, an affinity filter (its
 // AffinitySpec) or anything else (role and label filters, which may only come first).
 type ChainStage struct {
-	Tier     *TierFilter
-	Affinity *AffinitySpec
+	Tier          *TierFilter
+	Affinity      *AffinitySpec
+	ContextLength *ContextLengthAware // taken out of the chain by ContextLengthPlacement first
 }
 
 // ProfilePlacement places a profile's affinity and tier filters on the engine's chain

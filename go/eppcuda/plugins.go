@@ -35,6 +35,7 @@ func Register(e *Engine) {
 	shared = e
 	registerLabelFilters()
 	registerLatencyPlugins()
+	registerContextLengthPlugin()
 	plugin.Register(PrefixProducerType, func(name string, _ json.RawMessage, _ plugin.Handle) (plugin.Plugin, error) {
 		if shared == nil {
 			return nil, errors.New("eppcuda: engine not created")

@@ -95,7 +95,13 @@ func (s *Scheduler) Schedule(ctx context.Context, request *scheduling.InferenceR
 	}
 	mm := HasMultimodalContent != nil && HasMultimodalContent(request)
 	var d Decision
-	if s.Engine.latency && slots == nil {
+	if s.Engine.ctxLen {
+		var pred []C.epp_prediction
+		if s.Engine.latency {
+			pred = s.Engine.predictions(candidates)
+		}
+		d, err = s.Engine.scheduleCtx(model, prompt, mm, slots, pred, ContextLength(request))
+	} else if s.Engine.latency && slots == nil {
 		d, err = s.Engine.schedulePredicted(model, prompt, mm, s.Engine.predictions(candidates))
 	} else if s.Engine.latency {
 		d, err = s.Engine.scheduleSubsetPredicted(model, prompt, mm, slots, s.Engine.predictions(candidates))

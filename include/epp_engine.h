@@ -149,8 +149,10 @@ typedef enum {
                                   started and then Adds, for each cold request in request order, its pick and its
                                   prefill pick (PreRequest, :279-321): inside one batch cold requests do not rotate.
                                   Not available in the endpoint-sharded and peer-memory modes.                    */
-    EPP_SCORER_LATENCY = 10    /* "latency-scorer"               scorer/latency/plugin.go:144-395; reads the request's latency
+    EPP_SCORER_LATENCY = 10,   /* "latency-scorer"               scorer/latency/plugin.go:144-395; reads the request's latency
                                   predictions, configured by epp_latency_profile_set (see "Latency predictions")  */
+    EPP_SCORER_CONTEXT_LENGTH = 11 /* "context-length-aware"     scorer/contextlengthaware/context_length_aware.go; scorer and
+                                  filter, configured by epp_context_length_set (see "Context length")            */
 } epp_scorer_kind;
 
 /* Value of the llm-d.ai/role label (filter/bylabel/roles.go:25-44). */
@@ -642,6 +644,57 @@ EPP_API int32_t epp_schedule_subset_predicted(epp_engine *h, const epp_batch *ba
                                               const epp_predictions *preds, epp_decision *out, epp_decision_detail *detail,
                                               int32_t keep_hashes, const epp_topk_out *topk /* or NULL */);
 
+/* ---- Context length (scorer/contextlengthaware/context_length_aware.go, "context-length-aware") ---------------------
+ * One plugin that is both a scorer and a filter: it sends long prompts to endpoints whose range label covers them.  A
+ * profile lists it as EPP_SCORER_CONTEXT_LENGTH with its weight (at most one per profile) and is then a CHAIN profile,
+ * decided by the evaluation of "Latency predictions" (it counts as a latency profile wherever that section says so:
+ * subsets through epp_schedule_subset_predicted / epp_schedule_ctx, predictions accepted, no endpoint-sharded mode):
+ *     [role + label + context-length filters] -> [A1] -> [T] -> [A2] -> scorers in order -> picker
+ *   The context-length filter is a per-endpoint predicate on the request's context length, so it joins the role and label
+ *   filters in the first stage.  Everything taken "over the set" uses the final set: the affinity filters' gates and sticky
+ *   sets, the queue / running min-max, the active-request max, the latency scorer's buckets, tie_count, and the random
+ *   pickers' population (every candidate an explicit item).
+ * Range label: each profile names a label key (default "llm-d.ai/context-length-range"; profiles may name different keys);
+ *   epp_pool_set_labels parses the value of every slot (parseContextRange): split on "-" into exactly 2 parts, each part
+ *   trimmed of Unicode white space (strings.TrimSpace) and read by strconv.Atoi (base 10, optional sign, int64 range), and
+ *   min <= max; anything else, the empty value included, is an INVALID label.  Slots without the key have NO label.  The
+ *   ranges follow the label snapshot rule: batches enqueued before an epp_pool_set_labels decide on the ranges they were
+ *   enqueued under.
+ * Filter (enable_filtering != 0): no label keeps, an invalid label drops, else keep iff min <= ctx <= max.  A request whose
+ *   filter empties its decode set gets status -1 (that request only); an empty prefill or encode set omits that stage.
+ * Score: no label 0.5; invalid label 0.0; in range with w = max - min: 1.0 when w == 0, else 0.3 + raw * 0.7 with raw =
+ *   0.7 * (1 / (1 + w / 10000)) + 0.3 * ((max - ctx) / w); out of range 0.3 / (1 + d / 1000), d = the distance to the nearer
+ *   bound.  Integers convert to double rounding to nearest; every operation rounds on its own (no fused multiply-add).
+ * Request context length ctx: the caller's token count (len(TokenizedPrompt.TokenIDs), or its chat estimate) when it passes
+ *   one; else the reference's estimate of a completions request, ctx = int(float64(L) * 0.25) = floor(L / 4) for L < 2^53,
+ *   with L the true prompt length as est(L) of "In-flight load" reads it (lengths[r], the row length, input_len_bytes[r]).
+ *   Every scheduling call decides context-length profiles with that default.
+ * Refused (EPP_ERR_INVALID): a second context-length scorer in one profile; the no-hit-lru scorer or ttft_column >= 0 on a
+ *   profile that lists it; the endpoint-sharded and peer-memory modes; epp_score naming its index, or -1 on its profile. */
+#define EPP_CONTEXT_LENGTH_LABEL "llm-d.ai/context-length-range"
+/* Sets profile's label key (NUL-terminated, non-empty; NULL = the default) and filtering (0 or 1, default 0).  Only
+ * before the engine's first successful epp_pool_set / epp_pool_set_labels (EPP_ERR_STATE after), and only on a profile
+ * that lists the scorer. */
+EPP_API int32_t epp_context_length_set(epp_engine *h, int32_t profile, const char *label, int32_t enable_filtering);
+/* Per-request context lengths: tokens[r] >= 0 is request r's ctx, -1 the default above.  HOST memory for every batch kind,
+ * validated and copied before anything is launched; an entry < -1 or a wrong struct_size is EPP_ERR_INVALID and the call
+ * then changes no ordinal, LRU or counter state.  Accepted on every engine (read only by context-length profiles). */
+typedef struct {
+    uint32_t struct_size;              /* sizeof(epp_context_tokens)                                                   */
+    uint32_t reserved;
+    const int64_t *tokens;             /* [R]                                                                          */
+} epp_context_tokens;
+/* epp_schedule_subset_predicted plus context lengths; subset, preds, ctx and topk may each be NULL. */
+EPP_API int32_t epp_schedule_ctx(epp_engine *h, const epp_batch *batch, const epp_subset *subset, const epp_predictions *preds,
+                                 const epp_context_tokens *ctx, epp_decision *out, epp_decision_detail *detail,
+                                 int32_t keep_hashes, const epp_topk_out *topk);
+/* epp_schedule_with_match_predicted plus context lengths (ctx may be NULL). */
+EPP_API int32_t epp_schedule_with_match_ctx(epp_engine *h, int64_t n_requests, const int32_t *match, const int32_t *total,
+                                            const uint32_t *model_ids, const int64_t *input_len_bytes, int32_t block_size_tokens,
+                                            epp_decision *out, epp_decision_detail *detail, uint32_t flags,
+                                            const epp_topk_out *topk, const epp_predictions *preds,
+                                            const epp_context_tokens *ctx);
+
 /* PreRequest (approximateprefix/plugin.go:164-200): index the hashes of the LAST epp_schedule batch
  * (keep_hashes=1) for each request's primary pick and prefill pick. */
 EPP_API int32_t epp_index_add_picked(epp_engine *h);
@@ -797,6 +850,13 @@ EPP_API int32_t epp_submit_predicted(epp_batcher *b, uint32_t model_id, const vo
 EPP_API int32_t epp_submit_subset_predicted(epp_batcher *b, uint32_t model_id, const void *prompt, uint64_t prompt_len,
                                             uint32_t multimodal, uint32_t n_slots, const uint32_t *slots, uint32_t n_pred,
                                             const epp_prediction *entries, uint64_t *out_ticket);
+/* epp_submit with everything a request may carry (see "Context length"): an endpoint subset (slots == NULL: none, then
+ * n_slots must be 0), predictions (n_pred entries; a latency engine is required when n_pred > 0) and context_tokens (-1 =
+ * the default, < -1 EPP_ERR_INVALID), each checked here with the rules of epp_submit_subset_predicted.  A flush that holds
+ * such a request runs epp_schedule_ctx. */
+EPP_API int32_t epp_submit_ctx(epp_batcher *b, uint32_t model_id, const void *prompt, uint64_t prompt_len, uint32_t multimodal,
+                               uint32_t n_slots, const uint32_t *slots, uint32_t n_pred, const epp_prediction *entries,
+                               int64_t context_tokens, uint64_t *out_ticket);
 EPP_API int32_t epp_wait(epp_batcher *b, uint64_t ticket, epp_decision *out, epp_decision_detail *out_detail);
 /* The same on an engine created with pick_k > 1, plus the request's first-k lists (ProfileRunResult.TargetEndpoints of
  * each profile, see epp_topk_out): primary / prefill / encode receive pick_k slot ids each (EPP_NO_ENDPOINT padded); any

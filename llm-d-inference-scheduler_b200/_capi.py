@@ -18,7 +18,7 @@ EPP_BATCH_LENGTHS_EXCEED_ROWS = 4
 EPP_OK, EPP_ERR_INVALID, EPP_ERR_CUDA, EPP_ERR_NO_DEVICE, EPP_ERR_CAPACITY, EPP_ERR_STATE, EPP_ERR_NCCL = \
     0, -1, -2, -3, -4, -5, -6
 (SCORER_PREFIX, SCORER_KV_UTIL, SCORER_QUEUE, SCORER_LOAD_AWARE, SCORER_EXTERNAL, SCORER_RUNNING, SCORER_TOKEN_LOAD,
- SCORER_ACTIVE_REQUEST, SCORER_LORA_AFFINITY, SCORER_NO_HIT_LRU, SCORER_LATENCY) = range(11)
+ SCORER_ACTIVE_REQUEST, SCORER_LORA_AFFINITY, SCORER_NO_HIT_LRU, SCORER_LATENCY, SCORER_CONTEXT_LENGTH) = range(12)
 (ROLE_NONE, ROLE_DECODE, ROLE_PREFILL, ROLE_PREFILL_DECODE, ROLE_BOTH, ROLE_ENCODE, ROLE_ENCODE_PREFILL,
  ROLE_ENCODE_PREFILL_DECODE, ROLE_OTHER) = range(9)
 FILTER_NONE, FILTER_DECODE, FILTER_PREFILL, FILTER_ENCODE = range(4)
@@ -115,6 +115,13 @@ EPP_LABEL_MAX_REQS = 32
 LABEL_IN, LABEL_NOT_IN, LABEL_EXISTS, LABEL_DOES_NOT_EXIST, LABEL_BY_LABEL, LABEL_BY_LABEL_OR_ABSENT = range(6)
 
 
+CONTEXT_LENGTH_LABEL = "llm-d.ai/context-length-range"
+
+
+class ContextTokens(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("reserved", C.c_uint32), ("tokens", C.c_void_p)]
+
+
 class LabelReq(C.Structure):
     _fields_ = [("key", C.c_char_p), ("op", C.c_int32), ("n_values", C.c_int32), ("values", C.POINTER(C.c_char_p))]
 
@@ -182,6 +189,12 @@ SIGNATURES = {
                                                       C.POINTER(Predictions)]),
     "epp_schedule_subset_predicted": (C.c_int32, [C.c_void_p, C.POINTER(Batch), C.POINTER(Subset), C.POINTER(Predictions),
                                                   C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(TopkOut)]),
+    "epp_context_length_set": (C.c_int32, [C.c_void_p, C.c_int32, C.c_char_p, C.c_int32]),
+    "epp_schedule_ctx": (C.c_int32, [C.c_void_p, C.POINTER(Batch), C.POINTER(Subset), C.POINTER(Predictions),
+                                     C.POINTER(ContextTokens), C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(TopkOut)]),
+    "epp_schedule_with_match_ctx": (C.c_int32, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                C.c_int32, C.c_void_p, C.c_void_p, C.c_uint32, C.POINTER(TopkOut),
+                                                C.POINTER(Predictions), C.POINTER(ContextTokens)]),
     "epp_index_add_picked": (C.c_int32, [C.c_void_p]),
     "epp_nohit_lru_get": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(C.c_int32)]),
     "epp_inflight_release": (C.c_int32, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
@@ -213,6 +226,8 @@ SIGNATURES = {
                                          C.POINTER(C.c_uint64)]),
     "epp_submit_subset_predicted": (C.c_int32, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_uint32, C.c_uint32,
                                                 C.c_void_p, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint64)]),
+    "epp_submit_ctx": (C.c_int32, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_uint32, C.c_uint32, C.c_void_p,
+                                   C.c_uint32, C.c_void_p, C.c_int64, C.POINTER(C.c_uint64)]),
     "epp_wait": (C.c_int32, [C.c_void_p, C.c_uint64, C.POINTER(Decision), C.POINTER(DecisionDetail)]),
     "epp_wait_topk": (C.c_int32, [C.c_void_p, C.c_uint64, C.POINTER(Decision), C.POINTER(DecisionDetail), C.c_void_p,
                                   C.c_void_p, C.c_void_p]),

@@ -79,6 +79,9 @@ struct Staging {
     std::vector<uint64_t> pred_offsets;        // [max_batch]
     std::vector<epp_prediction> pred_entries;  // [max_batch][EPP_PRED_MAX_SLOTS], allocated by the first predicted submit
     std::atomic<int32_t> any_pred{0};          // some row of the batch using this buffer has predictions
+    // context lengths (epp_submit_ctx): per row its token count, -1 = the default
+    std::vector<int64_t> ctx;                  // [max_batch]
+    std::atomic<int32_t> any_ctx{0};           // some row of the batch using this buffer has a token count
     std::atomic<int32_t> ready{0};             // rows of the batch using this buffer whose copy is complete
     std::atomic<int64_t> first_arrival_ns{0};  // when row 0 of that batch was reserved
 };
@@ -180,7 +183,8 @@ static void flusher_main(epp_batcher *b) {
         tk.primary = st.topk[0]; tk.prefill = st.topk[1]; tk.encode = st.topk[2];
         const bool any_pred = st.any_pred.load(std::memory_order_acquire) != 0;
         const bool any_sub = st.any_subset.load(std::memory_order_acquire) != 0;
-        if (any_pred || any_sub) {
+        const bool any_ctx = st.any_ctx.load(std::memory_order_acquire) != 0;
+        if (any_pred || any_sub || any_ctx) {
             // predictions only reach a latency engine (every predicted submit checks it), where subsets and predictions
             // may share a batch and even a row: one epp_schedule_subset_predicted decides them all
             epp_predictions pr;
@@ -195,13 +199,21 @@ static void flusher_main(epp_batcher *b) {
             sub.counts = st.sub_counts.data();
             sub.offsets = st.sub_offsets.data();
             sub.slots = st.sub_slots.data();
-            if (engine_latency_mask(b->eng))
+            epp_context_tokens ct;
+            memset(&ct, 0, sizeof ct);
+            ct.struct_size = sizeof ct;
+            ct.tokens = st.ctx.data();
+            if (any_ctx)
+                rc = epp_schedule_ctx(b->eng, &batch, any_sub ? &sub : nullptr, any_pred ? &pr : nullptr, &ct, st.dec, st.det,
+                                      b->cfg.index_picks ? 1 : 0, b->pick_k > 1 ? &tk : nullptr);
+            else if (engine_latency_mask(b->eng))
                 rc = epp_schedule_subset_predicted(b->eng, &batch, any_sub ? &sub : nullptr, any_pred ? &pr : nullptr, st.dec, st.det,
                                                    b->cfg.index_picks ? 1 : 0, b->pick_k > 1 ? &tk : nullptr);
             else
                 rc = epp_schedule_subset(b->eng, &batch, &sub, st.dec, st.det, b->cfg.index_picks ? 1 : 0, b->pick_k > 1 ? &tk : nullptr);
             st.any_pred.store(0, std::memory_order_relaxed);
             st.any_subset.store(0, std::memory_order_relaxed);
+            st.any_ctx.store(0, std::memory_order_relaxed);
         } else if (b->pick_k > 1) {
             rc = epp_schedule_topk(b->eng, &batch, st.dec, st.det, b->cfg.index_picks ? 1 : 0, &tk);
         } else {
@@ -293,6 +305,7 @@ extern "C" int32_t epp_batcher_create(epp_engine *h, const epp_batcher_cfg *cfg,
         st.pred_counts.assign(mb, 0);
         st.pred_offsets.resize(mb);
         for (size_t r = 0; r < mb; r++) st.pred_offsets[r] = (uint64_t)r * EPP_PRED_MAX_SLOTS;
+        st.ctx.assign(mb, -1);
         if (b->pick_k > 1)
             for (int q = 0; q < 3; q++) {
                 rc = epp_host_alloc(sizeof(uint32_t) * mb * (size_t)b->pick_k, &p);
@@ -326,10 +339,10 @@ extern "C" int32_t epp_batcher_destroy(epp_batcher *b) {
 }
 
 // sub: the request's slots, sorted and deduplicated, or nullptr (the whole pool); pred: its predictions, validated and
-// sorted by slot, or nullptr (none)
+// sorted by slot, or nullptr (none); ctx: its context tokens, -1 = the default
 static int32_t submit_impl(epp_batcher *b, uint32_t model_id, const void *prompt, uint64_t prompt_len, uint32_t multimodal,
                            const std::vector<uint32_t> *sub, uint64_t *out_ticket,
-                           const std::vector<epp_prediction> *pred = nullptr) {
+                           const std::vector<epp_prediction> *pred = nullptr, int64_t ctx = -1) {
     const uint64_t max_batch = (uint64_t)b->cfg.max_batch;
     uint64_t seq, idx;
     for (int spin = 0;; spin++) {
@@ -378,6 +391,8 @@ static int32_t submit_impl(epp_batcher *b, uint32_t model_id, const void *prompt
     } else {
         st.pred_counts[idx] = 0;
     }
+    st.ctx[idx] = ctx;
+    if (ctx != -1) st.any_ctx.store(1, std::memory_order_relaxed);   // published by the release below
     st.ready.fetch_add(1, std::memory_order_release);              // the flusher waits for this before it reads the row
     *out_ticket = (seq << 20) | idx;
     return EPP_OK;
@@ -467,6 +482,20 @@ extern "C" int32_t epp_submit_subset_predicted(epp_batcher *b, uint32_t model_id
     if (rc == EPP_OK) rc = take_predictions(b, n_pred, entries, &pred);
     if (rc != EPP_OK) return rc;
     return submit_impl(b, model_id, prompt, prompt_len, multimodal, &sub, out_ticket, &pred);
+}
+
+extern "C" int32_t epp_submit_ctx(epp_batcher *b, uint32_t model_id, const void *prompt, uint64_t prompt_len, uint32_t multimodal,
+                                  uint32_t n_slots, const uint32_t *slots, uint32_t n_pred, const epp_prediction *entries,
+                                  int64_t context_tokens, uint64_t *out_ticket) {
+    if (!b || !out_ticket || (prompt_len && !prompt) || (n_slots && !slots) || (n_pred && !entries))
+        return bfail(EPP_ERR_INVALID, "NULL argument");
+    if (context_tokens < -1) return bfail(EPP_ERR_INVALID, "context tokens < -1");
+    std::vector<uint32_t> sub;
+    std::vector<epp_prediction> pred;
+    int32_t rc = slots ? take_subset(b, n_slots, slots, &sub) : EPP_OK;
+    if (rc == EPP_OK && n_pred) rc = take_predictions(b, n_pred, entries, &pred);
+    if (rc != EPP_OK) return rc;
+    return submit_impl(b, model_id, prompt, prompt_len, multimodal, slots ? &sub : nullptr, out_ticket, &pred, context_tokens);
 }
 
 extern "C" int32_t epp_wait(epp_batcher *b, uint64_t ticket, epp_decision *out, epp_decision_detail *out_detail) {

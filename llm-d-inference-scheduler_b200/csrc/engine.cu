@@ -132,6 +132,16 @@ struct epp_engine {
     void *lat_host = nullptr;       // pinned staging of counts, offsets and entries
     size_t lat_host_cap = 0;
     cudaEvent_t lat_up_ev = nullptr;    // behind the last upload from lat_host
+    // context length (include/epp_engine.h "Context length"): the profiles listing the plugin (they are in lat_mask too),
+    // each one's label key, filtering and per-slot ranges; the staged token counts of the call in progress (cur_ctx)
+    int cl_mask = 0, cl_filter = 0;
+    std::string cl_label[kMaxProfiles];
+    DevBuf cl_rng[kMaxProfiles];    // longlong2 [E] (kernels.h LatView::rng)
+    bool cur_ctx = false;
+    DevBuf ctx_dev;
+    int64_t *ctx_host = nullptr;    // pinned staging of the token counts
+    size_t ctx_host_cap = 0;
+    cudaEvent_t ctx_up_ev = nullptr;    // behind the last upload from ctx_host
     ProfileState prof[kMaxProfiles];
     // no-hit-lru scorer (nohit_lru.cu), allocated only when a profile lists it
     int nohit_mask = 0;             // bit pi: profile pi has the scorer
@@ -296,7 +306,7 @@ static int32_t validate_profile(const epp_profile_cfg &p, int n_ext, bool inflig
     if (p.n_scorers < 0 || p.n_scorers > EPP_MAX_SCORERS) return fail(EPP_ERR_INVALID, "%s: n_scorers %d out of range", name, p.n_scorers);
     for (int s = 0; s < p.n_scorers; s++) {
         const epp_scorer_cfg &sc = p.scorers[s];
-        if (sc.kind < EPP_SCORER_PREFIX || sc.kind > EPP_SCORER_LATENCY) return fail(EPP_ERR_INVALID, "%s: scorer %d has unknown kind %d", name, s, sc.kind);
+        if (sc.kind < EPP_SCORER_PREFIX || sc.kind > EPP_SCORER_CONTEXT_LENGTH) return fail(EPP_ERR_INVALID, "%s: scorer %d has unknown kind %d", name, s, sc.kind);
         if (!std::isfinite(sc.weight)) return fail(EPP_ERR_INVALID, "%s: scorer %d weight is not finite", name, s);
         if (!inflight && (sc.kind == EPP_SCORER_TOKEN_LOAD || sc.kind == EPP_SCORER_ACTIVE_REQUEST) && (sc.column < 0 || sc.column >= n_ext))
             return fail(EPP_ERR_INVALID, "%s: scorer %d reads ext column %d, out of range [0,%d)", name, s, sc.column, n_ext);
@@ -308,6 +318,9 @@ static int32_t validate_profile(const epp_profile_cfg &p, int n_ext, bool inflig
     if (!(p.max_ttft_penalty_ms >= 0.0)) return fail(EPP_ERR_INVALID, "%s: maxTTFTPenaltyMs must be >= 0, got %f", name, p.max_ttft_penalty_ms);
     if (p.affinity_threshold > 0.0 && p.ttft_column >= n_ext) return fail(EPP_ERR_INVALID, "%s: ttft_column %d out of range [0,%d)", name, p.ttft_column, n_ext);
     if (p.picker < EPP_PICKER_MAX_SCORE || p.picker > EPP_PICKER_WEIGHTED_RANDOM) return fail(EPP_ERR_INVALID, "%s: unknown picker %d", name, p.picker);
+    int n_cl = 0;
+    for (int s = 0; s < p.n_scorers; s++) n_cl += p.scorers[s].kind == EPP_SCORER_CONTEXT_LENGTH;
+    if (n_cl > 1) return fail(EPP_ERR_INVALID, "%s: the context-length scorer is listed %d times (at most once per profile)", name, n_cl);
     return EPP_OK;
 }
 
@@ -316,7 +329,14 @@ static bool lists_scorer(const epp_profile_cfg &p, int kind) {
         if (p.scorers[s].kind == kind) return true;
     return false;
 }
-// The rules a profile with a latency piece adds to validate_profile ("Latency predictions").
+static bool latency_piece(const epp_profile_cfg &p, const epp_latency_cfg &c) {
+    return c.tier_filter || c.a1_affinity_threshold > 0.0 || lists_scorer(p, EPP_SCORER_LATENCY);
+}
+// A profile decided by the chain of pick_latency.cuh: a latency piece or the context-length plugin ("Context length").
+static bool chain_profile(const epp_profile_cfg &p, const epp_latency_cfg &c) {
+    return latency_piece(p, c) || lists_scorer(p, EPP_SCORER_CONTEXT_LENGTH);
+}
+// The rules a chain profile adds to validate_profile ("Latency predictions", "Context length").
 static int32_t validate_latency(const epp_profile_cfg &p, const epp_latency_cfg &c, const char *name) {
     if (c.struct_size != sizeof(epp_latency_cfg)) return fail(EPP_ERR_INVALID, "epp_latency_cfg.struct_size %u != %zu", c.struct_size, sizeof(epp_latency_cfg));
     if (c.tier_filter != 0 && c.tier_filter != 1) return fail(EPP_ERR_INVALID, "%s: tier_filter %d must be 0 or 1", name, c.tier_filter);
@@ -328,13 +348,10 @@ static int32_t validate_latency(const epp_profile_cfg &p, const epp_latency_cfg 
     if (c.strategy != EPP_HEADROOM_LEAST && c.strategy != EPP_HEADROOM_MOST) return fail(EPP_ERR_INVALID, "%s: unknown headroom strategy %d", name, c.strategy);
     const double w[5] = {c.ttft_weight, c.tpot_weight, c.composite_kv_weight, c.composite_queue_weight, c.composite_prefix_weight};
     for (double x : w) if (!std::isfinite(x)) return fail(EPP_ERR_INVALID, "%s: latency-scorer weights must be finite", name);
-    const bool piece = c.tier_filter || c.a1_affinity_threshold > 0.0 || lists_scorer(p, EPP_SCORER_LATENCY);
-    if (piece && lists_scorer(p, EPP_SCORER_NO_HIT_LRU)) return fail(EPP_ERR_INVALID, "%s: the no-hit-lru scorer is not available on a latency profile", name);
-    if (piece && p.ttft_column >= 0) return fail(EPP_ERR_INVALID, "%s: a latency profile reads TTFT from the predictions: ttft_column must be < 0", name);
+    const bool piece = chain_profile(p, c);
+    if (piece && lists_scorer(p, EPP_SCORER_NO_HIT_LRU)) return fail(EPP_ERR_INVALID, "%s: the no-hit-lru scorer is not available on a latency or context-length profile", name);
+    if (piece && p.ttft_column >= 0) return fail(EPP_ERR_INVALID, "%s: a latency or context-length profile reads TTFT from the predictions: ttft_column must be < 0", name);
     return EPP_OK;
-}
-static bool latency_piece(const epp_profile_cfg &p, const epp_latency_cfg &c) {
-    return c.tier_filter || c.a1_affinity_threshold > 0.0 || lists_scorer(p, EPP_SCORER_LATENCY);
 }
 
 static int32_t alloc_profile(epp_engine *e, ProfileState &ps, bool random_picker) {
@@ -498,7 +515,13 @@ extern "C" int32_t epp_engine_create(const epp_config *cfg, epp_engine **out) {
         epp_latency_cfg_default(&e->lat_cfg[pi]);
         const epp_profile_cfg &pc = profile_cfg(e.get(), pi);
         EPP_TRY(validate_latency(pc, e->lat_cfg[pi], pi == 0 ? "primary profile" : (pi == 1 ? "prefill profile" : "encode profile")));
-        if (latency_piece(pc, e->lat_cfg[pi])) e->lat_mask |= 1 << pi;
+        if (chain_profile(pc, e->lat_cfg[pi])) e->lat_mask |= 1 << pi;
+        if (!lists_scorer(pc, EPP_SCORER_CONTEXT_LENGTH)) continue;
+        e->cl_mask |= 1 << pi;
+        e->cl_label[pi] = EPP_CONTEXT_LENGTH_LABEL;
+        const std::vector<longlong2> absent(E, longlong2{kRangeAbsent, 0});     // no labels yet
+        CUDA_TRY(e->cl_rng[pi].reserve(sizeof(longlong2) * E, &e->dev_bytes));
+        CUDA_TRY(cudaMemcpy(e->cl_rng[pi].p, absent.data(), sizeof(longlong2) * E, cudaMemcpyHostToDevice));
     }
     if (e->lat_mask) e->general = true;
     e->store.reset(new IndexStore((uint32_t)cfg->max_endpoints, cfg->lru_capacity_per_server, e->sm_count));
@@ -553,6 +576,8 @@ extern "C" int32_t epp_engine_destroy(epp_engine *h) {
     cudaDeviceSynchronize();
     if (h->lat_host) cudaFreeHost(h->lat_host);
     if (h->lat_up_ev) cudaEventDestroy(h->lat_up_ev);
+    if (h->ctx_host) cudaFreeHost(h->ctx_host);
+    if (h->ctx_up_ev) cudaEventDestroy(h->ctx_up_ev);
     for (int i = 0; i < 2; i++) {
         if (h->slot[i].stream) cudaStreamDestroy(h->slot[i].stream);
         if (h->slot[i].done) cudaEventDestroy(h->slot[i].done);
@@ -1037,6 +1062,88 @@ extern "C" int32_t epp_label_filters_set(epp_engine *h, int32_t profile, int32_t
     return EPP_OK;
 }
 
+// ---- context length ---------------------------------------------------------------------------------------------------
+// unicode.IsSpace
+static bool go_is_space(uint32_t r) {
+    if (r < 0x80) return r == ' ' || (r >= '\t' && r <= '\r');
+    return r == 0x85 || r == 0xA0 || r == 0x1680 || (r >= 0x2000 && r <= 0x200A) || r == 0x2028 || r == 0x2029 ||
+           r == 0x202F || r == 0x205F || r == 0x3000;
+}
+// The rune encoded by exactly the bytes [p, end), or -1 when they are not one valid UTF-8 sequence.
+static int64_t utf8_rune(const unsigned char *p, const unsigned char *end) {
+    const size_t n = (size_t)(end - p);
+    if (n == 1) return p[0] < 0x80 ? p[0] : -1;
+    const size_t want = (p[0] & 0xE0) == 0xC0 ? 2 : (p[0] & 0xF0) == 0xE0 ? 3 : (p[0] & 0xF8) == 0xF0 ? 4 : 0;
+    if (want != n) return -1;
+    uint32_t r = p[0] & (0x7F >> n);
+    for (size_t i = 1; i < n; i++) {
+        if ((p[i] & 0xC0) != 0x80) return -1;
+        r = (r << 6) | (p[i] & 0x3F);
+    }
+    static const uint32_t min_of[5] = {0, 0, 0x80, 0x800, 0x10000};
+    if (r < min_of[n] || r > 0x10FFFF || (r >= 0xD800 && r <= 0xDFFF)) return -1;
+    return r;
+}
+// strings.TrimSpace: white-space runes off both ends (an invalid byte stops the trim, as utf8.RuneError is no space).
+static std::string go_trim_space(const std::string &v) {
+    const unsigned char *b = reinterpret_cast<const unsigned char *>(v.data()), *e = b + v.size();
+    while (b < e) {
+        const ptrdiff_t want = *b < 0x80 ? 1 : (*b & 0xE0) == 0xC0 ? 2 : (*b & 0xF0) == 0xE0 ? 3 : 4;
+        const unsigned char *q = e - b < want ? e : b + want;
+        const int64_t r = utf8_rune(b, q);
+        if (r < 0 || !go_is_space((uint32_t)r)) break;
+        b = q;
+    }
+    while (e > b) {
+        const unsigned char *q = e - 1;
+        while (q > b && e - q < 4 && (*q & 0xC0) == 0x80) q--;
+        const int64_t r = utf8_rune(q, e);
+        if (r < 0 || !go_is_space((uint32_t)r)) break;
+        e = q;
+    }
+    return std::string(reinterpret_cast<const char *>(b), (size_t)(e - b));
+}
+// strconv.Atoi on a 64-bit platform: optional sign, then at least one decimal digit and nothing else, within int64.
+static bool go_atoi(const std::string &v, long long *out) {
+    size_t i = 0;
+    bool neg = false;
+    if (i < v.size() && (v[i] == '+' || v[i] == '-')) neg = v[i++] == '-';
+    if (i == v.size()) return false;
+    const unsigned long long lim = neg ? (1ull << 63) : (1ull << 63) - 1;
+    unsigned long long x = 0;
+    for (; i < v.size(); i++) {
+        if (v[i] < '0' || v[i] > '9') return false;
+        const unsigned d = (unsigned)(v[i] - '0');
+        if (x > (lim - d) / 10) return false;
+        x = x * 10 + d;
+    }
+    *out = neg ? (long long)(0ull - x) : (long long)x;
+    return true;
+}
+// parseContextRange: "min-max" split on "-" into exactly 2 parts, each TrimSpace + Atoi, min <= max.
+static bool parse_context_range(const std::string &v, long long *lo, long long *hi) {
+    const size_t dash = v.find('-');
+    if (v.empty() || dash == std::string::npos || v.find('-', dash + 1) != std::string::npos) return false;
+    if (!go_atoi(go_trim_space(v.substr(0, dash)), lo) || !go_atoi(go_trim_space(v.substr(dash + 1)), hi)) return false;
+    return *lo <= *hi;
+}
+
+extern "C" int32_t epp_context_length_set(epp_engine *h, int32_t profile, const char *label, int32_t enable_filtering) {
+    if (!h) return fail(EPP_ERR_INVALID, "NULL engine");
+    if (profile < 0 || profile >= h->n_alloc_profiles) return fail(EPP_ERR_INVALID, "profile %d is not configured", profile);
+    if (label && !label[0]) return fail(EPP_ERR_INVALID, "the context-length label must not be empty");
+    if (label && strpbrk(label, "=\n")) return fail(EPP_ERR_INVALID, "the context-length label holds '=' or a newline");
+    if (enable_filtering != 0 && enable_filtering != 1) return fail(EPP_ERR_INVALID, "enable_filtering %d must be 0 or 1", enable_filtering);
+    std::lock_guard<std::mutex> lk(h->mu);
+    if (h->pool_called) return fail(EPP_ERR_STATE, "context-length profiles are fixed once the pool has been set");
+    if (sharded(h) || h->p2p_buf) return fail(EPP_ERR_INVALID, "endpoint-sharded mode does not support the context-length scorer");
+    if (!((h->cl_mask >> profile) & 1)) return fail(EPP_ERR_INVALID, "profile %d does not list the context-length scorer", profile);
+    h->cl_label[profile] = label ? label : EPP_CONTEXT_LENGTH_LABEL;
+    if (enable_filtering) h->cl_filter |= 1 << profile;
+    else h->cl_filter &= ~(1 << profile);
+    return EPP_OK;
+}
+
 extern "C" int32_t epp_pool_set_labels(epp_engine *h, int32_t n, const uint32_t *ids, const uint64_t *offsets,
                                        const uint8_t *text) {
     if (!h) return fail(EPP_ERR_INVALID, "NULL engine");
@@ -1048,6 +1155,9 @@ extern "C" int32_t epp_pool_set_labels(epp_engine *h, int32_t n, const uint32_t 
     std::unordered_map<std::string, size_t> key_row;
     for (size_t k = 0; k < K; k++) key_row.emplace(h->labels.keys[k], k);
     std::vector<std::string> slot_keys;
+    std::vector<longlong2> rng[kMaxProfiles];          // context-length ranges of the profiles listing the plugin
+    for (int pi = 0; pi < kMaxProfiles; pi++)
+        if ((h->cl_mask >> pi) & 1) rng[pi].assign(E, longlong2{kRangeAbsent, 0});
     for (int32_t i = 0; i < n; i++) {
         const uint32_t id = ids[i];
         if (id >= E) return fail(EPP_ERR_INVALID, "label entry %d: slot id %u >= max_endpoints %u", i, id, E);
@@ -1066,6 +1176,11 @@ extern "C" int32_t epp_pool_set_labels(epp_engine *h, int32_t n, const uint32_t 
             if (std::find(slot_keys.begin(), slot_keys.end(), key) != slot_keys.end())
                 return fail(EPP_ERR_INVALID, "label entry %d: key \"%s\" repeated", i, key.c_str());
             slot_keys.push_back(key);
+            for (int pi = 0; pi < kMaxProfiles; pi++) {
+                if (!((h->cl_mask >> pi) & 1) || key != h->cl_label[pi]) continue;
+                long long lo, hi;
+                rng[pi][id] = parse_context_range(std::string(eq + 1, nl), &lo, &hi) ? longlong2{lo, hi} : longlong2{kRangeInvalid, 0};
+            }
             auto kr = key_row.find(key);
             if (kr != key_row.end()) {                     // keys no requirement references are dropped here
                 const auto &codes = h->labels.codes[kr->second];
@@ -1076,12 +1191,17 @@ extern "C" int32_t epp_pool_set_labels(epp_engine *h, int32_t n, const uint32_t 
         }
     }
     h->pool_called = true;
-    if (!K) return EPP_OK;                                 // no label filter: nothing on the device reads labels
+    if (!K && !h->cl_mask) return EPP_OK;                  // no label filter or range: nothing on the device reads labels
     EPP_TRY(set_device(h));
     EPP_TRY(join_streams(h));
     cudaStream_t s = h->slot[0].stream;
-    CUDA_TRY(cudaMemcpyAsync(h->lcode.p, lc.data(), lc.size(), cudaMemcpyHostToDevice, s));
-    if (h->pool_ready) EPP_TRY(derive_pool(h));
+    for (int pi = 0; pi < kMaxProfiles; pi++)
+        if ((h->cl_mask >> pi) & 1)
+            CUDA_TRY(cudaMemcpyAsync(h->cl_rng[pi].p, rng[pi].data(), sizeof(longlong2) * E, cudaMemcpyHostToDevice, s));
+    if (K) {
+        CUDA_TRY(cudaMemcpyAsync(h->lcode.p, lc.data(), lc.size(), cudaMemcpyHostToDevice, s));
+        if (h->pool_ready) EPP_TRY(derive_pool(h));
+    }
     CUDA_TRY(cudaStreamSynchronize(s));
     return EPP_OK;
 }
@@ -1614,6 +1734,9 @@ static LatView lat_view(epp_engine *h, int64_t r0) {
     v.mask = h->lat_mask;
     v.r0 = r0;
     for (int i = 0; i < kMaxProfiles; i++) v.cfg[i] = h->lat_cfg[i];
+    for (int i = 0; i < kMaxProfiles; i++) v.rng[i] = (h->cl_mask >> i) & 1 ? h->cl_rng[i].as<longlong2>() : nullptr;
+    v.cl_filter = h->cl_filter;
+    if (h->cur_ctx) v.ctx = h->ctx_dev.as<int64_t>();
     if (h->cur_pred) {
         v.cnt = h->lat_cnt.as<uint32_t>();
         v.off = h->lat_off.as<uint64_t>();
@@ -2268,7 +2391,7 @@ extern "C" int32_t epp_latency_profile_set(epp_engine *h, int32_t profile, const
     const epp_profile_cfg &pc = profile_cfg(h, profile);
     EPP_TRY(validate_latency(pc, *cfg, profile == 0 ? "primary profile" : (profile == 1 ? "prefill profile" : "encode profile")));
     h->lat_cfg[profile] = *cfg;
-    if (latency_piece(pc, *cfg)) h->lat_mask |= 1 << profile;
+    if (chain_profile(pc, *cfg)) h->lat_mask |= 1 << profile;
     else h->lat_mask &= ~(1 << profile);
     if (h->lat_mask) h->general = true;
     return EPP_OK;
@@ -2296,6 +2419,37 @@ static int32_t check_predictions(const epp_engine *h, int64_t R, const epp_predi
         total += n;
     }
     *n_ent = total;
+    return EPP_OK;
+}
+
+// Validates a call's context lengths (R entries, each >= -1).  Nothing of the engine changes.
+static int32_t check_ctx(int64_t R, const epp_context_tokens *c) {
+    if (c->struct_size != sizeof(epp_context_tokens)) return fail(EPP_ERR_INVALID, "epp_context_tokens.struct_size %u != %zu", c->struct_size, sizeof(epp_context_tokens));
+    if (R > 0 && !c->tokens) return fail(EPP_ERR_INVALID, "epp_context_tokens.tokens is NULL");
+    for (int64_t r = 0; r < R; r++)
+        if (c->tokens[r] < -1) return fail(EPP_ERR_INVALID, "request %lld: context tokens %lld < -1", (long long)r, (long long)c->tokens[r]);
+    return EPP_OK;
+}
+
+// The token counts to the device on stream 0, behind everything enqueued so far, through the engine's pinned staging
+// (refilled only once the previous call's copy has run), as upload_predictions does.
+static int32_t upload_ctx(epp_engine *h, int64_t R, const epp_context_tokens *c) {
+    cudaStream_t s0 = h->slot[0].stream;
+    EPP_TRY(join_streams(h));
+    const size_t bytes = sizeof(int64_t) * (size_t)R;
+    CUDA_TRY(h->ctx_dev.reserve(bytes, &h->dev_bytes));
+    if (!h->ctx_up_ev) CUDA_TRY(cudaEventCreateWithFlags(&h->ctx_up_ev, cudaEventDisableTiming));
+    else CUDA_TRY(cudaEventSynchronize(h->ctx_up_ev));
+    if (bytes > h->ctx_host_cap) {
+        if (h->ctx_host) CUDA_TRY(cudaFreeHost(h->ctx_host));
+        h->ctx_host = nullptr;
+        h->ctx_host_cap = 0;
+        CUDA_TRY(cudaHostAlloc(reinterpret_cast<void **>(&h->ctx_host), bytes, cudaHostAllocDefault));
+        h->ctx_host_cap = bytes;
+    }
+    memcpy(h->ctx_host, c->tokens, bytes);
+    CUDA_TRY(cudaMemcpyAsync(h->ctx_dev.p, h->ctx_host, bytes, cudaMemcpyHostToDevice, s0));
+    CUDA_TRY(cudaEventRecord(h->ctx_up_ev, s0));
     return EPP_OK;
 }
 
@@ -2341,7 +2495,8 @@ static int32_t upload_predictions(epp_engine *h, int64_t R, const epp_prediction
 
 static int32_t schedule_impl(epp_engine *h, const epp_batch *batch, epp_decision *out, epp_decision_detail *detail,
                              int32_t keep_hashes, const epp_topk_out *topk, const epp_subset *subset = nullptr,
-                             const epp_predictions *preds = nullptr, bool subset_latency_ok = false) {
+                             const epp_predictions *preds = nullptr, bool subset_latency_ok = false,
+                             const epp_context_tokens *ctx = nullptr) {
     if (!h) return fail(EPP_ERR_INVALID, "NULL engine");
     if (!out) return fail(EPP_ERR_INVALID, "out is NULL");
     std::lock_guard<std::mutex> lk(h->mu);
@@ -2355,19 +2510,24 @@ static int32_t schedule_impl(epp_engine *h, const epp_batch *batch, epp_decision
     if (subset) EPP_TRY(check_subset(h, v.R, subset, sub_rows, &sub_n_slots, subset_latency_ok));
     uint64_t n_ent = 0;
     if (preds) EPP_TRY(check_predictions(h, v.R, preds, &n_ent));
-    if (!sub_rows.empty() || (preds && v.R)) {
+    if (ctx) EPP_TRY(check_ctx(v.R, ctx));
+    const bool use_ctx = ctx && v.R && h->cl_mask;
+    if (!sub_rows.empty() || (preds && v.R) || use_ctx) {
         if (!h->pool_ready) return fail(EPP_ERR_STATE, "epp_pool_set has not been called");
     }
     if (!sub_rows.empty()) EPP_TRY(upload_subset(h, sub_rows, subset, sub_n_slots));
     if (preds && v.R) EPP_TRY(upload_predictions(h, v.R, preds, n_ent));
+    if (use_ctx) EPP_TRY(upload_ctx(h, v.R, ctx));
     h->kept_R = 0;
     h->cur_topk = topk;
     h->cur_sub = sub_rows.empty() ? nullptr : &sub_rows;
     h->cur_pred = preds && v.R;
+    h->cur_ctx = use_ctx;
     const int32_t rc = run_batch(h, v, Mode::Schedule, nullptr, nullptr, out, detail, nullptr, nullptr, keep_hashes != 0);
     h->cur_topk = nullptr;
     h->cur_sub = nullptr;
     h->cur_pred = false;
+    h->cur_ctx = false;
     EPP_TRY(rc);
     h->stats.n_batches++;
     h->stats.n_decisions += (uint64_t)v.R;
@@ -2410,6 +2570,12 @@ extern "C" int32_t epp_schedule_subset_predicted(epp_engine *h, const epp_batch 
                                                  const epp_predictions *preds, epp_decision *out, epp_decision_detail *detail,
                                                  int32_t keep_hashes, const epp_topk_out *topk) {
     return schedule_impl(h, batch, out, detail, keep_hashes, topk, subset, preds, true);
+}
+
+extern "C" int32_t epp_schedule_ctx(epp_engine *h, const epp_batch *batch, const epp_subset *subset, const epp_predictions *preds,
+                                    const epp_context_tokens *ctx, epp_decision *out, epp_decision_detail *detail,
+                                    int32_t keep_hashes, const epp_topk_out *topk) {
+    return schedule_impl(h, batch, out, detail, keep_hashes, topk, subset, preds, true, ctx);
 }
 
 // PreRequest: approximateprefix/plugin.go:164-200 (primary target + "prefill" profile target).
@@ -2470,8 +2636,10 @@ extern "C" int32_t epp_score(epp_engine *h, int64_t n_requests, const int32_t *m
     if (!h->pool_ready) return fail(EPP_ERR_STATE, "epp_pool_set has not been called");
     if (profile < 0 || profile >= h->n_alloc_profiles) return fail(EPP_ERR_INVALID, "profile %d out of range", profile);
     if (scorer_index < -1 || scorer_index >= profile_cfg(h, profile).n_scorers) return fail(EPP_ERR_INVALID, "scorer_index %d out of range", scorer_index);
-    if (((h->lat_mask >> profile) & 1) && (scorer_index < 0 || profile_cfg(h, profile).scorers[scorer_index].kind == EPP_SCORER_LATENCY))
-        return fail(EPP_ERR_INVALID, "epp_score does not evaluate latency pieces (the weighted sum of a latency profile, the latency scorer)");
+    if (((h->lat_mask >> profile) & 1) &&
+        (scorer_index < 0 || profile_cfg(h, profile).scorers[scorer_index].kind == EPP_SCORER_LATENCY ||
+         profile_cfg(h, profile).scorers[scorer_index].kind == EPP_SCORER_CONTEXT_LENGTH))
+        return fail(EPP_ERR_INVALID, "epp_score does not evaluate chain pieces (the weighted sum of a latency or context-length profile, the latency and context-length scorers)");
     if (n_requests == 0) return EPP_OK;
     const size_t E = (size_t)h->cfg.max_endpoints, n = (size_t)n_requests * E;
     cudaStream_t s = h->slot[0].stream;
@@ -2505,21 +2673,24 @@ extern "C" int32_t epp_score(epp_engine *h, int64_t n_requests, const int32_t *m
 static int32_t with_match_impl(epp_engine *h, int64_t n_requests, const int32_t *match, const int32_t *total,
                                const uint32_t *model_ids, const int64_t *input_len_bytes, int32_t block_size_tokens, epp_decision *out,
                                epp_decision_detail *detail, uint32_t flags, const epp_topk_out *topk,
-                               const epp_predictions *preds = nullptr) {
+                               const epp_predictions *preds = nullptr, const epp_context_tokens *ctx = nullptr) {
     if (!h || n_requests < 0 || (n_requests && (!match || !total || !out))) return fail(EPP_ERR_INVALID, "bad arguments");
     std::lock_guard<std::mutex> lk(h->mu);
     if (topk) EPP_TRY(check_topk(h, topk));
     uint64_t n_ent = 0;
     if (preds) EPP_TRY(check_predictions(h, n_requests, preds, &n_ent));
+    if (ctx) EPP_TRY(check_ctx(n_requests, ctx));
     EPP_TRY(set_device(h));
     EPP_TRY(join_streams(h));
     if (!h->pool_ready) return fail(EPP_ERR_STATE, "epp_pool_set has not been called");
     if (n_requests == 0) return EPP_OK;
     if (preds) EPP_TRY(upload_predictions(h, n_requests, preds, n_ent));
+    if (ctx && h->cl_mask) EPP_TRY(upload_ctx(h, n_requests, ctx));
     h->cur_pred = preds != nullptr;
-    struct PredReset {                             // the call's predictions end with it, whichever way it returns
+    h->cur_ctx = ctx && h->cl_mask;
+    struct PredReset {                             // the call's predictions and token counts end with it, whichever way it returns
         epp_engine *h;
-        ~PredReset() { h->cur_pred = false; }
+        ~PredReset() { h->cur_pred = false; h->cur_ctx = false; }
     } pred_reset{h};
     const size_t R = (size_t)n_requests;
     cudaStream_t s = h->slot[0].stream;
@@ -2583,6 +2754,15 @@ extern "C" int32_t epp_schedule_with_match_predicted(epp_engine *h, int64_t n_re
                                                      int32_t block_size_tokens, epp_decision *out, epp_decision_detail *detail,
                                                      uint32_t flags, const epp_topk_out *topk, const epp_predictions *preds) {
     return with_match_impl(h, n_requests, match, total, model_ids, input_len_bytes, block_size_tokens, out, detail, flags, topk, preds);
+}
+
+extern "C" int32_t epp_schedule_with_match_ctx(epp_engine *h, int64_t n_requests, const int32_t *match, const int32_t *total,
+                                               const uint32_t *model_ids, const int64_t *input_len_bytes,
+                                               int32_t block_size_tokens, epp_decision *out, epp_decision_detail *detail,
+                                               uint32_t flags, const epp_topk_out *topk, const epp_predictions *preds,
+                                               const epp_context_tokens *ctx) {
+    return with_match_impl(h, n_requests, match, total, model_ids, input_len_bytes, block_size_tokens, out, detail, flags, topk,
+                           preds, ctx);
 }
 
 extern "C" int32_t epp_schedule_with_match_topk(epp_engine *h, int64_t n_requests, const int32_t *match, const int32_t *total,

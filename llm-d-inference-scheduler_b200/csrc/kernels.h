@@ -348,9 +348,16 @@ struct LatView {
     const uint64_t *off;
     const epp_prediction *ent;
     int64_t r0;                // row of this launch's request 0
-    int32_t mask;              // profiles with a latency piece
+    int32_t mask;              // chain profiles: a latency piece or the context-length scorer
     epp_latency_cfg cfg[kMaxProfiles];
+    // context length ("Context length"): the call's per-row token counts ([batch R] absolute rows, -1 = the default from
+    // the prompt length; nullptr: all default), and per profile listing the scorer its slots' ranges ([E]: x = min, y = max
+    // when x >= 0; x = kRangeAbsent / kRangeInvalid otherwise) and whether it filters
+    const int64_t *ctx;
+    const longlong2 *rng[kMaxProfiles];
+    int32_t cl_filter;         // bit pi: profile pi's context-length filter is on
 };
+constexpr long long kRangeAbsent = -1, kRangeInvalid = -2;
 cudaError_t launch_match_pick_lat(const PickParams &p, const LatView &lv, uint32_t *gscratch, int grid, size_t smem,
                                   cudaStream_t s, int *launches);
 cudaError_t launch_dense_pick_lat(const DensePickParams &p, const LatView &lv, cudaStream_t s, int *launches);

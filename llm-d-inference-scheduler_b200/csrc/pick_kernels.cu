@@ -354,7 +354,7 @@ __device__ inline Best gen_eval_profile(const P &p, const ProfileDev &pf, int pi
                      (k > 1 && pi == 0 && p.gen.topk_scores) ? p.gen.topk_scores + r * k : nullptr);
 }
 
-// lat::eval for latency profile pi of request r (the row handling of gen_eval_profile).
+// lat::eval for chain profile pi of request r (the row handling of gen_eval_profile).
 template <bool kRand, typename P, typename CntOf>
 __device__ inline Best lat_eval_profile(const P &p, const LatView &lv, int pi, int64_t r, int32_t total, int lane,
                                         uint32_t adapter, uint64_t key, CntOf cnt_of) {
@@ -367,7 +367,8 @@ __device__ inline Best lat_eval_profile(const P &p, const LatView &lv, int pi, i
     lat::Req q;
     q.n = lv.cnt ? lv.cnt[lv.r0 + r] : 0u;
     q.ent = q.n ? lv.ent + lv.off[lv.r0 + r] : nullptr;
-    return lat::eval<kRand>(p.prof[pi], lv.cfg[pi], p.gen, q, p.E, total, lane, p.lora, adapter, p.tie_seed, key,
+    const lat::CtxLen cl = lat::ctx_len(lv, pi, lv.r0 + r, p.in_len ? p.in_len[r] : 0);
+    return lat::eval<kRand>(p.prof[pi], lv.cfg[pi], cl, p.gen, q, p.E, total, lane, p.lora, adapter, p.tie_seed, key,
                             lat::pool_dom(p.E, cnt_of), k,
                             (k > 1 && p.gen.topk_picks[pi]) ? p.gen.topk_picks[pi] + r * k : nullptr,
                             (k > 1 && pi == 0 && p.gen.topk_scores) ? p.gen.topk_scores + r * k : nullptr);

@@ -1,7 +1,8 @@
-// pick_latency.cuh -- the general evaluation of one SchedulerProfile with a latency piece for one request (one warp), as
-// defined in include/epp_engine.h ("Latency predictions"):
-//   [role + label filters] -> [affinity A1] -> [slo-headroom-tier-filter T] -> [affinity A2] -> scorers -> picker,
-// with the latency-scorer (scorer/latency/plugin.go:144-395) among the scorers.  The request-level state (the A1 / T / A2
+// pick_latency.cuh -- the general evaluation of one chain SchedulerProfile (a latency piece, the context-length-aware
+// plugin or both) for one request (one warp), as defined in include/epp_engine.h ("Latency predictions", "Context length"):
+//   [role + label + context-length filters] -> [affinity A1] -> [slo-headroom-tier-filter T] -> [affinity A2] -> scorers
+//   -> picker,
+// with the latency-scorer (scorer/latency/plugin.go:144-395) and the context-length scorer among the scorers.  The request-level state (the A1 / T / A2
 // decisions, the scored bucket, its per-dimension min / max, alpha and beta) is computed once per stage by warp
 // reductions; after that a slot's membership and score are per-slot predicates over its entry, which each lane finds by
 // binary search in the request's ascending entry list.
@@ -35,6 +36,48 @@ __device__ __forceinline__ uint32_t warp_sum(uint32_t v) {
     return v;
 }
 
+// The context-length-aware plugin of one profile for one request (context_length_aware.go): the first-stage filter
+// predicate and the score of slot e, from e's range (kernels.h LatView::rng) and the request's ctx.
+struct CtxLen {
+    const longlong2 *rng;          // nullptr: the profile does not list the plugin
+    long long ctx;
+    bool filter;
+    __device__ __forceinline__ bool keep(uint32_t e) const {
+        if (!filter) return true;
+        const longlong2 r = rng[e];
+        if (r.x < 0) return r.x == kRangeAbsent;                                      // no label keeps, invalid drops
+        return ctx >= r.x && ctx <= r.y;
+    }
+    // calculateRangeScore; differences wrap like Go's int arithmetic
+    __device__ __forceinline__ double score(uint32_t e) const {
+        const longlong2 r = rng[e];
+        if (r.x == kRangeAbsent) return 0.5;
+        if (r.x < 0) return 0.0;
+        if (ctx >= r.x && ctx <= r.y) {
+            const long long w = r.y - r.x;
+            if (w == 0) return 1.0;
+            const double ws = __ddiv_rn(1.0, __dadd_rn(1.0, __ddiv_rn((double)w, 10000.0)));
+            const double pos = __ddiv_rn((double)(r.y - ctx), (double)w);
+            const double raw = __dadd_rn(__dmul_rn(0.7, ws), __dmul_rn(0.3, pos));
+            return __dadd_rn(0.3, __dmul_rn(raw, 0.7));
+        }
+        const long long d = (long long)(ctx > r.y ? (unsigned long long)ctx - (unsigned long long)r.y
+                                                  : (unsigned long long)r.x - (unsigned long long)ctx);
+        return __ddiv_rn(0.3, __dadd_rn(1.0, __ddiv_rn((double)d, 1000.0)));
+    }
+};
+
+// Profile pi's plugin for absolute row `row` of the call, whose true prompt length is L: ctx is the caller's count, or
+// int(float64(L) * 0.25).
+__device__ __forceinline__ CtxLen ctx_len(const LatView &lv, int pi, int64_t row, int64_t L) {
+    CtxLen c;
+    c.rng = lv.rng[pi];
+    c.filter = c.rng && ((lv.cl_filter >> pi) & 1);
+    const long long t = (c.rng && lv.ctx) ? lv.ctx[row] : -1;
+    c.ctx = t >= 0 ? t : go_int(__dmul_rn((double)L, 0.25));
+    return c;
+}
+
 // The request's entries, ascending slot.
 struct Req {
     const epp_prediction *ent;
@@ -50,14 +93,20 @@ struct Req {
 };
 
 // The index domain of an evaluation: members i of [0, n), member i is slot at(i) with matchBlocks cnt(i);
-// n_cand(pf) is the number of members that are candidates of profile pf (role and label filters).
+// n_cand(pf, lane, cl) is the number of members that pass the first stage of profile pf (role, label and context-length
+// filters); with the context-length filter on it depends on the request.
 template <typename CntOf>
 struct PoolDom {                   // i -> i over the whole pool
     uint32_t n;
     CntOf cnt_of;
     __device__ __forceinline__ uint32_t at(uint32_t i) const { return i; }
     __device__ __forceinline__ int32_t cnt(uint32_t i) const { return cnt_of(i); }
-    __device__ __forceinline__ uint32_t n_cand(const ProfileDev &pf, int) const { return (uint32_t)*pf.n_cand; }
+    __device__ __forceinline__ uint32_t n_cand(const ProfileDev &pf, int lane, const CtxLen &cl) const {
+        if (!cl.filter) return (uint32_t)*pf.n_cand;
+        uint32_t c = 0;
+        for (uint32_t i = lane; i < n; i += 32) c += pf.cand[i] && cl.keep(i);
+        return warp_sum(c);
+    }
 };
 template <typename CntOf>
 __device__ __forceinline__ PoolDom<CntOf> pool_dom(int32_t E, CntOf cnt_of) { return PoolDom<CntOf>{(uint32_t)E, cnt_of}; }
@@ -68,9 +117,10 @@ struct ListDom {                   // i -> sl[i] over a restricted request's asc
     uint32_t n;
     __device__ __forceinline__ uint32_t at(uint32_t i) const { return sl[i]; }
     __device__ __forceinline__ int32_t cnt(uint32_t i) const { return hit[i]; }
-    __device__ __forceinline__ uint32_t n_cand(const ProfileDev &pf, int lane) const {
+    __device__ __forceinline__ uint32_t n_cand(const ProfileDev &pf, int lane, const CtxLen &cl) const {
         uint32_t c = 0;
-        for (uint32_t i0 = 0; i0 < n; i0 += 32) c += __popc(__ballot_sync(gen::kFull, i0 + lane < n && pf.cand[sl[i0 + lane]]));
+        for (uint32_t i0 = 0; i0 < n; i0 += 32)
+            c += __popc(__ballot_sync(gen::kFull, i0 + lane < n && pf.cand[sl[i0 + lane]] && cl.keep(sl[i0 + lane])));
         return c;
     }
 };
@@ -155,8 +205,8 @@ __device__ __forceinline__ double score_raw(const State &st, const PoolArrays &p
     return __ddiv_rn((double)(go_int(__dmul_rn(x, 100.0)) + 1), 100.0);
 }
 
-// runScorerPlugins over the final set (weighted_sum_over with the latency scorer).
-__device__ inline double weighted_sum(const ProfileDev &pf, const GenView &g, const State &st, uint32_t e,
+// runScorerPlugins over the final set (weighted_sum_over with the latency and context-length scorers).
+__device__ inline double weighted_sum(const ProfileDev &pf, const GenView &g, const State &st, const CtxLen &cl, uint32_t e,
                                       const epp_prediction *p, int32_t match, int32_t total, const LoraDev &L, int lora_st) {
     double acc = 0.0;
 #pragma unroll 1
@@ -166,6 +216,7 @@ __device__ inline double weighted_sum(const ProfileDev &pf, const GenView &g, co
         if (sc.kind == EPP_SCORER_PREFIX) raw = prefix_score(match, total);
         else if (sc.kind == EPP_SCORER_LORA_AFFINITY) raw = lora_score(L, e, lora_st);
         else if (sc.kind == EPP_SCORER_LATENCY) raw = score_raw(st, g.pool, e, p, match, total);
+        else if (sc.kind == EPP_SCORER_CONTEXT_LENGTH) raw = cl.score(e);
         else raw = pool_score(sc, s, g.pool, st.nm.q, (int32_t)e);
         acc = __dadd_rn(acc, __dmul_rn(clamp01(raw), sc.weight));
     }
@@ -175,12 +226,13 @@ __device__ inline double weighted_sum(const ProfileDev &pf, const GenView &g, co
 // The request-level state of the chain and the scorer over the members of ix (E: the pool's, the stride of its
 // columns).  Returns the final set's size.
 template <typename Dom>
-__device__ inline uint32_t prepare(const ProfileDev &pf, const epp_latency_cfg &lc, const GenView &g, const Req &q,
-                                   int32_t E, int32_t total, int lane, uint64_t seed, uint64_t key, const Dom &ix, State &st) {
+__device__ inline uint32_t prepare(const ProfileDev &pf, const epp_latency_cfg &lc, const CtxLen &cl, const GenView &g,
+                                   const Req &q, int32_t E, int32_t total, int lane, uint64_t seed, uint64_t key, const Dom &ix,
+                                   State &st) {
     const epp_profile_cfg &c = pf.cfg;
     st.a1 = st.a2 = false;
     st.tier = kTierAll;
-    auto in1 = [&](uint32_t i) { return pf.cand[ix.at(i)] && (!st.a1 || gen::is_sticky(ix.cnt(i), total, lc.a1_affinity_threshold)); };
+    auto in1 = [&](uint32_t i) { return pf.cand[ix.at(i)] && cl.keep(ix.at(i)) && (!st.a1 || gen::is_sticky(ix.cnt(i), total, lc.a1_affinity_threshold)); };
     auto in2 = [&](uint32_t i) {
         if (!in1(i)) return false;
         if (st.tier == kTierAll) return true;
@@ -191,7 +243,7 @@ __device__ inline uint32_t prepare(const ProfileDev &pf, const epp_latency_cfg &
     // A1 over the filtered candidates
     if (lc.tier_filter)
         st.a1 = affinity(lc.a1_affinity_threshold, lc.a1_exploration_probability, lc.a1_max_ttft_penalty_ms, kA1Domain,
-                         ix.n_cand(pf, lane), q, total, lane, seed, key, in1, ix);
+                         ix.n_cand(pf, lane, cl), q, total, lane, seed, key, in1, ix);
     // T over A1's set (sloheadroomtier/plugin.go:84-138)
     uint32_t n1 = 0, npos = 0, nneg = 0;
     for (uint32_t i = lane; i < ix.n; i += 32) {
@@ -298,22 +350,22 @@ __device__ inline uint32_t prepare(const ProfileDev &pf, const epp_latency_cfg &
 // contract of gen::eval, over the final set), all over the members of ix: the candidates are its members that pass
 // pf's filters, and every set size, range and draw population is taken over them.  Picks are slots.
 template <bool kRand, typename Dom>
-__device__ inline Best eval(const ProfileDev &pf, const epp_latency_cfg &lc, const GenView &g, const Req &q, int32_t E,
-                            int32_t total, int lane, const LoraDev &lora, uint32_t adapter, uint64_t seed, uint64_t key,
-                            const Dom &ix, int32_t k, uint32_t *picks_row, double *scores_row) {
+__device__ inline Best eval(const ProfileDev &pf, const epp_latency_cfg &lc, const CtxLen &cl, const GenView &g, const Req &q,
+                            int32_t E, int32_t total, int lane, const LoraDev &lora, uint32_t adapter, uint64_t seed,
+                            uint64_t key, const Dom &ix, int32_t k, uint32_t *picks_row, double *scores_row) {
     Best first;
     best_init(first);
     if (k < 1) k = 1;
     if (picks_row) for (int j = lane; j < k; j += 32) picks_row[j] = EPP_NO_ENDPOINT;
     if (scores_row) for (int j = lane; j < k; j += 32) scores_row[j] = 0.0;
     __syncwarp();
-    if (ix.n_cand(pf, lane) == 0) return first;
+    if (ix.n_cand(pf, lane, cl) == 0) return first;
     State st;
-    const uint32_t n = prepare(pf, lc, g, q, E, total, lane, seed, key, ix, st);
+    const uint32_t n = prepare(pf, lc, cl, g, q, E, total, lane, seed, key, ix, st);
     const bool use_lora = lora.enabled && lora.ptr;
     auto cand = [&](uint32_t i) {
         const uint32_t e = ix.at(i);
-        if (!pf.cand[e]) return false;
+        if (!pf.cand[e] || !cl.keep(e)) return false;
         if (st.a1 && !gen::is_sticky(ix.cnt(i), total, lc.a1_affinity_threshold)) return false;
         if (st.tier != kTierAll) {
             const epp_prediction *p = q.find(e);
@@ -324,7 +376,7 @@ __device__ inline Best eval(const ProfileDev &pf, const epp_latency_cfg &lc, con
     auto score = [&](uint32_t i) {
         const uint32_t e = ix.at(i);
         const int ls = use_lora ? lora_lookup(lora, adapter, e) : 0;
-        return weighted_sum(pf, g, st, e, q.find(e), ix.cnt(i), total, lora, ls);
+        return weighted_sum(pf, g, st, cl, e, q.find(e), ix.cnt(i), total, lora, ls);
     };
     if (kRand && pf.cfg.picker) {     // random pickers: every member is an explicit item
         uint32_t g0 = EPP_NO_ENDPOINT, g1 = EPP_NO_ENDPOINT;

@@ -369,7 +369,8 @@ __device__ __forceinline__ void subset_pick(const PickParams &p, const SubsetVie
                 lat::Req lq;
                 lq.n = lv->cnt ? lv->cnt[row.row] : 0u;
                 lq.ent = lq.n ? lv->ent + lv->off[row.row] : nullptr;
-                return lat::eval<true>(p.prof[pi], lv->cfg[pi], p.gen, lq, p.E, total, lane, p.lora, q.adapter, p.tie_seed, key,
+                const lat::CtxLen cl = lat::ctx_len(*lv, pi, row.row, p.in_len[r]);
+                return lat::eval<true>(p.prof[pi], lv->cfg[pi], cl, p.gen, lq, p.E, total, lane, p.lora, q.adapter, p.tie_seed, key,
                                        lat::ListDom{q.sl, q.hit, q.n}, k,
                                        (k > 1 && p.gen.topk_picks[pi]) ? p.gen.topk_picks[pi] + r * k : nullptr,
                                        (k > 1 && pi == 0 && p.gen.topk_scores) ? p.gen.topk_scores + r * k : nullptr);

@@ -56,6 +56,8 @@ class ProfileSpec:
     picker: int = capi.PICKER_MAX_SCORE
     labels: list = field(default_factory=list)
     latency: dict | None = None      # Engine.latency_profile_set fields of a profile with a latency piece, or None
+    context_length: dict | None = None   # Engine.context_length_set fields (label, enable_filtering) of a profile listing
+                                         # the context-length scorer, or None (the defaults)
 
 
 def _fill_profile(dst: capi.ProfileCfg, spec: ProfileSpec):
@@ -156,6 +158,30 @@ def pack_predictions(predictions):
     return counts, offsets, np.ascontiguousarray(entries)
 
 
+def _context_struct(context_tokens, R):
+    """epp_context_tokens over R int64 entries -> (struct, the array it points to: keep it alive through the call)."""
+    arr = np.ascontiguousarray(np.asarray(context_tokens, dtype=np.int64).reshape(-1))
+    if arr.shape[0] != R:
+        raise ValueError(f"context_tokens has {arr.shape[0]} entries for {R} requests")
+    ct = capi.ContextTokens()
+    ct.struct_size = C.sizeof(capi.ContextTokens)
+    ct.tokens = arr.ctypes.data if R else None
+    return ct, arr
+
+
+def _prediction_entries(predictions):
+    """One request's predictions (a PREDICTION_DTYPE array, or (slot, ttft, ttft_headroom, tpot_headroom, dispatched)
+    tuples) as a contiguous PREDICTION_DTYPE array."""
+    if isinstance(predictions, np.ndarray) and predictions.dtype == PREDICTION_DTYPE:
+        return np.ascontiguousarray(predictions)
+    ent = np.zeros(len(predictions), dtype=PREDICTION_DTYPE)
+    for i, (sl, tt, th, tp, d) in enumerate(predictions):
+        if not 0 <= int(sl) <= 0xFFFFFFFE:
+            raise ValueError(f"slot id {sl} out of range")
+        ent[i] = (int(sl), int(d), float(tt), float(th), float(tp))
+    return ent
+
+
 def _predictions_struct(packed):
     p = capi.Predictions()
     p.struct_size = C.sizeof(capi.Predictions)
@@ -203,6 +229,8 @@ class Engine:
                 self.label_filters_set(p, spec.labels)
             if spec is not None and spec.latency is not None:
                 self.latency_profile_set(p, **spec.latency)
+            if spec is not None and spec.context_length is not None:
+                self.context_length_set(p, **spec.context_length)
 
     # ---- plumbing ----
     def _check(self, rc: int):
@@ -447,9 +475,15 @@ class Engine:
             setattr(cfg, k, v)
         self._check(self._lib.epp_latency_profile_set(self._h, profile, C.byref(cfg)))
 
+    def context_length_set(self, profile: int, label: str | None = None, enable_filtering: bool = False):
+        """The context-length-aware plugin of profile 0 (primary / decode), 1 (prefill) or 2 (encode): its range label key
+        (None = capi.CONTEXT_LENGTH_LABEL) and whether it also filters (include/epp_engine.h "Context length")."""
+        self._check(self._lib.epp_context_length_set(self._h, profile, None if label is None else label.encode(),
+                                                     int(enable_filtering)))
+
     def schedule(self, data, offsets=None, uniform_len=None, model_ids=None, n_requests=None, keep_hashes=False,
                  detail=True, out=None, lengths=None, asynchronous=False, multimodal=None, topk=False, subsets=None,
-                 predictions=None):
+                 predictions=None, context_tokens=None):
         """a1-a14 Scheduler.Schedule for a batch -> (decisions, details).  asynchronous=True (CUDA tensors only)
         enqueues the batch and returns; the outputs are complete after synchronize().  topk=True (engines created with
         pick_k > 1) also returns the dict of the pickers' first-k lists (maxscore/picker.go:104-115): "primary",
@@ -458,7 +492,9 @@ class Engine:
         candidates (the gateway's endpoint subset, include/epp_engine.h "Endpoint subsets"); epp_schedule_subset.
         predictions: None, or a list of R entries in the form pack_predictions takes (include/epp_engine.h "Latency
         predictions"); epp_schedule_predicted.  Both together: epp_schedule_subset_predicted (a latency engine's
-        restricted requests decided with their predictions)."""
+        restricted requests decided with their predictions).
+        context_tokens: None, or R request context lengths (-1 = the default from the prompt length, include/epp_engine.h
+        "Context length"); with it every call goes through epp_schedule_ctx."""
         b, R, dev, keep = self._batch(data, offsets, uniform_len, model_ids, n_requests, lengths, multimodal)
         if asynchronous:
             b.flags |= capi.EPP_BATCH_ASYNC
@@ -482,7 +518,12 @@ class Engine:
             sub = capi.Subset()
             sub.struct_size = C.sizeof(capi.Subset)
             sub.counts, sub.offsets, sub.slots = (_ptr(a) for a in spacked)
-        if predictions is not None and subsets is not None:
+        if context_tokens is not None:
+            ct, ctx_arr = _context_struct(context_tokens, R)
+            self._check(self._lib.epp_schedule_ctx(self._h, C.byref(b), C.byref(sub) if subsets is not None else None,
+                                                   C.byref(pr) if predictions is not None else None, C.byref(ct), _ptr(dec),
+                                                   _ptr(det), int(keep_hashes), C.byref(tk) if topk else None))
+        elif predictions is not None and subsets is not None:
             self._check(self._lib.epp_schedule_subset_predicted(self._h, C.byref(b), C.byref(sub), C.byref(pr), _ptr(dec),
                                                                 _ptr(det), int(keep_hashes), C.byref(tk) if topk else None))
         elif predictions is not None:
@@ -516,7 +557,7 @@ class Engine:
         return lists, tk
 
     def schedule_with_match(self, match, total, input_len_bytes=None, block_size_tokens: int = 0, model_ids=None,
-                            topk=False, predictions=None):
+                            topk=False, predictions=None, context_tokens=None):
         match = np.ascontiguousarray(match, dtype=np.int32).reshape(-1, self.E)
         total = np.ascontiguousarray(total, dtype=np.int32)
         R = match.shape[0]
@@ -524,6 +565,17 @@ class Engine:
         dec = np.zeros(R, dtype=DECISION_DTYPE)
         det = np.zeros(R, dtype=DETAIL_DTYPE)
         mids = None if model_ids is None else np.ascontiguousarray(model_ids, dtype=np.uint32)
+        if context_tokens is not None:
+            ct, ctx_arr = _context_struct(context_tokens, R)
+            if predictions is not None and len(predictions) != R:
+                raise ValueError(f"predictions has {len(predictions)} entries for {R} requests")
+            packed = pack_predictions(predictions) if predictions is not None else None
+            pr = _predictions_struct(packed) if packed is not None else None
+            lists, tk = self._topk_out(R) if topk else (None, None)
+            self._check(self._lib.epp_schedule_with_match_ctx(
+                self._h, R, _ptr(match), _ptr(total), _ptr(mids), _ptr(il), block_size_tokens, _ptr(dec), _ptr(det), 0,
+                C.byref(tk) if topk else None, C.byref(pr) if pr is not None else None, C.byref(ct)))
+            return (dec, det, lists) if topk else (dec, det)
         if predictions is not None:
             if len(predictions) != R:
                 raise ValueError(f"predictions has {len(predictions)} entries for {R} requests")
@@ -635,14 +687,25 @@ class Batcher:
         if rc != 0:
             raise EngineError(rc, (self._lib.epp_batcher_last_error() or b"").decode())
 
-    def submit(self, prompt, model_id: int = 0, multimodal: bool = False, subset=None, predictions=None) -> int:
+    def submit(self, prompt, model_id: int = 0, multimodal: bool = False, subset=None, predictions=None,
+               context_tokens=None) -> int:
         """subset: None (the whole pool) or a sequence of slot ids, the request's candidates (epp_submit_subset).
         predictions: None or the request's entries in the form pack_predictions takes (epp_submit_predicted).  Both
-        together: epp_submit_subset_predicted."""
+        together: epp_submit_subset_predicted.  context_tokens: None, or the request's context length (-1 = the default);
+        with it the request goes through epp_submit_ctx with whatever else it carries."""
         buf = np.ascontiguousarray(prompt).view(np.uint8).reshape(-1) if not isinstance(prompt, (bytes, bytearray)) else prompt
         n = len(buf)
         ptr = buf.ctypes.data_as(C.c_void_p) if isinstance(buf, np.ndarray) else C.cast(C.c_char_p(bytes(buf)), C.c_void_p)
         t = C.c_uint64()
+        if context_tokens is not None:
+            ent = _prediction_entries(predictions) if predictions is not None else np.zeros(0, dtype=PREDICTION_DTYPE)
+            sl = None if subset is None else np.ascontiguousarray(np.asarray(subset, dtype=np.uint32).reshape(-1))
+            if sl is not None and sl.shape[0] == 0:
+                sl = np.zeros(1, dtype=np.uint32)[:0]
+            self._check(self._lib.epp_submit_ctx(self._b, model_id, ptr, n, int(multimodal), 0 if sl is None else sl.shape[0],
+                                                 None if sl is None else sl.ctypes.data_as(C.c_void_p), ent.shape[0],
+                                                 _ptr(ent), int(context_tokens), C.byref(t)))
+            return t.value
         if predictions is not None:
             if isinstance(predictions, np.ndarray) and predictions.dtype == PREDICTION_DTYPE:
                 ent = np.ascontiguousarray(predictions)

@@ -15,6 +15,7 @@ Reference interfaces mirrored (paths relative to the reference root):
   LatencyPredictionInfo (LatencyPredictionInfoKey)        .../datalayer/attribute/latency/data_types.go:23-96
   slo-headroom-tier-filter                                .../filter/sloheadroomtier/plugin.go:43-73
   latency-scorer                                          .../scorer/latency/plugin.go:59-125
+  context-length-aware (scorer and filter)                .../scorer/contextlengthaware/context_length_aware.go
 """
 from __future__ import annotations
 
@@ -457,6 +458,54 @@ def _latency_fields(tier, a1, scorer) -> dict:
     return f
 
 
+ContextLengthAwareType = "context-length-aware"
+DefaultContextLengthLabel = capi.CONTEXT_LENGTH_LABEL
+
+
+@dataclass
+class _ContextLengthAware(_Scorer):             # both a scorer and a filter (include/epp_engine.h "Context length")
+    label: str = DefaultContextLengthLabel
+    enableFiltering: bool = False
+
+
+def NewContextLengthAware(name: str, label: str = DefaultContextLengthLabel, enableFiltering: bool = False):
+    return _ContextLengthAware(capi.SCORER_CONTEXT_LENGTH, 0.0, name, label=label, enableFiltering=enableFiltering)
+
+
+def ContextLengthAwareFactory(name: str, rawParameters=None):
+    """ "context-length-aware" Factory: rawParameters is JSON text, bytes, a dict or None; json.Unmarshal into
+    {label string, enableFiltering bool} over the defaults, then an empty label is an error."""
+    raw = rawParameters
+    try:
+        if isinstance(raw, (str, bytes, bytearray)):
+            raw = json.loads(raw)
+        fields = {"label": str, "enablefiltering": bool}
+        params = {"label": DefaultContextLengthLabel, "enablefiltering": False}
+        if raw is not None:
+            if not isinstance(raw, dict):
+                raise ValueError(f"json: cannot unmarshal {type(raw).__name__} into Go value of type "
+                                 f"contextlengthaware.contextLengthAwareParameters")
+            for k, v in raw.items():
+                want = fields.get(k.lower())
+                if want is None or v is None:
+                    continue
+                if not isinstance(v, want):
+                    raise ValueError(f"json: cannot unmarshal {type(v).__name__} into Go struct field "
+                                     f"contextLengthAwareParameters.{k} of type {'string' if want is str else 'bool'}")
+                params[k.lower()] = v
+    except (ValueError, json.JSONDecodeError) as e:
+        raise ValueError(f"failed to parse the parameters of the '{ContextLengthAwareType}' plugin - {e}") from e
+    if params["label"] == "":
+        raise ValueError(f"invalid configuration for '{ContextLengthAwareType}' plugin: 'label' must be specified")
+    return NewContextLengthAware(name, params["label"], params["enablefiltering"])
+
+
+def _context_length_of(plugin):
+    """The context-length instance of a filter-list entry or WeightedScorer, or None."""
+    inner = plugin.scorer if isinstance(plugin, WeightedScorer) else plugin
+    return inner if isinstance(inner, _ContextLengthAware) else None
+
+
 @dataclass
 class PrefixCacheAffinityFilter:                 # filter/prefixcacheaffinity "prefix-cache-affinity-filter"; DefaultConfig :62-66
     affinityThreshold: float = 0.80
@@ -509,6 +558,7 @@ class SchedulerProfile:
         self.picker = MaxScorePicker()
 
     def WithFilters(self, *filters):
+        filters = [_context_length_of(f) or f for f in filters]
         _check_chain(filters)
         self.filters = list(filters)
         return self
@@ -519,7 +569,13 @@ class SchedulerProfile:
 
     def AddPlugins(self, *plugins):
         for p in plugins:
-            if isinstance(p, WeightedScorer):
+            if isinstance(p, _ContextLengthAware):
+                raise ValueError(f"plugin '{p.type_name}' is a scorer: it must be registered with a weight")
+            if isinstance(p, WeightedScorer) and isinstance(p.scorer, _ContextLengthAware):
+                _check_chain(self.filters + [p.scorer])              # scheduler_profile.go:76-95: also a filter, here
+                self.filters.append(p.scorer)
+                self.scorers.append(p)
+            elif isinstance(p, WeightedScorer):
                 self.scorers.append(p)
             elif isinstance(p, (_RoleFilter, _LabelFilter, PrefixCacheAffinityFilter, SLOHeadroomTierFilter)):
                 _check_chain(self.filters + [p])
@@ -544,19 +600,31 @@ class SchedulerProfile:
         lat_scorers = [ws.scorer for ws in self.scorers if isinstance(ws.scorer, _LatencyScorer)]
         assert len(lat_scorers) <= 1, "at most one latency-scorer per profile"
         tier = self.filters[tier_at[0]] if tier_at else None
+        cls = {id(f): f for f in self.filters if isinstance(f, _ContextLengthAware)}
+        cls.update({id(ws.scorer): ws.scorer for ws in self.scorers if isinstance(ws.scorer, _ContextLengthAware)})
+        assert len(cls) <= 1, "at most one context-length-aware instance per profile"
+        cl = next(iter(cls.values()), None)
+        scorers = [ScorerSpec(ws.scorer.kind, ws.weight, ws.scorer.param, ws.scorer.column, ws.scorer.param2)
+                   for ws in self.scorers]
+        context_length = None
+        if cl is not None:
+            in_filters = any(f is cl for f in self.filters)
+            context_length = dict(label=cl.label, enable_filtering=bool(cl.enableFiltering and in_filters))
+            if not any(ws.scorer is cl for ws in self.scorers):
+                scorers.append(ScorerSpec(capi.SCORER_CONTEXT_LENGTH, 0.0))    # a filter only: its score weighs 0
         latency = None
         if tier is not None or lat_scorers:
             latency = _latency_fields(tier, a1, lat_scorers[0] if lat_scorers else None)
             if a2:
                 assert a2[0].ttft_column < 0, "a latency profile reads TTFT from the predictions, not from an ext column"
-        return ProfileSpec(roles[0].kind if roles else capi.FILTER_NONE,
-                           [ScorerSpec(ws.scorer.kind, ws.weight, ws.scorer.param, ws.scorer.column, ws.scorer.param2)
-                            for ws in self.scorers],
+        if cl is not None and a2:
+            assert a2[0].ttft_column < 0, "a context-length profile reads TTFT from the predictions, not from an ext column"
+        return ProfileSpec(roles[0].kind if roles else capi.FILTER_NONE, scorers,
                            AffinityFilterSpec(a2[0].affinityThreshold, a2[0].explorationProbability,
                                               a2[0].maxTTFTPenaltyMs, a2[0].ttft_column) if a2 else None,
                            _PICKER_KIND[type(self.picker)],
                            [q for f in self.filters if isinstance(f, _LabelFilter) for q in f.reqs],
-                           latency)
+                           latency, context_length)
 
 
 def _check_chain(filters):
@@ -568,10 +636,16 @@ def _check_chain(filters):
     roles = [f for f in filters if isinstance(f, _RoleFilter)]
     aff = [i for i, f in enumerate(filters) if isinstance(f, PrefixCacheAffinityFilter)]
     tier = [i for i, f in enumerate(filters) if isinstance(f, SLOHeadroomTierFilter)]
-    assert all(isinstance(f, (_RoleFilter, _LabelFilter, PrefixCacheAffinityFilter, SLOHeadroomTierFilter))
-               for f in filters), \
-        "a profile's filters are role filters, label filters, the prefix-cache-affinity-filter and the " \
-        "slo-headroom-tier-filter"
+    assert all(isinstance(f, (_RoleFilter, _LabelFilter, PrefixCacheAffinityFilter, SLOHeadroomTierFilter,
+                              _ContextLengthAware)) for f in filters), \
+        "a profile's filters are role filters, label filters, the prefix-cache-affinity-filter, the " \
+        "slo-headroom-tier-filter and context-length-aware"
+    cls = [i for i, f in enumerate(filters) if isinstance(f, _ContextLengthAware)]
+    assert len({id(filters[i]) for i in cls}) <= 1, "at most one context-length-aware instance per profile"
+    gates = [i for i, f in enumerate(filters) if isinstance(f, (PrefixCacheAffinityFilter, SLOHeadroomTierFilter))]
+    assert not any(filters[i].enableFiltering and gates and i > gates[0] for i in cls), \
+        "a filtering context-length-aware comes before the affinity and tier filters (it is a per-endpoint predicate)"
+    filters = [f for f in filters if not isinstance(f, _ContextLengthAware)]   # the rest of the chain as without it
     assert len(roles) <= 1, "at most one role filter per profile"
     assert len(tier) <= 1, "at most one slo-headroom-tier-filter per profile"
     if tier:
@@ -639,6 +713,7 @@ class InferenceRequest:
     Prompt: bytes = b""                          # Body.Completions.Prompt.Raw as bytes
     CacheSalt: str = ""
     SchedulingResult: object = None              # set by the caller after Schedule (read by ResponseBody processors)
+    TokenizedPrompt: list | None = None          # Body.TokenizedPrompt.TokenIDs, or None (no token producer)
 
 
 class Scheduler:
@@ -676,7 +751,8 @@ class Scheduler:
                              max_prefix_blocks=max_prefix_blocks, non_cached_tokens=nct, always_disagg=always,
                              n_ext_cols=ext_columns, tie_seed=tie_seed, pick_k=self.pick_k, inflight_load=inflight_load)
         self.block_size_tokens = block_size_tokens
-        self.has_labels = any(p.spec().labels for p in profiles.values())
+        self.has_context_length = any(p.spec().context_length is not None for p in profiles.values())
+        self.has_labels = any(p.spec().labels for p in profiles.values()) or self.has_context_length
         self.has_latency = any(p.spec().latency is not None for p in profiles.values())
 
     def _push_pool(self, endpoints, ext=None):
@@ -720,10 +796,14 @@ class Scheduler:
             preds = [row] * len(reqs)
         if preds is not None and not self.has_latency:
             raise SchedulingError("latency predictions need a profile with a latency-scorer or slo-headroom-tier-filter")
+        # getContextLength: the token count, else the engine's default int(float64(len(prompt)) * 0.25) (-1)
+        ctx = np.array([len(r.TokenizedPrompt) if r.TokenizedPrompt else -1 for r in reqs], dtype=np.int64) \
+            if self.has_context_length else None
         if self.pick_k > 1:
-            dec, det, lists = self.engine.schedule_with_match(match, total, in_len, bst, topk=True, predictions=preds)
+            dec, det, lists = self.engine.schedule_with_match(match, total, in_len, bst, topk=True, predictions=preds,
+                                                              context_tokens=ctx)
         else:
-            dec, det = self.engine.schedule_with_match(match, total, in_len, bst, predictions=preds)
+            dec, det = self.engine.schedule_with_match(match, total, in_len, bst, predictions=preds, context_tokens=ctx)
             lists = {"primary": dec["pick"].reshape(-1, 1), "prefill": dec["prefill_pick"].reshape(-1, 1)}
         out = [self._result(dec[i], det[i], eps, lists["primary"][i], lists["prefill"][i]) for i in range(len(reqs))]
         return out[0] if single else out
