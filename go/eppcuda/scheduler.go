@@ -34,6 +34,8 @@ type Scheduler struct {
 	// the reference scheduler: used only for a candidate the engine has no slot for (not in its pool snapshot yet), or a
 	// subset of more than EPP_SUBSET_MAX_SLOTS endpoints
 	Fallback requestcontrol.Scheduler
+	// the engine-backed admitters (admission.go), or nil: Schedule then uses the decision AdmitRequest kept
+	Admitter *Admitter
 }
 
 var _ requestcontrol.Scheduler = (*Scheduler)(nil)
@@ -95,7 +97,12 @@ func (s *Scheduler) Schedule(ctx context.Context, request *scheduling.InferenceR
 	}
 	mm := HasMultimodalContent != nil && HasMultimodalContent(request)
 	var d Decision
-	if s.Engine.ctxLen {
+	admitted := false
+	if s.Admitter != nil { // the decision the engine made when it admitted the request (admission.go)
+		d, admitted = s.Admitter.take(request)
+	}
+	if admitted {
+	} else if s.Engine.ctxLen {
 		var pred []C.epp_prediction
 		if s.Engine.latency {
 			pred = s.Engine.predictions(candidates)

@@ -256,7 +256,8 @@ typedef struct {
 } epp_config;
 
 /* One routing decision (32 bytes).  status: 0 = ok, -1 = no endpoint available for the primary profile
- * (Schedule error: scheduler_profile.go:119-121 / disagg_profile_handler.go:335-338). */
+ * (Schedule error: scheduler_profile.go:119-121 / disagg_profile_handler.go:335-338), EPP_STATUS_REJECTED (-2) = an
+ * admitter rejected the request (see "Admission"). */
 typedef struct {
     int32_t status;
     uint32_t pick;             /* primary (decode) pick: lowest slot id of the arg-max set, or EPP_NO_ENDPOINT */
@@ -315,7 +316,9 @@ typedef struct {
     /* device-pointer batches only: CUDA-event time of each kernel of the last batch on the launch stream.
      * [0] prompt lengths  [1] block digests (dominant: reads every token once)  [2] chain  [3] match+score+pick
      * [4] the no-hit-lru update after the picks (engines with that scorer; 0 otherwise)
-     * [5] the in-flight counters' update after the picks (engines with inflight_load; 0 otherwise) */
+     * [5] the in-flight counters' update after the picks (engines with inflight_load; 0 otherwise)
+     * [6] the subset pick kernel (calls with restricted requests; 0 otherwise)
+     * [7] the admission kernel (calls with a row an admitter can reject, see "Admission"; 0 otherwise) */
     double last_kernel_ms[8];
     /* algorithmic work of the last batch (SURVEY.md 8(d)): table probes P = sum_r min(stop_r+1, B_r) and
      * postings consumed M = sum_r sum_{i<stop_r} |servers(h_i)| */
@@ -695,6 +698,79 @@ EPP_API int32_t epp_schedule_with_match_ctx(epp_engine *h, int64_t n_requests, c
                                             const epp_topk_out *topk, const epp_predictions *preds,
                                             const epp_context_tokens *ctx);
 
+/* ---- Admission (requestcontrol/admitter/latencyslo/plugin.go:99-158 "latency-slo-admitter",
+ * requestcontrol/admitter/probabilisticadmitter/plugin.go:125-162 "probabilistic-admitter") ---------------------------
+ * The director runs the Admitter plugins after the data producers and before Scheduler.Schedule, over the same candidate
+ * snapshot (requestcontrol/director.go:230-243); a rejected request is never scheduled.  The engine decides admission on
+ * the device after the picks of a call and rewrites the rows it rejects, so a rejected request makes none of the
+ * after-pick updates (no in-flight adds, no no-hit-lru Adds, nothing for epp_index_add_picked).
+ *   Candidates of a request: the pool slots, or, for a request with an endpoint subset, the subset's slots that are in the
+ *     pool.  Role, label, context-length and affinity filters do NOT apply (admission runs before any profile).  A request
+ *     without a candidate keeps status -1 (the director answers ServiceUnavailable before admission); every other row may
+ *     be rejected, a row whose decode profile found nobody included.
+ *   Per-request inputs (epp_admission): priority (< 0 = sheddable; both admitters admit priority >= 0), ttft_slo / tpot_slo
+ *     (parseFloatHeaderValue of x-slo-ttft-ms / x-slo-tpot-ms: 0 when absent, unparsable or out of range; only > 0 is
+ *     tested, any double is accepted), and pred_valid: one byte per entry of the call's epp_predictions, same layout,
+ *     bit 0 TTFTValid, bit 1 TPOTValid; IsValid() = both.  Validity is not derived from the headrooms (the producer
+ *     neutralises TPOT with headroom 0, and a streaming prediction at the buffered SLO has headroom 0 but is invalid).
+ *   latency-slo-admitter rejects iff the request is sheddable, ttft_slo > 0 || tpot_slo > 0, some candidate has an entry
+ *     (entries for other slots are ignored), no candidate's entry has both bits set, no candidate has running == 0 and no
+ *     candidate has kv_usage < 0.02.
+ *   probabilistic-admitter, for a sheddable request: sat = the left fold from +0.0, in ascending slot order over the
+ *     candidates, of math.Max(float64(waiting) / float64(queue_depth_threshold), kv_usage / kv_cache_util_threshold),
+ *     divided by the number of candidates; p = math.Min(math.Pow(sat, power) * k, 1.0); rejected iff u < p with
+ *     u = (mix64((tie_seed ^ 0x1D8E4E27C47D124F) ^ mix64(key)) >> 11) * 2^-53, key = 4 * ordinal + 3 (the one index of the
+ *     key space no profile uses), drawn for every tie_seed, 0 included.  math.Pow is Go's algorithm restated (special
+ *     cases, Modf, Exp(yf * Log(x)) for the fraction, the binary loop on Frexp's mantissa, Ldexp): bit-exact for an
+ *     integer power; with a fractional one Exp and Log are CUDA's exp and log.
+ *   Both admitters may be on: a row is rejected when either rejects it (the draw is keyed, so their order is irrelevant).
+ *   A rejected row: status EPP_STATUS_REJECTED, pick = prefill_pick = EPP_NO_ENDPOINT, score 0.0, tie_count 0,
+ *     match_blocks 0, total_blocks unchanged (the prefix producer ran before admission); its detail EPP_NO_ENDPOINT / 0 with
+ *     every *_ran 0; its first-k rows EPP_NO_ENDPOINT / 0.0.  It keeps its ordinal (n_decisions counts it), so every
+ *     admitted row is byte-identical to the same call made without admission inputs.
+ *   The whole-pool candidate set's idle and cold flags, count and saturation fold are derived by epp_pool_set and follow
+ *   the snapshot rule: an async batch decides on the pool it was enqueued under.  Only rows an admitter can reject are
+ *   examined, one warp each, by a kernel behind the call's picks (and before its after-pick updates); a call without such
+ *   a row launches nothing more and may take the small-batch path.  Its device time is epp_stats.last_kernel_ms[7] on
+ *   device-pointer batches (0 otherwise).
+ * The arrays are HOST memory for every batch kind, validated and copied before anything is launched.  A wrong struct_size,
+ * a NULL pred_valid on an engine with the latency-slo-admitter for a call with predictions, or epp_admission on an
+ * engine without admitters is EPP_ERR_INVALID; a refused call changes no ordinal, LRU, counter or index state.  With the
+ * latency-slo-admitter on, predictions are accepted on every engine (on an engine without a latency profile only the
+ * admitter reads them). */
+#define EPP_STATUS_REJECTED (-2)
+typedef struct {
+    uint32_t struct_size;              /* sizeof(epp_admission_cfg)                                                    */
+    int32_t latency_slo;               /* 1: the latency-slo-admitter                                                  */
+    int32_t probabilistic;             /* 1: the probabilistic-admitter                                                */
+    int32_t queue_depth_threshold;     /* queueDepthThreshold, > 0 (default 5)                                         */
+    double kv_cache_util_threshold;    /* kvCacheUtilThreshold, finite and > 0 (default 0.8)                           */
+    double power;                      /* power, finite and > 0 (default 5.0)                                          */
+    double k;                          /* k, finite and > 0 (default 300)                                              */
+} epp_admission_cfg;
+EPP_API void epp_admission_cfg_default(epp_admission_cfg *cfg);
+/* Sets the engine's admitters.  Only before the first successful epp_pool_set / epp_pool_set_labels (EPP_ERR_STATE after);
+ * refused on endpoint-sharded and peer-memory engines. */
+EPP_API int32_t epp_admission_set(epp_engine *h, const epp_admission_cfg *cfg);
+typedef struct {
+    uint32_t struct_size;              /* sizeof(epp_admission)                                                        */
+    uint32_t reserved;
+    const int32_t *priority;           /* [R] Objectives.Priority, or NULL = all 0                                     */
+    const double *ttft_slo;            /* [R] or NULL = all 0                                                          */
+    const double *tpot_slo;            /* [R] or NULL = all 0                                                          */
+    const uint8_t *pred_valid;         /* one byte per entry of the call's epp_predictions (entries[offsets[r] + i]), or NULL */
+} epp_admission;
+/* epp_schedule_ctx / epp_schedule_with_match_ctx with admission inputs (adm may be NULL: the call is then exactly the
+ * _ctx call). */
+EPP_API int32_t epp_schedule_admit(epp_engine *h, const epp_batch *batch, const epp_subset *subset, const epp_predictions *preds,
+                                   const epp_context_tokens *ctx, const epp_admission *adm, epp_decision *out,
+                                   epp_decision_detail *detail, int32_t keep_hashes, const epp_topk_out *topk);
+EPP_API int32_t epp_schedule_with_match_admit(epp_engine *h, int64_t n_requests, const int32_t *match, const int32_t *total,
+                                              const uint32_t *model_ids, const int64_t *input_len_bytes,
+                                              int32_t block_size_tokens, epp_decision *out, epp_decision_detail *detail,
+                                              uint32_t flags, const epp_topk_out *topk, const epp_predictions *preds,
+                                              const epp_context_tokens *ctx, const epp_admission *adm);
+
 /* PreRequest (approximateprefix/plugin.go:164-200): index the hashes of the LAST epp_schedule batch
  * (keep_hashes=1) for each request's primary pick and prefill pick. */
 EPP_API int32_t epp_index_add_picked(epp_engine *h);
@@ -857,6 +933,15 @@ EPP_API int32_t epp_submit_subset_predicted(epp_batcher *b, uint32_t model_id, c
 EPP_API int32_t epp_submit_ctx(epp_batcher *b, uint32_t model_id, const void *prompt, uint64_t prompt_len, uint32_t multimodal,
                                uint32_t n_slots, const uint32_t *slots, uint32_t n_pred, const epp_prediction *entries,
                                int64_t context_tokens, uint64_t *out_ticket);
+/* epp_submit_ctx plus the request's admission inputs (see "Admission"): pred_valid holds one byte per entry of `entries`
+ * (required when n_pred > 0 and the engine has the latency-slo-admitter), priority (< 0 = sheddable) and the two SLOs.  An
+ * engine without admitters is EPP_ERR_INVALID; predictions are accepted on an engine with the latency-slo-admitter.  A
+ * flush that holds such a request runs epp_schedule_admit; its rejected requests get status EPP_STATUS_REJECTED from
+ * epp_wait / epp_wait_topk like any other row. */
+EPP_API int32_t epp_submit_admit(epp_batcher *b, uint32_t model_id, const void *prompt, uint64_t prompt_len, uint32_t multimodal,
+                                 uint32_t n_slots, const uint32_t *slots, uint32_t n_pred, const epp_prediction *entries,
+                                 const uint8_t *pred_valid, int64_t context_tokens, int32_t priority, double ttft_slo,
+                                 double tpot_slo, uint64_t *out_ticket);
 EPP_API int32_t epp_wait(epp_batcher *b, uint64_t ticket, epp_decision *out, epp_decision_detail *out_detail);
 /* The same on an engine created with pick_k > 1, plus the request's first-k lists (ProfileRunResult.TargetEndpoints of
  * each profile, see epp_topk_out): primary / prefill / encode receive pick_k slot ids each (EPP_NO_ENDPOINT padded); any

@@ -122,6 +122,20 @@ class ContextTokens(C.Structure):
     _fields_ = [("struct_size", C.c_uint32), ("reserved", C.c_uint32), ("tokens", C.c_void_p)]
 
 
+EPP_STATUS_REJECTED = -2
+
+
+class AdmissionCfg(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("latency_slo", C.c_int32), ("probabilistic", C.c_int32),
+                ("queue_depth_threshold", C.c_int32), ("kv_cache_util_threshold", C.c_double), ("power", C.c_double),
+                ("k", C.c_double)]
+
+
+class Admission(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("reserved", C.c_uint32), ("priority", C.c_void_p), ("ttft_slo", C.c_void_p),
+                ("tpot_slo", C.c_void_p), ("pred_valid", C.c_void_p)]
+
+
 class LabelReq(C.Structure):
     _fields_ = [("key", C.c_char_p), ("op", C.c_int32), ("n_values", C.c_int32), ("values", C.POINTER(C.c_char_p))]
 
@@ -195,6 +209,14 @@ SIGNATURES = {
     "epp_schedule_with_match_ctx": (C.c_int32, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                                 C.c_int32, C.c_void_p, C.c_void_p, C.c_uint32, C.POINTER(TopkOut),
                                                 C.POINTER(Predictions), C.POINTER(ContextTokens)]),
+    "epp_admission_cfg_default": (None, [C.POINTER(AdmissionCfg)]),
+    "epp_admission_set": (C.c_int32, [C.c_void_p, C.POINTER(AdmissionCfg)]),
+    "epp_schedule_admit": (C.c_int32, [C.c_void_p, C.POINTER(Batch), C.POINTER(Subset), C.POINTER(Predictions),
+                                       C.POINTER(ContextTokens), C.POINTER(Admission), C.c_void_p, C.c_void_p, C.c_int32,
+                                       C.POINTER(TopkOut)]),
+    "epp_schedule_with_match_admit": (C.c_int32, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                  C.c_int32, C.c_void_p, C.c_void_p, C.c_uint32, C.POINTER(TopkOut),
+                                                  C.POINTER(Predictions), C.POINTER(ContextTokens), C.POINTER(Admission)]),
     "epp_index_add_picked": (C.c_int32, [C.c_void_p]),
     "epp_nohit_lru_get": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(C.c_int32)]),
     "epp_inflight_release": (C.c_int32, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
@@ -228,6 +250,9 @@ SIGNATURES = {
                                                 C.c_void_p, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint64)]),
     "epp_submit_ctx": (C.c_int32, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_uint32, C.c_uint32, C.c_void_p,
                                    C.c_uint32, C.c_void_p, C.c_int64, C.POINTER(C.c_uint64)]),
+    "epp_submit_admit": (C.c_int32, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_uint32, C.c_uint32, C.c_void_p,
+                                     C.c_uint32, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_double, C.c_double,
+                                     C.POINTER(C.c_uint64)]),
     "epp_wait": (C.c_int32, [C.c_void_p, C.c_uint64, C.POINTER(Decision), C.POINTER(DecisionDetail)]),
     "epp_wait_topk": (C.c_int32, [C.c_void_p, C.c_uint64, C.POINTER(Decision), C.POINTER(DecisionDetail), C.c_void_p,
                                   C.c_void_p, C.c_void_p]),

@@ -12,7 +12,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libepp_engine.so")
-SOURCES = ["engine.cu", "batcher.cu", "hash_kernels.cu", "hash_fused.cu", "index_kernels.cu", "index_store.cu", "pick_kernels.cu", "match_sparse.cu", "cycle_small.cu", "shard_p2p.cu", "nohit_lru.cu", "inflight.cu", "subset_pick.cu"]
+SOURCES = ["engine.cu", "batcher.cu", "hash_kernels.cu", "hash_fused.cu", "index_kernels.cu", "index_store.cu", "pick_kernels.cu", "match_sparse.cu", "cycle_small.cu", "shard_p2p.cu", "nohit_lru.cu", "inflight.cu", "subset_pick.cu", "admit.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",

@@ -35,9 +35,11 @@
 #include <vector>
 
 #include "../../include/epp_engine.h"
+#include "kernels.h"
 
 // engine.cu: the engine's profiles with a latency piece (0: none)
 int32_t engine_latency_mask(const epp_engine *h);
+int32_t engine_admission(const epp_engine *h);
 
 namespace {
 constexpr int kBufs = 4;                       // staging buffers: batches k .. k+3 can be filling / in flight at once
@@ -82,6 +84,11 @@ struct Staging {
     // context lengths (epp_submit_ctx): per row its token count, -1 = the default
     std::vector<int64_t> ctx;                  // [max_batch]
     std::atomic<int32_t> any_ctx{0};           // some row of the batch using this buffer has a token count
+    // admission (epp_submit_admit): per row its priority and SLOs, and its entries' validity bytes next to pred_entries
+    std::vector<int32_t> priority;             // [max_batch], 0 for rows submitted any other way
+    std::vector<double> ttft_slo, tpot_slo;    // [max_batch]
+    std::vector<uint8_t> pred_valid;           // [max_batch][EPP_PRED_MAX_SLOTS], allocated with pred_entries
+    std::atomic<int32_t> any_adm{0};           // some row of the batch using this buffer came through epp_submit_admit
     std::atomic<int32_t> ready{0};             // rows of the batch using this buffer whose copy is complete
     std::atomic<int64_t> first_arrival_ns{0};  // when row 0 of that batch was reserved
 };
@@ -184,7 +191,8 @@ static void flusher_main(epp_batcher *b) {
         const bool any_pred = st.any_pred.load(std::memory_order_acquire) != 0;
         const bool any_sub = st.any_subset.load(std::memory_order_acquire) != 0;
         const bool any_ctx = st.any_ctx.load(std::memory_order_acquire) != 0;
-        if (any_pred || any_sub || any_ctx) {
+        const bool any_adm = st.any_adm.load(std::memory_order_acquire) != 0;
+        if (any_pred || any_sub || any_ctx || any_adm) {
             // predictions only reach a latency engine (every predicted submit checks it), where subsets and predictions
             // may share a batch and even a row: one epp_schedule_subset_predicted decides them all
             epp_predictions pr;
@@ -203,9 +211,17 @@ static void flusher_main(epp_batcher *b) {
             memset(&ct, 0, sizeof ct);
             ct.struct_size = sizeof ct;
             ct.tokens = st.ctx.data();
-            if (any_ctx)
-                rc = epp_schedule_ctx(b->eng, &batch, any_sub ? &sub : nullptr, any_pred ? &pr : nullptr, &ct, st.dec, st.det,
-                                      b->cfg.index_picks ? 1 : 0, b->pick_k > 1 ? &tk : nullptr);
+            epp_admission adm;
+            memset(&adm, 0, sizeof adm);
+            adm.struct_size = sizeof adm;
+            adm.priority = st.priority.data();
+            adm.ttft_slo = st.ttft_slo.data();
+            adm.tpot_slo = st.tpot_slo.data();
+            adm.pred_valid = st.pred_valid.empty() ? nullptr : st.pred_valid.data();
+            // predictions on an engine without a latency profile are read by the latency-slo-admitter only (epp_schedule_admit)
+            if (any_ctx || any_adm || (any_pred && !engine_latency_mask(b->eng)))
+                rc = epp_schedule_admit(b->eng, &batch, any_sub ? &sub : nullptr, any_pred ? &pr : nullptr, &ct, any_adm ? &adm : nullptr,
+                                        st.dec, st.det, b->cfg.index_picks ? 1 : 0, b->pick_k > 1 ? &tk : nullptr);
             else if (engine_latency_mask(b->eng))
                 rc = epp_schedule_subset_predicted(b->eng, &batch, any_sub ? &sub : nullptr, any_pred ? &pr : nullptr, st.dec, st.det,
                                                    b->cfg.index_picks ? 1 : 0, b->pick_k > 1 ? &tk : nullptr);
@@ -214,6 +230,7 @@ static void flusher_main(epp_batcher *b) {
             st.any_pred.store(0, std::memory_order_relaxed);
             st.any_subset.store(0, std::memory_order_relaxed);
             st.any_ctx.store(0, std::memory_order_relaxed);
+            st.any_adm.store(0, std::memory_order_relaxed);
         } else if (b->pick_k > 1) {
             rc = epp_schedule_topk(b->eng, &batch, st.dec, st.det, b->cfg.index_picks ? 1 : 0, &tk);
         } else {
@@ -306,6 +323,9 @@ extern "C" int32_t epp_batcher_create(epp_engine *h, const epp_batcher_cfg *cfg,
         st.pred_offsets.resize(mb);
         for (size_t r = 0; r < mb; r++) st.pred_offsets[r] = (uint64_t)r * EPP_PRED_MAX_SLOTS;
         st.ctx.assign(mb, -1);
+        st.priority.assign(mb, 0);
+        st.ttft_slo.assign(mb, 0.0);
+        st.tpot_slo.assign(mb, 0.0);
         if (b->pick_k > 1)
             for (int q = 0; q < 3; q++) {
                 rc = epp_host_alloc(sizeof(uint32_t) * mb * (size_t)b->pick_k, &p);
@@ -338,11 +358,18 @@ extern "C" int32_t epp_batcher_destroy(epp_batcher *b) {
     return EPP_OK;
 }
 
+// The admission inputs of one request (epp_submit_admit): its entries' validity bytes in the order of its sorted predictions.
+struct AdmitIn {
+    int32_t priority;
+    double ttft_slo, tpot_slo;
+    const std::vector<uint8_t> *valid;
+};
+
 // sub: the request's slots, sorted and deduplicated, or nullptr (the whole pool); pred: its predictions, validated and
-// sorted by slot, or nullptr (none); ctx: its context tokens, -1 = the default
+// sorted by slot, or nullptr (none); ctx: its context tokens, -1 = the default; adm: its admission inputs, or nullptr
 static int32_t submit_impl(epp_batcher *b, uint32_t model_id, const void *prompt, uint64_t prompt_len, uint32_t multimodal,
                            const std::vector<uint32_t> *sub, uint64_t *out_ticket,
-                           const std::vector<epp_prediction> *pred = nullptr, int64_t ctx = -1) {
+                           const std::vector<epp_prediction> *pred = nullptr, int64_t ctx = -1, const AdmitIn *adm = nullptr) {
     const uint64_t max_batch = (uint64_t)b->cfg.max_batch;
     uint64_t seq, idx;
     for (int spin = 0;; spin++) {
@@ -393,6 +420,14 @@ static int32_t submit_impl(epp_batcher *b, uint32_t model_id, const void *prompt
     }
     st.ctx[idx] = ctx;
     if (ctx != -1) st.any_ctx.store(1, std::memory_order_relaxed);   // published by the release below
+    st.priority[idx] = adm ? adm->priority : 0;
+    st.ttft_slo[idx] = adm ? adm->ttft_slo : 0.0;
+    st.tpot_slo[idx] = adm ? adm->tpot_slo : 0.0;
+    if (adm) {
+        if (adm->valid && !adm->valid->empty())
+            memcpy(st.pred_valid.data() + (size_t)idx * EPP_PRED_MAX_SLOTS, adm->valid->data(), adm->valid->size());
+        st.any_adm.store(1, std::memory_order_relaxed);            // published by the release below
+    }
     st.ready.fetch_add(1, std::memory_order_release);              // the flusher waits for this before it reads the row
     *out_ticket = (seq << 20) | idx;
     return EPP_OK;
@@ -429,7 +464,8 @@ static int32_t take_subset(epp_batcher *b, uint32_t n_slots, const uint32_t *slo
 // prediction staging allocated.
 static int32_t take_predictions(epp_batcher *b, uint32_t n, const epp_prediction *entries, std::vector<epp_prediction> *pred) {
     if (n > EPP_PRED_MAX_SLOTS) return bfail(EPP_ERR_CAPACITY, "more than EPP_PRED_MAX_SLOTS predictions for one request");
-    if (!engine_latency_mask(b->eng)) return bfail(EPP_ERR_INVALID, "predictions passed to an engine without a latency profile");
+    if (!engine_latency_mask(b->eng) && !(engine_admission(b->eng) & epp::kAdmitLatencySlo))
+        return bfail(EPP_ERR_INVALID, "predictions passed to an engine without a latency profile or the latency-slo-admitter");
     pred->assign(entries, entries + n);
     for (const epp_prediction &p : *pred) {
         if (p.slot >= b->max_endpoints) return bfail(EPP_ERR_INVALID, "prediction slot >= max_endpoints");
@@ -441,7 +477,10 @@ static int32_t take_predictions(epp_batcher *b, uint32_t n, const epp_prediction
         if ((*pred)[i].slot == (*pred)[i - 1].slot) return bfail(EPP_ERR_INVALID, "two predictions for one slot");
     std::call_once(b->pred_once, [b] {
         try {
-            for (int i = 0; i < kBufs; i++) b->buf[i].pred_entries.resize((size_t)b->cfg.max_batch * EPP_PRED_MAX_SLOTS);
+            for (int i = 0; i < kBufs; i++) {
+                b->buf[i].pred_entries.resize((size_t)b->cfg.max_batch * EPP_PRED_MAX_SLOTS);
+                b->buf[i].pred_valid.resize((size_t)b->cfg.max_batch * EPP_PRED_MAX_SLOTS);
+            }
         } catch (...) {
             b->pred_alloc_failed = true;
         }
@@ -496,6 +535,37 @@ extern "C" int32_t epp_submit_ctx(epp_batcher *b, uint32_t model_id, const void 
     if (rc == EPP_OK && n_pred) rc = take_predictions(b, n_pred, entries, &pred);
     if (rc != EPP_OK) return rc;
     return submit_impl(b, model_id, prompt, prompt_len, multimodal, slots ? &sub : nullptr, out_ticket, &pred, context_tokens);
+}
+
+extern "C" int32_t epp_submit_admit(epp_batcher *b, uint32_t model_id, const void *prompt, uint64_t prompt_len, uint32_t multimodal,
+                                    uint32_t n_slots, const uint32_t *slots, uint32_t n_pred, const epp_prediction *entries,
+                                    const uint8_t *pred_valid, int64_t context_tokens, int32_t priority, double ttft_slo,
+                                    double tpot_slo, uint64_t *out_ticket) {
+    if (!b || !out_ticket || (prompt_len && !prompt) || (n_slots && !slots) || (n_pred && !entries))
+        return bfail(EPP_ERR_INVALID, "NULL argument");
+    if (context_tokens < -1) return bfail(EPP_ERR_INVALID, "context tokens < -1");
+    const int32_t admitters = engine_admission(b->eng);
+    if (!admitters) return bfail(EPP_ERR_INVALID, "admission inputs passed to an engine without admitters (epp_admission_set)");
+    if (n_pred && (admitters & epp::kAdmitLatencySlo) && !pred_valid)
+        return bfail(EPP_ERR_INVALID, "pred_valid is NULL: the latency-slo-admitter needs it for a request with predictions");
+    if (n_pred > EPP_PRED_MAX_SLOTS) return bfail(EPP_ERR_CAPACITY, "more than EPP_PRED_MAX_SLOTS predictions for one request");
+    // the entries and their validity bytes sorted together by slot (take_predictions keeps an ascending list as it is)
+    std::vector<uint32_t> order(n_pred);
+    for (uint32_t i = 0; i < n_pred; i++) order[i] = i;
+    std::stable_sort(order.begin(), order.end(), [entries](uint32_t x, uint32_t y) { return entries[x].slot < entries[y].slot; });
+    std::vector<epp_prediction> sorted(n_pred);
+    std::vector<uint8_t> valid(n_pred, 0);
+    for (uint32_t i = 0; i < n_pred; i++) {
+        sorted[i] = entries[order[i]];
+        if (pred_valid) valid[i] = pred_valid[order[i]];
+    }
+    std::vector<uint32_t> sub;
+    std::vector<epp_prediction> pred;
+    int32_t rc = slots ? take_subset(b, n_slots, slots, &sub) : EPP_OK;
+    if (rc == EPP_OK && n_pred) rc = take_predictions(b, n_pred, sorted.data(), &pred);
+    if (rc != EPP_OK) return rc;
+    const AdmitIn adm{priority, ttft_slo, tpot_slo, &valid};
+    return submit_impl(b, model_id, prompt, prompt_len, multimodal, slots ? &sub : nullptr, out_ticket, &pred, context_tokens, &adm);
 }
 
 extern "C" int32_t epp_wait(epp_batcher *b, uint64_t ticket, epp_decision *out, epp_decision_detail *out_detail) {

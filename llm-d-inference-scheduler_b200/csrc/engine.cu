@@ -233,6 +233,20 @@ struct epp_engine {
     size_t sub_host_cap = 0;
     cudaEvent_t sub_up_ev = nullptr;    // behind the last upload from sub_host
     DevBuf topk_picks[kMaxProfiles], topk_scores;   // device staging of the lists for host batches
+    // admission (include/epp_engine.h "Admission", admit.cu): the admitters, the whole pool's candidate aggregates of the
+    // current snapshot (derived by epp_pool_set), and the rows of the call in progress an admitter can reject (cur_adm,
+    // ascending; their rows and packed entries were validated on the host and copied to adm_rows / adm_ent)
+    epp_admission_cfg adm{};
+    bool adm_on = false;
+    int32_t adm_pool_n = 0, adm_idle = 0, adm_cold = 0;
+    double adm_sat = 0.0;
+    const std::vector<AdmitRow> *cur_adm = nullptr;
+    DevBuf adm_rows, adm_ent;
+    std::vector<cudaEvent_t> adm_ev;    // pairs bracketing the admission launches of the device batch in flight
+    int adm_ev_used = 0;                // events of adm_ev recorded for it (last_kernel_ms[7])
+    void *adm_host = nullptr;           // pinned staging of the rows and entries being uploaded
+    size_t adm_host_cap = 0;
+    cudaEvent_t adm_up_ev = nullptr;    // behind the last upload from adm_host
     int64_t kept_R = 0;             // rows of `hashes` valid for epp_index_add_picked
     int64_t shard_R = 0;            // rows of `hashes` valid for epp_shard_pick / epp_shard_merge
     bool shard_models = false;      // the probed batch had model ids: its copy in `model_ids` feeds epp_shard_pick
@@ -587,6 +601,9 @@ extern "C" int32_t epp_engine_destroy(epp_engine *h) {
     for (auto &ev : h->sub_ev) cudaEventDestroy(ev);
     if (h->sub_up_ev) cudaEventDestroy(h->sub_up_ev);
     if (h->sub_host) cudaFreeHost(h->sub_host);
+    for (auto &ev : h->adm_ev) cudaEventDestroy(ev);
+    if (h->adm_up_ev) cudaEventDestroy(h->adm_up_ev);
+    if (h->adm_host) cudaFreeHost(h->adm_host);
     if (h->wc_host) cudaFreeHost(h->wc_host);
     if (h->small_host) cudaFreeHost(h->small_host);
     if (h->small_epoch_host) cudaFreeHost(h->small_epoch_host);
@@ -869,6 +886,71 @@ static int32_t inflight_flush(epp_engine *h, cudaStream_t s, int *launches) {
     return inflight_rederive(h, s, launches);
 }
 
+// ---- admission (admit.cu) ------------------------------------------------------------------------------------------
+// Go's math.Max (Inf, then NaN, then the sign of zero): the probabilistic-admitter's per-endpoint saturation term.
+static double go_max(double x, double y) {
+    if (std::isinf(x) && x > 0) return x;
+    if (std::isinf(y) && y > 0) return y;
+    if (std::isnan(x) || std::isnan(y)) return std::nan("");
+    if (x == 0 && x == y) return std::signbit(x) ? y : x;
+    return x > y ? x : y;
+}
+
+// The whole pool's candidate aggregates of a new snapshot (slot-indexed arrays, role 0xFF = absent): the count, whether
+// one is idle (running == 0) or cold (kv < 0.02), and the saturation terms folded from +0.0 in ascending slot order.  They
+// reach k_admit as launch arguments, so a batch enqueued before the next epp_pool_set keeps deciding on these.
+static void admission_derive(epp_engine *h, const std::vector<uint8_t> &role, const std::vector<double> &kv,
+                             const std::vector<int32_t> &waiting, const std::vector<int32_t> &running) {
+    const double qdt = (double)h->adm.queue_depth_threshold, kvt = h->adm.kv_cache_util_threshold;
+    int32_t n = 0, idle = 0, cold = 0;
+    double sat = 0.0;
+    for (size_t e = 0; e < role.size(); e++) {
+        if (role[e] == 0xFF) continue;
+        n++;
+        idle |= running[e] == 0;
+        cold |= kv[e] < 0.02;
+        sat += go_max((double)waiting[e] / qdt, kv[e] / kvt);
+    }
+    h->adm_pool_n = n;
+    h->adm_idle = idle;
+    h->adm_cold = cold;
+    h->adm_sat = sat;
+}
+
+extern "C" void epp_admission_cfg_default(epp_admission_cfg *cfg) {
+    if (!cfg) return;
+    memset(cfg, 0, sizeof *cfg);
+    cfg->struct_size = sizeof(epp_admission_cfg);
+    cfg->queue_depth_threshold = 5;                   // probabilisticadmitter/plugin.go:38-41
+    cfg->kv_cache_util_threshold = 0.8;
+    cfg->power = 5.0;
+    cfg->k = 300.0;
+}
+
+extern "C" int32_t epp_admission_set(epp_engine *h, const epp_admission_cfg *cfg) {
+    if (!h || !cfg) return fail(EPP_ERR_INVALID, "NULL engine or configuration");
+    if (cfg->struct_size != sizeof(epp_admission_cfg))
+        return fail(EPP_ERR_INVALID, "epp_admission_cfg.struct_size %u != %zu", cfg->struct_size, sizeof(epp_admission_cfg));
+    std::lock_guard<std::mutex> lk(h->mu);
+    if (h->pool_called) return fail(EPP_ERR_STATE, "the admitters are fixed once the pool has been set");
+    if (sharded(h) || h->p2p_buf)
+        return fail(EPP_ERR_INVALID, "admission is not available in the endpoint-sharded and peer-memory modes");
+    if ((cfg->latency_slo != 0 && cfg->latency_slo != 1) || (cfg->probabilistic != 0 && cfg->probabilistic != 1))
+        return fail(EPP_ERR_INVALID, "latency_slo and probabilistic must be 0 or 1");
+    // probabilisticadmitter.Factory's checks and messages (plugin.go:71-84); the finiteness checks are the C side's own
+    if (cfg->queue_depth_threshold <= 0)
+        return fail(EPP_ERR_INVALID, "plugin 'probabilistic-admitter': queueDepthThreshold must be > 0, got %d", cfg->queue_depth_threshold);
+    if (!(cfg->kv_cache_util_threshold > 0.0) || !std::isfinite(cfg->kv_cache_util_threshold))
+        return fail(EPP_ERR_INVALID, "plugin 'probabilistic-admitter': kvCacheUtilThreshold must be > 0, got %g", cfg->kv_cache_util_threshold);
+    if (!(cfg->power > 0) || !std::isfinite(cfg->power))
+        return fail(EPP_ERR_INVALID, "plugin 'probabilistic-admitter': power must be > 0, got %g", cfg->power);
+    if (!(cfg->k > 0) || !std::isfinite(cfg->k))
+        return fail(EPP_ERR_INVALID, "plugin 'probabilistic-admitter': k must be > 0, got %g", cfg->k);
+    h->adm = *cfg;
+    h->adm_on = cfg->latency_slo || cfg->probabilistic;
+    return EPP_OK;
+}
+
 extern "C" int32_t epp_pool_set(epp_engine *h, int32_t n, const uint32_t *ids, const uint8_t *role,
                                 const double *kv_usage, const int32_t *waiting, const int32_t *running,
                                 const double *ext) {
@@ -908,6 +990,7 @@ extern "C" int32_t epp_pool_set(epp_engine *h, int32_t n, const uint32_t *ids, c
         CUDA_TRY(cudaMemcpyAsync(h->ext.p, ex.data(), sizeof(double) * E * (size_t)h->cfg.n_ext_cols, cudaMemcpyHostToDevice, s));
     EPP_TRY(derive_pool(h));
     CUDA_TRY(cudaStreamSynchronize(s));
+    if (h->adm_on) admission_derive(h, r, kv, w, run);
     h->pool_ready = true;
     h->pool_called = true;
     return EPP_OK;
@@ -1855,6 +1938,14 @@ static int32_t finish_async(epp_engine *h) {
     }
     h->stats.last_kernel_ms[6] = ts;
     h->sub_ev_used = 0;
+    double ta = 0.0;
+    for (int i = 0; i + 1 < h->adm_ev_used; i += 2) {
+        float t1 = 0;
+        cudaEventElapsedTime(&t1, h->adm_ev[i], h->adm_ev[i + 1]);
+        ta += t1;
+    }
+    h->stats.last_kernel_ms[7] = ta;
+    h->adm_ev_used = 0;
     return EPP_OK;
 }
 
@@ -1889,6 +1980,60 @@ static int32_t launch_subset(epp_engine *h, const PickParams &pp, int64_t r0, in
     if (timed) {
         CUDA_TRY(cudaEventRecord(h->sub_ev[h->sub_ev_used + 1], s));
         h->sub_ev_used += 2;
+    }
+    return EPP_OK;
+}
+
+// The listed admission rows among rows [r0, r1) of a call, decided on s by k_admit after the picks (subset launch
+// included) of the same rows.  dec / det / tk: the call's rows from request 0 on.  timed: bracket it for last_kernel_ms[7].
+static int32_t launch_admission(epp_engine *h, int64_t r0, int64_t r1, epp_decision *dec, epp_decision_detail *det,
+                                const TopkRows &tk, cudaStream_t s, int *launches, bool timed) {
+    if (!h->cur_adm) return EPP_OK;
+    const std::vector<AdmitRow> &rows = *h->cur_adm;
+    auto below = [](const AdmitRow &a, int64_t r) { return (int64_t)a.row < r; };
+    const size_t lo = std::lower_bound(rows.begin(), rows.end(), r0, below) - rows.begin();
+    const size_t hi = std::lower_bound(rows.begin(), rows.end(), r1, below) - rows.begin();
+    if (lo == hi) return EPP_OK;
+    AdmitParams p;
+    memset(&p, 0, sizeof p);
+    p.rows = h->adm_rows.as<AdmitRow>() + lo;
+    p.n_rows = (int32_t)(hi - lo);
+    p.E = h->cfg.max_endpoints;
+    p.ent = h->adm_ent.as<uint32_t>();
+    p.sub_slots = h->sub_slots.as<uint32_t>();
+    p.role = h->role.as<uint8_t>();
+    p.kv = h->kv.as<double>();
+    p.waiting = h->waiting.as<int32_t>();
+    p.running = h->running.as<int32_t>();
+    p.pool_n = h->adm_pool_n;
+    p.pool_idle = h->adm_idle;
+    p.pool_cold = h->adm_cold;
+    p.pool_sat = h->adm_sat;
+    p.qdt = (double)h->adm.queue_depth_threshold;
+    p.kvt = h->adm.kv_cache_util_threshold;
+    p.power = h->adm.power;
+    p.k = h->adm.k;
+    p.tie_seed = h->cfg.tie_seed;
+    p.ord_base = h->stats.n_decisions;
+    p.dec = dec;
+    p.det = det;
+    if (tk.on) {
+        p.topk = h->cfg.pick_k;
+        for (int i = 0; i < kMaxProfiles; i++) p.topk_picks[i] = tk.picks[i];
+        p.topk_scores = tk.scores;
+    }
+    if (timed) {
+        while ((int)h->adm_ev.size() < h->adm_ev_used + 2) {
+            cudaEvent_t ev;
+            CUDA_TRY(cudaEventCreate(&ev));
+            h->adm_ev.push_back(ev);
+        }
+        CUDA_TRY(cudaEventRecord(h->adm_ev[h->adm_ev_used], s));
+    }
+    CUDA_TRY(launch_admit(p, s, launches));
+    if (timed) {
+        CUDA_TRY(cudaEventRecord(h->adm_ev[h->adm_ev_used + 1], s));
+        h->adm_ev_used += 2;
     }
     return EPP_OK;
 }
@@ -2075,6 +2220,7 @@ static int32_t run_device(epp_engine *h, const BatchView &v, Call &call) {
     CUDA_TRY(cudaMemsetAsync(h->work_counters.p, 0, sizeof(unsigned long long) * 4, s0));
     const int64_t min_chunk = 4096;
     h->sub_ev_used = 0;
+    h->adm_ev_used = 0;
     epp_decision *dec = call.out_dec ? call.out_dec : h->decisions.as<epp_decision>();
     PickParams pp;                                 // the rows of the last launch_rows, for their subset launch
     if (call.pipelined) {
@@ -2098,6 +2244,7 @@ static int32_t run_device(epp_engine *h, const BatchView &v, Call &call) {
             EPP_TRY(launch_rows(h, sl, device_work(h, v, r0, r1, or_bits), call, dec + r0,
                                 call.det_out ? call.det_out + r0 : nullptr, nullptr, false, pp, &call.launches));
             EPP_TRY(launch_subset(h, pp, r0, r1, sl.stream, &call.launches, true));
+            EPP_TRY(launch_admission(h, r0, r1, dec, call.det_out, call.tk, sl.stream, &call.launches, true));
         }
         h->s1_unjoined = true;
         // the next call's picks must see both chunks' Adds: join the chunks on stream 0 for the update (below), and the
@@ -2115,7 +2262,10 @@ static int32_t run_device(epp_engine *h, const BatchView &v, Call &call) {
     }
     CUDA_TRY(cudaEventRecord(h->ev[4], s0));
     if (call.mode == Mode::Schedule) {             // after ev[4]: last_kernel_ms[3] stays the match + pick time
-        if (!call.pipelined) EPP_TRY(launch_subset(h, pp, 0, R, s0, &call.launches, true));
+        if (!call.pipelined) {
+            EPP_TRY(launch_subset(h, pp, 0, R, s0, &call.launches, true));
+            EPP_TRY(launch_admission(h, 0, R, dec, call.det_out, call.tk, s0, &call.launches, true));
+        }
         EPP_TRY(after_picks(h, dec, call.det_out, h->in_len.as<int64_t>(), R, s0, &call.launches, true));
     }
     CUDA_TRY(cudaMemcpyAsync(h->wc_host, h->work_counters.p, sizeof(unsigned long long) * 4, cudaMemcpyDeviceToHost, s0));
@@ -2196,6 +2346,8 @@ static int32_t run_host(epp_engine *h, const BatchView &v, Call &call) {
             if (call.out_nblocks) CUDA_TRY(cudaMemcpyAsync(call.out_nblocks + c.r0, w.nblocks_out, sizeof(int32_t) * nreq, cudaMemcpyDeviceToHost, s));
         } else if (call.mode == Mode::Schedule) {
             EPP_TRY(launch_subset(h, pp, c.r0, c.r1, s, &call.launches, false));
+            EPP_TRY(launch_admission(h, c.r0, c.r1, h->decisions.as<epp_decision>(), h->details.as<epp_decision_detail>(),
+                                     call.tk, s, &call.launches, false));
             if (call.out_dec) CUDA_TRY(cudaMemcpyAsync(call.out_dec + c.r0, dec, sizeof(epp_decision) * nreq, cudaMemcpyDeviceToHost, s));
             if (call.out_detail) CUDA_TRY(cudaMemcpyAsync(call.out_detail + c.r0, det, sizeof(epp_decision_detail) * nreq, cudaMemcpyDeviceToHost, s));
             if (call.tk.on) EPP_TRY(topk_copy_back(h, call.tk, c.r0, (int64_t)nreq, s));
@@ -2213,7 +2365,8 @@ static int32_t run_host(epp_engine *h, const BatchView &v, Call &call) {
     float t_all = 0;
     cudaEventElapsedTime(&t_all, h->ev[0], h->ev[1]);
     h->stats.last_kernels_ms = t_all;
-    h->stats.last_kernel_ms[6] = 0.0;              // the subset kernel is timed on device batches only
+    h->stats.last_kernel_ms[6] = 0.0;              // the subset and admission kernels are timed on device batches only
+    h->stats.last_kernel_ms[7] = 0.0;
     h->stats.last_hash_ms = h->stats.last_match_pick_ms = 0;
     h->stats.last_kernel_launches = (uint64_t)call.launches;
     return EPP_OK;
@@ -2256,8 +2409,9 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
     if (v.device) return run_device(h, v, call);
 
     // small host batch in pinned memory: one zero-copy launch, no copy engine, no stream synchronisation (not for a batch
-    // with restricted requests: the kernel hands the decisions to the host before a subset launch could rewrite them)
-    if (mode == Mode::Schedule && !call.tk.on && out_dec && !h->cur_sub) {
+    // with restricted requests or admission rows: the kernel hands the decisions to the host before a subset or admission
+    // launch could rewrite them)
+    if (mode == Mode::Schedule && !call.tk.on && out_dec && !h->cur_sub && !h->cur_adm) {
         const uint8_t *data_dev = nullptr;
         const int sm = small_batch_mode(h, v, &data_dev);
         if (sm) return run_small(h, v, sm, data_dev, out_dec, out_detail);
@@ -2366,6 +2520,11 @@ static int32_t upload_subset(epp_engine *h, const std::vector<SubsetRow> &rows, 
 // For the batcher (batcher.cu), which refuses subsets and checks predictions at submit time.  The mask is fixed once the
 // pool is set, and no batch is scheduled before that.
 int32_t engine_latency_mask(const epp_engine *h) { return h->lat_mask; }
+// The admitters (kAdmitProbabilistic | kAdmitLatencySlo), for the batcher's submit-time checks; fixed once the pool is set.
+int32_t engine_admission(const epp_engine *h) {
+    if (!h->adm_on) return 0;
+    return (h->adm.probabilistic ? (int32_t)kAdmitProbabilistic : 0) | (h->adm.latency_slo ? (int32_t)kAdmitLatencySlo : 0);
+}
 
 extern "C" void epp_latency_cfg_default(epp_latency_cfg *cfg) {
     if (!cfg) return;
@@ -2400,7 +2559,8 @@ extern "C" int32_t epp_latency_profile_set(epp_engine *h, int32_t profile, const
 // Validates the predictions of a batch of R requests on the host (*n_ent entries in all).  Nothing of the engine changes.
 static int32_t check_predictions(const epp_engine *h, int64_t R, const epp_predictions *p, uint64_t *n_ent) {
     if (p->struct_size != sizeof(epp_predictions)) return fail(EPP_ERR_INVALID, "epp_predictions.struct_size %u != %zu", p->struct_size, sizeof(epp_predictions));
-    if (!h->lat_mask) return fail(EPP_ERR_INVALID, "predictions passed to an engine without a latency profile");
+    if (!h->lat_mask && !(h->adm_on && h->adm.latency_slo))
+        return fail(EPP_ERR_INVALID, "predictions passed to an engine without a latency profile or the latency-slo-admitter");
     if (R > 0 && !p->counts) return fail(EPP_ERR_INVALID, "epp_predictions.counts is NULL");
     const uint32_t E = (uint32_t)h->cfg.max_endpoints;
     uint64_t total = 0;
@@ -2493,10 +2653,71 @@ static int32_t upload_predictions(epp_engine *h, int64_t R, const epp_prediction
     return EPP_OK;
 }
 
+// Validates a call's admission inputs (R requests; preds: the call's predictions, validated, or nullptr; sub: its
+// restricted rows, ascending) and lists, in ascending request order, the rows an admitter can reject, with the packed
+// entries of the latency-slo-admitter's rows (slot | both validity bits << 31).  Nothing of the engine changes.
+static int32_t check_admission(const epp_engine *h, int64_t R, const epp_admission *a, const epp_predictions *preds,
+                               const std::vector<SubsetRow> &sub, std::vector<AdmitRow> &rows, std::vector<uint32_t> &ent) {
+    if (a->struct_size != sizeof(epp_admission)) return fail(EPP_ERR_INVALID, "epp_admission.struct_size %u != %zu", a->struct_size, sizeof(epp_admission));
+    if (!h->adm_on) return fail(EPP_ERR_INVALID, "admission inputs passed to an engine without admitters (epp_admission_set)");
+    const bool lat = h->adm.latency_slo != 0, with_pred = lat && preds && R > 0;
+    if (with_pred && !a->pred_valid)
+        return fail(EPP_ERR_INVALID, "epp_admission.pred_valid is NULL: the latency-slo-admitter needs it for a call with predictions");
+    if (!a->priority) return EPP_OK;              // nobody is sheddable
+    size_t si = 0;
+    for (int64_t r = 0; r < R; r++) {
+        while (si < sub.size() && (int64_t)sub[si].row < r) si++;
+        if (a->priority[r] >= 0) continue;
+        const bool restricted = si < sub.size() && (int64_t)sub[si].row == r;
+        if (restricted && sub[si].n == 0) continue;    // no candidate: status -1 stands
+        AdmitRow row{(uint32_t)r, 0u, restricted ? sub[si].off : 0ull, restricted ? sub[si].n : EPP_SUBSET_ALL, 0u, 0ull};
+        if (h->adm.probabilistic) row.flags |= kAdmitProbabilistic;
+        const double ttft = a->ttft_slo ? a->ttft_slo[r] : 0.0, tpot = a->tpot_slo ? a->tpot_slo[r] : 0.0;
+        if (with_pred && preds->counts[r] && (ttft > 0 || tpot > 0)) {
+            row.flags |= kAdmitLatencySlo;
+            row.pred_off = ent.size();
+            row.pred_n = preds->counts[r];
+            const uint64_t o = preds->offsets[r];
+            for (uint32_t i = 0; i < row.pred_n; i++)
+                ent.push_back(preds->entries[o + i].slot | ((a->pred_valid[o + i] & 3u) == 3u ? 0x80000000u : 0u));
+        }
+        if (row.flags) rows.push_back(row);
+    }
+    return EPP_OK;
+}
+
+// The listed rows and their entries to the device on stream 0, behind everything enqueued so far (a pipelined batch's
+// stream 1 joins first), through the engine's pinned staging, as upload_subset does.
+static int32_t upload_admission(epp_engine *h, const std::vector<AdmitRow> &rows, const std::vector<uint32_t> &ent) {
+    cudaStream_t s0 = h->slot[0].stream;
+    EPP_TRY(join_streams(h));
+    CUDA_TRY(h->adm_rows.reserve(sizeof(AdmitRow) * rows.size(), &h->dev_bytes));
+    CUDA_TRY(h->adm_ent.reserve(sizeof(uint32_t) * std::max<size_t>(ent.size(), 1), &h->dev_bytes));
+    if (!h->adm_up_ev) CUDA_TRY(cudaEventCreateWithFlags(&h->adm_up_ev, cudaEventDisableTiming));
+    else CUDA_TRY(cudaEventSynchronize(h->adm_up_ev));
+    const size_t rows_bytes = sizeof(AdmitRow) * rows.size();
+    const size_t need = rows_bytes + sizeof(uint32_t) * ent.size();
+    if (need > h->adm_host_cap) {
+        if (h->adm_host) CUDA_TRY(cudaFreeHost(h->adm_host));
+        h->adm_host = nullptr;
+        h->adm_host_cap = 0;
+        CUDA_TRY(cudaHostAlloc(&h->adm_host, need, cudaHostAllocDefault));
+        h->adm_host_cap = need;
+    }
+    uint8_t *stage = static_cast<uint8_t *>(h->adm_host);
+    memcpy(stage, rows.data(), rows_bytes);
+    if (!ent.empty()) memcpy(stage + rows_bytes, ent.data(), sizeof(uint32_t) * ent.size());
+    CUDA_TRY(cudaMemcpyAsync(h->adm_rows.p, stage, rows_bytes, cudaMemcpyHostToDevice, s0));
+    if (!ent.empty())
+        CUDA_TRY(cudaMemcpyAsync(h->adm_ent.p, stage + rows_bytes, sizeof(uint32_t) * ent.size(), cudaMemcpyHostToDevice, s0));
+    CUDA_TRY(cudaEventRecord(h->adm_up_ev, s0));
+    return EPP_OK;
+}
+
 static int32_t schedule_impl(epp_engine *h, const epp_batch *batch, epp_decision *out, epp_decision_detail *detail,
                              int32_t keep_hashes, const epp_topk_out *topk, const epp_subset *subset = nullptr,
                              const epp_predictions *preds = nullptr, bool subset_latency_ok = false,
-                             const epp_context_tokens *ctx = nullptr) {
+                             const epp_context_tokens *ctx = nullptr, const epp_admission *adm = nullptr) {
     if (!h) return fail(EPP_ERR_INVALID, "NULL engine");
     if (!out) return fail(EPP_ERR_INVALID, "out is NULL");
     std::lock_guard<std::mutex> lk(h->mu);
@@ -2511,23 +2732,30 @@ static int32_t schedule_impl(epp_engine *h, const epp_batch *batch, epp_decision
     uint64_t n_ent = 0;
     if (preds) EPP_TRY(check_predictions(h, v.R, preds, &n_ent));
     if (ctx) EPP_TRY(check_ctx(v.R, ctx));
+    std::vector<AdmitRow> adm_rows;
+    std::vector<uint32_t> adm_ent;
+    if (adm) EPP_TRY(check_admission(h, v.R, adm, preds, sub_rows, adm_rows, adm_ent));
     const bool use_ctx = ctx && v.R && h->cl_mask;
-    if (!sub_rows.empty() || (preds && v.R) || use_ctx) {
+    const bool use_pred = preds && v.R && h->lat_mask;     // without a latency profile only the admitter reads them
+    if (!sub_rows.empty() || use_pred || use_ctx || !adm_rows.empty()) {
         if (!h->pool_ready) return fail(EPP_ERR_STATE, "epp_pool_set has not been called");
     }
     if (!sub_rows.empty()) EPP_TRY(upload_subset(h, sub_rows, subset, sub_n_slots));
-    if (preds && v.R) EPP_TRY(upload_predictions(h, v.R, preds, n_ent));
+    if (use_pred) EPP_TRY(upload_predictions(h, v.R, preds, n_ent));
     if (use_ctx) EPP_TRY(upload_ctx(h, v.R, ctx));
+    if (!adm_rows.empty()) EPP_TRY(upload_admission(h, adm_rows, adm_ent));
     h->kept_R = 0;
     h->cur_topk = topk;
     h->cur_sub = sub_rows.empty() ? nullptr : &sub_rows;
-    h->cur_pred = preds && v.R;
+    h->cur_pred = use_pred;
     h->cur_ctx = use_ctx;
+    h->cur_adm = adm_rows.empty() ? nullptr : &adm_rows;
     const int32_t rc = run_batch(h, v, Mode::Schedule, nullptr, nullptr, out, detail, nullptr, nullptr, keep_hashes != 0);
     h->cur_topk = nullptr;
     h->cur_sub = nullptr;
     h->cur_pred = false;
     h->cur_ctx = false;
+    h->cur_adm = nullptr;
     EPP_TRY(rc);
     h->stats.n_batches++;
     h->stats.n_decisions += (uint64_t)v.R;
@@ -2576,6 +2804,12 @@ extern "C" int32_t epp_schedule_ctx(epp_engine *h, const epp_batch *batch, const
                                     const epp_context_tokens *ctx, epp_decision *out, epp_decision_detail *detail,
                                     int32_t keep_hashes, const epp_topk_out *topk) {
     return schedule_impl(h, batch, out, detail, keep_hashes, topk, subset, preds, true, ctx);
+}
+
+extern "C" int32_t epp_schedule_admit(epp_engine *h, const epp_batch *batch, const epp_subset *subset, const epp_predictions *preds,
+                                      const epp_context_tokens *ctx, const epp_admission *adm, epp_decision *out,
+                                      epp_decision_detail *detail, int32_t keep_hashes, const epp_topk_out *topk) {
+    return schedule_impl(h, batch, out, detail, keep_hashes, topk, subset, preds, true, ctx, adm);
 }
 
 // PreRequest: approximateprefix/plugin.go:164-200 (primary target + "prefill" profile target).
@@ -2673,24 +2907,31 @@ extern "C" int32_t epp_score(epp_engine *h, int64_t n_requests, const int32_t *m
 static int32_t with_match_impl(epp_engine *h, int64_t n_requests, const int32_t *match, const int32_t *total,
                                const uint32_t *model_ids, const int64_t *input_len_bytes, int32_t block_size_tokens, epp_decision *out,
                                epp_decision_detail *detail, uint32_t flags, const epp_topk_out *topk,
-                               const epp_predictions *preds = nullptr, const epp_context_tokens *ctx = nullptr) {
+                               const epp_predictions *preds = nullptr, const epp_context_tokens *ctx = nullptr,
+                               const epp_admission *adm = nullptr) {
     if (!h || n_requests < 0 || (n_requests && (!match || !total || !out))) return fail(EPP_ERR_INVALID, "bad arguments");
     std::lock_guard<std::mutex> lk(h->mu);
     if (topk) EPP_TRY(check_topk(h, topk));
     uint64_t n_ent = 0;
     if (preds) EPP_TRY(check_predictions(h, n_requests, preds, &n_ent));
     if (ctx) EPP_TRY(check_ctx(n_requests, ctx));
+    std::vector<AdmitRow> adm_rows;
+    std::vector<uint32_t> adm_ent;
+    if (adm) EPP_TRY(check_admission(h, n_requests, adm, preds, {}, adm_rows, adm_ent));
     EPP_TRY(set_device(h));
     EPP_TRY(join_streams(h));
     if (!h->pool_ready) return fail(EPP_ERR_STATE, "epp_pool_set has not been called");
     if (n_requests == 0) return EPP_OK;
-    if (preds) EPP_TRY(upload_predictions(h, n_requests, preds, n_ent));
+    const bool use_pred = preds && h->lat_mask;    // without a latency profile only the admitter reads them
+    if (use_pred) EPP_TRY(upload_predictions(h, n_requests, preds, n_ent));
     if (ctx && h->cl_mask) EPP_TRY(upload_ctx(h, n_requests, ctx));
-    h->cur_pred = preds != nullptr;
+    if (!adm_rows.empty()) EPP_TRY(upload_admission(h, adm_rows, adm_ent));
+    h->cur_pred = use_pred;
     h->cur_ctx = ctx && h->cl_mask;
-    struct PredReset {                             // the call's predictions and token counts end with it, whichever way it returns
-        epp_engine *h;
-        ~PredReset() { h->cur_pred = false; h->cur_ctx = false; }
+    h->cur_adm = adm_rows.empty() ? nullptr : &adm_rows;
+    struct PredReset {                             // the call's predictions, token counts and admission rows end with it,
+        epp_engine *h;                             // whichever way it returns
+        ~PredReset() { h->cur_pred = false; h->cur_ctx = false; h->cur_adm = nullptr; }
     } pred_reset{h};
     const size_t R = (size_t)n_requests;
     cudaStream_t s = h->slot[0].stream;
@@ -2731,6 +2972,7 @@ static int32_t with_match_impl(epp_engine *h, int64_t n_requests, const int32_t 
     } else {
         CUDA_TRY(launch_dense_pick(p, s, &launches));
     }
+    EPP_TRY(launch_admission(h, 0, n_requests, p.out, p.detail, tk, s, &launches, false));
     EPP_TRY(after_picks(h, p.out, p.detail, p.in_len, n_requests, s, &launches, false));
     if (!dev) {
         CUDA_TRY(cudaMemcpyAsync(out, p.out, sizeof(epp_decision) * R, cudaMemcpyDeviceToHost, s));
@@ -2763,6 +3005,15 @@ extern "C" int32_t epp_schedule_with_match_ctx(epp_engine *h, int64_t n_requests
                                                const epp_context_tokens *ctx) {
     return with_match_impl(h, n_requests, match, total, model_ids, input_len_bytes, block_size_tokens, out, detail, flags, topk,
                            preds, ctx);
+}
+
+extern "C" int32_t epp_schedule_with_match_admit(epp_engine *h, int64_t n_requests, const int32_t *match, const int32_t *total,
+                                                 const uint32_t *model_ids, const int64_t *input_len_bytes,
+                                                 int32_t block_size_tokens, epp_decision *out, epp_decision_detail *detail,
+                                                 uint32_t flags, const epp_topk_out *topk, const epp_predictions *preds,
+                                                 const epp_context_tokens *ctx, const epp_admission *adm) {
+    return with_match_impl(h, n_requests, match, total, model_ids, input_len_bytes, block_size_tokens, out, detail, flags, topk,
+                           preds, ctx, adm);
 }
 
 extern "C" int32_t epp_schedule_with_match_topk(epp_engine *h, int64_t n_requests, const int32_t *match, const int32_t *total,
@@ -2906,6 +3157,7 @@ static int32_t check_shardable(const epp_engine *h) {
     if (h->nohit_mask) return fail(EPP_ERR_INVALID, "endpoint-sharded mode does not support the no-hit-lru scorer (coldness needs every rank's match)");
     if (any_random_picker(h)) return fail(EPP_ERR_INVALID, "endpoint-sharded mode does not support the random pickers (a weighted draw needs every rank's scores)");
     if (h->inflight) return fail(EPP_ERR_INVALID, "endpoint-sharded mode does not support the inflight-load producer");
+    if (h->adm_on) return fail(EPP_ERR_INVALID, "endpoint-sharded mode does not support the admitters");
     return EPP_OK;
 }
 

@@ -382,6 +382,41 @@ struct SubsetView {
     const int32_t *nohit_pos;  // [E] position in the no-hit-lru LRU (oldest 0, -1 = never used), or nullptr
 };
 cudaError_t launch_subset_pick(const PickParams &p, const SubsetView &sv, const LatView *lv, cudaStream_t s, int *launches);
+
+// ------------------------------------------------------------------------------------------------
+// admission (admit.cu, include/epp_engine.h "Admission"): k_admit rewrites the rows an admitter rejects, one warp per
+// listed row, behind the call's picks and before its after-pick updates.
+// ------------------------------------------------------------------------------------------------
+constexpr uint32_t kAdmitProbabilistic = 1u, kAdmitLatencySlo = 2u;
+struct AdmitRow {
+    uint32_t row;              // absolute request index in the call
+    uint32_t flags;            // kAdmitProbabilistic: sheddable; kAdmitLatencySlo: sheddable with an SLO and entries
+    uint64_t sub_off;          // subset slots sub_slots[sub_off .. + sub_n), ascending
+    uint32_t sub_n;            // EPP_SUBSET_ALL: the whole pool
+    uint32_t pred_n;           // entries ent[pred_off .. + pred_n)
+    uint64_t pred_off;
+};
+struct AdmitParams {
+    const AdmitRow *rows;      // [n_rows] ascending by row
+    int32_t n_rows;
+    int32_t E;
+    const uint32_t *ent;       // slot | (both validity bits set) << 31
+    const uint32_t *sub_slots;
+    const uint8_t *role;       // the pool snapshot (PoolArrays)
+    const double *kv;
+    const int32_t *waiting, *running;
+    int32_t pool_n, pool_idle, pool_cold;   // the whole pool's candidates, idle and cold flags, saturation fold
+    double pool_sat;
+    double qdt, kvt, power, k;
+    uint64_t tie_seed, ord_base;            // ordinal of row r = ord_base + r
+    epp_decision *dec;                      // [R] of the call
+    epp_decision_detail *det;               // [R] or nullptr
+    int32_t topk;                           // row stride of the lists (0 = none)
+    uint32_t *topk_picks[kMaxProfiles];
+    double *topk_scores;
+};
+cudaError_t launch_admit(const AdmitParams &p, cudaStream_t s, int *launches);
+
 // Scorer.Score parity: out[R][E].  scorer_index -1 => weighted ordered sum (-1.0 for non-candidates).
 // cold != nullptr (the profile has a no-hit-lru scorer): cold[r] selects prof_cold and the raw cold column nohit_col
 // for request r.

@@ -169,6 +169,46 @@ def _context_struct(context_tokens, R):
     return ct, arr
 
 
+def _admission_struct(admission, R, predictions=None):
+    """epp_admission for R requests -> (struct, the arrays it points to: keep them alive through the call).
+    admission: a dict with any of "priority" (R ints, < 0 = sheddable), "ttft_slo" / "tpot_slo" (R doubles, the parsed
+    x-slo-ttft-ms / x-slo-tpot-ms headers) and "pred_valid" (R entries, each None or one validity byte -- bit 0 TTFTValid,
+    bit 1 TPOTValid -- per entry of that request's predictions, in the order given to pack_predictions, which sorts both
+    alike)."""
+    keep = []
+    a = capi.Admission()
+    a.struct_size = C.sizeof(capi.Admission)
+    for name, dt in (("priority", np.int32), ("ttft_slo", np.float64), ("tpot_slo", np.float64)):
+        if admission.get(name) is None:
+            continue
+        arr = np.ascontiguousarray(np.asarray(admission[name], dtype=dt).reshape(-1))
+        if arr.shape[0] != R:
+            raise ValueError(f"admission {name} has {arr.shape[0]} entries for {R} requests")
+        keep.append(arr)
+        setattr(a, name, arr.ctypes.data if R else None)
+    pv = admission.get("pred_valid")
+    if pv is not None:
+        if len(pv) != R:
+            raise ValueError(f"admission pred_valid has {len(pv)} entries for {R} requests")
+        parts = []
+        for r, v in enumerate(pv):
+            p = None if predictions is None else predictions[r]
+            n = 0 if p is None else len(p)
+            v = np.zeros(0, dtype=np.uint8) if v is None else np.asarray(v, dtype=np.uint8).reshape(-1)
+            if v.shape[0] != n:
+                raise ValueError(f"request {r}: {v.shape[0]} validity bytes for {n} predictions")
+            if n:
+                slots = p["slot"] if isinstance(p, np.ndarray) and p.dtype == PREDICTION_DTYPE else [int(e[0]) for e in p]
+                v = v[np.argsort(np.asarray(slots, dtype=np.int64), kind="stable")]
+            parts.append(v)
+        arr = np.ascontiguousarray(np.concatenate(parts) if parts else np.zeros(0, dtype=np.uint8))
+        if arr.shape[0] == 0:
+            arr = np.zeros(1, dtype=np.uint8)          # a valid pointer for a call whose requests have no entries
+        keep.append(arr)
+        a.pred_valid = arr.ctypes.data
+    return a, keep
+
+
 def _prediction_entries(predictions):
     """One request's predictions (a PREDICTION_DTYPE array, or (slot, ttft, ttft_headroom, tpot_headroom, dispatched)
     tuples) as a contiguous PREDICTION_DTYPE array."""
@@ -475,6 +515,22 @@ class Engine:
             setattr(cfg, k, v)
         self._check(self._lib.epp_latency_profile_set(self._h, profile, C.byref(cfg)))
 
+    def admission_set(self, latency_slo: bool = False, probabilistic: bool = False, **fields):
+        """The engine's admitters (include/epp_engine.h "Admission"): the latency-slo-admitter and / or the
+        probabilistic-admitter with the epp_admission_cfg fields given as keywords (queue_depth_threshold,
+        kv_cache_util_threshold, power, k), the others at the reference's defaults.  Only before the first pool_set /
+        pool_set_labels."""
+        cfg = capi.AdmissionCfg()
+        self._lib.epp_admission_cfg_default(C.byref(cfg))
+        cfg.latency_slo = int(latency_slo)
+        cfg.probabilistic = int(probabilistic)
+        names = {n for n, _ in capi.AdmissionCfg._fields_} - {"struct_size", "latency_slo", "probabilistic"}
+        for k, v in fields.items():
+            if k not in names:
+                raise TypeError(f"unknown admission configuration field {k!r}")
+            setattr(cfg, k, v)
+        self._check(self._lib.epp_admission_set(self._h, C.byref(cfg)))
+
     def context_length_set(self, profile: int, label: str | None = None, enable_filtering: bool = False):
         """The context-length-aware plugin of profile 0 (primary / decode), 1 (prefill) or 2 (encode): its range label key
         (None = capi.CONTEXT_LENGTH_LABEL) and whether it also filters (include/epp_engine.h "Context length")."""
@@ -483,7 +539,7 @@ class Engine:
 
     def schedule(self, data, offsets=None, uniform_len=None, model_ids=None, n_requests=None, keep_hashes=False,
                  detail=True, out=None, lengths=None, asynchronous=False, multimodal=None, topk=False, subsets=None,
-                 predictions=None, context_tokens=None):
+                 predictions=None, context_tokens=None, admission=None):
         """a1-a14 Scheduler.Schedule for a batch -> (decisions, details).  asynchronous=True (CUDA tensors only)
         enqueues the batch and returns; the outputs are complete after synchronize().  topk=True (engines created with
         pick_k > 1) also returns the dict of the pickers' first-k lists (maxscore/picker.go:104-115): "primary",
@@ -494,7 +550,10 @@ class Engine:
         predictions"); epp_schedule_predicted.  Both together: epp_schedule_subset_predicted (a latency engine's
         restricted requests decided with their predictions).
         context_tokens: None, or R request context lengths (-1 = the default from the prompt length, include/epp_engine.h
-        "Context length"); with it every call goes through epp_schedule_ctx."""
+        "Context length"); with it every call goes through epp_schedule_ctx.
+        admission: None, or the requests' admission inputs as _admission_struct takes them (include/epp_engine.h
+        "Admission", engines with admission_set); with it the call goes through epp_schedule_admit and rejected requests
+        come back with status capi.EPP_STATUS_REJECTED."""
         b, R, dev, keep = self._batch(data, offsets, uniform_len, model_ids, n_requests, lengths, multimodal)
         if asynchronous:
             b.flags |= capi.EPP_BATCH_ASYNC
@@ -518,7 +577,14 @@ class Engine:
             sub = capi.Subset()
             sub.struct_size = C.sizeof(capi.Subset)
             sub.counts, sub.offsets, sub.slots = (_ptr(a) for a in spacked)
-        if context_tokens is not None:
+        if admission is not None:
+            ad, ad_keep = _admission_struct(admission, R, predictions)
+            ct, ctx_arr = _context_struct(context_tokens, R) if context_tokens is not None else (None, None)
+            self._check(self._lib.epp_schedule_admit(self._h, C.byref(b), C.byref(sub) if subsets is not None else None,
+                                                     C.byref(pr) if predictions is not None else None,
+                                                     C.byref(ct) if ct is not None else None, C.byref(ad), _ptr(dec),
+                                                     _ptr(det), int(keep_hashes), C.byref(tk) if topk else None))
+        elif context_tokens is not None:
             ct, ctx_arr = _context_struct(context_tokens, R)
             self._check(self._lib.epp_schedule_ctx(self._h, C.byref(b), C.byref(sub) if subsets is not None else None,
                                                    C.byref(pr) if predictions is not None else None, C.byref(ct), _ptr(dec),
@@ -557,7 +623,7 @@ class Engine:
         return lists, tk
 
     def schedule_with_match(self, match, total, input_len_bytes=None, block_size_tokens: int = 0, model_ids=None,
-                            topk=False, predictions=None, context_tokens=None):
+                            topk=False, predictions=None, context_tokens=None, admission=None):
         match = np.ascontiguousarray(match, dtype=np.int32).reshape(-1, self.E)
         total = np.ascontiguousarray(total, dtype=np.int32)
         R = match.shape[0]
@@ -565,6 +631,19 @@ class Engine:
         dec = np.zeros(R, dtype=DECISION_DTYPE)
         det = np.zeros(R, dtype=DETAIL_DTYPE)
         mids = None if model_ids is None else np.ascontiguousarray(model_ids, dtype=np.uint32)
+        if admission is not None:
+            ad, ad_keep = _admission_struct(admission, R, predictions)
+            ct, ctx_arr = _context_struct(context_tokens, R) if context_tokens is not None else (None, None)
+            if predictions is not None and len(predictions) != R:
+                raise ValueError(f"predictions has {len(predictions)} entries for {R} requests")
+            packed = pack_predictions(predictions) if predictions is not None else None
+            pr = _predictions_struct(packed) if packed is not None else None
+            lists, tk = self._topk_out(R) if topk else (None, None)
+            self._check(self._lib.epp_schedule_with_match_admit(
+                self._h, R, _ptr(match), _ptr(total), _ptr(mids), _ptr(il), block_size_tokens, _ptr(dec), _ptr(det), 0,
+                C.byref(tk) if topk else None, C.byref(pr) if pr is not None else None,
+                C.byref(ct) if ct is not None else None, C.byref(ad)))
+            return (dec, det, lists) if topk else (dec, det)
         if context_tokens is not None:
             ct, ctx_arr = _context_struct(context_tokens, R)
             if predictions is not None and len(predictions) != R:
@@ -688,15 +767,33 @@ class Batcher:
             raise EngineError(rc, (self._lib.epp_batcher_last_error() or b"").decode())
 
     def submit(self, prompt, model_id: int = 0, multimodal: bool = False, subset=None, predictions=None,
-               context_tokens=None) -> int:
+               context_tokens=None, admission=None) -> int:
         """subset: None (the whole pool) or a sequence of slot ids, the request's candidates (epp_submit_subset).
         predictions: None or the request's entries in the form pack_predictions takes (epp_submit_predicted).  Both
         together: epp_submit_subset_predicted.  context_tokens: None, or the request's context length (-1 = the default);
-        with it the request goes through epp_submit_ctx with whatever else it carries."""
+        with it the request goes through epp_submit_ctx with whatever else it carries.  admission: None, or a dict with
+        the request's "priority", "ttft_slo", "tpot_slo" and "pred_valid" (one byte per prediction, in the order given);
+        with it the request goes through epp_submit_admit with whatever else it carries."""
         buf = np.ascontiguousarray(prompt).view(np.uint8).reshape(-1) if not isinstance(prompt, (bytes, bytearray)) else prompt
         n = len(buf)
         ptr = buf.ctypes.data_as(C.c_void_p) if isinstance(buf, np.ndarray) else C.cast(C.c_char_p(bytes(buf)), C.c_void_p)
         t = C.c_uint64()
+        if admission is not None:
+            ent = _prediction_entries(predictions) if predictions is not None else np.zeros(0, dtype=PREDICTION_DTYPE)
+            pv = admission.get("pred_valid")
+            pv = None if pv is None else np.ascontiguousarray(np.asarray(pv, dtype=np.uint8).reshape(-1))
+            if pv is not None and pv.shape[0] != ent.shape[0]:
+                raise ValueError(f"{pv.shape[0]} validity bytes for {ent.shape[0]} predictions")
+            sl = None if subset is None else np.ascontiguousarray(np.asarray(subset, dtype=np.uint32).reshape(-1))
+            if sl is not None and sl.shape[0] == 0:
+                sl = np.zeros(1, dtype=np.uint32)[:0]
+            self._check(self._lib.epp_submit_admit(
+                self._b, model_id, ptr, n, int(multimodal), 0 if sl is None else sl.shape[0],
+                None if sl is None else sl.ctypes.data_as(C.c_void_p), ent.shape[0], _ptr(ent),
+                None if pv is None else pv.ctypes.data_as(C.c_void_p),
+                -1 if context_tokens is None else int(context_tokens), int(admission.get("priority", 0)),
+                float(admission.get("ttft_slo", 0.0)), float(admission.get("tpot_slo", 0.0)), C.byref(t)))
+            return t.value
         if context_tokens is not None:
             ent = _prediction_entries(predictions) if predictions is not None else np.zeros(0, dtype=PREDICTION_DTYPE)
             sl = None if subset is None else np.ascontiguousarray(np.asarray(subset, dtype=np.uint32).reshape(-1))

@@ -20,6 +20,7 @@ Reference interfaces mirrored (paths relative to the reference root):
 from __future__ import annotations
 
 import json
+import math
 import re
 from dataclasses import dataclass, field
 
@@ -500,6 +501,151 @@ def ContextLengthAwareFactory(name: str, rawParameters=None):
     return NewContextLengthAware(name, params["label"], params["enablefiltering"])
 
 
+# ---- strconv.ParseFloat, as parseFloatHeaderValue (latencyslo/plugin.go:150-158) uses it --------------------------------------------------------------
+def _underscore_ok(s: str) -> bool:
+    saw, i = "^", 0
+    if s[:1] in ("+", "-"):
+        s = s[1:]
+    hexa = False
+    if len(s) >= 2 and s[0] == "0" and s[1].lower() in "box":
+        i, saw, hexa = 2, "0", s[1].lower() == "x"
+    while i < len(s):
+        c = s[i]
+        if "0" <= c <= "9" or (hexa and "a" <= c.lower() <= "f"):
+            saw = "0"
+        elif c == "_":
+            if saw != "0":
+                return False
+            saw = "_"
+        else:
+            if saw == "_":
+                return False
+            saw = "!"
+        i += 1
+    return saw != "_"
+
+
+_DEC = re.compile(r"[+-]?([0-9_]*)(\.[0-9_]*)?([eE][+-]?[0-9_]+)?\Z")
+_HEX = re.compile(r"[+-]?0[xX]([0-9a-fA-F_]*)(\.[0-9a-fA-F_]*)?[pP][+-]?[0-9_]+\Z")
+
+
+def ParseFloat(s: str):
+    """strconv.ParseFloat(s, 64) -> (value, ok): ok is False for a syntax or range error."""
+    if not s:
+        return 0.0, False
+    m = re.fullmatch(r"([+-]?)(inf|infinity|nan)", s, flags=re.IGNORECASE)
+    if m:
+        if m.group(2).lower() == "nan":
+            return (math.nan, True) if not m.group(1) else (0.0, False)
+        return (-math.inf if m.group(1) == "-" else math.inf), True
+    hexa = _HEX.match(s)
+    dec = None if hexa else _DEC.match(s)
+    mm = hexa or dec
+    if not mm:
+        return 0.0, False
+    mant = (mm.group(1) or "") + (mm.group(2) or "").lstrip(".")
+    if not any(c != "_" for c in mant):
+        return 0.0, False                          # no mantissa digit
+    if "_" in s and not _underscore_ok(s):
+        return 0.0, False
+    t = s.replace("_", "")
+    try:
+        v = float.fromhex(t) if hexa else float(t)
+    except OverflowError:
+        return 0.0, False
+    if math.isinf(v):
+        return v, False                            # ErrRange
+    return v, True
+
+
+def parseFloatHeaderValue(s: str) -> float:
+    """parseFloatHeaderValue (latencyslo/plugin.go:150-158): 0 when absent, unparsable or out of range."""
+    v, ok = ParseFloat(s or "")
+    return v if ok else 0.0
+
+
+LatencyAdmissionPluginType = "latency-slo-admitter"
+ProbabilisticAdmitterType = "probabilistic-admitter"
+
+
+class AdmissionError(SchedulingError):
+    """A request an admitter rejected (status capi.EPP_STATUS_REJECTED): the director answers it with "request cannot be
+    admitted" (requestcontrol/director.go:238-240) and never schedules it."""
+
+
+@dataclass
+class LatencyAdmission:                          # requestcontrol/admitter/latencyslo; LatencyAdmissionConfig has no fields
+    name: str = LatencyAdmissionPluginType
+
+
+def NewLatencyAdmission(name: str = LatencyAdmissionPluginType) -> LatencyAdmission:
+    return LatencyAdmission(name)
+
+
+def LatencyAdmissionFactory(name: str, rawParameters=None) -> LatencyAdmission:
+    try:
+        _unmarshal(rawParameters, {}, "latencyslo.LatencyAdmissionConfig")
+    except ValueError as e:
+        raise ValueError(f"failed to unmarshal config for LatencyAdmission: {e}") from e
+    return NewLatencyAdmission(name)
+
+
+@dataclass
+class ProbabilisticAdmitter:                     # requestcontrol/admitter/probabilisticadmitter; defaults :37-42
+    queueDepthThreshold: int = 5
+    kvCacheUtilThreshold: float = 0.8
+    power: float = 5.0
+    k: float = 300.0
+    name: str = ProbabilisticAdmitterType
+
+
+def ProbabilisticAdmitterFactory(name: str, rawParameters=None) -> ProbabilisticAdmitter:
+    """probabilisticadmitter.Factory: json.Unmarshal over the defaults, then the four range checks (plugin.go:71-84)."""
+    t = ProbabilisticAdmitterType
+    p = ProbabilisticAdmitter(name=name)
+    try:
+        got = _unmarshal(rawParameters, {"queueDepthThreshold": float, "kvCacheUtilThreshold": float, "power": float,
+                                         "k": float}, "probabilisticadmitter.Parameters")
+    except ValueError as e:
+        raise ValueError(f"failed to parse parameters for '{t}' plugin: {e}") from e
+    if "queueDepthThreshold" in got:
+        q = got.pop("queueDepthThreshold")
+        if q != int(q) or not -2 ** 63 <= q < 2 ** 63:
+            raise ValueError(f"failed to parse parameters for '{t}' plugin: json: cannot unmarshal number {q} into Go "
+                             f"struct field Parameters.queueDepthThreshold of type int")
+        p.queueDepthThreshold = int(q)
+    for k, v in got.items():
+        setattr(p, k, v)
+    if p.queueDepthThreshold <= 0:
+        raise ValueError(f"plugin '{t}': queueDepthThreshold must be > 0, got {p.queueDepthThreshold}")
+    if p.kvCacheUtilThreshold <= 0.0:
+        raise ValueError(f"plugin '{t}': kvCacheUtilThreshold must be > 0, got {p.kvCacheUtilThreshold:g}")
+    if p.power <= 0:
+        raise ValueError(f"plugin '{t}': power must be > 0, got {p.power:g}")
+    if p.k <= 0:
+        raise ValueError(f"plugin '{t}': k must be > 0, got {p.k:g}")
+    return p
+
+
+Factory = ProbabilisticAdmitterFactory           # the reference's name for the probabilistic-admitter's factory
+
+
+def admission_fields(admitters) -> dict:
+    """Engine.admission_set keywords for a list of admitter instances."""
+    out = dict(latency_slo=False, probabilistic=False)
+    for a in admitters:
+        if isinstance(a, LatencyAdmission):
+            out["latency_slo"] = True
+        elif isinstance(a, ProbabilisticAdmitter):
+            if out["probabilistic"]:
+                raise ValueError("the engine runs one probabilistic-admitter")
+            out.update(probabilistic=True, queue_depth_threshold=a.queueDepthThreshold,
+                       kv_cache_util_threshold=a.kvCacheUtilThreshold, power=a.power, k=a.k)
+        else:
+            raise TypeError(f"not an admitter: {a!r}")
+    return out
+
+
 def _context_length_of(plugin):
     """The context-length instance of a filter-list entry or WeightedScorer, or None."""
     inner = plugin.scorer if isinstance(plugin, WeightedScorer) else plugin
@@ -707,6 +853,11 @@ class SchedulingResult:
 
 
 @dataclass
+class RequestObjectives:
+    Priority: int = 0
+
+
+@dataclass
 class InferenceRequest:
     RequestID: str = ""
     TargetModel: str = ""
@@ -714,6 +865,8 @@ class InferenceRequest:
     CacheSalt: str = ""
     SchedulingResult: object = None              # set by the caller after Schedule (read by ResponseBody processors)
     TokenizedPrompt: list | None = None          # Body.TokenizedPrompt.TokenIDs, or None (no token producer)
+    Objectives: "RequestObjectives" = None       # Objectives.Priority (< 0 = sheddable); None = priority 0
+    Headers: dict = field(default_factory=dict)  # request headers (the admitters read x-slo-ttft-ms / x-slo-tpot-ms)
 
 
 class Scheduler:
@@ -725,9 +878,10 @@ class Scheduler:
 
     def __init__(self, profileHandler, profiles: dict, *, max_endpoints: int = 64, block_size_tokens: int = 16,
                  max_prefix_blocks: int = 256, ext_columns: int = 0, device: int = 0, tie_seed: int = 0,
-                 inflight_load: bool = False):
+                 inflight_load: bool = False, admitters=()):
         """inflight_load: the engine runs the inflight-load producer's counters (InFlightLoadProducer) and the token-load /
-        active-request scorers read them."""
+        active-request scorers read them.  admitters: LatencyAdmission / ProbabilisticAdmitter instances the engine runs
+        before its picks take effect (include/epp_engine.h "Admission"); a rejected request raises AdmissionError."""
         self.handler = profileHandler
         self.profiles = profiles
         if isinstance(profileHandler, DisaggProfileHandler):
@@ -754,6 +908,9 @@ class Scheduler:
         self.has_context_length = any(p.spec().context_length is not None for p in profiles.values())
         self.has_labels = any(p.spec().labels for p in profiles.values()) or self.has_context_length
         self.has_latency = any(p.spec().latency is not None for p in profiles.values())
+        self.admission = admission_fields(admitters) if admitters else None
+        if self.admission:
+            self.engine.admission_set(**self.admission)
 
     def _push_pool(self, endpoints, ext=None):
         n = len(endpoints)
@@ -789,26 +946,39 @@ class Scheduler:
             if single:
                 predictions = [predictions]
             assert len(predictions) == len(reqs), "one predictions entry per request"
-            preds = [None if p is None else [info.entry(i) for i, info in sorted(p.items())] for p in predictions]
-        elif self.has_latency:
+            infos = [None if p is None else sorted(p.items()) for p in predictions]
+        elif self.has_latency or (self.admission and self.admission["latency_slo"]):
             attrs = [(i, ep.Get(LatencyPredictionInfoKey)) for i, ep in enumerate(eps)]
-            row = [info.entry(i) for i, (info, ok) in attrs if ok and info is not None]
-            preds = [row] * len(reqs)
-        if preds is not None and not self.has_latency:
+            infos = [[(i, info) for i, (info, ok) in attrs if ok and info is not None]] * len(reqs)
+        else:
+            infos = None
+        preds = None if infos is None else [None if p is None else [info.entry(i) for i, info in p] for p in infos]
+        if preds is not None and not self.has_latency and not (self.admission and self.admission["latency_slo"]):
             raise SchedulingError("latency predictions need a profile with a latency-scorer or slo-headroom-tier-filter")
+        admission = None
+        if self.admission:
+            admission = dict(priority=[r.Objectives.Priority if r.Objectives else 0 for r in reqs],
+                             ttft_slo=[parseFloatHeaderValue(r.Headers.get("x-slo-ttft-ms", "")) for r in reqs],
+                             tpot_slo=[parseFloatHeaderValue(r.Headers.get("x-slo-tpot-ms", "")) for r in reqs])
+            if infos is not None:
+                admission["pred_valid"] = [None if p is None else [int(info.TTFTValid()) | int(info.TPOTValid()) << 1
+                                                                   for _, info in p] for p in infos]
         # getContextLength: the token count, else the engine's default int(float64(len(prompt)) * 0.25) (-1)
         ctx = np.array([len(r.TokenizedPrompt) if r.TokenizedPrompt else -1 for r in reqs], dtype=np.int64) \
             if self.has_context_length else None
         if self.pick_k > 1:
             dec, det, lists = self.engine.schedule_with_match(match, total, in_len, bst, topk=True, predictions=preds,
-                                                              context_tokens=ctx)
+                                                              context_tokens=ctx, admission=admission)
         else:
-            dec, det = self.engine.schedule_with_match(match, total, in_len, bst, predictions=preds, context_tokens=ctx)
+            dec, det = self.engine.schedule_with_match(match, total, in_len, bst, predictions=preds, context_tokens=ctx,
+                                                       admission=admission)
             lists = {"primary": dec["pick"].reshape(-1, 1), "prefill": dec["prefill_pick"].reshape(-1, 1)}
         out = [self._result(dec[i], det[i], eps, lists["primary"][i], lists["prefill"][i]) for i in range(len(reqs))]
         return out[0] if single else out
 
     def _result(self, d, dd, eps, primary, prefill):
+        if d["status"] == capi.EPP_STATUS_REJECTED:
+            raise AdmissionError("request cannot be admitted")
         if d["status"] != 0:
             raise SchedulingError("failed to find available decode workers" if self.prefill_name
                                   else "no endpoints available for the given request")
