@@ -166,7 +166,8 @@ def profile_decide(orc, filter_kind, scorers, picker, role, kv, waiting, running
     if picker and final:
         weights = [s[1] for s in scorers]
         score = {e: float(allsc[e]) for e in final}
-        drawn = pm.draw_k(picker, final, None, score, set(final), seed, key, weights, k, gaps=False)
+        # candidates in ascending slot order, as tools/latency_model.py draws them
+        drawn = pm.draw_k(picker, sorted(final), None, score, set(final), seed, key, weights, k, gaps=False)
         picks = [p for p, _ in drawn]
         pscores = [s for _, s in drawn]
         ties = len(final)

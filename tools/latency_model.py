@@ -277,7 +277,9 @@ def profile_decide(orc, filter_kind, scorers, picker, role, kv, waiting, running
     if picker and final:
         weights = [s[1] for s in scorers]
         score = {e: float(allsc[e]) for e in final}
-        drawn = pm.draw_k(picker, final, None, score, set(final), seed, key, weights, k, gaps=False)
+        # the draws rank the candidates in ascending slot order; the tier filter's negative side lists the endpoints
+        # without a prediction last, so the chain's order is not that order
+        drawn = pm.draw_k(picker, sorted(final), None, score, set(final), seed, key, weights, k, gaps=False)
         picks = [p for p, _ in drawn]
         pscores = [s for _, s in drawn]
         ties = len(final)
