@@ -57,7 +57,8 @@
  *       decode, 1 prefill, 2 encode): uniform over the set like the reference, reproducible by the oracle
  *       (oracle/epp_oracle.c: orc_tie_rank).  Without it every tied request of a batch (cold prompts on a balanced
  *       pool) would land on the same endpoint.  The P/D decider reads the match count of the member picked, as the
- *       reference does (disagg_profile_handler.go:300).  Endpoint-sharded mode always uses the lowest slot.
+ *       reference does (disagg_profile_handler.go:300).  Endpoint-sharded mode uses the lowest slot unless it was set
+ *       with epp_shard_set_seeded (see "Seeded ties").
  *
  * Top-k (epp_config.pick_k > 1, epp_schedule_topk): maxscore/picker.go:91-110 shuffles, stable-sorts by score descending
  * and keeps the first k, i.e. the endpoints come out group by group in descending score order and every group of equal
@@ -869,6 +870,36 @@ EPP_API int32_t epp_shard_schedule_p2p_detail(epp_engine *h, const epp_batch *ba
                                               epp_decision_detail *out_detail);
 EPP_API int32_t epp_shard_p2p_phase_detail(epp_engine *h, const epp_batch *batch, epp_decision *out,
                                            epp_decision_detail *out_detail, int32_t phase);
+
+/* Seeded ties: the tie rule of epp_config.tie_seed != 0 (see "Tie rule") in the endpoint-sharded mode, with a third
+ * exchange.  epp_shard_set_seeded does what epp_shard_set_staged does (same *out_stages) and selects the seeded rule; it
+ * is EPP_ERR_INVALID when tie_seed == 0 and for every configuration epp_shard_set_staged refuses.  A later epp_shard_set
+ * or epp_shard_set_staged returns the engine to the lowest-slot rule.
+ * Phase 2 is unchanged: each record holds this rank's max, its lowest tied slot and its local tie count.  For request r
+ * and stage st every rank then computes from the gathered records the global max, N = the sum of the tied counts and
+ * rho = tie_rank(tie_seed, 4 * (n_decisions + r) + st, N).  The shard ranges are disjoint, so the arg-max set in
+ * ascending slot order is the ranks' local sets taken in the order of their records' picks; that order gives the OWNER
+ * rank of member rho and its rank in the owner's local set.  The owner selects that member (its match kernel again, the
+ * rank forced) and publishes {pick, match_blocks}; every other rank publishes EPP_NO_ENDPOINT for that entry.  The
+ * decisions are then built from the selected members, the P/D decider reading the seeded decode member's match_blocks,
+ * and are bit for bit those of an unsharded engine with the same tie_seed and ordinal.
+ * Host-driven exchanges: probe -> OR of the masks -> epp_shard_pick -> all-gather of the records -> epp_shard_select
+ * (writes this rank's [R][S] entries to out_sel) -> all-gather of the entries -> epp_shard_finish (the decisions; it
+ * advances epp_stats.n_decisions by R, the ordinal of the next batch).  epp_shard_merge(_detail) is EPP_ERR_STATE on a
+ * seeded engine.  all_best and all_sel are stacked in the same rank order.
+ * Peer memory: epp_shard_set_seeded must come before epp_shard_p2p_export, which then also sizes the entries (an export
+ * made for the other rule is EPP_ERR_STATE for both set calls).  A batch is four phases: 0 and 1 as above; 2 waits for
+ * the records, resolves, selects and raises flag 3; 3 waits for flag 3, gathers the entries and writes the decisions.
+ * epp_shard_p2p_phase(_detail) takes phase 0..3 on a seeded engine (0..2 otherwise: 3 is EPP_ERR_INVALID). */
+typedef struct {
+    uint32_t pick;             /* the selected member, EPP_NO_ENDPOINT on the ranks that do not own the entry */
+    int32_t match_blocks;      /* its match count */
+} epp_shard_sel;               /* 8 bytes */
+EPP_API int32_t epp_shard_set_seeded(epp_engine *h, uint32_t ep_begin, uint32_t ep_end, int32_t *out_stages);
+EPP_API int32_t epp_shard_select(epp_engine *h, int64_t n_requests, int32_t n_ranks, const epp_shard_best *all_best,
+                                 epp_shard_sel *out_sel);
+EPP_API int32_t epp_shard_finish(epp_engine *h, int64_t n_requests, int32_t n_ranks, const epp_shard_best *all_best,
+                                 const epp_shard_sel *all_sel, epp_decision *out, epp_decision_detail *out_detail);
 
 /* The configuration the engine was created with. */
 EPP_API int32_t epp_get_config(epp_engine *h, epp_config *out);

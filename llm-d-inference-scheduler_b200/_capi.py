@@ -238,6 +238,9 @@ SIGNATURES = {
     "epp_shard_merge_detail": (C.c_int32, [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "epp_shard_schedule_p2p_detail": (C.c_int32, [C.c_void_p, C.POINTER(Batch), C.c_void_p, C.c_void_p]),
     "epp_shard_p2p_phase_detail": (C.c_int32, [C.c_void_p, C.POINTER(Batch), C.c_void_p, C.c_void_p, C.c_int32]),
+    "epp_shard_set_seeded": (C.c_int32, [C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(C.c_int32)]),
+    "epp_shard_select": (C.c_int32, [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p]),
+    "epp_shard_finish": (C.c_int32, [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "epp_get_config": (C.c_int32, [C.c_void_p, C.POINTER(Config)]),
     "epp_batcher_create": (C.c_int32, [C.c_void_p, C.POINTER(BatcherCfg), C.POINTER(C.c_void_p)]),
     "epp_batcher_destroy": (C.c_int32, [C.c_void_p]),

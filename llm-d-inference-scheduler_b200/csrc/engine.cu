@@ -252,15 +252,21 @@ struct epp_engine {
     bool shard_models = false;      // the probed batch had model ids: its copy in `model_ids` feeds epp_shard_pick
     bool shard_mm = false;          // the probed batch had multimodal flags: its copy in `multimodal` feeds pick and merge
     int32_t shard_stages = 1;       // records per request of the sharded protocol (epp_shard_set_staged)
+    bool shard_seeded = false;      // the seeded tie rule (epp_shard_set_seeded): resolve, select, finish
+    bool shard_picked = false;      // epp_shard_pick ran on the probed batch: its global masks are in sel_gmasks
+    DevBuf sel_gmasks;              // seeded host-driven exchanges: the OR of the masks, kept for epp_shard_select
+    DevBuf sel_work, sel_dense;     // seeded: [R][S] work items of k_shard_resolve and the dense-select list (slot counters
+                                    // overflow_n[2] and [3])
     // endpoint-sharded mode over NVLink peer memory (shard_p2p.cu)
     void *p2p_buf = nullptr;        // this rank's exchange buffer {flags, masks, records} (cudaMalloc, IPC-exported)
-    size_t p2p_bytes = 0, p2p_masks_off = 0, p2p_best_off = 0;
+    size_t p2p_bytes = 0, p2p_masks_off = 0, p2p_best_off = 0, p2p_sel_off = 0;
+    bool p2p_seeded = false;        // the buffer was exported for the seeded tie rule (it holds the selected entries)
     int64_t p2p_R = 0;              // requests the buffer was sized for
     int32_t p2p_stages = 1;         // records per request the buffer was sized for
     int p2p_ranks = 0, p2p_rank = 0;
     bool p2p_ipc = false;
     std::vector<void *> p2p_peer;   // peers' buffers in this process's address space (own buffer at [p2p_rank])
-    DevBuf p2p_peer_dev, p2p_gmasks, p2p_allbest, p2p_err;
+    DevBuf p2p_peer_dev, p2p_gmasks, p2p_allbest, p2p_allsel, p2p_err;
     unsigned long long p2p_epoch = 0;
     uint64_t p2p_or_bits = 0;       // offsets alignment of the batch being stepped through epp_shard_p2p_phase
     bool p2p_broken = false;        // a wait timed out: the ranks are out of step until the buffers are connected again
@@ -1760,7 +1766,7 @@ static PickParams pick_params(epp_engine *h, const Work &w, epp_decision *out, e
     p.max_blocks = h->cfg.max_prefix_blocks;
     p.encode_on = h->cfg.encode_enabled ? 1 : 0;
     p.multimodal = w.multimodal_dev ? w.multimodal_dev + w.r0 : nullptr;
-    p.tie_seed = sharded(h) ? 0 : h->cfg.tie_seed;      // sharded mode: lowest slot
+    p.tie_seed = sharded(h) ? 0 : h->cfg.tie_seed;      // sharded mode: the records hold the lowest slot
     p.hashes = w.hashes_out;
     p.nblocks = w.nblocks_out;
     p.bound = nullptr;
@@ -3161,10 +3167,13 @@ static int32_t check_shardable(const epp_engine *h) {
     return EPP_OK;
 }
 
-// epp_shard_set (staged == false: the single-profile handler only) and epp_shard_set_staged.
-static int32_t shard_set(epp_engine *h, uint32_t ep_begin, uint32_t ep_end, bool staged, int32_t *out_stages) {
+// epp_shard_set (staged == false: the single-profile handler only), epp_shard_set_staged and (seeded)
+// epp_shard_set_seeded.
+static int32_t shard_set(epp_engine *h, uint32_t ep_begin, uint32_t ep_end, bool staged, int32_t *out_stages,
+                         bool seeded = false) {
     if (!h || ep_begin > ep_end) return fail(EPP_ERR_INVALID, "bad shard range");
     std::lock_guard<std::mutex> lk(h->mu);
+    if (seeded && h->cfg.tie_seed == 0) return fail(EPP_ERR_INVALID, "epp_shard_set_seeded needs epp_config.tie_seed != 0");
     if (!staged && h->cfg.handler != EPP_HANDLER_SINGLE) return fail(EPP_ERR_INVALID, "endpoint-sharded mode supports the single-profile handler only");
     if (h->general) return fail(EPP_ERR_INVALID, "endpoint-sharded mode supports neither pick_k > 1 nor the prefix-cache-affinity-filter (both need every candidate's score on one rank)");
     EPP_TRY(check_shardable(h));
@@ -3172,9 +3181,13 @@ static int32_t shard_set(epp_engine *h, uint32_t ep_begin, uint32_t ep_end, bool
     const int32_t stages = h->cfg.encode_enabled ? 3 : h->n_profiles;
     if (h->p2p_buf && h->p2p_stages != stages)
         return fail(EPP_ERR_STATE, "the exchange buffer was exported for %d record(s) per request, this handler needs %d: call epp_shard_set_staged before epp_shard_p2p_export", (int)h->p2p_stages, (int)stages);
+    if (h->p2p_buf && h->p2p_seeded != seeded)
+        return fail(EPP_ERR_STATE, "the exchange buffer was exported for the %s tie rule: set the rule before epp_shard_p2p_export",
+                    h->p2p_seeded ? "seeded" : "lowest-slot");
     h->shard_begin = ep_begin;
     h->shard_end = ep_end;
     h->shard_stages = stages;
+    h->shard_seeded = seeded;
     h->pool_ready = false;          // candidates are derived per shard: epp_pool_set must follow
     if (out_stages) *out_stages = stages;
     return EPP_OK;
@@ -3186,6 +3199,10 @@ extern "C" int32_t epp_shard_set(epp_engine *h, uint32_t ep_begin, uint32_t ep_e
 extern "C" int32_t epp_shard_set_staged(epp_engine *h, uint32_t ep_begin, uint32_t ep_end, int32_t *out_stages) {
     if (!out_stages) return fail(EPP_ERR_INVALID, "NULL argument");
     return shard_set(h, ep_begin, ep_end, true, out_stages);
+}
+extern "C" int32_t epp_shard_set_seeded(epp_engine *h, uint32_t ep_begin, uint32_t ep_end, int32_t *out_stages) {
+    if (!out_stages) return fail(EPP_ERR_INVALID, "NULL argument");
+    return shard_set(h, ep_begin, ep_end, true, out_stages, true);
 }
 
 static int32_t mask_words_of(const epp_engine *h) { return (h->cfg.max_prefix_blocks + 31) / 32; }
@@ -3202,6 +3219,7 @@ extern "C" int32_t epp_shard_probe(epp_engine *h, const epp_batch *batch, uint32
     h->shard_R = 0;
     h->shard_models = false;
     h->shard_mm = false;
+    h->shard_picked = false;
     EPP_TRY(commit_locked(h));
     EPP_TRY(run_batch(h, v, Mode::HashOnly, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr));
     int launches = 0;
@@ -3268,7 +3286,13 @@ extern "C" int32_t epp_shard_pick(epp_engine *h, int64_t n_requests, const uint3
     cudaStream_t s = h->slot[0].stream;
     EPP_TRY(reserve_batch(h, n_requests));
     EPP_TRY(launch_match(h, h->slot[0], pp, &launches));
+    if (h->shard_seeded) {          // epp_shard_select walks the same prompts again: keep the OR of the masks
+        const size_t bytes = sizeof(uint32_t) * (size_t)n_requests * (size_t)pp.mask_words;
+        CUDA_TRY(h->sel_gmasks.reserve(bytes, &h->dev_bytes));
+        CUDA_TRY(cudaMemcpyAsync(h->sel_gmasks.p, global_masks, bytes, cudaMemcpyDeviceToDevice, s));
+    }
     CUDA_TRY(cudaStreamSynchronize(s));
+    h->shard_picked = true;
     return EPP_OK;
 }
 
@@ -3278,6 +3302,7 @@ extern "C" int32_t epp_shard_merge_detail(epp_engine *h, int64_t n_requests, int
     std::lock_guard<std::mutex> lk(h->mu);
     EPP_TRY(set_device(h));
     EPP_TRY(join_streams(h));
+    if (h->shard_seeded) return fail(EPP_ERR_STATE, "the engine was set with epp_shard_set_seeded: epp_shard_select and epp_shard_finish replace epp_shard_merge");
     if (n_requests != h->shard_R) return fail(EPP_ERR_STATE, "epp_shard_merge: n_requests does not match the probed batch");
     EPP_TRY(check_encode_detail(h, h->shard_mm, out_detail));
     int launches = 0;
@@ -3292,10 +3317,104 @@ extern "C" int32_t epp_shard_merge(epp_engine *h, int64_t n_requests, int32_t n_
     return epp_shard_merge_detail(h, n_requests, n_ranks, all_best, out, nullptr);
 }
 
+// ---- seeded ties (include/epp_engine.h, "Seeded ties") ------------------------------------------------------------
+static ShardSeedParams shard_seed_params(const epp_engine *h, int64_t r0) {
+    ShardSeedParams sp;
+    memset(&sp, 0, sizeof sp);
+    sp.tie_seed = h->cfg.tie_seed;
+    sp.tie_base = h->stats.n_decisions + (uint64_t)r0;
+    sp.ep_begin = h->shard_begin;
+    sp.ep_end = h->shard_end;
+    return sp;
+}
+
+static int32_t reserve_select(epp_engine *h, int64_t R) {
+    const size_t n = (size_t)std::max<int64_t>(R, 1) * (size_t)h->shard_stages;
+    CUDA_TRY(h->sel_work.reserve(sizeof(uint2) * n, &h->dev_bytes));
+    CUDA_TRY(h->sel_dense.reserve(sizeof(int32_t) * n, &h->dev_bytes));
+    return EPP_OK;
+}
+
+// Resolve rows [r0, r0 + mp.R) over the gathered records and select the members this rank owns: k_shard_resolve, the
+// sparse select, the dense-counter select over its overflows.  pp: the rows' match launch (global masks set); own_sel:
+// this rank's [R][S] entries of the rows.  Work items at sel_work[r0 * S ..], counters in the slot's overflow_n[2], [3].
+static int32_t launch_select(epp_engine *h, Slot &sl, const ShardMergeParams &mp, const PickParams &pp, int64_t r0,
+                             epp_shard_sel *own_sel, int *launches) {
+    cudaStream_t s = sl.stream;
+    const size_t at = (size_t)r0 * (size_t)h->shard_stages;
+    int32_t *counts = sl.overflow_n.as<int32_t>() + 2;
+    CUDA_TRY(cudaMemsetAsync(counts, 0, sizeof(int32_t) * 2, s));
+    ShardSeedParams sp = shard_seed_params(h, r0);
+    sp.sel = own_sel;
+    sp.work = h->sel_work.as<uint2>() + at;
+    sp.work_n = counts;
+    CUDA_TRY(launch_shard_resolve(mp, sp, s, launches));
+    ShardSelView sv;
+    sv.work = sp.work;
+    sv.work_n = counts;
+    sv.stages = h->shard_stages;
+    sv.sel = own_sel;
+    sv.dense_list = h->sel_dense.as<int32_t>() + at;
+    sv.dense_n = counts + 1;
+    CUDA_TRY(launch_match_pick_sparse_select(pp, sv, h->sm_count, s, launches));
+    CUDA_TRY(launch_match_pick_select(pp, sv, h->pick_global ? sl.pick_scratch.as<uint32_t>() : nullptr, h->pick_grid,
+                                      h->pick_smem, s, launches));
+    return EPP_OK;
+}
+
+extern "C" int32_t epp_shard_select(epp_engine *h, int64_t n_requests, int32_t n_ranks, const epp_shard_best *all_best,
+                                    epp_shard_sel *out_sel) {
+    if (!h || !all_best || !out_sel || n_ranks <= 0) return fail(EPP_ERR_INVALID, "bad arguments");
+    std::lock_guard<std::mutex> lk(h->mu);
+    EPP_TRY(set_device(h));
+    EPP_TRY(join_streams(h));
+    if (!h->shard_seeded) return fail(EPP_ERR_STATE, "epp_shard_select needs an engine set with epp_shard_set_seeded");
+    if (!h->pool_ready) return fail(EPP_ERR_STATE, "epp_pool_set has not been called (after epp_shard_set_seeded)");
+    if (n_requests != h->shard_R || (n_requests && !h->shard_picked))
+        return fail(EPP_ERR_STATE, "epp_shard_select: n_requests %lld does not match the picked batch", (long long)n_requests);
+    if (n_requests == 0) return EPP_OK;
+    Work w{0, n_requests, nullptr, nullptr, nullptr, 0, h->shard_models ? h->model_ids.as<uint32_t>() : nullptr, 0,
+           h->hashes.as<uint64_t>(), h->nblocks.as<int32_t>(), h->shard_mm ? h->multimodal.as<uint8_t>() : nullptr};
+    PickParams pp = pick_params(h, w, h->decisions.as<epp_decision>(), nullptr, nullptr);
+    pp.global_masks = h->sel_gmasks.as<uint32_t>();
+    pp.mask_words = mask_words_of(h);
+    EPP_TRY(reserve_select(h, n_requests));
+    int launches = 0;
+    cudaStream_t s = h->slot[0].stream;
+    EPP_TRY(launch_select(h, h->slot[0], shard_merge_params(h, 0, n_requests, n_ranks, all_best, nullptr, nullptr, nullptr),
+                          pp, 0, out_sel, &launches));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    return EPP_OK;
+}
+
+extern "C" int32_t epp_shard_finish(epp_engine *h, int64_t n_requests, int32_t n_ranks, const epp_shard_best *all_best,
+                                    const epp_shard_sel *all_sel, epp_decision *out, epp_decision_detail *out_detail) {
+    if (!h || !all_best || !all_sel || !out || n_ranks <= 0) return fail(EPP_ERR_INVALID, "bad arguments");
+    std::lock_guard<std::mutex> lk(h->mu);
+    EPP_TRY(set_device(h));
+    EPP_TRY(join_streams(h));
+    if (!h->shard_seeded) return fail(EPP_ERR_STATE, "epp_shard_finish needs an engine set with epp_shard_set_seeded");
+    if (n_requests != h->shard_R) return fail(EPP_ERR_STATE, "epp_shard_finish: n_requests does not match the probed batch");
+    EPP_TRY(check_encode_detail(h, h->shard_mm, out_detail));
+    int launches = 0;
+    cudaStream_t s = h->slot[0].stream;
+    ShardSeedParams sp = shard_seed_params(h, 0);
+    sp.all_sel = all_sel;
+    CUDA_TRY(launch_shard_finish(shard_merge_params(h, 0, n_requests, n_ranks, all_best,
+                                                    h->shard_mm ? h->multimodal.as<uint8_t>() : nullptr, out, out_detail),
+                                 sp, s, &launches));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    h->stats.n_batches++;
+    h->stats.n_decisions += (uint64_t)n_requests;    // the next batch's ordinals follow this one's
+    return EPP_OK;
+}
+
 // ---- endpoint-sharded mode with the exchanges over NVLink peer memory (shard_p2p.cu) ------------------------------
-// flags of chunk c of a batch: flag 1 at c * 256, flag 2 at c * 256 + 128 (two chunks: the halves of a batch travel through
-// the exchange on the engine's two streams, so that a rank computes on one half while it waits for its peers on the other)
-static constexpr size_t kP2pFlag1 = 0, kP2pFlag2 = 128, kP2pChunkFlags = 256, kP2pChunks = 2, kP2pHeader = kP2pChunkFlags * kP2pChunks;
+// flags of chunk c of a batch: flag 1 at c * 256, flag 2 at c * 256 + 128, and with the seeded tie rule flag 3 at
+// c * 256 + 64 (two chunks: the halves of a batch travel through the exchange on the engine's two streams, so that a rank
+// computes on one half while it waits for its peers on the other)
+static constexpr size_t kP2pFlag1 = 0, kP2pFlag2 = 128, kP2pFlag3 = 64, kP2pChunkFlags = 256, kP2pChunks = 2,
+                        kP2pHeader = kP2pChunkFlags * kP2pChunks;
 
 extern "C" int32_t epp_shard_p2p_export(epp_engine *h, int64_t max_requests, uint8_t *out_handle, uint64_t *out_ptr) {
     if (!h || max_requests <= 0 || !out_handle || !out_ptr) return fail(EPP_ERR_INVALID, "bad arguments");
@@ -3317,6 +3436,9 @@ extern "C" int32_t epp_shard_p2p_export(epp_engine *h, int64_t max_requests, uin
     h->p2p_masks_off = kP2pHeader;
     h->p2p_best_off = (kP2pHeader + (size_t)max_requests * W * sizeof(uint32_t) + 255) & ~(size_t)255;
     h->p2p_bytes = (h->p2p_best_off + (size_t)max_requests * (size_t)h->shard_stages * sizeof(epp_shard_best) + 255) & ~(size_t)255;
+    h->p2p_seeded = h->shard_seeded;
+    h->p2p_sel_off = h->p2p_bytes;                              // seeded: the selected entries follow the records
+    if (h->p2p_seeded) h->p2p_bytes += ((size_t)max_requests * (size_t)h->shard_stages * sizeof(epp_shard_sel) + 255) & ~(size_t)255;
     CUDA_TRY(cudaMalloc(&h->p2p_buf, h->p2p_bytes));
     CUDA_TRY(cudaMemset(h->p2p_buf, 0, h->p2p_bytes));
     h->dev_bytes += h->p2p_bytes;
@@ -3362,13 +3484,18 @@ extern "C" int32_t epp_shard_p2p_connect(epp_engine *h, int32_t n_ranks, int32_t
     CUDA_TRY(h->p2p_gmasks.reserve(((size_t)h->p2p_R * W * sizeof(uint32_t) + 15) & ~(size_t)15, &h->dev_bytes));
     CUDA_TRY(h->p2p_allbest.reserve(sizeof(epp_shard_best) * (size_t)h->p2p_R * (size_t)h->p2p_stages * (size_t)n_ranks,
                                      &h->dev_bytes));
+    if (h->p2p_seeded) {
+        CUDA_TRY(h->p2p_allsel.reserve(sizeof(epp_shard_sel) * (size_t)h->p2p_R * (size_t)h->p2p_stages * (size_t)n_ranks,
+                                        &h->dev_bytes));
+        EPP_TRY(reserve_select(h, h->p2p_R));
+    }
     EPP_TRY(reserve_batch(h, h->p2p_R));
     return EPP_OK;
 }
 
 // One batch of the sharded protocol with both exchanges done by this rank's own kernels over peer memory.  Every rank
 // calls it with the same batch; the decisions (identical on every rank) land in `out` (device pointer).
-// The protocol is three phases; epp_shard_schedule_p2p runs them back to back (the waits happen ON THE DEVICE, the host
+// The protocol is three phases (four with the seeded tie rule); epp_shard_schedule_p2p runs them back to back (the waits happen ON THE DEVICE, the host
 // only waits at the end), epp_shard_p2p_phase runs ONE phase and synchronises, so that ranks which share a GPU -- whose
 // spin-wait kernels could starve each other -- can be stepped phase by phase from one host thread (tests, small setups).
 static constexpr unsigned long long kP2pPoison = ~0ull;
@@ -3392,6 +3519,7 @@ static int32_t p2p_check(epp_engine *h, cudaStream_t s, unsigned long long epoch
     for (size_t c = 0; c < kP2pChunks; c++) {
         CUDA_TRY(launch_p2p_signal(reinterpret_cast<unsigned long long *>(own + c * kP2pChunkFlags + kP2pFlag1), kP2pPoison, s));
         CUDA_TRY(launch_p2p_signal(reinterpret_cast<unsigned long long *>(own + c * kP2pChunkFlags + kP2pFlag2), kP2pPoison, s));
+        CUDA_TRY(launch_p2p_signal(reinterpret_cast<unsigned long long *>(own + c * kP2pChunkFlags + kP2pFlag3), kP2pPoison, s));
     }
     CUDA_TRY(cudaMemsetAsync(h->p2p_err.p, 0, sizeof(int), s));
     CUDA_TRY(cudaStreamSynchronize(s));
@@ -3402,7 +3530,7 @@ static int32_t p2p_check(epp_engine *h, cudaStream_t s, unsigned long long epoch
 }
 
 // One phase of the exchange for rows [r0, r1) of the batch (chunk c: its own flag words, stream of slot c).  Phase 0
-// expects ++p2p_epoch and the commit to have happened; the caller checks p2p_err after phase 2 of every chunk.
+// expects ++p2p_epoch and the commit to have happened; the caller checks p2p_err after the last phase of every chunk.
 static int32_t p2p_phase_rows(epp_engine *h, const BatchView &v, epp_decision *out, epp_decision_detail *detail, int phase,
                               int c, int64_t r0, int64_t r1, uint64_t or_bits) {
     const int64_t R = r1 - r0;
@@ -3447,14 +3575,40 @@ static int32_t p2p_phase_rows(epp_engine *h, const BatchView &v, epp_decision *o
         h->p2p_launches += launches + 3;
         return EPP_OK;
     }
-    // exchange 2: gather every rank's records from the peers and merge
-    CUDA_TRY(launch_p2p_wait(peers, n, flag2, epoch, h->p2p_err.as<int>(), timeout_ns, s));
-    CUDA_TRY(launch_p2p_gather(peers, n, best_off, sizeof(epp_shard_best) * S * (size_t)R, allbest, s));
-    CUDA_TRY(launch_shard_merge(shard_merge_params(h, r0, R, n, allbest, v.multimodal, out + r0, detail ? detail + r0 : nullptr),
-                                s, &launches));
+    const ShardMergeParams mp = shard_merge_params(h, r0, R, n, allbest, v.multimodal, out + r0, detail ? detail + r0 : nullptr);
+    const size_t flag3 = (size_t)c * kP2pChunkFlags + kP2pFlag3;
+    const size_t sel_off = h->p2p_sel_off + (size_t)r0 * S * sizeof(epp_shard_sel);
+    if (phase == 2) {
+        // exchange 2: gather every rank's records from the peers; then merge (lowest slot), or (seeded) resolve the tie
+        // rule, select the members this rank owns into the own exchange buffer and raise flag 3
+        CUDA_TRY(launch_p2p_wait(peers, n, flag2, epoch, h->p2p_err.as<int>(), timeout_ns, s));
+        CUDA_TRY(launch_p2p_gather(peers, n, best_off, sizeof(epp_shard_best) * S * (size_t)R, allbest, s));
+        if (!h->p2p_seeded) {
+            CUDA_TRY(launch_shard_merge(mp, s, &launches));
+            h->p2p_launches += launches + 2;
+            return EPP_OK;
+        }
+        PickParams pp = pick_params(h, w, h->decisions.as<epp_decision>() + r0, nullptr, nullptr);
+        pp.global_masks = gmasks;
+        pp.mask_words = (int32_t)W;
+        EPP_TRY(launch_select(h, sl, mp, pp, r0, reinterpret_cast<epp_shard_sel *>(own + sel_off), &launches));
+        CUDA_TRY(launch_p2p_signal_unless(reinterpret_cast<unsigned long long *>(own + flag3), epoch, h->p2p_err.as<int>(), s));
+        h->p2p_launches += launches + 3;
+        return EPP_OK;
+    }
+    // exchange 3 (seeded): gather every rank's selected entries and build the decisions
+    epp_shard_sel *allsel = h->p2p_allsel.as<epp_shard_sel>() + (size_t)r0 * (size_t)n * S;
+    CUDA_TRY(launch_p2p_wait(peers, n, flag3, epoch, h->p2p_err.as<int>(), timeout_ns, s));
+    CUDA_TRY(launch_p2p_gather(peers, n, sel_off, sizeof(epp_shard_sel) * S * (size_t)R, allsel, s));
+    ShardSeedParams sp = shard_seed_params(h, r0);
+    sp.all_sel = allsel;
+    CUDA_TRY(launch_shard_finish(mp, sp, s, &launches));
     h->p2p_launches += launches + 2;
     return EPP_OK;
 }
+
+// Phases of a batch: the seeded tie rule adds the third exchange.
+static int p2p_phases(const epp_engine *h) { return h->p2p_seeded ? 4 : 3; }
 
 // Start / end of a batch of the exchange.
 static int32_t p2p_begin(epp_engine *h, const BatchView &v, uint64_t *or_bits) {
@@ -3510,7 +3664,7 @@ extern "C" int32_t epp_shard_schedule_p2p_detail(epp_engine *h, const epp_batch 
         CUDA_TRY(cudaEventRecord(h->slot[0].done, h->slot[0].stream));
         CUDA_TRY(cudaStreamWaitEvent(h->slot[1].stream, h->slot[0].done, 0));
     }
-    for (int phase = 0; phase < 3; phase++) {
+    for (int phase = 0; phase < p2p_phases(h); phase++) {
         EPP_TRY(p2p_phase_rows(h, v, out, out_detail, phase, 0, 0, half, or_bits));
         if (split) EPP_TRY(p2p_phase_rows(h, v, out, out_detail, phase, 1, half, v.R, or_bits));
     }
@@ -3526,14 +3680,14 @@ extern "C" int32_t epp_shard_schedule_p2p(epp_engine *h, const epp_batch *batch,
 extern "C" int32_t epp_shard_p2p_phase_detail(epp_engine *h, const epp_batch *batch, epp_decision *out,
                                               epp_decision_detail *out_detail, int32_t phase) {
     if (!h) return fail(EPP_ERR_INVALID, "NULL argument");
-    if (phase < 0 || phase > 2) return fail(EPP_ERR_INVALID, "phase %d out of range [0,2]", phase);
     std::lock_guard<std::mutex> lk(h->mu);
+    if (phase < 0 || phase >= p2p_phases(h)) return fail(EPP_ERR_INVALID, "phase %d out of range [0,%d]", phase, p2p_phases(h) - 1);
     BatchView v;
     EPP_TRY(p2p_prepare(h, batch, out, out_detail, v));
     if (v.R == 0) return EPP_OK;
     if (phase == 0) EPP_TRY(p2p_begin(h, v, &h->p2p_or_bits));
     EPP_TRY(p2p_phase_rows(h, v, out, out_detail, phase, 0, 0, v.R, h->p2p_or_bits));
-    if (phase == 2) return p2p_end(h, v.R);
+    if (phase == p2p_phases(h) - 1) return p2p_end(h, v.R);
     CUDA_TRY(cudaStreamSynchronize(h->slot[0].stream));
     return EPP_OK;
 }

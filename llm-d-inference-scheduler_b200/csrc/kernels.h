@@ -450,6 +450,35 @@ struct ShardMergeParams {
 };
 cudaError_t launch_shard_merge(const ShardMergeParams &p, cudaStream_t s, int *launches);
 
+// Seeded ties (include/epp_engine.h, "Seeded ties"): every rank resolves the global tie rule over the gathered records
+// (k_shard_resolve: the owner of each arg-max member and its rank in the owner's local set), the owner selects that
+// member (the _select builds of the match kernels), and k_shard_finish builds the decisions from the gathered selects.
+// A work item is x = r * stages + st (r: row of the launch), y = the member's rank in this rank's local set (>= 1).
+struct ShardSeedParams {
+    uint64_t tie_seed;
+    uint64_t tie_base;                  // ordinal of request 0 of the launch
+    uint32_t ep_begin, ep_end;          // resolve: this rank's shard (the owner's pick lies in its range)
+    epp_shard_sel *sel;                 // resolve: [R][stages] this rank's entries (EPP_NO_ENDPOINT where it owns none)
+    uint2 *work;                        // resolve: the selects this rank owns, appended at work[*work_n]
+    int32_t *work_n;
+    const epp_shard_sel *all_sel;       // finish: [n_ranks][R][stages], in the order of all_best
+};
+cudaError_t launch_shard_resolve(const ShardMergeParams &p, const ShardSeedParams &sp, cudaStream_t s, int *launches);
+cudaError_t launch_shard_finish(const ShardMergeParams &p, const ShardSeedParams &sp, cudaStream_t s, int *launches);
+struct ShardSelView {
+    const uint2 *work;                  // [*work_n] items of k_shard_resolve
+    const int32_t *work_n;
+    int32_t stages;
+    epp_shard_sel *sel;                 // [R][stages]: the selected member and its match count
+    int32_t *dense_list;                // items whose lane map overflowed, for the dense-counter select
+    int32_t *dense_n;
+};
+// The sparse select (one warp per item; overflows to sv.dense_list) and the dense-counter select over sv.dense_list.
+cudaError_t launch_match_pick_sparse_select(const PickParams &p, const ShardSelView &sv, int sm_count, cudaStream_t s,
+                                            int *launches);
+cudaError_t launch_match_pick_select(const PickParams &p, const ShardSelView &sv, uint32_t *gscratch, int grid, size_t smem,
+                                     cudaStream_t s, int *launches);
+
 // shard_p2p.cu: exchanges of the endpoint-sharded mode over NVLink peer memory (no NCCL)
 cudaError_t launch_p2p_signal(unsigned long long *flag, unsigned long long epoch, cudaStream_t s);
 cudaError_t launch_p2p_signal_unless(unsigned long long *flag, unsigned long long epoch, const int *err_dev, cudaStream_t s);

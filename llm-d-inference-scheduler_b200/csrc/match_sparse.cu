@@ -59,6 +59,19 @@ __global__ void __launch_bounds__(kWarps * 32, 6) k_match_pick_sparse_rand(PickP
     match_pick_sparse<false, true, 3, true, true>(p);
 }
 
+// The seeded sharded select (include/epp_engine.h "Seeded ties"): one warp per work item of k_shard_resolve, the items
+// taken in grid stride (their count is on the device).
+__global__ void __launch_bounds__(kWarps * 32, 6) k_match_pick_sparse_select(PickParams p, ShardSelView sv) {
+    const int lane = threadIdx.x & 31;
+    const int32_t nwarps = (int32_t)(gridDim.x * kWarps);
+    const int32_t n = *sv.work_n;
+    for (int32_t wi = (int32_t)(blockIdx.x * kWarps + (threadIdx.x >> 5)); wi < n; wi += nwarps) {
+        int32_t ticket = 0;
+        sparse::match_request<false, true, true, 1, sparse::NoFollow, false, false, true>(
+            p, sv.work[wi].x / (uint32_t)sv.stages, lane, false, nullptr, nullptr, ticket, sparse::NoFollow(), &sv, wi);
+    }
+}
+
 namespace {
 template <void (*kernel)(PickParams)>
 cudaError_t launch_kernel(const PickParams &p, int sm_count, cudaStream_t s) {
@@ -85,6 +98,18 @@ cudaError_t launch_nohit(const PickParams &p, int sm_count, cudaStream_t s) {
     return launch_kernel<k_match_pick_sparse_nohit<6, kTie, kStages>>(p, sm_count, s);
 }
 }  // namespace
+
+cudaError_t launch_match_pick_sparse_select(const PickParams &p, const ShardSelView &sv, int sm_count, cudaStream_t s,
+                                            int *launches) {
+    const int64_t items = p.R * (int64_t)sv.stages;          // at most one item per request and stage
+    if (items <= 0) return cudaSuccess;
+    if (sm_count <= 0) sm_count = 132;
+    const int64_t need = (items + kWarps - 1) / kWarps;
+    const int grid = (int)(need < (int64_t)sm_count * 6 ? need : (int64_t)sm_count * 6);
+    k_match_pick_sparse_select<<<grid, kWarps * 32, 0, s>>>(p, sv);
+    if (launches) *launches += 1;
+    return cudaGetLastError();
+}
 
 cudaError_t launch_match_pick_sparse(const PickParams &p, int sm_count, cudaStream_t s, int *launches) {
     if (p.R <= 0) return cudaSuccess;

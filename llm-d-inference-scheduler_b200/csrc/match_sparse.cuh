@@ -110,10 +110,11 @@ static __device__ __noinline__ uint32_t select_tied(const ProfileDev &pf, const 
 // group G of the order (only when that base IS the maximum); X = matched candidates sitting inside G.  G is sorted by
 // slot, |A|, |X| <= 32: the rank of a slot x in S is #{a in A: a < x} + lower_bound_G(x) - #{x' in X: x' < x}, so the
 // member is found with one lower bound per A lane (in parallel) and, failing that, one warp-uniform binary search over G.
-template <bool kTie>
+// kForce: the member of rank force_rank (>= 1) instead (the seeded sharded select, include/epp_engine.h "Seeded ties").
+template <bool kTie, bool kForce = false>
 __device__ __forceinline__ Best eval_profile_lanes(const ProfileDev &pf, int32_t E, const LaneMap &m, int32_t total,
                                                    int lane, const LoraDev &lora, int lora_st, uint64_t tie_seed,
-                                                   uint64_t tie_key) {
+                                                   uint64_t tie_key, uint32_t force_rank = 0) {
     Best b;
     best_init(b);
     const int32_t ncand = *pf.n_cand;
@@ -121,7 +122,8 @@ __device__ __forceinline__ Best eval_profile_lanes(const ProfileDev &pf, int32_t
     if (m.n == 0) {                                   // nobody holds a block of this prompt: the head of the order wins
         const uint32_t ue = pf.order[0];
         best_add(b, pf.base[ue], ue, pf.grp_size[0]);
-        if (kTie && tie_seed && b.ties > 1) b.pick = pf.order[tie_rank(tie_seed, tie_key, b.ties)];
+        if (kForce) b.pick = pf.order[force_rank];
+        else if (kTie && tie_seed && b.ties > 1) b.pick = pf.order[tie_rank(tie_seed, tie_key, b.ties)];
         return b;
     }
     const bool mine = (uint32_t)lane < m.n && pf.cand[m.e];
@@ -154,9 +156,9 @@ __device__ __forceinline__ Best eval_profile_lanes(const ProfileDev &pf, int32_t
             break;
         }
     }
-    if (kTie && tie_seed && b.ties > 1)
+    if (kForce || (kTie && tie_seed && b.ties > 1))
         b.pick = select_tied(pf, m, lane, mine && myv == b.val, in_x, have_u && ubase == b.val, gpos, ue,
-                             tie_rank(tie_seed, tie_key, b.ties));
+                             kForce ? force_rank : tie_rank(tie_seed, tie_key, b.ties));
     return b;
 }
 
@@ -292,9 +294,14 @@ struct NoFollow {
 // kNoHit: a profile has a no-hit-lru scorer (PickParams::nohit): the lane map decides, with one ballot, whether the request
 // is cold for the profile, which selects the profile's warm or cold set (same candidates, different base / order / groups).
 // kRand: some profile has a random picker (epp_profile_cfg.picker): those profiles are decided by eval_random_lanes.
-template <bool kCg, bool kSharded, bool kTie, int kStages, typename Follow = NoFollow, bool kNoHit = false, bool kRand = false>
+// kSel: the seeded sharded select (k_match_pick_sparse_select): request r is work item sv->work[wi], whose one profile
+// is evaluated with the rank of its member forced; the member and its match count go to sv->sel, an overflow appends wi
+// to sv->dense_list.
+template <bool kCg, bool kSharded, bool kTie, int kStages, typename Follow = NoFollow, bool kNoHit = false, bool kRand = false,
+          bool kSel = false>
 __device__ __forceinline__ bool match_request(const PickParams &p, const uint32_t r, const int lane, const bool counting,
-                                              Work *wk, int32_t *req_next, int32_t &ticket, const Follow fw = Follow()) {
+                                              Work *wk, int32_t *req_next, int32_t &ticket, const Follow fw = Follow(),
+                                              const ShardSelView *sv = nullptr, int32_t wi = 0) {
     const uint32_t shard_lo = p.index.ep_begin, shard_hi = min(p.index.ep_end, (uint32_t)p.E);
     const IndexSlot *slots = p.index.slots;
     const uint32_t mask32 = (uint32_t)p.index.mask;
@@ -388,8 +395,25 @@ __device__ __forceinline__ bool match_request(const PickParams &p, const uint32_
     }
     if (m.overflow()) {
         // hand the request to the dense-counter kernel
-        if (lane == 0 && p.overflow_list) p.overflow_list[atomicAdd(p.overflow_n, 1)] = (int32_t)r;
+        if constexpr (kSel) {
+            if (lane == 0) sv->dense_list[atomicAdd(sv->dense_n, 1)] = wi;
+        } else {
+            if (lane == 0 && p.overflow_list) p.overflow_list[atomicAdd(p.overflow_n, 1)] = (int32_t)r;
+        }
         return false;
+    }
+    if constexpr (kSel) {
+        const uint2 it = sv->work[wi];
+        const Best b = eval_profile_lanes<true, true>(p.prof[it.x % (uint32_t)sv->stages], p.E, m, total, lane, p.lora,
+                                                      lora_st, 0, 0, it.y);
+        const uint32_t mb = m.n ? map_get(m, b.pick) : 0u;
+        if (lane == 0) {
+            epp_shard_sel s;
+            s.pick = b.pick;
+            s.match_blocks = (int32_t)mb;
+            sv->sel[it.x] = s;
+        }
+        return true;
     }
     // ---- a5-a14: the profiles of the handler
     if constexpr (kSharded && kStages > 1) {

@@ -257,11 +257,12 @@ __device__ __forceinline__ uint32_t cnt_get(const uint32_t *cnt32, uint32_t e) {
 __device__ inline Best eval_profile_inner(const ProfileDev &pf, int32_t E, const uint32_t *cnt32, const uint32_t *list,
                                           uint32_t nl, int32_t total, int lane, const LoraDev &lora, uint32_t adapter);
 
-// + the tie rule (score.cuh): the member of rank k of the arg-max set, found by one more scan over the slots
-template <bool kRand>
+// + the tie rule (score.cuh): the member of rank k of the arg-max set, found by one more scan over the slots.
+// kForce: the member of rank force_rank instead (the seeded sharded select, include/epp_engine.h "Seeded ties").
+template <bool kRand, bool kForce = false>
 __device__ inline Best eval_profile(const ProfileDev &pf, int32_t E, const uint32_t *cnt32, const uint32_t *list,
                                     uint32_t nl, int32_t total, int lane, const LoraDev &lora, uint32_t adapter,
-                                    uint64_t tie_seed, uint64_t tie_key) {
+                                    uint64_t tie_seed, uint64_t tie_key, uint32_t force_rank = 0) {
     if (kRand && pf.cfg.picker) {                     // random pickers: explicit = matched or lora-resident candidates
         const bool use_lora = lora.enabled && lora.ptr;
         return rnd::draw_scan(pf, E, lane, true, (uint32_t)*pf.n_cand, 0u, tie_seed, tie_key,
@@ -275,9 +276,9 @@ __device__ inline Best eval_profile(const ProfileDev &pf, int32_t E, const uint3
                               [](uint32_t) { return false; });
     }
     Best b = eval_profile_inner(pf, E, cnt32, list, nl, total, lane, lora, adapter);
-    if (tie_seed && b.ties > 1) {
+    if (kForce || (tie_seed && b.ties > 1)) {
         const bool use_lora = lora.enabled && lora.ptr;
-        b.pick = select_kth_scan(pf, E, b.val, tie_rank(tie_seed, tie_key, b.ties), lane, [&](uint32_t e) {
+        b.pick = select_kth_scan(pf, E, b.val, kForce ? force_rank : tie_rank(tie_seed, tie_key, b.ties), lane, [&](uint32_t e) {
             const uint32_t c = cnt_get(cnt32, e);
             if (use_lora) return weighted_sum(pf, E, e, (int32_t)c, total, lora, lora_lookup(lora, adapter, e));
             return c ? weighted_sum(pf, E, e, (int32_t)c, total) : pf.base[e];
@@ -376,9 +377,11 @@ __device__ inline Best lat_eval_profile(const P &p, const LatView &lv, int pi, i
 
 // kRand: the engine has a random picker (k_match_pick_rand); the max-score build carries none of its code.
 // kLat: the engine has latency profiles (k_match_pick_lat*): those evaluate through lat::eval with the request's entries.
-template <bool kRand, bool kLat = false>
+// kSel: the seeded sharded select (k_match_pick_select): the items of sv->dense_list, each one profile with the rank of
+// its member forced, written to sv->sel.
+template <bool kRand, bool kLat = false, bool kSel = false>
 __device__ __forceinline__ void match_pick_dense(const PickParams &p, int32_t cnt_words, uint32_t *gscratch,
-                                                 const LatView *lv = nullptr) {
+                                                 const LatView *lv = nullptr, const ShardSelView *sv = nullptr) {
     extern __shared__ uint32_t smem[];
     const int lane = threadIdx.x & 31;
     const int warp = threadIdx.x >> 5;
@@ -386,7 +389,7 @@ __device__ __forceinline__ void match_pick_dense(const PickParams &p, int32_t cn
     const int64_t nwarps = (int64_t)gridDim.x * kPickWarps;
     // the overflow pass runs over a full grid and its list is almost always empty: a warp without a request leaves
     // before it clears its counters (no block-wide barrier below)
-    const int64_t n_work = p.req_list ? (int64_t)*p.req_list_n : p.R;
+    const int64_t n_work = kSel ? (int64_t)*sv->dense_n : (p.req_list ? (int64_t)*p.req_list_n : p.R);
     if (gwarp >= n_work) return;
     uint32_t *cnt32;
     uint32_t *list;
@@ -404,7 +407,8 @@ __device__ __forceinline__ void match_pick_dense(const PickParams &p, int32_t cn
     __syncwarp();
 
     for (int64_t wi = gwarp; wi < n_work; wi += nwarps) {
-        const int64_t r = p.req_list ? (int64_t)p.req_list[wi] : wi;
+        const int64_t r = kSel ? (int64_t)(sv->work[sv->dense_list[wi]].x / (uint32_t)sv->stages)
+                               : (p.req_list ? (int64_t)p.req_list[wi] : wi);
         const int32_t total = p.nblocks[r];
         const int32_t stored = p.bound ? p.bound[r] : total;      // block `stored` < total: a proven miss
         if (lane == 0) *list_n = 0;
@@ -457,7 +461,18 @@ __device__ __forceinline__ void match_pick_dense(const PickParams &p, int32_t cn
         bool cold = false;
         auto is_cold = [&](const ProfileDev &pf) { return cold_scan(pf, p.E, lane, cnt_of); };
         bool staged = false;
-        if constexpr (kLat) {
+        if constexpr (kSel) {
+            const uint2 it = sv->work[sv->dense_list[wi]];
+            const Best b = eval_profile<false, true>(p.prof[it.x % (uint32_t)sv->stages], p.E, cnt32, list, nl, total, lane,
+                                                     p.lora, adapter, 0, 0, it.y);
+            if (lane == 0) {
+                epp_shard_sel s;
+                s.pick = b.pick;
+                s.match_blocks = (int32_t)cnt_get(cnt32, b.pick);
+                sv->sel[it.x] = s;
+            }
+            staged = true;                               // nothing else is written
+        } else if constexpr (kLat) {
             decide_stages<3>(p, r, total, p.n_profiles >= 2 ? p.in_len[r] : 0,
                           [&](int pi, uint64_t key) {
                               if ((lv->mask >> pi) & 1) return lat_eval_profile<kRand>(p, *lv, pi, r, total, lane, adapter, key, cnt_of);
@@ -484,15 +499,17 @@ __device__ __forceinline__ void match_pick_dense(const PickParams &p, int32_t cn
                               cnt_of, d, dd);
         }
         if (lane == 0 && p.nohit.cold_out) p.nohit.cold_out[r] = cold ? 1 : 0;
-        if (lane == 0 && !staged) {
-            if (p.shard_out) {
-                epp_shard_best sb;
-                sb.score = d.score; sb.pick = d.pick; sb.tie_count = d.tie_count;
-                sb.match_blocks = d.match_blocks; sb.status = d.status;
-                p.shard_out[r] = sb;
-            } else {
-                p.out[r] = d;
-                if (p.detail) p.detail[r] = dd;
+        if constexpr (!kSel) {
+            if (lane == 0 && !staged) {
+                if (p.shard_out) {
+                    epp_shard_best sb;
+                    sb.score = d.score; sb.pick = d.pick; sb.tie_count = d.tie_count;
+                    sb.match_blocks = d.match_blocks; sb.status = d.status;
+                    p.shard_out[r] = sb;
+                } else {
+                    p.out[r] = d;
+                    if (p.detail) p.detail[r] = dd;
+                }
             }
         }
         // ---- a4: dense match row (Produce parity mode only)
@@ -531,6 +548,10 @@ __global__ void __launch_bounds__(kPickWarps * 32) k_match_pick_rand(PickParams 
     match_pick_dense<true>(p, cnt_words, gscratch);
 }
 
+__global__ void __launch_bounds__(kPickWarps * 32) k_match_pick_select(PickParams p, int32_t cnt_words, uint32_t *gscratch, ShardSelView sv) {
+    match_pick_dense<false, false, true>(p, cnt_words, gscratch, nullptr, &sv);
+}
+
 __global__ void __launch_bounds__(kPickWarps * 32) k_match_pick_lat(PickParams p, int32_t cnt_words, uint32_t *gscratch, LatView lv) {
     match_pick_dense<false, true>(p, cnt_words, gscratch, &lv);
 }
@@ -560,6 +581,21 @@ cudaError_t launch_match_pick(const PickParams &p, uint32_t *gscratch, int grid,
     int32_t cnt_words = (p.E + 1) / 2;
     if (any_random_picker(p)) k_match_pick_rand<<<grid, kPickWarps * 32, smem, s>>>(p, cnt_words, gscratch);
     else k_match_pick<<<grid, kPickWarps * 32, smem, s>>>(p, cnt_words, gscratch);
+    if (launches) *launches += 1;
+    return cudaGetLastError();
+}
+
+cudaError_t launch_match_pick_select(const PickParams &p, const ShardSelView &sv, uint32_t *gscratch, int grid, size_t smem,
+                                     cudaStream_t s, int *launches) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    static bool attr_set[64] = {};
+    if (!attr_set[dev & 63]) {
+        const cudaError_t e = cudaFuncSetAttribute(k_match_pick_select, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+        if (e != cudaSuccess) return e;
+        attr_set[dev & 63] = true;
+    }
+    k_match_pick_select<<<grid, kPickWarps * 32, smem, s>>>(p, (p.E + 1) / 2, gscratch, sv);
     if (launches) *launches += 1;
     return cudaGetLastError();
 }
@@ -761,12 +797,12 @@ __device__ __forceinline__ Best merge_stage(const ShardMergeParams &p, int64_t r
     return b;
 }
 
-// The decision of request r from the merged stages, as decide_stages makes it from one pool.
-__global__ void k_shard_merge(ShardMergeParams p) {
-    int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= p.R) return;
+// The decision of request r from the reduced stages (stage(st, mb) -> the stage's Best, mb = its pick's match count), as
+// decide_stages makes it from one pool.
+template <typename Stage>
+__device__ __forceinline__ void shard_decide(const ShardMergeParams &p, int64_t r, Stage stage) {
     int32_t mb;
-    const Best b = merge_stage(p, r, 0, mb);
+    const Best b = stage(0, mb);
     epp_decision d;
     d.status = b.ties ? 0 : -1;
     d.pick = b.ties ? b.pick : EPP_NO_ENDPOINT;
@@ -780,22 +816,117 @@ __global__ void k_shard_merge(ShardMergeParams p) {
     dd.encode_score = 0.0; dd.encode_pick = EPP_NO_ENDPOINT; dd.encode_tie_count = 0; dd.encode_ran = 0; dd.reserved = 0;
     if (b.ties && p.stages >= 3 && p.multimodal && p.multimodal[r]) {   // no decode pick: no other stage runs
         dd.encode_ran = 1;
-        const Best b2 = merge_stage(p, r, 2, mb);
+        const Best b2 = stage(2, mb);
         if (b2.ties) { dd.encode_pick = b2.pick; dd.encode_score = b2.val; dd.encode_tie_count = b2.ties; }
     }
     if (b.ties && p.stages >= 2 &&
         (p.always_disagg || pd_decide(p.non_cached_tokens, p.in_len[r], d.match_blocks, p.block_size_tokens))) {
         dd.prefill_ran = 1;
-        const Best b1 = merge_stage(p, r, 1, mb);
+        const Best b1 = stage(1, mb);
         if (b1.ties) { d.prefill_pick = b1.pick; dd.prefill_score = b1.val; dd.prefill_tie_count = b1.ties; }
     }
     p.out[r] = d;
     if (p.detail) p.detail[r] = dd;
 }
 
+__global__ void k_shard_merge(ShardMergeParams p) {
+    int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= p.R) return;
+    shard_decide(p, r, [&](int st, int32_t &mb) { return merge_stage(p, r, st, mb); });
+}
+
 cudaError_t launch_shard_merge(const ShardMergeParams &p, cudaStream_t s, int *launches) {
     if (p.R <= 0) return cudaSuccess;
     k_shard_merge<<<(unsigned)((p.R + 255) / 256), 256, 0, s>>>(p);
+    if (launches) *launches += 1;
+    return cudaGetLastError();
+}
+
+// Seeded ties (include/epp_engine.h, "Seeded ties").  The arg-max set of stage st over every rank is the union of the
+// local sets of the records at the max (b, from merge_stage); the shard ranges are disjoint, so in ascending slot order
+// it is those local sets taken in the order of their lowest members, the records' picks.  -> the rank (index in
+// all_best) that owns member tie_rank(seed, 4 * (tie_base + r) + st, b.ties) and its rank in that rank's local set;
+// rank -1 when no rank has a candidate.  At most n_ranks passes over n_ranks records.
+struct ShardOwner {
+    int32_t rank;
+    uint32_t local;
+};
+__device__ __forceinline__ ShardOwner shard_owner(const ShardMergeParams &p, const ShardSeedParams &sp, int64_t r, int st,
+                                                  const Best &b) {
+    ShardOwner o{-1, 0u};
+    if (!b.ties) return o;
+    uint32_t rho = b.ties > 1 ? tie_rank(sp.tie_seed, 4 * (sp.tie_base + (uint64_t)r) + (uint64_t)st, b.ties) : 0u;
+    int64_t after = -1;                                  // the pick of the last local set passed
+    for (int32_t n = 0; n < p.n_ranks; n++) {
+        int32_t next = -1;
+        uint32_t lo = EPP_NO_ENDPOINT;
+        for (int32_t k = 0; k < p.n_ranks; k++) {
+            const epp_shard_best sb = p.all_best[((int64_t)k * p.R + r) * p.stages + st];
+            if (sb.status == 0 && sb.score == b.val && (int64_t)sb.pick > after && (next < 0 || sb.pick < lo)) {
+                next = k;
+                lo = sb.pick;
+            }
+        }
+        if (next < 0) break;
+        const uint32_t c = p.all_best[((int64_t)next * p.R + r) * p.stages + st].tie_count;
+        if (rho < c) { o.rank = next; o.local = rho; break; }
+        rho -= c;
+        after = lo;
+    }
+    return o;
+}
+
+// One thread per (request, stage): this rank's entry -- the owner's record pick when this rank owns it (the member of
+// local rank 0 is that pick), EPP_NO_ENDPOINT otherwise -- and a work item for each owned member of local rank >= 1.
+__global__ void k_shard_resolve(ShardMergeParams p, ShardSeedParams sp) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= p.R * p.stages) return;
+    const int64_t r = i / p.stages;
+    const int st = (int)(i % p.stages);
+    int32_t mb;
+    const Best b = merge_stage(p, r, st, mb);
+    const ShardOwner o = shard_owner(p, sp, r, st, b);
+    epp_shard_sel s;
+    s.pick = EPP_NO_ENDPOINT;
+    s.match_blocks = 0;
+    if (o.rank >= 0) {
+        const epp_shard_best own = p.all_best[((int64_t)o.rank * p.R + r) * p.stages + st];
+        if (own.pick >= sp.ep_begin && own.pick < sp.ep_end) {
+            s.pick = own.pick;
+            s.match_blocks = own.match_blocks;
+            if (o.local) sp.work[atomicAdd(sp.work_n, 1)] = make_uint2((uint32_t)i, o.local);
+        }
+    }
+    sp.sel[i] = s;
+}
+
+cudaError_t launch_shard_resolve(const ShardMergeParams &p, const ShardSeedParams &sp, cudaStream_t s, int *launches) {
+    const int64_t n = p.R * p.stages;
+    if (n <= 0) return cudaSuccess;
+    k_shard_resolve<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(p, sp);
+    if (launches) *launches += 1;
+    return cudaGetLastError();
+}
+
+// The decisions as k_shard_merge builds them, each stage's pick and match count taken from its owner's entry.
+__global__ void k_shard_finish(ShardMergeParams p, ShardSeedParams sp) {
+    const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= p.R) return;
+    shard_decide(p, r, [&](int st, int32_t &mb) {
+        Best b = merge_stage(p, r, st, mb);
+        const ShardOwner o = shard_owner(p, sp, r, st, b);
+        if (o.rank >= 0) {
+            const epp_shard_sel s = sp.all_sel[((int64_t)o.rank * p.R + r) * p.stages + st];
+            b.pick = s.pick;
+            mb = s.match_blocks;
+        }
+        return b;
+    });
+}
+
+cudaError_t launch_shard_finish(const ShardMergeParams &p, const ShardSeedParams &sp, cudaStream_t s, int *launches) {
+    if (p.R <= 0) return cudaSuccess;
+    k_shard_finish<<<(unsigned)((p.R + 255) / 256), 256, 0, s>>>(p, sp);
     if (launches) *launches += 1;
     return cudaGetLastError();
 }

@@ -262,6 +262,7 @@ class Engine:
         self.E = max_endpoints
         self.B = max_prefix_blocks
         self.shard_stages = 1           # records per request of the endpoint-sharded protocol (shard_set_staged)
+        self.shard_seeded = False       # the sharded protocol resolves the seeded tie rule (shard_set_seeded)
         self._h = C.c_void_p()
         self._check(self._lib.epp_engine_create(C.byref(cfg), C.byref(self._h)))
         for p, spec in enumerate((primary, prefill, encode)):
@@ -697,6 +698,7 @@ class Engine:
     def shard_set(self, ep_begin: int, ep_end: int):
         self._check(self._lib.epp_shard_set(self._h, ep_begin, ep_end))
         self.shard_stages = 1
+        self.shard_seeded = False
 
     def shard_set_staged(self, ep_begin: int, ep_end: int) -> int:
         """shard_set that also takes the disagg handler -> S, the records per request of shard_pick (1 single profile,
@@ -704,6 +706,17 @@ class Engine:
         s = C.c_int32(0)
         self._check(self._lib.epp_shard_set_staged(self._h, ep_begin, ep_end, C.byref(s)))
         self.shard_stages = s.value
+        self.shard_seeded = False
+        return s.value
+
+    def shard_set_seeded(self, ep_begin: int, ep_end: int) -> int:
+        """shard_set_staged with the engine's tie_seed rule across the shards (epp_engine.h, "Seeded ties") -> S.  A batch
+        then takes shard_select and shard_finish (a third exchange) instead of shard_merge, and the peer-memory exchange
+        four phases."""
+        s = C.c_int32(0)
+        self._check(self._lib.epp_shard_set_seeded(self._h, ep_begin, ep_end, C.byref(s)))
+        self.shard_stages = s.value
+        self.shard_seeded = True
         return s.value
 
     def shard_probe(self, data, out_masks, offsets=None, uniform_len=None, model_ids=None, n_requests=None,
@@ -736,7 +749,8 @@ class Engine:
 
     def shard_p2p_phase(self, data, out_decisions, phase: int, offsets=None, uniform_len=None, model_ids=None,
                         n_requests=None, lengths=None, multimodal=None, out_detail=None):
-        """One phase (0, 1, 2) of shard_schedule_p2p, synchronised: for ranks that share a GPU."""
+        """One phase (0, 1, 2; and 3 on a seeded engine) of shard_schedule_p2p, synchronised: for ranks that share a
+        GPU."""
         b, R, dev, keep = self._batch(data, offsets, uniform_len, model_ids, n_requests, lengths, multimodal)
         self._check(self._lib.epp_shard_p2p_phase_detail(self._h, C.byref(b), _ptr(out_decisions), _ptr(out_detail), phase))
         return R
@@ -745,6 +759,17 @@ class Engine:
         """all_best: [n_ranks, R, S * 24] records; out_detail as in shard_schedule_p2p."""
         self._check(self._lib.epp_shard_merge_detail(self._h, n_requests, n_ranks, _ptr(all_best), _ptr(out_decisions),
                                                      _ptr(out_detail)))
+
+    def shard_select(self, n_requests, n_ranks, all_best, out_sel):
+        """Seeded engines: all_best [n_ranks, R, S * 24] records -> out_sel [R, S * 8] bytes, this rank's entries
+        (epp_shard_sel: the member it owns, else EPP_NO_ENDPOINT)."""
+        self._check(self._lib.epp_shard_select(self._h, n_requests, n_ranks, _ptr(all_best), _ptr(out_sel)))
+
+    def shard_finish(self, n_requests, n_ranks, all_best, all_sel, out_decisions, out_detail=None):
+        """Seeded engines: the decisions from the records and every rank's entries ([n_ranks, R, S * 8], stacked in the
+        order of all_best)."""
+        self._check(self._lib.epp_shard_finish(self._h, n_requests, n_ranks, _ptr(all_best), _ptr(all_sel),
+                                               _ptr(out_decisions), _ptr(out_detail)))
 
 
 class Batcher:

@@ -10,7 +10,11 @@ at the first block NO server holds (approximateprefix/plugin.go:219-223), a shar
     phase 3  epp_shard_merge   per stage: max score, lowest slot id among equals, ties summed; then the deciders
 
 S is the engine's number of stages (Engine.shard_set_staged): 1 for the single-profile handler, 2 for the disagg
-handler's decode + prefill, 3 with its encode stage.  The prefill and encode profiles do not depend on the decode pick,
+handler's decode + prefill, 3 with its encode stage.
+
+Seeded ties (Engine.shard_set_seeded, epp_engine.h "Seeded ties") add a third exchange: phase 3 becomes epp_shard_select,
+which resolves the tie rule over the gathered records (resolve_records_host restates it) and selects the arg-max members
+this rank owns; the 8-byte entries are all-gathered and epp_shard_finish builds the decisions from them.  The prefill and encode profiles do not depend on the decode pick,
 only whether they run does: every rank publishes its best record of each stage (prefill whenever the P/D decider can
 still say yes, encode for multimodal requests), and the merge applies the deciders to the merged decode pick -- still two
 exchanges.
@@ -46,7 +50,8 @@ def or_allgather(local_masks, dist=None):
 
 
 def allgather_records(local_best, dist=None):
-    """All-gather the 24-byte best records.  local_best: torch uint8 tensor [R, S * 24] -> [world, R, S * 24]."""
+    """All-gather the 24-byte best records (or the 8-byte selected entries).  local_best: torch uint8 tensor [R, X]
+    -> [world, R, X]."""
     import torch
     if dist is None or not dist.is_initialized() or dist.get_world_size() == 1:
         return local_best.unsqueeze(0).clone()
@@ -78,6 +83,47 @@ def merge_records_host(all_best: np.ndarray) -> np.ndarray:
         out["score"] = np.where(better, rec["score"], out["score"])
         out["status"] = np.where(ok, 0, out["status"])
     return out
+
+
+SHARD_SEL_DTYPE = np.dtype([("pick", "<u4"), ("match_blocks", "<i4")])
+
+
+def _mix64(z: int) -> int:
+    m = (1 << 64) - 1
+    z = (z + 0x9E3779B97F4A7C15) & m
+    z = ((z ^ (z >> 30)) * 0xBF58476D1CE4E5B9) & m
+    z = ((z ^ (z >> 27)) * 0x94D049BB133111EB) & m
+    return z ^ (z >> 31)
+
+
+def tie_rank_host(seed: int, key: int, n: int) -> int:
+    """The tie rule's member rank (epp_engine.h, "Tie rule")."""
+    return ((_mix64((seed ^ _mix64(key)) & ((1 << 64) - 1)) >> 32) * n) >> 32
+
+
+def resolve_records_host(all_best: np.ndarray, tie_seed: int, tie_base: int, stage: int = 0):
+    """The owner computation of epp_shard_select on the host: all_best [world, R] of SHARD_BEST_DTYPE (one stage) ->
+    (merged records [R] as merge_records_host returns them, owner [R] (index in all_best, -1 when no rank has a
+    candidate), rho_local [R]: the rank of member tie_rank(seed, 4 * (tie_base + r) + stage, N) in the owner's local
+    set).  The shard ranges are disjoint, so the global arg-max set in ascending slot order is the local sets taken in
+    the order of their records' picks."""
+    world, R = all_best.shape
+    merged = merge_records_host(all_best)
+    owner = np.full(R, -1, np.int64)
+    local = np.zeros(R, np.uint32)
+    for r in range(R):
+        if merged["status"][r] != 0:
+            continue
+        n = int(merged["tie_count"][r])
+        rho = tie_rank_host(tie_seed, 4 * (tie_base + r) + stage, n) if n > 1 else 0
+        at_max = [g for g in range(world) if all_best[g, r]["status"] == 0 and all_best[g, r]["score"] == merged["score"][r]]
+        for g in sorted(at_max, key=lambda g: int(all_best[g, r]["pick"])):
+            c = int(all_best[g, r]["tie_count"])
+            if rho < c:
+                owner[r], local[r] = g, rho
+                break
+            rho -= c
+    return merged, owner, local
 
 
 STAGE_DETAIL_DTYPE = np.dtype([("prefill_pick", "<u4"), ("prefill_score", "<f8"), ("prefill_tie_count", "<u4"),
@@ -142,7 +188,15 @@ def schedule_sharded(engine, tokens_dev, uniform_len: int, dist=None, detail=Non
     allb = allgather_records(best, dist)
     dec = torch.empty((R, 32), dtype=torch.uint8, device=dev)
     torch.cuda.current_stream(dev).synchronize()
-    engine.shard_merge(R, allb.shape[0], allb, dec, out_detail=detail)
+    if not getattr(engine, "shard_seeded", False):
+        engine.shard_merge(R, allb.shape[0], allb, dec, out_detail=detail)
+        return dec
+    # seeded ties: the third exchange carries the members each rank selected
+    sel = torch.empty((R, 8 * engine.shard_stages), dtype=torch.uint8, device=dev)
+    engine.shard_select(R, allb.shape[0], allb, sel)
+    alls = allgather_records(sel, dist)
+    torch.cuda.current_stream(dev).synchronize()
+    engine.shard_finish(R, allb.shape[0], allb, alls, dec, out_detail=detail)
     return dec
 
 
