@@ -182,7 +182,6 @@ static void flusher_main(epp_batcher *b) {
         batch.model_ids = st.model_ids;
         batch.multimodal = st.multimodal;
         batch.flags = EPP_BATCH_LENGTHS_EXCEED_ROWS;
-        int32_t rc;
         epp_topk_out tk;
         memset(&tk, 0, sizeof tk);
         tk.struct_size = sizeof tk;
@@ -192,50 +191,38 @@ static void flusher_main(epp_batcher *b) {
         const bool any_sub = st.any_subset.load(std::memory_order_acquire) != 0;
         const bool any_ctx = st.any_ctx.load(std::memory_order_acquire) != 0;
         const bool any_adm = st.any_adm.load(std::memory_order_acquire) != 0;
-        if (any_pred || any_sub || any_ctx || any_adm) {
-            // predictions only reach a latency engine (every predicted submit checks it), where subsets and predictions
-            // may share a batch and even a row: one epp_schedule_subset_predicted decides them all
-            epp_predictions pr;
-            memset(&pr, 0, sizeof pr);
-            pr.struct_size = sizeof pr;
-            pr.counts = st.pred_counts.data();
-            pr.offsets = st.pred_offsets.data();
-            pr.entries = st.pred_entries.data();
-            epp_subset sub;
-            memset(&sub, 0, sizeof sub);
-            sub.struct_size = sizeof sub;
-            sub.counts = st.sub_counts.data();
-            sub.offsets = st.sub_offsets.data();
-            sub.slots = st.sub_slots.data();
-            epp_context_tokens ct;
-            memset(&ct, 0, sizeof ct);
-            ct.struct_size = sizeof ct;
-            ct.tokens = st.ctx.data();
-            epp_admission adm;
-            memset(&adm, 0, sizeof adm);
-            adm.struct_size = sizeof adm;
-            adm.priority = st.priority.data();
-            adm.ttft_slo = st.ttft_slo.data();
-            adm.tpot_slo = st.tpot_slo.data();
-            adm.pred_valid = st.pred_valid.empty() ? nullptr : st.pred_valid.data();
-            // predictions on an engine without a latency profile are read by the latency-slo-admitter only (epp_schedule_admit)
-            if (any_ctx || any_adm || (any_pred && !engine_latency_mask(b->eng)))
-                rc = epp_schedule_admit(b->eng, &batch, any_sub ? &sub : nullptr, any_pred ? &pr : nullptr, &ct, any_adm ? &adm : nullptr,
-                                        st.dec, st.det, b->cfg.index_picks ? 1 : 0, b->pick_k > 1 ? &tk : nullptr);
-            else if (engine_latency_mask(b->eng))
-                rc = epp_schedule_subset_predicted(b->eng, &batch, any_sub ? &sub : nullptr, any_pred ? &pr : nullptr, st.dec, st.det,
-                                                   b->cfg.index_picks ? 1 : 0, b->pick_k > 1 ? &tk : nullptr);
-            else
-                rc = epp_schedule_subset(b->eng, &batch, &sub, st.dec, st.det, b->cfg.index_picks ? 1 : 0, b->pick_k > 1 ? &tk : nullptr);
-            st.any_pred.store(0, std::memory_order_relaxed);
-            st.any_subset.store(0, std::memory_order_relaxed);
-            st.any_ctx.store(0, std::memory_order_relaxed);
-            st.any_adm.store(0, std::memory_order_relaxed);
-        } else if (b->pick_k > 1) {
-            rc = epp_schedule_topk(b->eng, &batch, st.dec, st.det, b->cfg.index_picks ? 1 : 0, &tk);
-        } else {
-            rc = epp_schedule(b->eng, &batch, st.dec, st.det, b->cfg.index_picks ? 1 : 0);
-        }
+        // each input is passed exactly when some row carries it; predictions only reach a latency engine or the
+        // latency-slo-admitter (every predicted submit checks it)
+        epp_predictions pr;
+        memset(&pr, 0, sizeof pr);
+        pr.struct_size = sizeof pr;
+        pr.counts = st.pred_counts.data();
+        pr.offsets = st.pred_offsets.data();
+        pr.entries = st.pred_entries.data();
+        epp_subset sub;
+        memset(&sub, 0, sizeof sub);
+        sub.struct_size = sizeof sub;
+        sub.counts = st.sub_counts.data();
+        sub.offsets = st.sub_offsets.data();
+        sub.slots = st.sub_slots.data();
+        epp_context_tokens ct;
+        memset(&ct, 0, sizeof ct);
+        ct.struct_size = sizeof ct;
+        ct.tokens = st.ctx.data();
+        epp_admission adm;
+        memset(&adm, 0, sizeof adm);
+        adm.struct_size = sizeof adm;
+        adm.priority = st.priority.data();
+        adm.ttft_slo = st.ttft_slo.data();
+        adm.tpot_slo = st.tpot_slo.data();
+        adm.pred_valid = st.pred_valid.empty() ? nullptr : st.pred_valid.data();
+        const int32_t rc = epp_schedule_admit(b->eng, &batch, any_sub ? &sub : nullptr, any_pred ? &pr : nullptr,
+                                              any_ctx ? &ct : nullptr, any_adm ? &adm : nullptr, st.dec, st.det,
+                                              b->cfg.index_picks ? 1 : 0, b->pick_k > 1 ? &tk : nullptr);
+        st.any_pred.store(0, std::memory_order_relaxed);
+        st.any_subset.store(0, std::memory_order_relaxed);
+        st.any_ctx.store(0, std::memory_order_relaxed);
+        st.any_adm.store(0, std::memory_order_relaxed);
         if (rc != EPP_OK) {
             std::lock_guard<std::mutex> lk(b->err_mu);
             b->last_error = epp_last_error();

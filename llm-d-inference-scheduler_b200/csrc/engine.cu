@@ -83,6 +83,66 @@ struct Slot {                       // per-stream staging for host-pointer batch
     cudaEvent_t done = nullptr;
 };
 
+// Event pairs bracketing the launches of one kernel in the device batch in flight; their elapsed times are summed once
+// it completes.
+struct EventSpans {
+    std::vector<cudaEvent_t> ev;
+    int used = 0;                   // events recorded for the batch in flight
+    EventSpans() = default;
+    EventSpans(const EventSpans &) = delete;
+    EventSpans &operator=(const EventSpans &) = delete;
+    ~EventSpans() { for (cudaEvent_t e : ev) cudaEventDestroy(e); }
+    cudaError_t begin(cudaStream_t s) {
+        while ((int)ev.size() < used + 2) {
+            cudaEvent_t e;
+            cudaError_t err = cudaEventCreate(&e);
+            if (err != cudaSuccess) return err;
+            ev.push_back(e);
+        }
+        return cudaEventRecord(ev[used], s);
+    }
+    cudaError_t end(cudaStream_t s) {
+        const cudaError_t err = cudaEventRecord(ev[used + 1], s);
+        if (err == cudaSuccess) used += 2;
+        return err;
+    }
+    double take_ms() {
+        double t = 0.0;
+        for (int i = 0; i + 1 < used; i += 2) {
+            float t1 = 0;
+            cudaEventElapsedTime(&t1, ev[i], ev[i + 1]);
+            t += t1;
+        }
+        used = 0;
+        return t;
+    }
+};
+
+// The side inputs of one scheduling call: validated on the host by check_inputs before any engine state changes, then
+// staged to the device by stage_inputs.  A call without them stages nothing.
+struct CallInputs {
+    int64_t R = 0;
+    const epp_topk_out *topk = nullptr;
+    const epp_subset *subset = nullptr;         // the caller's arrays, packed by stage_inputs
+    const epp_predictions *preds = nullptr;
+    const epp_context_tokens *ctx = nullptr;
+    std::vector<SubsetRow> sub_rows;            // the restricted requests, ascending
+    uint64_t sub_n_slots = 0;
+    bool use_pred = false;                      // staged: without a latency profile only the admitter reads predictions
+    bool use_ctx = false;                       // staged: only a context-length profile reads the token counts
+    uint64_t n_ent = 0;                         // prediction entries
+    std::vector<AdmitRow> adm_rows;             // the rows an admitter can reject, ascending
+    std::vector<uint32_t> adm_ent;
+    // the staged sections on the device (nullptr: not staged)
+    const SubsetRow *d_sub_rows = nullptr;
+    const uint32_t *d_sub_slots = nullptr, *d_cnt = nullptr, *d_adm_ent = nullptr;
+    const uint64_t *d_off = nullptr;
+    const epp_prediction *d_ent = nullptr;
+    const int64_t *d_ctx = nullptr;
+    const AdmitRow *d_adm_rows = nullptr;
+    bool staged() const { return !sub_rows.empty() || use_pred || use_ctx || !adm_rows.empty(); }
+};
+
 struct epp_engine {
     std::mutex mu;
     epp_config cfg;
@@ -123,25 +183,15 @@ struct epp_engine {
     LabelPlan labels;
     DevBuf lcode;                   // uint8 [labels.keys.size()][E] (LabelFilterDev)
     bool pool_called = false;       // epp_pool_set / epp_pool_set_labels succeeded once: the label filters are fixed
-    // latency predictions (include/epp_engine.h "Latency predictions"): each profile's configuration, the profiles with a
-    // latency piece, and the staged entries of the call in progress (cur_pred: the call passed predictions)
+    // latency predictions (include/epp_engine.h "Latency predictions"): each profile's configuration and the profiles with
+    // a latency piece
     epp_latency_cfg lat_cfg[kMaxProfiles] = {};
     int lat_mask = 0;
-    bool cur_pred = false;
-    DevBuf lat_cnt, lat_off, lat_ent;
-    void *lat_host = nullptr;       // pinned staging of counts, offsets and entries
-    size_t lat_host_cap = 0;
-    cudaEvent_t lat_up_ev = nullptr;    // behind the last upload from lat_host
     // context length (include/epp_engine.h "Context length"): the profiles listing the plugin (they are in lat_mask too),
-    // each one's label key, filtering and per-slot ranges; the staged token counts of the call in progress (cur_ctx)
+    // each one's label key, filtering and per-slot ranges
     int cl_mask = 0, cl_filter = 0;
     std::string cl_label[kMaxProfiles];
     DevBuf cl_rng[kMaxProfiles];    // longlong2 [E] (kernels.h LatView::rng)
-    bool cur_ctx = false;
-    DevBuf ctx_dev;
-    int64_t *ctx_host = nullptr;    // pinned staging of the token counts
-    size_t ctx_host_cap = 0;
-    cudaEvent_t ctx_up_ev = nullptr;    // behind the last upload from ctx_host
     ProfileState prof[kMaxProfiles];
     // no-hit-lru scorer (nohit_lru.cu), allocated only when a profile lists it
     int nohit_mask = 0;             // bit pi: profile pi has the scorer
@@ -158,8 +208,7 @@ struct epp_engine {
     std::mutex if_mu;               // guards if_pending only: releases and resets never wait for a batch
     std::unordered_map<uint32_t, InflightDelta> if_pending;   // folded releases / resets not applied yet
     // two staging sets for the folded deltas: a set is refilled once the apply kernel that read it has run (if_ev)
-    InflightDelta *if_host[2] = {};
-    size_t if_host_cap[2] = {};
+    HostBuf if_host[2];
     DevBuf if_dev[2];
     cudaEvent_t if_ev[2] = {};
     int if_flip = 0;
@@ -222,31 +271,22 @@ struct epp_engine {
     bool committed_once = false;
     bool general = false;           // a profile configures the prefix-cache-affinity-filter or pick_k > 1: every batch takes
                                     // the dense-counter kernel with the full-scan evaluation of pick_general.cuh
-    const epp_topk_out *cur_topk = nullptr;   // top-k destination of the call in progress (under mu)
-    // endpoint subsets of the call in progress (epp_schedule_subset, subset_pick.cu): its restricted requests in ascending
-    // order, or nullptr; their rows and slot lists were validated on the host and copied to sub_rows / sub_slots
-    const std::vector<SubsetRow> *cur_sub = nullptr;
-    DevBuf sub_rows, sub_slots, sub_hits, sub_scratch;
-    std::vector<cudaEvent_t> sub_ev;    // pairs bracketing the subset launches of the device batch in flight
-    int sub_ev_used = 0;                // events of sub_ev recorded for it (last_kernel_ms[6])
-    void *sub_host = nullptr;           // pinned staging of the rows and slots being uploaded
-    size_t sub_host_cap = 0;
-    cudaEvent_t sub_up_ev = nullptr;    // behind the last upload from sub_host
+    // the side inputs of the scheduling call in progress (under mu): set by schedule_impl and with_match_impl for the whole
+    // call (CallScope), nullptr otherwise
+    const CallInputs *cur = nullptr;
+    HostBuf in_host;                // pinned staging of the call's side inputs (stage_inputs)
+    DevBuf in_dev;
+    cudaEvent_t in_ev = nullptr;    // behind the last copy from in_host
+    DevBuf sub_hits, sub_scratch;   // endpoint subsets (subset_pick.cu): written by the subset kernel, parallel to its slots
+    EventSpans sub_spans;           // the subset launches of the device batch in flight (last_kernel_ms[6])
     DevBuf topk_picks[kMaxProfiles], topk_scores;   // device staging of the lists for host batches
-    // admission (include/epp_engine.h "Admission", admit.cu): the admitters, the whole pool's candidate aggregates of the
-    // current snapshot (derived by epp_pool_set), and the rows of the call in progress an admitter can reject (cur_adm,
-    // ascending; their rows and packed entries were validated on the host and copied to adm_rows / adm_ent)
+    // admission (include/epp_engine.h "Admission", admit.cu): the admitters and the whole pool's candidate aggregates of the
+    // current snapshot (derived by epp_pool_set)
     epp_admission_cfg adm{};
     bool adm_on = false;
     int32_t adm_pool_n = 0, adm_idle = 0, adm_cold = 0;
     double adm_sat = 0.0;
-    const std::vector<AdmitRow> *cur_adm = nullptr;
-    DevBuf adm_rows, adm_ent;
-    std::vector<cudaEvent_t> adm_ev;    // pairs bracketing the admission launches of the device batch in flight
-    int adm_ev_used = 0;                // events of adm_ev recorded for it (last_kernel_ms[7])
-    void *adm_host = nullptr;           // pinned staging of the rows and entries being uploaded
-    size_t adm_host_cap = 0;
-    cudaEvent_t adm_up_ev = nullptr;    // behind the last upload from adm_host
+    EventSpans adm_spans;           // the admission launches of the device batch in flight (last_kernel_ms[7])
     int64_t kept_R = 0;             // rows of `hashes` valid for epp_index_add_picked
     int64_t shard_R = 0;            // rows of `hashes` valid for epp_shard_pick / epp_shard_merge
     bool shard_models = false;      // the probed batch had model ids: its copy in `model_ids` feeds epp_shard_pick
@@ -594,29 +634,17 @@ extern "C" int32_t epp_engine_destroy(epp_engine *h) {
     if (!h) return EPP_OK;
     cudaSetDevice(h->cfg.device);
     cudaDeviceSynchronize();
-    if (h->lat_host) cudaFreeHost(h->lat_host);
-    if (h->lat_up_ev) cudaEventDestroy(h->lat_up_ev);
-    if (h->ctx_host) cudaFreeHost(h->ctx_host);
-    if (h->ctx_up_ev) cudaEventDestroy(h->ctx_up_ev);
+    if (h->in_ev) cudaEventDestroy(h->in_ev);
     for (int i = 0; i < 2; i++) {
         if (h->slot[i].stream) cudaStreamDestroy(h->slot[i].stream);
         if (h->slot[i].done) cudaEventDestroy(h->slot[i].done);
     }
     for (auto &ev : h->ev) if (ev) cudaEventDestroy(ev);
     for (auto &ev : h->user_ev) if (ev) cudaEventDestroy(ev);
-    for (auto &ev : h->sub_ev) cudaEventDestroy(ev);
-    if (h->sub_up_ev) cudaEventDestroy(h->sub_up_ev);
-    if (h->sub_host) cudaFreeHost(h->sub_host);
-    for (auto &ev : h->adm_ev) cudaEventDestroy(ev);
-    if (h->adm_up_ev) cudaEventDestroy(h->adm_up_ev);
-    if (h->adm_host) cudaFreeHost(h->adm_host);
     if (h->wc_host) cudaFreeHost(h->wc_host);
     if (h->small_host) cudaFreeHost(h->small_host);
     if (h->small_epoch_host) cudaFreeHost(h->small_epoch_host);
-    for (int i = 0; i < 2; i++) {
-        if (h->if_host[i]) cudaFreeHost(h->if_host[i]);
-        if (h->if_ev[i]) cudaEventDestroy(h->if_ev[i]);
-    }
+    for (auto &ev : h->if_ev) if (ev) cudaEventDestroy(ev);
     for (int g = 0; g < (int)h->p2p_peer.size(); g++)
         if (h->p2p_ipc && g != h->p2p_rank && h->p2p_peer[g]) cudaIpcCloseMemHandle(h->p2p_peer[g]);
     if (h->p2p_buf) cudaFree(h->p2p_buf);
@@ -876,17 +904,10 @@ static int32_t inflight_flush(epp_engine *h, cudaStream_t s, int *launches) {
     h->if_flip ^= 1;
     CUDA_TRY(cudaEventSynchronize(h->if_ev[k]));      // the apply kernel that last read staging set k has run
     const size_t bytes = sizeof(InflightDelta) * d.size();
-    if (h->if_host_cap[k] < bytes) {
-        if (h->if_host[k]) CUDA_TRY(cudaFreeHost(h->if_host[k]));
-        h->if_host[k] = nullptr;
-        h->if_host_cap[k] = 0;
-        const size_t cap = std::max<size_t>(bytes * 2, 4096);
-        CUDA_TRY(cudaHostAlloc(reinterpret_cast<void **>(&h->if_host[k]), cap, cudaHostAllocDefault));
-        h->if_host_cap[k] = cap;
-    }
-    memcpy(h->if_host[k], d.data(), bytes);
+    CUDA_TRY(h->if_host[k].reserve(bytes));
+    memcpy(h->if_host[k].p, d.data(), bytes);
     CUDA_TRY(h->if_dev[k].reserve(bytes, &h->dev_bytes));
-    CUDA_TRY(cudaMemcpyAsync(h->if_dev[k].p, h->if_host[k], bytes, cudaMemcpyHostToDevice, s));
+    CUDA_TRY(cudaMemcpyAsync(h->if_dev[k].p, h->if_host[k].p, bytes, cudaMemcpyHostToDevice, s));
     CUDA_TRY(launch_inflight_apply(inflight_state(h), h->if_dev[k].as<InflightDelta>(), (int32_t)d.size(), s, launches));
     CUDA_TRY(cudaEventRecord(h->if_ev[k], s));
     return inflight_rederive(h, s, launches);
@@ -1825,12 +1846,10 @@ static LatView lat_view(epp_engine *h, int64_t r0) {
     for (int i = 0; i < kMaxProfiles; i++) v.cfg[i] = h->lat_cfg[i];
     for (int i = 0; i < kMaxProfiles; i++) v.rng[i] = (h->cl_mask >> i) & 1 ? h->cl_rng[i].as<longlong2>() : nullptr;
     v.cl_filter = h->cl_filter;
-    if (h->cur_ctx) v.ctx = h->ctx_dev.as<int64_t>();
-    if (h->cur_pred) {
-        v.cnt = h->lat_cnt.as<uint32_t>();
-        v.off = h->lat_off.as<uint64_t>();
-        v.ent = h->lat_ent.as<epp_prediction>();
-    }
+    v.ctx = h->cur->d_ctx;
+    v.cnt = h->cur->d_cnt;
+    v.off = h->cur->d_off;
+    v.ent = h->cur->d_ent;
     return v;
 }
 
@@ -1936,22 +1955,8 @@ static int32_t finish_async(epp_engine *h) {
         h->stats.last_kernel_ms[4 + u] = tu;
         h->post_pick_timed[u] = false;
     }
-    double ts = 0.0;
-    for (int i = 0; i + 1 < h->sub_ev_used; i += 2) {
-        float t1 = 0;
-        cudaEventElapsedTime(&t1, h->sub_ev[i], h->sub_ev[i + 1]);
-        ts += t1;
-    }
-    h->stats.last_kernel_ms[6] = ts;
-    h->sub_ev_used = 0;
-    double ta = 0.0;
-    for (int i = 0; i + 1 < h->adm_ev_used; i += 2) {
-        float t1 = 0;
-        cudaEventElapsedTime(&t1, h->adm_ev[i], h->adm_ev[i + 1]);
-        ta += t1;
-    }
-    h->stats.last_kernel_ms[7] = ta;
-    h->adm_ev_used = 0;
+    h->stats.last_kernel_ms[6] = h->sub_spans.take_ms();
+    h->stats.last_kernel_ms[7] = h->adm_spans.take_ms();
     return EPP_OK;
 }
 
@@ -1959,34 +1964,23 @@ static int32_t finish_async(epp_engine *h) {
 // kernels of the same rows (pp: their PickParams, trimmed rows included).  timed: bracket it for last_kernel_ms[6].
 static int32_t launch_subset(epp_engine *h, const PickParams &pp, int64_t r0, int64_t r1, cudaStream_t s, int *launches,
                              bool timed) {
-    if (!h->cur_sub) return EPP_OK;
-    const std::vector<SubsetRow> &rows = *h->cur_sub;
+    const std::vector<SubsetRow> &rows = h->cur->sub_rows;
     auto below = [](const SubsetRow &a, int64_t r) { return (int64_t)a.row < r; };
     const size_t lo = std::lower_bound(rows.begin(), rows.end(), r0, below) - rows.begin();
     const size_t hi = std::lower_bound(rows.begin(), rows.end(), r1, below) - rows.begin();
     if (lo == hi) return EPP_OK;
     SubsetView sv;
-    sv.rows = h->sub_rows.as<SubsetRow>() + lo;
+    sv.rows = h->cur->d_sub_rows + lo;
     sv.n_rows = (int32_t)(hi - lo);
     sv.r0 = r0;
-    sv.slots = h->sub_slots.as<uint32_t>();
+    sv.slots = h->cur->d_sub_slots;
     sv.hits = h->sub_hits.as<int32_t>();
     sv.scratch = h->sub_scratch.as<int32_t>();
     sv.nohit_pos = h->nohit_mask ? h->nh_pos.as<int32_t>() : nullptr;
-    if (timed) {
-        while ((int)h->sub_ev.size() < h->sub_ev_used + 2) {
-            cudaEvent_t ev;
-            CUDA_TRY(cudaEventCreate(&ev));
-            h->sub_ev.push_back(ev);
-        }
-        CUDA_TRY(cudaEventRecord(h->sub_ev[h->sub_ev_used], s));
-    }
+    if (timed) CUDA_TRY(h->sub_spans.begin(s));
     const LatView lv = lat_view(h, r0);
     CUDA_TRY(launch_subset_pick(pp, sv, h->lat_mask ? &lv : nullptr, s, launches));
-    if (timed) {
-        CUDA_TRY(cudaEventRecord(h->sub_ev[h->sub_ev_used + 1], s));
-        h->sub_ev_used += 2;
-    }
+    if (timed) CUDA_TRY(h->sub_spans.end(s));
     return EPP_OK;
 }
 
@@ -1994,19 +1988,18 @@ static int32_t launch_subset(epp_engine *h, const PickParams &pp, int64_t r0, in
 // included) of the same rows.  dec / det / tk: the call's rows from request 0 on.  timed: bracket it for last_kernel_ms[7].
 static int32_t launch_admission(epp_engine *h, int64_t r0, int64_t r1, epp_decision *dec, epp_decision_detail *det,
                                 const TopkRows &tk, cudaStream_t s, int *launches, bool timed) {
-    if (!h->cur_adm) return EPP_OK;
-    const std::vector<AdmitRow> &rows = *h->cur_adm;
+    const std::vector<AdmitRow> &rows = h->cur->adm_rows;
     auto below = [](const AdmitRow &a, int64_t r) { return (int64_t)a.row < r; };
     const size_t lo = std::lower_bound(rows.begin(), rows.end(), r0, below) - rows.begin();
     const size_t hi = std::lower_bound(rows.begin(), rows.end(), r1, below) - rows.begin();
     if (lo == hi) return EPP_OK;
     AdmitParams p;
     memset(&p, 0, sizeof p);
-    p.rows = h->adm_rows.as<AdmitRow>() + lo;
+    p.rows = h->cur->d_adm_rows + lo;
     p.n_rows = (int32_t)(hi - lo);
     p.E = h->cfg.max_endpoints;
-    p.ent = h->adm_ent.as<uint32_t>();
-    p.sub_slots = h->sub_slots.as<uint32_t>();
+    p.ent = h->cur->d_adm_ent;
+    p.sub_slots = h->cur->d_sub_slots;
     p.role = h->role.as<uint8_t>();
     p.kv = h->kv.as<double>();
     p.waiting = h->waiting.as<int32_t>();
@@ -2028,19 +2021,9 @@ static int32_t launch_admission(epp_engine *h, int64_t r0, int64_t r1, epp_decis
         for (int i = 0; i < kMaxProfiles; i++) p.topk_picks[i] = tk.picks[i];
         p.topk_scores = tk.scores;
     }
-    if (timed) {
-        while ((int)h->adm_ev.size() < h->adm_ev_used + 2) {
-            cudaEvent_t ev;
-            CUDA_TRY(cudaEventCreate(&ev));
-            h->adm_ev.push_back(ev);
-        }
-        CUDA_TRY(cudaEventRecord(h->adm_ev[h->adm_ev_used], s));
-    }
+    if (timed) CUDA_TRY(h->adm_spans.begin(s));
     CUDA_TRY(launch_admit(p, s, launches));
-    if (timed) {
-        CUDA_TRY(cudaEventRecord(h->adm_ev[h->adm_ev_used + 1], s));
-        h->adm_ev_used += 2;
-    }
+    if (timed) CUDA_TRY(h->adm_spans.end(s));
     return EPP_OK;
 }
 
@@ -2225,8 +2208,8 @@ static int32_t run_device(epp_engine *h, const BatchView &v, Call &call) {
     if (v.offsets) EPP_TRY(device_offsets_or_bits(h, v.offsets, R, s0, &or_bits));
     CUDA_TRY(cudaMemsetAsync(h->work_counters.p, 0, sizeof(unsigned long long) * 4, s0));
     const int64_t min_chunk = 4096;
-    h->sub_ev_used = 0;
-    h->adm_ev_used = 0;
+    h->sub_spans.used = 0;
+    h->adm_spans.used = 0;
     epp_decision *dec = call.out_dec ? call.out_dec : h->decisions.as<epp_decision>();
     PickParams pp;                                 // the rows of the last launch_rows, for their subset launch
     if (call.pipelined) {
@@ -2401,7 +2384,7 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
     }
     if (h->async_pending && !(v.device && v.async)) EPP_TRY(finish_async(h));
     Call call{mode, out_hashes, out_nblocks, out_match, out_total, out_dec, out_detail, out_detail};
-    EPP_TRY(topk_rows(h, mode == Mode::Schedule ? h->cur_topk : nullptr, v.device, R, call.tk));
+    EPP_TRY(topk_rows(h, mode == Mode::Schedule ? h->cur->topk : nullptr, v.device, R, call.tk));
     call.pipelined = v.device && v.async && mode == Mode::Schedule && h->dev_chunks > 1 && R >= 2 * 4096 && !h->pick_global;
     // the endpoint-sharded mode's local table is not the global one: its rows stay whole
     call.trim = mode == Mode::Schedule && !keep_hashes && h->hash_trim && !sharded(h);
@@ -2417,7 +2400,7 @@ static int32_t run_batch(epp_engine *h, const BatchView &v, Mode mode, uint64_t 
     // small host batch in pinned memory: one zero-copy launch, no copy engine, no stream synchronisation (not for a batch
     // with restricted requests or admission rows: the kernel hands the decisions to the host before a subset or admission
     // launch could rewrite them)
-    if (mode == Mode::Schedule && !call.tk.on && out_dec && !h->cur_sub && !h->cur_adm) {
+    if (mode == Mode::Schedule && !call.tk.on && out_dec && h->cur->sub_rows.empty() && h->cur->adm_rows.empty()) {
         const uint8_t *data_dev = nullptr;
         const int sm = small_batch_mode(h, v, &data_dev);
         if (sm) return run_small(h, v, sm, data_dev, out_dec, out_detail);
@@ -2487,39 +2470,6 @@ static int32_t check_subset(const epp_engine *h, int64_t R, const epp_subset *s,
         total += n;
     }
     *n_slots = total;
-    return EPP_OK;
-}
-
-// The restricted rows and their slots to the device on stream 0, behind everything enqueued so far (a pipelined batch's
-// stream 1 joins first), through the engine's pinned staging: the slots are packed into it straight from the caller's
-// arrays and copied asynchronously.  The staging is refilled only once the previous call's copy has run (sub_up_ev).
-static int32_t upload_subset(epp_engine *h, const std::vector<SubsetRow> &rows, const epp_subset *s, uint64_t n_slots) {
-    cudaStream_t s0 = h->slot[0].stream;
-    EPP_TRY(join_streams(h));
-    const size_t ns = (size_t)std::max<uint64_t>(n_slots, 1);
-    CUDA_TRY(h->sub_rows.reserve(sizeof(SubsetRow) * rows.size(), &h->dev_bytes));
-    CUDA_TRY(h->sub_slots.reserve(sizeof(uint32_t) * ns, &h->dev_bytes));
-    CUDA_TRY(h->sub_hits.reserve(sizeof(int32_t) * ns, &h->dev_bytes));
-    CUDA_TRY(h->sub_scratch.reserve(sizeof(int32_t) * ns, &h->dev_bytes));
-    if (!h->sub_up_ev) CUDA_TRY(cudaEventCreateWithFlags(&h->sub_up_ev, cudaEventDisableTiming));
-    else CUDA_TRY(cudaEventSynchronize(h->sub_up_ev));
-    const size_t rows_bytes = (sizeof(SubsetRow) * rows.size() + 15) & ~(size_t)15;
-    const size_t need = rows_bytes + sizeof(uint32_t) * (size_t)n_slots;
-    if (need > h->sub_host_cap) {
-        if (h->sub_host) CUDA_TRY(cudaFreeHost(h->sub_host));
-        h->sub_host = nullptr;
-        h->sub_host_cap = 0;
-        CUDA_TRY(cudaHostAlloc(&h->sub_host, need, cudaHostAllocDefault));
-        h->sub_host_cap = need;
-    }
-    uint8_t *stage = static_cast<uint8_t *>(h->sub_host);
-    memcpy(stage, rows.data(), sizeof(SubsetRow) * rows.size());
-    uint32_t *dst = reinterpret_cast<uint32_t *>(stage + rows_bytes);
-    for (const SubsetRow &row : rows)
-        if (row.n) memcpy(dst + row.off, s->slots + s->offsets[row.row], sizeof(uint32_t) * row.n);
-    CUDA_TRY(cudaMemcpyAsync(h->sub_rows.p, stage, sizeof(SubsetRow) * rows.size(), cudaMemcpyHostToDevice, s0));
-    if (n_slots) CUDA_TRY(cudaMemcpyAsync(h->sub_slots.p, dst, sizeof(uint32_t) * (size_t)n_slots, cudaMemcpyHostToDevice, s0));
-    CUDA_TRY(cudaEventRecord(h->sub_up_ev, s0));
     return EPP_OK;
 }
 
@@ -2597,68 +2547,6 @@ static int32_t check_ctx(int64_t R, const epp_context_tokens *c) {
     return EPP_OK;
 }
 
-// The token counts to the device on stream 0, behind everything enqueued so far, through the engine's pinned staging
-// (refilled only once the previous call's copy has run), as upload_predictions does.
-static int32_t upload_ctx(epp_engine *h, int64_t R, const epp_context_tokens *c) {
-    cudaStream_t s0 = h->slot[0].stream;
-    EPP_TRY(join_streams(h));
-    const size_t bytes = sizeof(int64_t) * (size_t)R;
-    CUDA_TRY(h->ctx_dev.reserve(bytes, &h->dev_bytes));
-    if (!h->ctx_up_ev) CUDA_TRY(cudaEventCreateWithFlags(&h->ctx_up_ev, cudaEventDisableTiming));
-    else CUDA_TRY(cudaEventSynchronize(h->ctx_up_ev));
-    if (bytes > h->ctx_host_cap) {
-        if (h->ctx_host) CUDA_TRY(cudaFreeHost(h->ctx_host));
-        h->ctx_host = nullptr;
-        h->ctx_host_cap = 0;
-        CUDA_TRY(cudaHostAlloc(reinterpret_cast<void **>(&h->ctx_host), bytes, cudaHostAllocDefault));
-        h->ctx_host_cap = bytes;
-    }
-    memcpy(h->ctx_host, c->tokens, bytes);
-    CUDA_TRY(cudaMemcpyAsync(h->ctx_dev.p, h->ctx_host, bytes, cudaMemcpyHostToDevice, s0));
-    CUDA_TRY(cudaEventRecord(h->ctx_up_ev, s0));
-    return EPP_OK;
-}
-
-// Counts, packed offsets and entries to the device on stream 0, behind everything enqueued so far, through the engine's
-// pinned staging (refilled only once the previous call's copy has run), as upload_subset does.
-static int32_t upload_predictions(epp_engine *h, int64_t R, const epp_predictions *p, uint64_t n_ent) {
-    cudaStream_t s0 = h->slot[0].stream;
-    EPP_TRY(join_streams(h));
-    const size_t nr = (size_t)std::max<int64_t>(R, 1), ne = (size_t)std::max<uint64_t>(n_ent, 1);
-    CUDA_TRY(h->lat_cnt.reserve(sizeof(uint32_t) * nr, &h->dev_bytes));
-    CUDA_TRY(h->lat_off.reserve(sizeof(uint64_t) * nr, &h->dev_bytes));
-    CUDA_TRY(h->lat_ent.reserve(sizeof(epp_prediction) * ne, &h->dev_bytes));
-    if (!h->lat_up_ev) CUDA_TRY(cudaEventCreateWithFlags(&h->lat_up_ev, cudaEventDisableTiming));
-    else CUDA_TRY(cudaEventSynchronize(h->lat_up_ev));
-    const size_t off_at = (sizeof(uint32_t) * nr + 15) & ~(size_t)15;
-    const size_t ent_at = off_at + sizeof(uint64_t) * nr;
-    const size_t need = ent_at + sizeof(epp_prediction) * (size_t)n_ent;
-    if (need > h->lat_host_cap) {
-        if (h->lat_host) CUDA_TRY(cudaFreeHost(h->lat_host));
-        h->lat_host = nullptr;
-        h->lat_host_cap = 0;
-        CUDA_TRY(cudaHostAlloc(&h->lat_host, need, cudaHostAllocDefault));
-        h->lat_host_cap = need;
-    }
-    uint8_t *stage = static_cast<uint8_t *>(h->lat_host);
-    uint32_t *cnt = reinterpret_cast<uint32_t *>(stage);
-    uint64_t *off = reinterpret_cast<uint64_t *>(stage + off_at);
-    epp_prediction *ent = reinterpret_cast<epp_prediction *>(stage + ent_at);
-    uint64_t o = 0;
-    for (int64_t r = 0; r < R; r++) {
-        const uint32_t n = p->counts[r];
-        cnt[r] = n;
-        off[r] = o;
-        if (n) memcpy(ent + o, p->entries + p->offsets[r], sizeof(epp_prediction) * n);
-        o += n;
-    }
-    CUDA_TRY(cudaMemcpyAsync(h->lat_cnt.p, cnt, sizeof(uint32_t) * (size_t)R, cudaMemcpyHostToDevice, s0));
-    CUDA_TRY(cudaMemcpyAsync(h->lat_off.p, off, sizeof(uint64_t) * (size_t)R, cudaMemcpyHostToDevice, s0));
-    if (n_ent) CUDA_TRY(cudaMemcpyAsync(h->lat_ent.p, ent, sizeof(epp_prediction) * (size_t)n_ent, cudaMemcpyHostToDevice, s0));
-    CUDA_TRY(cudaEventRecord(h->lat_up_ev, s0));
-    return EPP_OK;
-}
-
 // Validates a call's admission inputs (R requests; preds: the call's predictions, validated, or nullptr; sub: its
 // restricted rows, ascending) and lists, in ascending request order, the rows an admitter can reject, with the packed
 // entries of the latency-slo-admitter's rows (slot | both validity bits << 31).  Nothing of the engine changes.
@@ -2692,33 +2580,104 @@ static int32_t check_admission(const epp_engine *h, int64_t R, const epp_admissi
     return EPP_OK;
 }
 
-// The listed rows and their entries to the device on stream 0, behind everything enqueued so far (a pipelined batch's
-// stream 1 joins first), through the engine's pinned staging, as upload_subset does.
-static int32_t upload_admission(epp_engine *h, const std::vector<AdmitRow> &rows, const std::vector<uint32_t> &ent) {
-    cudaStream_t s0 = h->slot[0].stream;
-    EPP_TRY(join_streams(h));
-    CUDA_TRY(h->adm_rows.reserve(sizeof(AdmitRow) * rows.size(), &h->dev_bytes));
-    CUDA_TRY(h->adm_ent.reserve(sizeof(uint32_t) * std::max<size_t>(ent.size(), 1), &h->dev_bytes));
-    if (!h->adm_up_ev) CUDA_TRY(cudaEventCreateWithFlags(&h->adm_up_ev, cudaEventDisableTiming));
-    else CUDA_TRY(cudaEventSynchronize(h->adm_up_ev));
-    const size_t rows_bytes = sizeof(AdmitRow) * rows.size();
-    const size_t need = rows_bytes + sizeof(uint32_t) * ent.size();
-    if (need > h->adm_host_cap) {
-        if (h->adm_host) CUDA_TRY(cudaFreeHost(h->adm_host));
-        h->adm_host = nullptr;
-        h->adm_host_cap = 0;
-        CUDA_TRY(cudaHostAlloc(&h->adm_host, need, cudaHostAllocDefault));
-        h->adm_host_cap = need;
-    }
-    uint8_t *stage = static_cast<uint8_t *>(h->adm_host);
-    memcpy(stage, rows.data(), rows_bytes);
-    if (!ent.empty()) memcpy(stage + rows_bytes, ent.data(), sizeof(uint32_t) * ent.size());
-    CUDA_TRY(cudaMemcpyAsync(h->adm_rows.p, stage, rows_bytes, cudaMemcpyHostToDevice, s0));
-    if (!ent.empty())
-        CUDA_TRY(cudaMemcpyAsync(h->adm_ent.p, stage + rows_bytes, sizeof(uint32_t) * ent.size(), cudaMemcpyHostToDevice, s0));
-    CUDA_TRY(cudaEventRecord(h->adm_up_ev, s0));
+// Validates a call's side inputs (R requests; each input nullptr when not passed) into in: subsets, predictions, context
+// lengths, then admission, and which of them the engine reads.  Nothing of the engine changes.
+// latency_ok: as check_subset.
+static int32_t check_inputs(const epp_engine *h, int64_t R, const epp_subset *subset, bool latency_ok,
+                            const epp_predictions *preds, const epp_context_tokens *ctx, const epp_admission *adm,
+                            CallInputs &in) {
+    in.R = R;
+    in.subset = subset;
+    in.preds = preds;
+    in.ctx = ctx;
+    if (subset) EPP_TRY(check_subset(h, R, subset, in.sub_rows, &in.sub_n_slots, latency_ok));
+    if (preds) EPP_TRY(check_predictions(h, R, preds, &in.n_ent));
+    if (ctx) EPP_TRY(check_ctx(R, ctx));
+    if (adm) EPP_TRY(check_admission(h, R, adm, preds, in.sub_rows, in.adm_rows, in.adm_ent));
+    in.use_pred = preds && R && h->lat_mask;
+    in.use_ctx = ctx && R && h->cl_mask;
     return EPP_OK;
 }
+
+// A validated call's staged inputs to the device on stream 0, behind everything enqueued so far (a pipelined batch's
+// stream 1 joins first): the sections are packed into the engine's pinned staging, each from a 256-byte boundary (the
+// alignment of a cudaMalloc), and go over in one copy.  The staging is refilled only once the previous call's copy has
+// run (in_ev).  Sets in's device pointers.
+static int32_t stage_inputs(epp_engine *h, CallInputs &in) {
+    if (!in.staged()) return EPP_OK;
+    const size_t R = (size_t)in.R;
+    size_t total = 0;
+    auto section = [&total](size_t bytes) {
+        const size_t at = (total + 255) & ~(size_t)255;
+        total = at + bytes;
+        return at;
+    };
+    const size_t at_rows = section(sizeof(SubsetRow) * in.sub_rows.size());
+    const size_t at_slots = section(sizeof(uint32_t) * (size_t)in.sub_n_slots);
+    const size_t at_cnt = section(in.use_pred ? sizeof(uint32_t) * R : 0);
+    const size_t at_off = section(in.use_pred ? sizeof(uint64_t) * R : 0);
+    const size_t at_ent = section(in.use_pred ? sizeof(epp_prediction) * (size_t)in.n_ent : 0);
+    const size_t at_ctx = section(in.use_ctx ? sizeof(int64_t) * R : 0);
+    const size_t at_adm = section(sizeof(AdmitRow) * in.adm_rows.size());
+    const size_t at_adm_ent = section(sizeof(uint32_t) * in.adm_ent.size());
+    cudaStream_t s0 = h->slot[0].stream;
+    EPP_TRY(join_streams(h));
+    CUDA_TRY(h->in_dev.reserve(total, &h->dev_bytes));
+    if (!in.sub_rows.empty()) {
+        const size_t ns = (size_t)std::max<uint64_t>(in.sub_n_slots, 1);
+        CUDA_TRY(h->sub_hits.reserve(sizeof(int32_t) * ns, &h->dev_bytes));
+        CUDA_TRY(h->sub_scratch.reserve(sizeof(int32_t) * ns, &h->dev_bytes));
+    }
+    if (!h->in_ev) CUDA_TRY(cudaEventCreateWithFlags(&h->in_ev, cudaEventDisableTiming));
+    else CUDA_TRY(cudaEventSynchronize(h->in_ev));
+    CUDA_TRY(h->in_host.reserve(total));
+    uint8_t *stage = h->in_host.as<uint8_t>();
+    const uint8_t *dev = h->in_dev.as<uint8_t>();
+    if (!in.sub_rows.empty()) {
+        memcpy(stage + at_rows, in.sub_rows.data(), sizeof(SubsetRow) * in.sub_rows.size());
+        uint32_t *slots = reinterpret_cast<uint32_t *>(stage + at_slots);
+        for (const SubsetRow &row : in.sub_rows)
+            if (row.n) memcpy(slots + row.off, in.subset->slots + in.subset->offsets[row.row], sizeof(uint32_t) * row.n);
+        in.d_sub_rows = reinterpret_cast<const SubsetRow *>(dev + at_rows);
+        in.d_sub_slots = reinterpret_cast<const uint32_t *>(dev + at_slots);
+    }
+    if (in.use_pred) {
+        uint32_t *cnt = reinterpret_cast<uint32_t *>(stage + at_cnt);
+        uint64_t *off = reinterpret_cast<uint64_t *>(stage + at_off);
+        epp_prediction *ent = reinterpret_cast<epp_prediction *>(stage + at_ent);
+        uint64_t o = 0;
+        for (size_t r = 0; r < R; r++) {
+            const uint32_t n = in.preds->counts[r];
+            cnt[r] = n;
+            off[r] = o;
+            if (n) memcpy(ent + o, in.preds->entries + in.preds->offsets[r], sizeof(epp_prediction) * n);
+            o += n;
+        }
+        in.d_cnt = reinterpret_cast<const uint32_t *>(dev + at_cnt);
+        in.d_off = reinterpret_cast<const uint64_t *>(dev + at_off);
+        in.d_ent = reinterpret_cast<const epp_prediction *>(dev + at_ent);
+    }
+    if (in.use_ctx) {
+        memcpy(stage + at_ctx, in.ctx->tokens, sizeof(int64_t) * R);
+        in.d_ctx = reinterpret_cast<const int64_t *>(dev + at_ctx);
+    }
+    if (!in.adm_rows.empty()) {
+        memcpy(stage + at_adm, in.adm_rows.data(), sizeof(AdmitRow) * in.adm_rows.size());
+        if (!in.adm_ent.empty()) memcpy(stage + at_adm_ent, in.adm_ent.data(), sizeof(uint32_t) * in.adm_ent.size());
+        in.d_adm_rows = reinterpret_cast<const AdmitRow *>(dev + at_adm);
+        in.d_adm_ent = reinterpret_cast<const uint32_t *>(dev + at_adm_ent);
+    }
+    CUDA_TRY(cudaMemcpyAsync(h->in_dev.p, stage, total, cudaMemcpyHostToDevice, s0));
+    CUDA_TRY(cudaEventRecord(h->in_ev, s0));
+    return EPP_OK;
+}
+
+// The engine's call in progress (epp_engine::cur) for the life of a scheduling call, whichever way it returns.
+struct CallScope {
+    epp_engine *h;
+    CallScope(epp_engine *e, const CallInputs *in) : h(e) { h->cur = in; }
+    ~CallScope() { h->cur = nullptr; }
+};
 
 static int32_t schedule_impl(epp_engine *h, const epp_batch *batch, epp_decision *out, epp_decision_detail *detail,
                              int32_t keep_hashes, const epp_topk_out *topk, const epp_subset *subset = nullptr,
@@ -2732,37 +2691,14 @@ static int32_t schedule_impl(epp_engine *h, const epp_batch *batch, epp_decision
     EPP_TRY(check_batch(h, batch, v));
     if (topk) EPP_TRY(check_topk(h, topk));
     if (h->cfg.encode_enabled && v.multimodal && !detail) return fail(EPP_ERR_INVALID, "an encode profile is configured and the batch flags multimodal requests: `detail` (which carries the encode pick) must not be NULL");
-    std::vector<SubsetRow> sub_rows;
-    uint64_t sub_n_slots = 0;
-    if (subset) EPP_TRY(check_subset(h, v.R, subset, sub_rows, &sub_n_slots, subset_latency_ok));
-    uint64_t n_ent = 0;
-    if (preds) EPP_TRY(check_predictions(h, v.R, preds, &n_ent));
-    if (ctx) EPP_TRY(check_ctx(v.R, ctx));
-    std::vector<AdmitRow> adm_rows;
-    std::vector<uint32_t> adm_ent;
-    if (adm) EPP_TRY(check_admission(h, v.R, adm, preds, sub_rows, adm_rows, adm_ent));
-    const bool use_ctx = ctx && v.R && h->cl_mask;
-    const bool use_pred = preds && v.R && h->lat_mask;     // without a latency profile only the admitter reads them
-    if (!sub_rows.empty() || use_pred || use_ctx || !adm_rows.empty()) {
-        if (!h->pool_ready) return fail(EPP_ERR_STATE, "epp_pool_set has not been called");
-    }
-    if (!sub_rows.empty()) EPP_TRY(upload_subset(h, sub_rows, subset, sub_n_slots));
-    if (use_pred) EPP_TRY(upload_predictions(h, v.R, preds, n_ent));
-    if (use_ctx) EPP_TRY(upload_ctx(h, v.R, ctx));
-    if (!adm_rows.empty()) EPP_TRY(upload_admission(h, adm_rows, adm_ent));
+    CallInputs in;
+    in.topk = topk;
+    EPP_TRY(check_inputs(h, v.R, subset, subset_latency_ok, preds, ctx, adm, in));
+    if (in.staged() && !h->pool_ready) return fail(EPP_ERR_STATE, "epp_pool_set has not been called");
+    EPP_TRY(stage_inputs(h, in));
     h->kept_R = 0;
-    h->cur_topk = topk;
-    h->cur_sub = sub_rows.empty() ? nullptr : &sub_rows;
-    h->cur_pred = use_pred;
-    h->cur_ctx = use_ctx;
-    h->cur_adm = adm_rows.empty() ? nullptr : &adm_rows;
-    const int32_t rc = run_batch(h, v, Mode::Schedule, nullptr, nullptr, out, detail, nullptr, nullptr, keep_hashes != 0);
-    h->cur_topk = nullptr;
-    h->cur_sub = nullptr;
-    h->cur_pred = false;
-    h->cur_ctx = false;
-    h->cur_adm = nullptr;
-    EPP_TRY(rc);
+    const CallScope scope(h, &in);
+    EPP_TRY(run_batch(h, v, Mode::Schedule, nullptr, nullptr, out, detail, nullptr, nullptr, keep_hashes != 0));
     h->stats.n_batches++;
     h->stats.n_decisions += (uint64_t)v.R;
     if (keep_hashes && v.R) {
@@ -2918,27 +2854,15 @@ static int32_t with_match_impl(epp_engine *h, int64_t n_requests, const int32_t 
     if (!h || n_requests < 0 || (n_requests && (!match || !total || !out))) return fail(EPP_ERR_INVALID, "bad arguments");
     std::lock_guard<std::mutex> lk(h->mu);
     if (topk) EPP_TRY(check_topk(h, topk));
-    uint64_t n_ent = 0;
-    if (preds) EPP_TRY(check_predictions(h, n_requests, preds, &n_ent));
-    if (ctx) EPP_TRY(check_ctx(n_requests, ctx));
-    std::vector<AdmitRow> adm_rows;
-    std::vector<uint32_t> adm_ent;
-    if (adm) EPP_TRY(check_admission(h, n_requests, adm, preds, {}, adm_rows, adm_ent));
+    CallInputs in;
+    in.topk = topk;
+    EPP_TRY(check_inputs(h, n_requests, nullptr, false, preds, ctx, adm, in));
     EPP_TRY(set_device(h));
     EPP_TRY(join_streams(h));
     if (!h->pool_ready) return fail(EPP_ERR_STATE, "epp_pool_set has not been called");
     if (n_requests == 0) return EPP_OK;
-    const bool use_pred = preds && h->lat_mask;    // without a latency profile only the admitter reads them
-    if (use_pred) EPP_TRY(upload_predictions(h, n_requests, preds, n_ent));
-    if (ctx && h->cl_mask) EPP_TRY(upload_ctx(h, n_requests, ctx));
-    if (!adm_rows.empty()) EPP_TRY(upload_admission(h, adm_rows, adm_ent));
-    h->cur_pred = use_pred;
-    h->cur_ctx = ctx && h->cl_mask;
-    h->cur_adm = adm_rows.empty() ? nullptr : &adm_rows;
-    struct PredReset {                             // the call's predictions, token counts and admission rows end with it,
-        epp_engine *h;                             // whichever way it returns
-        ~PredReset() { h->cur_pred = false; h->cur_ctx = false; h->cur_adm = nullptr; }
-    } pred_reset{h};
+    EPP_TRY(stage_inputs(h, in));
+    const CallScope scope(h, &in);
     const size_t R = (size_t)n_requests;
     cudaStream_t s = h->slot[0].stream;
     const bool dev = (flags & EPP_BATCH_DEVICE_PTRS) != 0;

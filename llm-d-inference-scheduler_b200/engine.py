@@ -634,46 +634,28 @@ class Engine:
         mids = None if model_ids is None else np.ascontiguousarray(model_ids, dtype=np.uint32)
         if admission is not None:
             ad, ad_keep = _admission_struct(admission, R, predictions)
-            ct, ctx_arr = _context_struct(context_tokens, R) if context_tokens is not None else (None, None)
-            if predictions is not None and len(predictions) != R:
-                raise ValueError(f"predictions has {len(predictions)} entries for {R} requests")
-            packed = pack_predictions(predictions) if predictions is not None else None
-            pr = _predictions_struct(packed) if packed is not None else None
-            lists, tk = self._topk_out(R) if topk else (None, None)
-            self._check(self._lib.epp_schedule_with_match_admit(
-                self._h, R, _ptr(match), _ptr(total), _ptr(mids), _ptr(il), block_size_tokens, _ptr(dec), _ptr(det), 0,
-                C.byref(tk) if topk else None, C.byref(pr) if pr is not None else None,
-                C.byref(ct) if ct is not None else None, C.byref(ad)))
-            return (dec, det, lists) if topk else (dec, det)
-        if context_tokens is not None:
-            ct, ctx_arr = _context_struct(context_tokens, R)
-            if predictions is not None and len(predictions) != R:
-                raise ValueError(f"predictions has {len(predictions)} entries for {R} requests")
-            packed = pack_predictions(predictions) if predictions is not None else None
-            pr = _predictions_struct(packed) if packed is not None else None
-            lists, tk = self._topk_out(R) if topk else (None, None)
-            self._check(self._lib.epp_schedule_with_match_ctx(
-                self._h, R, _ptr(match), _ptr(total), _ptr(mids), _ptr(il), block_size_tokens, _ptr(dec), _ptr(det), 0,
-                C.byref(tk) if topk else None, C.byref(pr) if pr is not None else None, C.byref(ct)))
-            return (dec, det, lists) if topk else (dec, det)
-        if predictions is not None:
-            if len(predictions) != R:
-                raise ValueError(f"predictions has {len(predictions)} entries for {R} requests")
-            packed = pack_predictions(predictions)
-            pr = _predictions_struct(packed)
-            lists, tk = self._topk_out(R) if topk else (None, None)
-            self._check(self._lib.epp_schedule_with_match_predicted(
-                self._h, R, _ptr(match), _ptr(total), _ptr(mids), _ptr(il), block_size_tokens, _ptr(dec), _ptr(det), 0,
-                C.byref(tk) if topk else None, C.byref(pr)))
-            return (dec, det, lists) if topk else (dec, det)
-        if not topk:
-            self._check(self._lib.epp_schedule_with_match(self._h, R, _ptr(match), _ptr(total), _ptr(mids), _ptr(il),
-                                                          block_size_tokens, _ptr(dec), _ptr(det), 0))
-            return dec, det
-        lists, tk = self._topk_out(R)
-        self._check(self._lib.epp_schedule_with_match_topk(self._h, R, _ptr(match), _ptr(total), _ptr(mids), _ptr(il),
-                                                           block_size_tokens, _ptr(dec), _ptr(det), 0, C.byref(tk)))
-        return dec, det, lists
+        ct, ctx_arr = _context_struct(context_tokens, R) if context_tokens is not None else (None, None)
+        if predictions is not None and len(predictions) != R:
+            raise ValueError(f"predictions has {len(predictions)} entries for {R} requests")
+        packed = pack_predictions(predictions) if predictions is not None else None
+        pr = _predictions_struct(packed) if packed is not None else None
+        lists, tk = self._topk_out(R) if topk else (None, None)
+        args = (self._h, R, _ptr(match), _ptr(total), _ptr(mids), _ptr(il), block_size_tokens, _ptr(dec), _ptr(det), 0)
+        tkp = C.byref(tk) if topk else None
+        prp = C.byref(pr) if pr is not None else None
+        if admission is not None:
+            rc = self._lib.epp_schedule_with_match_admit(*args, tkp, prp, C.byref(ct) if ct is not None else None,
+                                                         C.byref(ad))
+        elif ct is not None:
+            rc = self._lib.epp_schedule_with_match_ctx(*args, tkp, prp, C.byref(ct))
+        elif pr is not None:
+            rc = self._lib.epp_schedule_with_match_predicted(*args, tkp, prp)
+        elif topk:
+            rc = self._lib.epp_schedule_with_match_topk(*args, tkp)
+        else:
+            rc = self._lib.epp_schedule_with_match(*args)
+        self._check(rc)
+        return (dec, det, lists) if topk else (dec, det)
 
     def synchronize(self):
         self._check(self._lib.epp_synchronize(self._h))
@@ -803,53 +785,35 @@ class Batcher:
         n = len(buf)
         ptr = buf.ctypes.data_as(C.c_void_p) if isinstance(buf, np.ndarray) else C.cast(C.c_char_p(bytes(buf)), C.c_void_p)
         t = C.c_uint64()
+        ent = None if predictions is None else _prediction_entries(predictions)
+        n_ent = 0 if ent is None else ent.shape[0]
         if admission is not None:
-            ent = _prediction_entries(predictions) if predictions is not None else np.zeros(0, dtype=PREDICTION_DTYPE)
             pv = admission.get("pred_valid")
             pv = None if pv is None else np.ascontiguousarray(np.asarray(pv, dtype=np.uint8).reshape(-1))
-            if pv is not None and pv.shape[0] != ent.shape[0]:
-                raise ValueError(f"{pv.shape[0]} validity bytes for {ent.shape[0]} predictions")
-            sl = None if subset is None else np.ascontiguousarray(np.asarray(subset, dtype=np.uint32).reshape(-1))
-            if sl is not None and sl.shape[0] == 0:
-                sl = np.zeros(1, dtype=np.uint32)[:0]
-            self._check(self._lib.epp_submit_admit(
-                self._b, model_id, ptr, n, int(multimodal), 0 if sl is None else sl.shape[0],
-                None if sl is None else sl.ctypes.data_as(C.c_void_p), ent.shape[0], _ptr(ent),
-                None if pv is None else pv.ctypes.data_as(C.c_void_p),
+            if pv is not None and pv.shape[0] != n_ent:
+                raise ValueError(f"{pv.shape[0]} validity bytes for {n_ent} predictions")
+        sl = None if subset is None else np.ascontiguousarray(np.asarray(subset, dtype=np.uint32).reshape(-1))
+        if sl is not None and sl.shape[0] == 0:
+            sl = np.zeros(1, dtype=np.uint32)[:0]          # a non-NULL pointer: an empty subset, not the whole pool
+        n_sl = 0 if sl is None else sl.shape[0]
+        if admission is not None:
+            rc = self._lib.epp_submit_admit(
+                self._b, model_id, ptr, n, int(multimodal), n_sl, _ptr(sl), n_ent, _ptr(ent), _ptr(pv),
                 -1 if context_tokens is None else int(context_tokens), int(admission.get("priority", 0)),
-                float(admission.get("ttft_slo", 0.0)), float(admission.get("tpot_slo", 0.0)), C.byref(t)))
-            return t.value
-        if context_tokens is not None:
-            ent = _prediction_entries(predictions) if predictions is not None else np.zeros(0, dtype=PREDICTION_DTYPE)
-            sl = None if subset is None else np.ascontiguousarray(np.asarray(subset, dtype=np.uint32).reshape(-1))
-            if sl is not None and sl.shape[0] == 0:
-                sl = np.zeros(1, dtype=np.uint32)[:0]
-            self._check(self._lib.epp_submit_ctx(self._b, model_id, ptr, n, int(multimodal), 0 if sl is None else sl.shape[0],
-                                                 None if sl is None else sl.ctypes.data_as(C.c_void_p), ent.shape[0],
-                                                 _ptr(ent), int(context_tokens), C.byref(t)))
-            return t.value
-        if predictions is not None:
-            if isinstance(predictions, np.ndarray) and predictions.dtype == PREDICTION_DTYPE:
-                ent = np.ascontiguousarray(predictions)
-            else:
-                ent = np.zeros(len(predictions), dtype=PREDICTION_DTYPE)
-            for i, (sl, tt, th, tp, d) in enumerate(() if ent is predictions else predictions):
-                if not 0 <= int(sl) <= 0xFFFFFFFE:
-                    raise ValueError(f"slot id {sl} out of range")
-                ent[i] = (int(sl), int(d), float(tt), float(th), float(tp))
-            if subset is not None:
-                sl = np.ascontiguousarray(np.asarray(subset, dtype=np.uint32).reshape(-1))
-                self._check(self._lib.epp_submit_subset_predicted(self._b, model_id, ptr, n, int(multimodal), sl.shape[0],
-                                                                  _ptr(sl), ent.shape[0], _ptr(ent), C.byref(t)))
-            else:
-                self._check(self._lib.epp_submit_predicted(self._b, model_id, ptr, n, int(multimodal), ent.shape[0],
-                                                           _ptr(ent), C.byref(t)))
-        elif subset is None:
-            self._check(self._lib.epp_submit(self._b, model_id, ptr, n, int(multimodal), C.byref(t)))
+                float(admission.get("ttft_slo", 0.0)), float(admission.get("tpot_slo", 0.0)), C.byref(t))
+        elif context_tokens is not None:
+            rc = self._lib.epp_submit_ctx(self._b, model_id, ptr, n, int(multimodal), n_sl, _ptr(sl), n_ent, _ptr(ent),
+                                          int(context_tokens), C.byref(t))
+        elif ent is not None and sl is not None:
+            rc = self._lib.epp_submit_subset_predicted(self._b, model_id, ptr, n, int(multimodal), n_sl, _ptr(sl), n_ent,
+                                                       _ptr(ent), C.byref(t))
+        elif ent is not None:
+            rc = self._lib.epp_submit_predicted(self._b, model_id, ptr, n, int(multimodal), n_ent, _ptr(ent), C.byref(t))
+        elif sl is not None:
+            rc = self._lib.epp_submit_subset(self._b, model_id, ptr, n, int(multimodal), n_sl, _ptr(sl), C.byref(t))
         else:
-            sl = np.ascontiguousarray(np.asarray(subset, dtype=np.uint32).reshape(-1))
-            self._check(self._lib.epp_submit_subset(self._b, model_id, ptr, n, int(multimodal), sl.shape[0], _ptr(sl),
-                                                    C.byref(t)))
+            rc = self._lib.epp_submit(self._b, model_id, ptr, n, int(multimodal), C.byref(t))
+        self._check(rc)
         return t.value
 
     def wait(self, ticket: int):
